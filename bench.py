@@ -1,14 +1,14 @@
 #!/usr/bin/env python
 """bench.py -- throughput of the wave-generation hot path (spectrum propagation -> 4 packed N x N
-inverse FFTs -> displacement/normal/foam maps) on B200, per the driver contract.
+inverse FFTs -> displacement/normal/foam maps) on H100, per the driver contract.
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched by torch.distributed.run)
   python bench.py --impl reference ...                      (CPU arm: the oracle on the host cores)
 
 One "step" = one batched update of every cascade resident on a GPU (default workload: BASELINE.json
 configs[1], 256x256 x 4 cascades, batched as --sets independent 4-cascade sets per GPU so that the
-working set, 40 B/texel algorithmic + 64 B/texel scratch, exceeds the 126 MB L2).
-Prints ONE JSON line on rank 0.
+working set, 40 B/texel algorithmic + 64 B/texel scratch, exceeds the 50 MB L2).
+Prints ONE JSON line on rank 0.  --dump-outputs DIR writes the maps of the last timed step (native arm, rank 0).
 """
 from __future__ import annotations
 
@@ -48,27 +48,13 @@ def synth_params(cls, global_index: int):
     return cls(**kw)
 
 
-def ncu_traffic():
-    """DRAM bytes per launch of the dominant kernel from the newest committed ncu capture (profiles/*traffic*.json)."""
-    import glob
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "*traffic*.json")))
-    if not files:
-        return None, None
-    try:
-        with open(files[-1]) as f:
-            t = json.load(f)
-        return float(t["dram_bytes_per_launch"]), os.path.relpath(files[-1], ROOT)
-    except Exception:
-        return None, None
-
-
 def measured_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     try:
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 class ClockSampler:
@@ -203,8 +189,8 @@ def workload_config(args, world: int) -> dict:
     return {"workload": f"{N}x{N} x {args.cascades_per_set} cascades, full pipeline incl. foam, {args.sets} independent sets per GPU per step",
             "map_size": N, "cascades_per_set": args.cascades_per_set, "sets_per_gpu": args.sets,
             "cascades_per_step_per_gpu": C, "parallelism": f"cascade-sharded x{world}, no data-path collective",
-            "l2": (lambda mib: f"working set {mib:.0f} MiB per step " + ("> 126 MB L2 (inputs larger than L2)" if mib * 2**20 > 126e6
-                                                                         else "fits the 126 MB L2 (NOT an HBM-bound measurement)"))(
+            "l2": (lambda mib: f"working set {mib:.0f} MiB per step " + ("> 50 MB L2 (inputs larger than L2)" if mib * 2**20 > 50e6
+                                                                         else "fits the 50 MB L2 (NOT an HBM-bound measurement)"))(
                 (ALGO_BYTES_PER_TEXEL + 64) * C * N * N / 2**20)}
 
 
@@ -282,6 +268,26 @@ def preflight_sharding_check(world: int, local_rank: int, dist):
     return {"ok": True, "what": f"{C} cascades of {N}x{N}, {frames} updates: round-robin over {world} GPU(s) == one GPU, CRC-32 of both RGBA16F maps per cascade"}
 
 
+DUMP_BYTES = 48 << 20       # --dump-outputs budget for both maps together
+
+
+def dump_outputs(out_dir: str, gen, cascades: int, N: int) -> None:
+    """Both RGBA16F maps as the caller of update_all would read them (maps_to_host), widened exactly to float32: every
+    cascade when they fit DUMP_BYTES, else a fixed seeded sample of whole cascades (their indices in cascade_index.npy)."""
+    import numpy as np
+    k = max(1, min(cascades, DUMP_BYTES // (2 * N * N * 4 * 4)))
+    pick = np.sort(np.random.default_rng(0).choice(cascades, k, replace=False))
+    disp = np.empty((k, N, N, 4), np.float32)
+    norm = np.empty((k, N, N, 4), np.float32)
+    for i, c in enumerate(pick):
+        d, n = gen.maps_to_host(int(c), 1)
+        disp[i], norm[i] = d[0], n[0]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "displacement_map.npy"), disp)
+    np.save(os.path.join(out_dir, "normal_map.npy"), norm)
+    np.save(os.path.join(out_dir, "cascade_index.npy"), pick.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -294,10 +300,14 @@ def main():
     ap.add_argument("--cpu-seconds", type=float, default=20.0, help="CPU-baseline sample budget inside the native arm")
     ap.add_argument("--reference-seconds", type=float, default=240.0, help="time budget of the whole --impl reference run")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the displacement / normal maps of the last timed step as DIR/<name>.npy (float32, <= 48 MiB)")
     ap.add_argument("--workload", default="cfg2", choices=["cfg2", "cfg4-strong"],
                     help="cfg2: BASELINE configs[1], weak scaling (default, the driver's contract); cfg4-strong: BASELINE configs[3], "
                          "1024x1024 x 8 cascades split over the GPUs (8/4/2/1 per GPU), strong scaling")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     args.warmup = max(args.warmup, 3)
     # the CPU arm's OpenMP runtime: threads pinned to cores, sleeping (not spinning) between parallel regions -- must be in
     # the environment before the first OpenMP library is loaded
@@ -383,6 +393,8 @@ def main():
     for _ in range(args.steps):
         gen.update_all(delta, params)
     ms = gen.timer_stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, gen, C, N)           # before any further update overwrites the maps
     if len(sampler.samples) < 5:
         # the timed region is only tens of milliseconds and the submitting thread rarely yields the GIL: keep the
         # same workload running (untimed) for ~0.5 s so that NVML sees the clocks under this load
@@ -454,9 +466,6 @@ def main():
         return
 
     peak_gbs, peak_src = measured_peaks()
-    traffic, traffic_src = ncu_traffic()
-    if not (N == 256 and C == 128):
-        traffic, traffic_src = None, None          # the capture is of the default workload only
     step_s = ms * 1e-3 / args.steps
     achieved = ALGO_BYTES_PER_TEXEL * texels_per_step / step_s / 1e9
     line = {
@@ -466,8 +475,6 @@ def main():
         "config": workload_config(args, world),
         "mtexels_per_sec": value * N * N / 1e6,
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak_gbs, "unit": "GB/s", "frac": achieved / peak_gbs,
-                     "traffic": traffic, "traffic_source": traffic_src,
-                     "traffic_kind": "static: dram__bytes_read.sum + dram__bytes_write.sum of one launch from the committed ncu --set full capture, not measured in this run",
                      "peak_source": peak_src,
                      "kernel": "k_update_persistent (one launch per step: time propagation + row IFFT items and column IFFT + map items)",
                      "algorithmic_bytes_per_step": ALGO_BYTES_PER_TEXEL * texels_per_step,

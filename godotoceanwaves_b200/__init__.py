@@ -1,4 +1,4 @@
-"""godotoceanwaves_b200 -- B200-native drop-in for the wave-generation hot path of
+"""godotoceanwaves_b200 -- H100-native drop-in for the wave-generation hot path of
 2Retr0/GodotOceanWaves (spectrum -> time propagation -> packed inverse FFTs -> maps).
 
 The product is the CUDA library ``libocean.so`` (C ABI in ``include/ocean.h``); this package is
@@ -10,7 +10,7 @@ the Python host-side mirror of the reference's GDScript interface for that path:
   RenderingContext.create_push_constant <- assets/render_context.gd:122-135
 
 There is no CPU fallback: importing works anywhere, but creating a generator without the
-compiled extension or without an sm_100 GPU raises ``OceanError``.
+compiled extension or without an sm_90 GPU (H100) raises ``OceanError``.
 """
 from .native import OceanError, load_library, native_library_path  # noqa: F401
 from .render_context import RenderingContext  # noqa: F401

@@ -1,4 +1,4 @@
-"""Builds libocean.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a."""
+"""Builds libocean.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ SOURCES = ["ocean_kernels.cu", "ocean_sample.cu", "ocean_spray.cu", "ocean_api.c
 HEADERS = ["ocean_kernels.cuh", "ocean_texture.cuh", "detmath.cuh", "fft_core.cuh", os.path.join("..", "..", "include", "ocean.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-fmad=false",                      # no implicit contraction: every FMA in the kernels is explicit
     "-Xcompiler", "-fPIC", "-shared",

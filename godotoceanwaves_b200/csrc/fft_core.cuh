@@ -1,4 +1,4 @@
-// fft_core.cuh -- register-resident radix-2 Stockham passes on packed f32x2 lanes (sm_100a).
+// fft_core.cuh -- register-resident radix-2 Stockham passes on lane pairs of fp32 (sm_90a).
 //
 // The reference's inverse FFT (assets/shaders/compute/fft_butterfly.glsl:24-34 + fft_compute.glsl:47-58)
 // is a radix-2 decimation-in-time Stockham network: stage s (stride = 2^s, mid = N >> (s+1))
@@ -31,25 +31,27 @@ __device__ __forceinline__ u64 pk(float lo, float hi) {
 __device__ __forceinline__ void upk(u64 v, float& lo, float& hi) {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
+// Lane-wise operations on a pair.  sm_90 has no packed fp32 instruction: each lane is one scalar FFMA / FMUL / FADD
+// with an explicit .rn rounding, which ptxas never contracts, so every lane rounds exactly once as the GLSL text does.
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-    u64 d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
+    float a0, a1, b0, b1, c0, c1;
+    upk(a, a0, a1); upk(b, b0, b1); upk(c, c0, c1);
+    return pk(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-    u64 d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    float a0, a1, b0, b1;
+    upk(a, a0, a1); upk(b, b0, b1);
+    return pk(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ u64 add2(u64 a, u64 b) {
-    u64 d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    float a0, a1, b0, b1;
+    upk(a, a0, a1); upk(b, b0, b1);
+    return pk(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ u64 sub2(u64 a, u64 b) {
-    u64 d;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    float a0, a1, b0, b1;
+    upk(a, a0, a1); upk(b, b0, b1);
+    return pk(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
 }
 
 // Two complex numbers (spectrum layers a and b of one layer pair) in SoA form.

@@ -2,7 +2,7 @@
 // the reference's WaveGenerator (assets/water/wave_generator.gd:17-121): resource allocation,
 // dirty-flag handling, push-constant rounding (assets/render_context.gd:122-135), the
 // update / _process pending-cascade state machine, and the hand-off of the finished maps.
-// No CPU fallback exists: every compute entry point launches the sm_100a kernels or fails.
+// No CPU fallback exists: every compute entry point launches the sm_90a kernels or fails.
 #include "../../include/ocean.h"
 #include "ocean_kernels.cuh"
 
@@ -410,7 +410,7 @@ int check_cascade(ocean_generator* g, int cascade) {
 extern "C" {
 
 const char* ocean_last_error(void) { return g_last_error.c_str(); }
-const char* ocean_version(void) { return "godotoceanwaves_b200 0.1 (sm_100a)"; }
+const char* ocean_version(void) { return "godotoceanwaves_b200 0.1 (sm_90a)"; }
 
 double ocean_jonswap_alpha(double wind_speed, double fetch_length) {             // wave_generator.gd:116-117
     return 0.076 * std::pow(wind_speed * wind_speed / (fetch_length * kG), 0.22);
@@ -452,8 +452,8 @@ int ocean_create(int device, int map_size, int num_cascades, ocean_generator** o
     OCEAN_CUDA(device_scope.enter(device));
     cudaDeviceProp prop;
     OCEAN_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
-        return fail(OCEAN_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(OCEAN_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
 
     ocean_generator* g = new (std::nothrow) ocean_generator();
     if (!g) return fail(OCEAN_ERR_STATE, "out of host memory");

@@ -1,5 +1,5 @@
 // ocean_kernels.cuh -- launch interface between the C-ABI layer (ocean_api.cu) and the
-// sm_100a kernels (ocean_kernels.cu).  Internal; the public surface is include/ocean.h.
+// sm_90a kernels (ocean_kernels.cu).  Internal; the public surface is include/ocean.h.
 #pragma once
 #include <cstdint>
 #include <cuda.h>

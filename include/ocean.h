@@ -1,5 +1,5 @@
 /*
- * include/ocean.h -- C ABI of libocean.so, the B200-native drop-in for the wave-generation
+ * include/ocean.h -- C ABI of libocean.so, the H100-native drop-in for the wave-generation
  * hot path of 2Retr0/GodotOceanWaves (spectrum -> time propagation -> 4 packed N x N inverse
  * FFTs -> displacement / normal / Jacobian-foam maps).
  *

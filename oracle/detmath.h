@@ -7,7 +7,7 @@
  * IEEE-754 binary64 add/mul/div/fma operations (round-to-nearest-even) whose
  * result is then rounded ONCE to binary32.  Because only correctly-rounded
  * basic operations are used, the same sequence executed by gcc on x86-64
- * (-ffp-contract=off, explicit fma()) and by nvcc on sm_100a (-fmad=false,
+ * (-ffp-contract=off, explicit fma()) and by nvcc on sm_90a (-fmad=false,
  * explicit fma()) yields bit-identical results.  The binary64 results are
  * accurate to ~1e-14 relative, so the binary32 result equals the correctly
  * rounded value of the true function except with probability ~1e-6 per call

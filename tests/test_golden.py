@@ -1,5 +1,5 @@
 """Committed golden vectors (tests/golden/*.json, written by tools/make_golden.py FROM THE REFERENCE'S OWN SHADERS compiled
-for the CPU, oracle/_ref): the C oracle and oracle/_ref reproduce them here, the CUDA path reproduces them on the B200."""
+for the CPU, oracle/_ref): the C oracle and oracle/_ref reproduce them here, the CUDA path reproduces them on the H100."""
 import glob
 import json
 import os

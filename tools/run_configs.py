@@ -77,7 +77,7 @@ def run_spectrum(N, C, reps, label):
     texels = C * N * N
     out = {"config": label, "map_size": N, "cascades": C, "kernel": "k_spectrum_compute", "us_per_launch": 1e3 * ms,
            "gtexels_per_s": texels / (ms * 1e-3) / 1e9, "algorithmic_GBps": 16.0 * texels / (ms * 1e-3) / 1e9,
-           "frac_of_hbm_peak_6572.5": 16.0 * texels / (ms * 1e-3) / 1e9 / 6572.5, "bound": "fp64 pipe (see profiles/r02_spectrum_summary.txt)"}
+           "frac_of_hbm_datasheet_3350": 16.0 * texels / (ms * 1e-3) / 1e9 / 3350.0, "bound": "fp64 pipe"}
     g.free()
     print(json.dumps(out), flush=True)
 
