@@ -41,6 +41,16 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanSurfaceSample                         // struct ocean_surface_sample (40 B) <- water.gdshader:28,37 inverted
+    {
+        public float source_x, source_z;
+        public fixed float displacement[3];                         // displacement[1] = water height at the query point
+        public fixed float gradient_foam[3];                        // normal = normalize(-g.x, 1, -g.y), water.gdshader:90
+        public float residual;
+        public uint iterations;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public struct OceanInfo
     {
         public int device, map_size, num_cascades, pending_cascades;
@@ -111,6 +121,10 @@ namespace OceanB200
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_extract_spray(IntPtr handle, int num_candidates, float* points_xz, int num_cascades, float* map_scales,
                                                         float* particle_scale, int max_records, OceanSprayRecord* records, int* num_active);
+        // surface query: the surface at world positions points [n][2] (P + D_xz(P) = Q solved for P, then the map query at P)
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,
+                                                        float tolerance, int max_iterations, OceanSurfaceSample* samples);
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_get_info(IntPtr handle, OceanInfo* info);
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]

@@ -65,6 +65,10 @@ struct ocean_generator {
     int spray_count_capacity = 0;
     void* spray_records = nullptr;                      // spray op staging for the host entry point
     size_t spray_record_capacity = 0;
+    int* surf_scratch = nullptr;                        // surface query scratch: pending count, layer maxima, pending list
+    size_t surf_scratch_capacity = 0;                   // (ints), grown on demand
+    ocean_surface_sample* surf_records = nullptr;       // surface query staging for the host entry point
+    size_t surf_record_capacity = 0;
     ocean::CascadeDispatch* d_cascade = nullptr;        // [num_cascades] (two-kernel path only)
     ocean::SpectrumDispatch* d_spectrum = nullptr;      // [num_cascades]
     ocean::TableDispatch* d_tables = nullptr;           // [num_cascades]
@@ -161,6 +165,8 @@ void release(ocean_generator* g) {
     if (g->snap_free) cudaEventDestroy(g->snap_free);
     cudaFree(g->spray_counts);
     cudaFree(g->spray_records);
+    cudaFree(g->surf_scratch);
+    cudaFree(g->surf_records);
     cudaFree(g->d_cascade);
     cudaFree(g->d_spectrum);
     cudaFree(g->d_queue);
@@ -949,6 +955,19 @@ int upload_scales(ocean_generator* gen, int num_cascades, const float* map_scale
     OCEAN_CUDA(cudaMemcpyAsync(gen->q_scales, map_scales_host, sizeof(float4) * (size_t)num_cascades, cudaMemcpyHostToDevice, gen->stream));
     return OCEAN_OK;
 }
+
+// The host-side query entry points stage their points (and the map-query outputs) in buffers they share, grown on demand.
+int grow_query_staging(ocean_generator* gen, size_t n) {
+    if (n <= gen->q_capacity) return OCEAN_OK;
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    cudaFree(gen->q_points); cudaFree(gen->q_disp); cudaFree(gen->q_grad);
+    gen->q_points = nullptr; gen->q_disp = gen->q_grad = nullptr; gen->q_capacity = 0;
+    OCEAN_CUDA(dev_alloc(gen, &gen->q_points, n));
+    OCEAN_CUDA(dev_alloc(gen, &gen->q_disp, 3 * n));
+    OCEAN_CUDA(dev_alloc(gen, &gen->q_grad, 3 * n));
+    gen->q_capacity = n;
+    return OCEAN_OK;
+}
 }  // namespace
 
 int ocean_sample_maps_device(ocean_generator* gen, int num_points, const float* points_xz_dev, int num_cascades, const float* map_scales_host,
@@ -973,15 +992,7 @@ int ocean_sample_maps(ocean_generator* gen, int num_points, const float* points_
     if (num_points == 0) return OCEAN_OK;
     if (!points_xz_host || !displacement_host || !gradient_foam_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
     const size_t n = (size_t)num_points;
-    if (n > gen->q_capacity) {
-        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-        cudaFree(gen->q_points); cudaFree(gen->q_disp); cudaFree(gen->q_grad);
-        gen->q_points = nullptr; gen->q_disp = gen->q_grad = nullptr; gen->q_capacity = 0;
-        OCEAN_CUDA(dev_alloc(gen, &gen->q_points, n));
-        OCEAN_CUDA(dev_alloc(gen, &gen->q_disp, 3 * n));
-        OCEAN_CUDA(dev_alloc(gen, &gen->q_grad, 3 * n));
-        gen->q_capacity = n;
-    }
+    if ((rc = grow_query_staging(gen, n))) return rc;
     OCEAN_CUDA(cudaMemcpyAsync(gen->q_points, points_xz_host, sizeof(float2) * n, cudaMemcpyHostToDevice, gen->stream));
     if ((rc = ocean_sample_maps_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points), num_cascades, map_scales_host,
                                        gen->q_disp, gen->q_grad)))
@@ -1062,15 +1073,7 @@ int ocean_extract_spray(ocean_generator* gen, int num_candidates, const float* p
     if (num_candidates == 0) return OCEAN_OK;
     if (!points_xz_host || (max_records > 0 && !records_host)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
     const size_t n = (size_t)num_candidates;
-    if (n > gen->q_capacity) {                       // the candidate staging buffer is shared with the map-query op
-        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-        cudaFree(gen->q_points); cudaFree(gen->q_disp); cudaFree(gen->q_grad);
-        gen->q_points = nullptr; gen->q_disp = gen->q_grad = nullptr; gen->q_capacity = 0;
-        OCEAN_CUDA(dev_alloc(gen, &gen->q_points, n));
-        OCEAN_CUDA(dev_alloc(gen, &gen->q_disp, 3 * n));
-        OCEAN_CUDA(dev_alloc(gen, &gen->q_grad, 3 * n));
-        gen->q_capacity = n;
-    }
+    if ((rc = grow_query_staging(gen, n))) return rc;
     const size_t rec_bytes = ((size_t)max_records + 1) * sizeof(ocean_spray_record);    // + one slot for the count
     if (rec_bytes > gen->spray_record_capacity) {
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
@@ -1093,6 +1096,67 @@ int ocean_extract_spray(ocean_generator* gen, int num_candidates, const float* p
     const int kept = count < max_records ? count : max_records;
     if (kept > 0) OCEAN_CUDA(cudaMemcpy(records_host, recs, sizeof(ocean_spray_record) * (size_t)kept, cudaMemcpyDeviceToHost));
     *num_active = count;
+    return OCEAN_OK;
+}
+
+// ---- surface query: the surface at a world position (inverse of the horizontal displacement, then the map query) ----
+static_assert(sizeof(ocean_surface_sample) == 40, "ocean_surface_sample layout");
+
+namespace {
+int check_surface_args(int num_points, float tolerance, int max_iterations) {
+    if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
+    if (!(tolerance > 0.0f) || !std::isfinite(tolerance)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "tolerance %g is not finite and > 0", tolerance);
+    if (max_iterations < 0 || max_iterations > 64) return fail(OCEAN_ERR_INVALID_ARGUMENT, "max_iterations %d outside [0, 64]", max_iterations);
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_query_surface_device(ocean_generator* gen, int num_points, const float* points_xz_dev, int num_cascades, const float* map_scales_host,
+                               float tolerance, int max_iterations, ocean_surface_sample* out_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_surface_args(num_points, tolerance, max_iterations))) return rc;
+    if (num_points == 0) return OCEAN_OK;
+    if (!points_xz_dev || !out_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
+    const size_t ints = ocean::surface_scratch_ints(gen->num_cascades, num_points);
+    if (ints > gen->surf_scratch_capacity) {
+        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+        cudaFree(gen->surf_scratch);
+        gen->surf_scratch = nullptr;
+        gen->surf_scratch_capacity = 0;
+        OCEAN_CUDA(dev_alloc(gen, &gen->surf_scratch, ints));
+        gen->surf_scratch_capacity = ints;
+    }
+    OCEAN_CUDA(ocean::launch_query_surface(gen->buf, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_points, gen->q_scales,
+                                           tolerance, max_iterations, out_dev, gen->surf_scratch, gen->stream));
+    gen->kernel_launches += max_iterations > 0 ? 3 : 1;
+    return OCEAN_OK;
+}
+
+int ocean_query_surface(ocean_generator* gen, int num_points, const float* points_xz_host, int num_cascades, const float* map_scales_host,
+                        float tolerance, int max_iterations, ocean_surface_sample* out_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_surface_args(num_points, tolerance, max_iterations))) return rc;
+    if (num_points == 0) return OCEAN_OK;
+    if (!points_xz_host || !out_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
+    const size_t n = (size_t)num_points;
+    if ((rc = grow_query_staging(gen, n))) return rc;
+    if (n > gen->surf_record_capacity) {
+        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+        cudaFree(gen->surf_records);
+        gen->surf_records = nullptr;
+        gen->surf_record_capacity = 0;
+        OCEAN_CUDA(dev_alloc(gen, &gen->surf_records, n));
+        gen->surf_record_capacity = n;
+    }
+    OCEAN_CUDA(cudaMemcpyAsync(gen->q_points, points_xz_host, sizeof(float2) * n, cudaMemcpyHostToDevice, gen->stream));
+    if ((rc = ocean_query_surface_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points), num_cascades, map_scales_host,
+                                         tolerance, max_iterations, gen->surf_records)))
+        return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->surf_records, sizeof(ocean_surface_sample) * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
 

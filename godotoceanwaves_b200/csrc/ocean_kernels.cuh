@@ -117,6 +117,11 @@ cudaError_t launch_rowpass_export(const DeviceBuffers& b, int scratch_layer, flo
 // ocean_sample.cu: batched map queries (water.gdshader:27-39,42-84); scales_dev = map_scales[num_cascades] as float4
 cudaError_t launch_sample_maps(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
                                float* disp_out_dev, float* grad_out_dev, cudaStream_t stream);
+// ocean_sample.cu: surface query (P + D_xz(P) = Q solved for P, then sampled; oracle/surface.py); out_dev = ocean_surface_sample[n],
+// scratch_dev = [surface_scratch_ints(num_cascades, n)] ints
+size_t surface_scratch_ints(int num_cascades, int n);
+cudaError_t launch_query_surface(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
+                                 float tolerance, int max_iterations, void* out_dev, int* scratch_dev, cudaStream_t stream);
 
 // ocean_spray.cu: spray candidates (sea_spray_particle.gdshader:80-94) as a stable stream compaction; counts_dev is
 // [spray_blocks(n) + 1] ints of scratch whose last element receives the number of active candidates

@@ -230,6 +230,22 @@ class WaveGenerator:
                                                disp.ctypes.data, grad.ctypes.data))
         return disp, grad
 
+    # -- surface query: the surface at a world position (inverts the horizontal displacement, then samples) ----------
+    SURFACE_SAMPLE = np.dtype([("source_x", np.float32), ("source_z", np.float32), ("displacement", np.float32, 3),
+                               ("gradient_foam", np.float32, 3), ("residual", np.float32), ("iterations", np.uint32)])  # struct ocean_surface_sample
+
+    def query_surface(self, points_xz, map_scales, tolerance: float = 1e-3, max_iterations: int = 8) -> np.ndarray:
+        """SURFACE_SAMPLE rows for world positions points_xz [n][2]: the undisplaced point P whose rendered surface point
+        lies over the query (P + D_xz(P) = Q within `tolerance` where residual <= tolerance), and the maps sampled at P:
+        displacement[1] is the water height at Q, normalize(-g.x, 1, -g.y) of gradient_foam the normal (include/ocean.h)."""
+        self._require()
+        pts = np.ascontiguousarray(points_xz, np.float32).reshape(-1, 2)
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        out = np.zeros(pts.shape[0], self.SURFACE_SAMPLE)
+        check(load_library().ocean_query_surface(self.context, pts.shape[0], pts.ctypes.data, sc.shape[0], sc.ctypes.data,
+                                                 float(tolerance), int(max_iterations), out.ctypes.data))
+        return out
+
     # -- spray candidates: the spawn test of sea_spray_particle.gdshader:80-94 as a stream compaction --------------
     SPRAY_RECORD = np.dtype([("index", np.uint32), ("start_x", np.float32), ("start_z", np.float32), ("scale_factor", np.float32),
                              ("particle_scale", np.float32, 3), ("foam", np.float32)])     # struct ocean_spray_record

@@ -167,7 +167,8 @@ int ocean_set_spectrum_amplitudes(ocean_generator* gen, int cascade, const float
  * that the agreement can be checked without a GPU (tests/test_abi_cpu.py). */
 float ocean_detmath_expf(float x);
 
-/* Batched map queries -- the sampling contract of the water shader as an op (what buoyancy / gameplay code needs):
+/* Batched map queries -- the sampling contract of the water shader as an op, at UNDISPLACED points (the surface at a
+ * world position, what buoyancy / gameplay code needs, is ocean_query_surface below):
  *   displacement[p]   = sum_i texture(displacements, vec3(xz*scales_i.xy, i)).xyz * scales_i.z         water.gdshader:27-39
  *   gradient_foam[p]  = sum_i mix(texture_bicubic(normals, c_i), texture(normals, c_i), min(1, ppm_i*0.1)).xyw
  *                             * vec3(scales_i.ww, 1),  ppm_i = map_size * min(scales_i.x, scales_i.y)   water.gdshader:42-84
@@ -181,6 +182,37 @@ int ocean_sample_maps(ocean_generator* gen, int num_points, const float* points_
                       float* displacement_host, float* gradient_foam_host);
 int ocean_sample_maps_device(ocean_generator* gen, int num_points, const float* points_xz_dev, int num_cascades, const float* map_scales_host,
                              float* displacement_dev, float* gradient_foam_dev);
+
+/* Surface query -- the water surface at a WORLD position, what a boat, a buoy or a splash test asks.  ocean_sample_maps
+ * reads the maps at the undisplaced grid point (UV = VERTEX.xz before VERTEX += displacement, water.gdshader:28,37), so
+ * the rendered point it describes sits at P + D_xz(P), not at P.  For each point Q this op solves P + D_xz(P) = Q for P
+ * (damped Newton steps on the bilinear displacement sum and its exact Jacobian; where det(I + J) <= 1e-3 a fixed-point
+ * step; if the start from Q does not converge, restarts from Q - D_xz(Q) and from Q +- rho along x and z, rho = half the
+ * horizontal displacement bound of the maps) and then samples the maps at P as ocean_sample_maps does:
+ *   source_x/z     P, the undisplaced point whose rendered surface point is (P.x + dx, dy, P.z + dz)
+ *   displacement   D(P); the water height at Q is displacement[1]
+ *   gradient_foam  the gradient and foam at P; the normal is normalize(-g.x, 1, -g.y) (water.gdshader:90)
+ *   residual       max(|E.x|, |E.z|), E = P + D_xz(P) - Q; the point converged iff residual <= tolerance
+ *   iterations     Newton steps taken over all starts
+ * The end point with the smallest residual is returned, converged or not.  max_iterations = 0 returns the map query at Q
+ * unchanged (source = Q).  oracle/surface.py is the specification (binary32, bit-exact).
+ * Limits: the query describes the surface as rendered within 150 m of the camera, where distance_factor is exactly 1
+ * (water.gdshader:29); the camera-dependent flattening beyond that is render LOD and is not modelled.  Where the surface
+ * folds, several points P may map to Q, and any converged one may be returned.  tolerance (metres) must exceed a few
+ * binary32 ulps of |Q|, or points far from the origin cannot converge.  tolerance must be finite and > 0, max_iterations in
+ * [0, 64].  ocean_query_surface takes host buffers and is synchronous; ocean_query_surface_device takes device pointers for
+ * the points and the records (map_scales stays a host array) and is asynchronous on the generator's stream. */
+typedef struct ocean_surface_sample {
+    float source_x, source_z;
+    float displacement[3];
+    float gradient_foam[3];
+    float residual;
+    uint32_t iterations;
+} ocean_surface_sample;   /* 40 B */
+int ocean_query_surface(ocean_generator* gen, int num_points, const float* points_xz_host, int num_cascades, const float* map_scales_host,
+                        float tolerance, int max_iterations, ocean_surface_sample* out_host);
+int ocean_query_surface_device(ocean_generator* gen, int num_points, const float* points_xz_dev, int num_cascades, const float* map_scales_host,
+                               float tolerance, int max_iterations, ocean_surface_sample* out_dev);
 
 /* Spray candidates -- the spawn test of the sea-spray particle shader as a stream-compaction op
  * (assets/shaders/spatial/sea_spray_particle.gdshader:80-94; the reference evaluates it for every particle of the emitter and

@@ -162,6 +162,51 @@ def run_query(N, C, n_points, reps, label):
     print(json.dumps(out), flush=True)
 
 
+def run_surface(N, C, n_points, reps, label, tolerance=1e-3, max_iterations=8):
+    """Surface-query op (ocean_query_surface_device) on device-resident points: kernel time from CUDA events, against
+    ocean_sample_maps_device on the same points in the same run.  restarted = points that took more than max_iterations
+    steps, i.e. ran the restart kernel (a first start that stalls early and then converges on a restart is not counted)."""
+    import numpy as np
+    import torch
+    from godotoceanwaves_b200.native import load_library, check
+    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
+    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
+    for _ in range(2):
+        g.update_all(0.02, p)
+    scales = gow.WaveGenerator.map_scales(p)
+    dev = torch.device("cuda", 0)
+    pts = (torch.rand(n_points, 2, device=dev, generator=torch.Generator(dev).manual_seed(1)) * 600.0 - 300.0).contiguous()
+    recs = torch.empty(n_points * 10, dtype=torch.int32, device=dev)        # ocean_surface_sample: 40 B
+    disp = torch.empty(n_points, 3, device=dev)
+    grad = torch.empty(n_points, 3, device=dev)
+    torch.cuda.synchronize()
+    lib = load_library()
+    query = lambda: check(lib.ocean_query_surface_device(g.context, n_points, pts.data_ptr(), C, scales.ctypes.data, tolerance, max_iterations,
+                                                         recs.data_ptr()))
+    sample = lambda: check(lib.ocean_sample_maps_device(g.context, n_points, pts.data_ptr(), C, scales.ctypes.data, disp.data_ptr(), grad.data_ptr()))
+
+    def timed(call):
+        for _ in range(3):
+            call()
+        g.synchronize()
+        g.timer_start()
+        for _ in range(reps):
+            call()
+        return g.timer_stop() / reps
+
+    t_query, t_sample = timed(query), timed(sample)
+    t_query = min(t_query, timed(query))        # alternate: the first window also absorbs clock ramp-up
+    rec = recs.cpu().numpy().view(gow.WaveGenerator.SURFACE_SAMPLE)
+    out = {"config": label, "map_size": N, "cascades": C, "points": n_points, "tolerance": tolerance, "max_iterations": max_iterations,
+           "us_per_call": 1e3 * t_query, "mpoints_per_s": n_points / (t_query * 1e-3) / 1e6, "sample_maps_us_per_call": 1e3 * t_sample,
+           "ratio_to_sample_maps": t_query / t_sample, "frac_restarted": float(np.mean(rec["iterations"] > max_iterations)),
+           "frac_converged": float(np.mean(rec["residual"] <= np.float32(tolerance))), "mean_iterations": float(np.mean(rec["iterations"]))}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
 if "--query" in sys.argv or os.environ.get("OCEAN_RUN_QUERY", "1") != "0":
     run_query(256, 4, 1 << 20, 50, "query op: 2^20 random points x 4 cascades of 256x256 (maps L2-resident)")
     run_query(1024, 8, 1 << 20, 20, "query op: 2^20 random points x 8 cascades of 1024x1024 (maps 128 MiB)")
+    run_surface(256, 4, 1 << 20, 50, "surface query: 2^20 points in [-300, 300]^2 m x 4 cascades of 256x256")
+    run_surface(1024, 8, 1 << 20, 20, "surface query: 2^20 points in [-300, 300]^2 m x 8 cascades of 1024x1024")
