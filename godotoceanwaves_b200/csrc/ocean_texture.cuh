@@ -19,13 +19,20 @@ __device__ __forceinline__ float4 mix4(const float4 a, const float4 b, float t) 
     return make_float4(mixf(a.x, b.x, t), mixf(a.y, b.y, t), mixf(a.z, b.z, t), mixf(a.w, b.w, t));
 }
 
-// texture(): bilinear, REPEAT.  N is a power of two (128..1024), so the wrap is a mask.
+// REPEAT texel index of floor(x): x0 mod N.  N is a power of two (128..1024), so the wrap is a mask.  The conversion to
+// int64 saturates beyond +-2^63, so x0 is clamped to [-2^62, 2^62] first; that is exact, because every binary32 of
+// magnitude >= 2^62 is a multiple of 2^39, hence of N, and so is 2^62.  fmaxf sends NaN to -2^62, i.e. to texel 0.
+__device__ __forceinline__ int wrap_texel(float x0, int N) {
+    return (int)(long long)fminf(fmaxf(x0, -0x1p62f), 0x1p62f) & (N - 1);
+}
+
+// texture(): bilinear, REPEAT.
 __device__ __forceinline__ float4 texture_bilinear(const uint2* __restrict__ layer, int N, float u, float v) {
     const float n = (float)N;
     const float x = u * n - 0.5f, y = v * n - 0.5f;
     const float x0 = floorf(x), y0 = floorf(y);
     const float fx = x - x0, fy = y - y0;
-    const int ix0 = (int)(long long)x0 & (N - 1), iy0 = (int)(long long)y0 & (N - 1);
+    const int ix0 = wrap_texel(x0, N), iy0 = wrap_texel(y0, N);
     const int ix1 = (ix0 + 1) & (N - 1), iy1 = (iy0 + 1) & (N - 1);
     const float4 t00 = texel(layer, N, ix0, iy0), t10 = texel(layer, N, ix1, iy0);
     const float4 t01 = texel(layer, N, ix0, iy1), t11 = texel(layer, N, ix1, iy1);
@@ -40,7 +47,7 @@ __device__ __forceinline__ float4 texture_bilinear_slopes(const uint2* __restric
     const float x = u * n - 0.5f, y = v * n - 0.5f;
     const float x0 = floorf(x), y0 = floorf(y);
     const float fx = x - x0, fy = y - y0;
-    const int ix0 = (int)(long long)x0 & (N - 1), iy0 = (int)(long long)y0 & (N - 1);
+    const int ix0 = wrap_texel(x0, N), iy0 = wrap_texel(y0, N);
     const int ix1 = (ix0 + 1) & (N - 1), iy1 = (iy0 + 1) & (N - 1);
     const float4 t00 = texel(layer, N, ix0, iy0), t10 = texel(layer, N, ix1, iy0);
     const float4 t01 = texel(layer, N, ix0, iy1), t11 = texel(layer, N, ix1, iy1);

@@ -30,6 +30,14 @@ def _mix(a, b, t):
     return a * (F(1.0) - t) + b * t
 
 
+def wrap_texel(x0: np.ndarray, N: int) -> np.ndarray:
+    """REPEAT texel index x0 mod N of floor(x) = x0, defined for every binary32: x0 is clamped to [-2^62, 2^62] before
+    the conversion to int64, which is exact (a binary32 of magnitude >= 2^62 is a multiple of 2^39, hence of N, and so is
+    2^62); fmax sends NaN to -2^62, i.e. to texel 0."""
+    lim = F(2.0 ** 62)
+    return np.mod(np.fmin(np.fmax(x0, -lim), lim).astype(np.int64), N)
+
+
 def texture_bilinear(tex: np.ndarray, u: np.ndarray, v: np.ndarray) -> np.ndarray:
     """tex: [N][N][4] float16 (row y, column x); u, v: float32 [n] normalised coordinates.  Returns float32 [n][4]."""
     N = tex.shape[0]
@@ -40,8 +48,8 @@ def texture_bilinear(tex: np.ndarray, u: np.ndarray, v: np.ndarray) -> np.ndarra
     y0 = np.floor(y)
     fx = (x - x0)[:, None]
     fy = (y - y0)[:, None]
-    ix0 = np.mod(x0.astype(np.int64), N)
-    iy0 = np.mod(y0.astype(np.int64), N)
+    ix0 = wrap_texel(x0, N)
+    iy0 = wrap_texel(y0, N)
     ix1 = np.mod(ix0 + 1, N)
     iy1 = np.mod(iy0 + 1, N)
     t = tex.astype(np.float32)

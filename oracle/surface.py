@@ -34,7 +34,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .sampling import F, _mix, sample_maps, texture_bilinear
+from .sampling import F, _mix, sample_maps, texture_bilinear, wrap_texel
 
 RECORD = np.dtype([("source_x", np.float32), ("source_z", np.float32), ("displacement", np.float32, 3),
                    ("gradient_foam", np.float32, 3), ("residual", np.float32), ("iterations", np.uint32)])   # 40 B
@@ -52,8 +52,8 @@ def bilinear_slopes(tex: np.ndarray, u: np.ndarray, v: np.ndarray):
     y0 = np.floor(y)
     fx = (x - x0)[:, None]
     fy = (y - y0)[:, None]
-    ix0 = np.mod(x0.astype(np.int64), N)
-    iy0 = np.mod(y0.astype(np.int64), N)
+    ix0 = wrap_texel(x0, N)
+    iy0 = wrap_texel(y0, N)
     ix1 = np.mod(ix0 + 1, N)
     iy1 = np.mod(iy0 + 1, N)
     t = tex.astype(np.float32)

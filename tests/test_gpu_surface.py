@@ -7,7 +7,7 @@ import pytest
 
 from conftest import demo_params
 from oracle import surface as su
-from test_gpu_sampling import _gen, _points
+from test_gpu_sampling import _aniso_gen, _extreme_points, _gen, _points, _same_or_both_nan
 
 pytestmark = pytest.mark.gpu
 
@@ -19,7 +19,13 @@ def _scales(gow, params, C):
     return scales
 
 
-@pytest.mark.parametrize("N,C", [(128, 3), (256, 4), (512, 2)])
+def _records_match(rec, ref):
+    """bit-identical records, except that a NaN only has to meet a NaN (see _same_or_both_nan)"""
+    return all(_same_or_both_nan(rec[f], ref[f]) for f in ("source_x", "source_z", "displacement", "gradient_foam", "residual")) and \
+        np.array_equal(rec["iterations"], ref["iterations"])
+
+
+@pytest.mark.parametrize("N,C", [(128, 3), (256, 4), (512, 2), (1024, 2)])
 def test_query_surface_bit_exact(N, C):
     gow, g, params = _gen(N, C)
     d16, n16 = g.maps_to_host(0, C)
@@ -54,6 +60,55 @@ def test_query_surface_device_equals_host():
     check(load_library().ocean_query_surface_device(g.context, pts.shape[0], pts_d.data_ptr(), 4, scales.ctypes.data, 1e-3, 8, out_d.data_ptr()))
     g.synchronize()
     assert out_d.cpu().numpy().tobytes() == host.tobytes()
+    g.free()
+
+
+def test_query_surface_anisotropic_signed_scales():
+    """Non-square tiles make the Jacobian terms du*s.x and dv*s.y differ; negative displacement and normal scales."""
+    gow, g, scales = _aniso_gen()
+    d16, n16 = g.maps_to_host(0, 4)
+    pts = _points(20000, 33, 300.0)
+    rec = g.query_surface(pts, scales, 1e-3, 8)
+    ref = su.query_surface(d16, n16, pts, scales, 1e-3, 8)
+    assert rec.tobytes() == ref.tobytes()
+    assert np.any(rec["iterations"] > 8)                        # the restart kernel ran
+    assert np.mean(rec["residual"] <= np.float32(1e-3)) > 0.95
+    g.free()
+
+
+def test_query_surface_extreme_coordinates():
+    """Huge, overflowing and non-finite world positions.  A non-finite query has a NaN residual: the GPU sends it to the
+    restart list (r <= tol is false) and the specification does not (r > tol is false), yet both take no step."""
+    gow, g, params = _gen(256, 4)
+    d16, n16 = g.maps_to_host(0, 4)
+    scales = _scales(gow, params, 4)
+    pts, mask = _extreme_points(4000, 43)
+    rec = g.query_surface(pts, scales, 1e-3, 8)
+    with np.errstate(all="ignore"):
+        ref = su.query_surface(d16, n16, pts, scales, 1e-3, 8)
+    assert _records_match(rec, ref)
+    bad = ~np.isfinite(pts).all(1)
+    for r in (rec[bad], ref[bad]):
+        assert np.all(r["iterations"] == 0) and np.isnan(r["residual"]).all()
+        assert np.isnan(r["displacement"]).all() and np.isnan(r["gradient_foam"]).all()
+    assert g.query_surface(pts[~mask], scales, 1e-3, 8).tobytes() == rec[~mask].tobytes()
+    g.free()
+
+
+def test_query_surface_restart_grid_stride():
+    """More pending queries than k_surface_restart has threads (2048 blocks x 64): every thread runs its grid-stride loop
+    more than once."""
+    gow, g, params = _gen(256, 4)
+    d16, n16 = g.maps_to_host(0, 4)
+    scales = _scales(gow, params, 4)
+    scales[:, 2] *= np.float32(2.0)
+    pts = _points(200000, 47, 300.0)
+    tol = np.float32(1e-6)
+    qx, qz = pts[:, 0].copy(), pts[:, 1].copy()
+    _, _, r0, _ = su._solve(d16, scales, qx, qz, qx, qz, tol, 1)
+    assert np.count_nonzero(r0 > tol) > 2048 * 64                # pending after the first start
+    rec = g.query_surface(pts, scales, 1e-6, 1)
+    assert rec.tobytes() == su.query_surface(d16, n16, pts, scales, 1e-6, 1).tobytes()
     g.free()
 
 

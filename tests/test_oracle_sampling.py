@@ -23,6 +23,36 @@ def test_bilinear_hits_texel_centres_and_wraps():
         assert np.array_equal(sp.texture_bilinear(t, u + np.float32(shift), v - np.float32(shift)), out)
 
 
+def test_bilinear_wraps_beyond_the_int64_range():
+    """At |u*N| >= 2^63 the texel index still follows REPEAT addressing (floor(u*N - 0.5) mod N, computed here with
+    Python integers), without a RuntimeWarning from an out-of-range conversion; so does bilinear_slopes."""
+    import warnings
+    from oracle import surface as su
+    N = 8
+    t = _tex(N, 9)
+    # x = u*N - 0.5 rounds to u*N at these magnitudes, all beyond 2^63 (3e37*8 near FLT_MAX); the saturating conversion
+    # of the GPU would give INT64_MAX mod N = N - 1 for the positive ones, REPEAT gives texel 0
+    big =np.array([1e20, -1e20, 2.0 ** 61, -(2.0 ** 61), 3e37, -3e37, 3.0 * 2.0 ** 61, 1e19], np.float32)
+    v = np.full(big.size, np.float32(2.5 / N), np.float32)               # texel row 2, fy = 0
+    with warnings.catch_warnings():
+        warnings.simplefilter("error")
+        out = sp.texture_bilinear(t, big, v)
+        du, dv = su.bilinear_slopes(t, big, v)
+    x = big * np.float32(N) - np.float32(0.5)
+    assert np.all(np.abs(x) >= 2.0 ** 63) and np.array_equal(x, np.floor(x))
+    ix = [int(xi) % N for xi in x]                                          # exact: Python int of a binary32
+    assert np.array_equal(out, t.astype(np.float32)[2, ix])
+    # the same texels at an in-range coordinate: u = (ix + 0.5) / N
+    u_in = ((np.array(ix) + 0.5) / N).astype(np.float32)
+    assert np.array_equal(out, sp.texture_bilinear(t, u_in, v))
+    du_in, dv_in = su.bilinear_slopes(t, u_in, v)
+    assert np.array_equal(du, du_in) and np.array_equal(dv, dv_in)
+    # NaN and infinities: index 0, NaN fields
+    with np.errstate(invalid="ignore"):
+        odd = sp.texture_bilinear(t, np.array([np.nan, np.inf, -np.inf], np.float32), v[:3])
+    assert np.isnan(odd).all()
+
+
 def test_bilinear_matches_scipy_grid_wrap():
     ndi = pytest.importorskip("scipy.ndimage")
     N = 128
