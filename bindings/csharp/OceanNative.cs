@@ -51,6 +51,32 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanBuoyancyPoint                         // struct ocean_buoyancy_point (20 B), body-local
+    {
+        public fixed float position[3];
+        public float volume;                                        // m^3 of the vertical column element centred on the point
+        public float half_height;                                   // m above and below the point
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanBuoyancyBody                          // struct ocean_buoyancy_body (56 B)
+    {
+        public fixed float transform[12];                           // 3 x 4 row-major body-to-world [R | t]
+        public int first_point, num_points;                         // hull-point range; bodies may share a hull
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanBuoyancyResult                        // struct ocean_buoyancy_result (48 B)
+    {
+        public fixed float force[3];                                // apply_force(force, center_offset) in Godot
+        public fixed float torque[3];                               // about the body origin
+        public float submerged_volume;
+        public fixed float center_offset[3];                        // centre of buoyancy - body origin
+        public float max_residual;
+        public uint unconverged;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public struct OceanInfo
     {
         public int device, map_size, num_cascades, pending_cascades;
@@ -125,6 +151,15 @@ namespace OceanB200
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,
                                                         float tolerance, int max_iterations, OceanSurfaceSample* samples);
+        // buoyancy: per-body force and torque from hull points on the surface; samples may be null
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_buoyancy(IntPtr handle, int num_bodies, OceanBuoyancyBody* bodies, int num_points, OceanBuoyancyPoint* points,
+                                                   int num_cascades, float* map_scales, float density, float tolerance, int max_iterations,
+                                                   OceanBuoyancyResult* results, OceanSurfaceSample* samples);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_buoyancy_device(IntPtr handle, int num_bodies, OceanBuoyancyBody* bodies, int num_points, void* points_dev,
+                                                          int num_cascades, float* map_scales, float density, float tolerance, int max_iterations,
+                                                          void* results_dev, void* samples_dev);
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_get_info(IntPtr handle, OceanInfo* info);
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]

@@ -69,6 +69,21 @@ struct ocean_generator {
     size_t surf_scratch_capacity = 0;                   // (ints), grown on demand
     ocean_surface_sample* surf_records = nullptr;       // surface query staging for the host entry point
     size_t surf_record_capacity = 0;
+    // buoyancy staging, each grown on demand: body table and world-point offsets, query positions, surface records (when the
+    // caller wants none), and the host entry point's hull points and results
+    ocean_buoyancy_body* buoy_bodies = nullptr;
+    size_t buoy_bodies_capacity = 0;
+    int* buoy_offsets = nullptr;
+    size_t buoy_offsets_capacity = 0;
+    std::vector<int> buoy_offsets_host;
+    float2* buoy_q = nullptr;
+    size_t buoy_q_capacity = 0;
+    ocean_surface_sample* buoy_samples = nullptr;
+    size_t buoy_samples_capacity = 0;
+    ocean_buoyancy_point* buoy_points = nullptr;
+    size_t buoy_points_capacity = 0;
+    ocean_buoyancy_result* buoy_results = nullptr;
+    size_t buoy_results_capacity = 0;
     ocean::CascadeDispatch* d_cascade = nullptr;        // [num_cascades] (two-kernel path only)
     ocean::SpectrumDispatch* d_spectrum = nullptr;      // [num_cascades]
     ocean::TableDispatch* d_tables = nullptr;           // [num_cascades]
@@ -137,6 +152,20 @@ cudaError_t dev_alloc(ocean_generator* g, T** p, size_t count) {
     return e;
 }
 
+// A staging buffer of at least n elements (grown on demand; its contents are not kept).
+template <typename T>
+int grow_buffer(ocean_generator* g, T** p, size_t* capacity, size_t n) {
+    if (n <= *capacity) return OCEAN_OK;
+    OCEAN_CUDA(cudaStreamSynchronize(g->stream));        // an earlier call may still read it
+    cudaFree(*p);
+    *p = nullptr;
+    g->device_bytes -= *capacity * sizeof(T);
+    *capacity = 0;
+    OCEAN_CUDA(dev_alloc(g, p, n));
+    *capacity = n;
+    return OCEAN_OK;
+}
+
 void release(ocean_generator* g) {
     if (!g) return;
     DeviceScope scope;
@@ -167,6 +196,12 @@ void release(ocean_generator* g) {
     cudaFree(g->spray_records);
     cudaFree(g->surf_scratch);
     cudaFree(g->surf_records);
+    cudaFree(g->buoy_bodies);
+    cudaFree(g->buoy_offsets);
+    cudaFree(g->buoy_results);
+    cudaFree(g->buoy_q);
+    cudaFree(g->buoy_samples);
+    cudaFree(g->buoy_points);
     cudaFree(g->d_cascade);
     cudaFree(g->d_spectrum);
     cudaFree(g->d_queue);
@@ -1109,6 +1144,25 @@ int check_surface_args(int num_points, float tolerance, int max_iterations) {
     if (max_iterations < 0 || max_iterations > 64) return fail(OCEAN_ERR_INVALID_ARGUMENT, "max_iterations %d outside [0, 64]", max_iterations);
     return OCEAN_OK;
 }
+
+// The surface query on validated arguments, with the map scales already in gen->q_scales (ocean_query_surface_device and
+// ocean_buoyancy_device).
+int run_query_surface(ocean_generator* gen, int num_points, const float2* points_xz_dev, int num_cascades, float tolerance,
+                      int max_iterations, ocean_surface_sample* out_dev) {
+    const size_t ints = ocean::surface_scratch_ints(gen->num_cascades, num_points);
+    if (ints > gen->surf_scratch_capacity) {
+        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+        cudaFree(gen->surf_scratch);
+        gen->surf_scratch = nullptr;
+        gen->surf_scratch_capacity = 0;
+        OCEAN_CUDA(dev_alloc(gen, &gen->surf_scratch, ints));
+        gen->surf_scratch_capacity = ints;
+    }
+    OCEAN_CUDA(ocean::launch_query_surface(gen->buf, num_cascades, points_xz_dev, num_points, gen->q_scales, tolerance, max_iterations,
+                                           out_dev, gen->surf_scratch, gen->stream));
+    gen->kernel_launches += max_iterations > 0 ? 3 : 1;
+    return OCEAN_OK;
+}
 }  // namespace
 
 int ocean_query_surface_device(ocean_generator* gen, int num_points, const float* points_xz_dev, int num_cascades, const float* map_scales_host,
@@ -1119,19 +1173,7 @@ int ocean_query_surface_device(ocean_generator* gen, int num_points, const float
     if (num_points == 0) return OCEAN_OK;
     if (!points_xz_dev || !out_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
-    const size_t ints = ocean::surface_scratch_ints(gen->num_cascades, num_points);
-    if (ints > gen->surf_scratch_capacity) {
-        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-        cudaFree(gen->surf_scratch);
-        gen->surf_scratch = nullptr;
-        gen->surf_scratch_capacity = 0;
-        OCEAN_CUDA(dev_alloc(gen, &gen->surf_scratch, ints));
-        gen->surf_scratch_capacity = ints;
-    }
-    OCEAN_CUDA(ocean::launch_query_surface(gen->buf, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_points, gen->q_scales,
-                                           tolerance, max_iterations, out_dev, gen->surf_scratch, gen->stream));
-    gen->kernel_launches += max_iterations > 0 ? 3 : 1;
-    return OCEAN_OK;
+    return run_query_surface(gen, num_points, reinterpret_cast<const float2*>(points_xz_dev), num_cascades, tolerance, max_iterations, out_dev);
 }
 
 int ocean_query_surface(ocean_generator* gen, int num_points, const float* points_xz_host, int num_cascades, const float* map_scales_host,
@@ -1156,6 +1198,94 @@ int ocean_query_surface(ocean_generator* gen, int num_points, const float* point
                                          tolerance, max_iterations, gen->surf_records)))
         return rc;
     OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->surf_records, sizeof(ocean_surface_sample) * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+// ---- buoyancy: per-body force and torque from hull points on the surface (the surface query between two buoyancy kernels) ----
+static_assert(sizeof(ocean_buoyancy_point) == 20, "ocean_buoyancy_point layout");
+static_assert(sizeof(ocean_buoyancy_body) == 56, "ocean_buoyancy_body layout");
+static_assert(sizeof(ocean_buoyancy_result) == 48, "ocean_buoyancy_result layout");
+
+namespace {
+// The checks both entry points make; *world receives the number of world points, the sum of the bodies' num_points.
+int check_buoyancy_args(int num_bodies, const ocean_buoyancy_body* bodies, int num_points, float density, float tolerance,
+                        int max_iterations, int* world) {
+    int rc = check_surface_args(num_points, tolerance, max_iterations);
+    if (rc) return rc;
+    if (num_bodies < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_bodies %d is negative", num_bodies);
+    if (!(density > 0.0f) || !std::isfinite(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
+    if (num_bodies > 0 && !bodies) return fail(OCEAN_ERR_INVALID_ARGUMENT, "bodies is NULL");
+    long long total = 0;
+    for (int b = 0; b < num_bodies; ++b) {
+        const long long first = bodies[b].first_point, n = bodies[b].num_points;
+        if (n < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: num_points %lld is negative", b, n);
+        if (first < 0 || first + n > num_points)
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: points [%lld, %lld) outside [0, %d)", b, first, first + n, num_points);
+        total += n;
+    }
+    if (total > INT32_MAX) return fail(OCEAN_ERR_INVALID_ARGUMENT, "%lld world points exceed INT32_MAX", total);
+    *world = (int)total;
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int num_points,
+                          const ocean_buoyancy_point* points_dev, int num_cascades, const float* map_scales_host, float density,
+                          float tolerance, int max_iterations, ocean_buoyancy_result* results_dev, ocean_surface_sample* samples_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_buoyancy_args(num_bodies, bodies_host, num_points, density, tolerance, max_iterations, &world))) return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (!results_dev || (world > 0 && !points_dev)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
+    const size_t B = (size_t)num_bodies;
+    if ((rc = grow_buffer(gen, &gen->buoy_bodies, &gen->buoy_bodies_capacity, B))) return rc;
+    if ((rc = grow_buffer(gen, &gen->buoy_offsets, &gen->buoy_offsets_capacity, B))) return rc;
+    if ((rc = grow_buffer(gen, &gen->buoy_q, &gen->buoy_q_capacity, (size_t)world))) return rc;
+    if (!samples_dev && (rc = grow_buffer(gen, &gen->buoy_samples, &gen->buoy_samples_capacity, (size_t)world))) return rc;
+    ocean_surface_sample* samples = samples_dev ? samples_dev : gen->buoy_samples;
+    std::vector<int>& offsets = gen->buoy_offsets_host;              // kept in the generator: the copy below is asynchronous
+    offsets.resize(B);
+    for (size_t b = 0, start = 0; b < B; start += (size_t)bodies_host[b].num_points, ++b) offsets[b] = (int)start;
+    OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_bodies, bodies_host, sizeof(ocean_buoyancy_body) * B, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_offsets, offsets.data(), sizeof(int) * B, cudaMemcpyHostToDevice, gen->stream));
+    if (world > 0) {
+        OCEAN_CUDA(ocean::launch_buoyancy_transform(gen->buoy_bodies, gen->buoy_offsets, num_bodies, points_dev, world, gen->buoy_q, gen->stream));
+        gen->kernel_launches += 1;
+        if ((rc = run_query_surface(gen, world, gen->buoy_q, num_cascades, tolerance, max_iterations, samples))) return rc;
+    }
+    const float rho_g = density * 9.81f;                                 // G, wave_generator.gd:5, in binary32
+    OCEAN_CUDA(ocean::launch_buoyancy_reduce(gen->buoy_bodies, gen->buoy_offsets, num_bodies, points_dev, samples, rho_g, tolerance,
+                                             results_dev, gen->stream));
+    gen->kernel_launches += 1;
+    return OCEAN_OK;
+}
+
+int ocean_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int num_points,
+                   const ocean_buoyancy_point* points_host, int num_cascades, const float* map_scales_host, float density,
+                   float tolerance, int max_iterations, ocean_buoyancy_result* results_host, ocean_surface_sample* samples_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_buoyancy_args(num_bodies, bodies_host, num_points, density, tolerance, max_iterations, &world))) return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (!results_host || (world > 0 && !points_host)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
+    if ((rc = grow_buffer(gen, &gen->buoy_results, &gen->buoy_results_capacity, (size_t)num_bodies))) return rc;
+    if (world > 0) {
+        if ((rc = grow_buffer(gen, &gen->buoy_points, &gen->buoy_points_capacity, (size_t)num_points))) return rc;
+        OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_points, points_host, sizeof(ocean_buoyancy_point) * (size_t)num_points, cudaMemcpyHostToDevice,
+                                   gen->stream));
+    }
+    if ((rc = ocean_buoyancy_device(gen, num_bodies, bodies_host, num_points, world > 0 ? gen->buoy_points : nullptr, num_cascades,
+                                    map_scales_host, density, tolerance, max_iterations, gen->buoy_results, nullptr)))
+        return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(results_host, gen->buoy_results, sizeof(ocean_buoyancy_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost,
+                               gen->stream));
+    if (samples_host && world > 0)
+        OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
+                                   gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }

@@ -123,6 +123,14 @@ size_t surface_scratch_ints(int num_cascades, int n);
 cudaError_t launch_query_surface(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
                                  float tolerance, int max_iterations, void* out_dev, int* scratch_dev, cudaStream_t stream);
 
+// ocean_buoyancy.cu: buoyancy (oracle/buoyancy.py).  bodies_dev = ocean_buoyancy_body[num_bodies], offsets_dev = the exclusive
+// prefix of their num_points (body-major world points), points_dev = ocean_buoyancy_point[], q_dev / samples_dev = [n] world
+// points' (x, z) / surface records, results_dev = ocean_buoyancy_result[num_bodies]
+cudaError_t launch_buoyancy_transform(const void* bodies_dev, const int* offsets_dev, int num_bodies, const void* points_dev, int n,
+                                      float2* q_dev, cudaStream_t stream);
+cudaError_t launch_buoyancy_reduce(const void* bodies_dev, const int* offsets_dev, int num_bodies, const void* points_dev,
+                                   const void* samples_dev, float rho_g, float tolerance, void* results_dev, cudaStream_t stream);
+
 // ocean_spray.cu: spray candidates (sea_spray_particle.gdshader:80-94) as a stable stream compaction; counts_dev is
 // [spray_blocks(n) + 1] ints of scratch whose last element receives the number of active candidates
 int spray_blocks(int n);

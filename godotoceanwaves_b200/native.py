@@ -35,6 +35,22 @@ class InfoC(C.Structure):
                 ("cascade_updates", C.c_uint64), ("device_bytes", C.c_uint64)]
 
 
+class BuoyancyPointC(C.Structure):
+    """struct ocean_buoyancy_point (include/ocean.h), 20 B: body-local position, volume (m^3), half height (m)"""
+    _fields_ = [("position", C.c_float * 3), ("volume", C.c_float), ("half_height", C.c_float)]
+
+
+class BuoyancyBodyC(C.Structure):
+    """struct ocean_buoyancy_body (include/ocean.h), 56 B: 3 x 4 row-major body-to-world [R | t], hull-point range"""
+    _fields_ = [("transform", C.c_float * 12), ("first_point", C.c_int32), ("num_points", C.c_int32)]
+
+
+class BuoyancyResultC(C.Structure):
+    """struct ocean_buoyancy_result (include/ocean.h), 48 B"""
+    _fields_ = [("force", C.c_float * 3), ("torque", C.c_float * 3), ("submerged_volume", C.c_float),
+                ("center_offset", C.c_float * 3), ("max_residual", C.c_float), ("unconverged", C.c_uint32)]
+
+
 # every symbol include/ocean.h declares: name -> (restype, argtypes)
 _H = C.c_void_p
 _P = C.POINTER
@@ -73,6 +89,10 @@ SIGNATURES = {
     "ocean_sample_maps_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ocean_query_surface": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_int, C.c_void_p]),
     "ocean_query_surface_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_int, C.c_void_p]),
+    "ocean_buoyancy": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int,
+                                 C.c_void_p, C.c_void_p]),
+    "ocean_buoyancy_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int,
+                                        C.c_void_p, C.c_void_p]),
     "ocean_spray_grid":(C.c_int, [C.c_int, C.c_void_p, C.c_void_p]),
     "ocean_extract_spray": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, _P(C.c_int)]),
     "ocean_extract_spray_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),

@@ -246,6 +246,31 @@ class WaveGenerator:
                                                  float(tolerance), int(max_iterations), out.ctypes.data))
         return out
 
+    # -- buoyancy: per-body hydrostatic force and torque from hull points on the displaced surface -------------------
+    BUOYANCY_POINT = np.dtype([("position", np.float32, 3), ("volume", np.float32), ("half_height", np.float32)])   # struct ocean_buoyancy_point
+    BUOYANCY_BODY = np.dtype([("transform", np.float32, 12), ("first_point", np.int32), ("num_points", np.int32)])  # struct ocean_buoyancy_body
+    BUOYANCY_RESULT = np.dtype([("force", np.float32, 3), ("torque", np.float32, 3), ("submerged_volume", np.float32),
+                                ("center_offset", np.float32, 3), ("max_residual", np.float32),
+                                ("unconverged", np.uint32)])                                  # struct ocean_buoyancy_result
+
+    def buoyancy(self, bodies, points, map_scales, density: float = 1025.0, tolerance: float = 1e-3, max_iterations: int = 8,
+                 return_samples: bool = False):
+        """BUOYANCY_RESULT rows, one per BUOYANCY_BODY row of `bodies` (a 3 x 4 row-major body-to-world transform and a range
+        of the BUOYANCY_POINT rows of `points`; ranges may overlap): the hydrostatic force, the torque about the body origin,
+        the submerged volume and the centre-of-buoyancy offset this tick (include/ocean.h, ocean_buoyancy).  With
+        return_samples, also the SURFACE_SAMPLE of every world point, body by body."""
+        self._require()
+        b = np.ascontiguousarray(bodies, self.BUOYANCY_BODY).reshape(-1)
+        p = np.ascontiguousarray(points, self.BUOYANCY_POINT).reshape(-1)
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        out = np.zeros(len(b), self.BUOYANCY_RESULT)
+        world = int(np.maximum(b["num_points"], 0).astype(np.int64).sum())
+        samples = np.zeros(world, self.SURFACE_SAMPLE) if return_samples else None
+        check(load_library().ocean_buoyancy(self.context, len(b), b.ctypes.data, len(p), p.ctypes.data, sc.shape[0], sc.ctypes.data,
+                                            float(density), float(tolerance), int(max_iterations), out.ctypes.data,
+                                            None if samples is None else samples.ctypes.data))
+        return (out, samples) if return_samples else out
+
     # -- spray candidates: the spawn test of sea_spray_particle.gdshader:80-94 as a stream compaction --------------
     SPRAY_RECORD = np.dtype([("index", np.uint32), ("start_x", np.float32), ("start_z", np.float32), ("scale_factor", np.float32),
                              ("particle_scale", np.float32, 3), ("foam", np.float32)])     # struct ocean_spray_record

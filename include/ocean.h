@@ -214,6 +214,58 @@ int ocean_query_surface(ocean_generator* gen, int num_points, const float* point
 int ocean_query_surface_device(ocean_generator* gen, int num_points, const float* points_xz_dev, int num_cascades, const float* map_scales_host,
                                float tolerance, int max_iterations, ocean_surface_sample* out_dev);
 
+/* Buoyancy -- per-body hydrostatic force and torque for this physics tick, from hull sample points on the displaced surface.
+ * A hull point (body-local position, volume in m^3, half_height in m) stands for a vertical column element of that volume,
+ * centred on the point and reaching half_height above and below it.  A body is a 3 x 4 row-major body-to-world matrix [R | t]
+ * (the layout of ocean_spray_grid's emission_transform) and a range [first_point, first_point + num_points) into the hull
+ * points; ranges may overlap, so a thousand identical crates share one hull.  For world point j of a body (p = its hull point):
+ *   r = R p (rotated, not translated), w = r + t, eta = the water height over (w.x, w.z) from ocean_query_surface,
+ *   f = h > 0 ? min(max((eta - (w.y - h)) / (h + h), 0), 1) : (w.y <= eta),  v = f * volume,
+ * with NaN-dropping min/max (a NaN height gives f = 0).  Per body S0 = sum v and S1 = sum v * r, summed in a fixed order
+ * (point j in lane j mod 32, lanes in increasing j from +0, then the tree of a warp shuffle reduction), so the results are
+ * deterministic and bit-identical to oracle/buoyancy.py, the specification.  With rho_g = density * 9.81f:
+ *   submerged_volume  S0
+ *   force             (0, rho_g S0, 0)
+ *   torque            (-(rho_g S1.z), 0, rho_g S1.x), about the body origin t (the sum of r x F over the points)
+ *   center_offset     S1 / S0, or 0 when S0 is not > 0; the centre of buoyancy is t + center_offset, and a Godot host calls
+ *                     apply_force(force, center_offset), which gives the same torque
+ *   max_residual      NaN-dropping max of the points' surface-query residuals
+ *   unconverged       points whose residual is not <= tolerance
+ * A body with num_points = 0 gets an all-zero record.  num_cascades, map_scales, tolerance and max_iterations mean what they
+ * mean for ocean_query_surface, whose limits carry over (within 150 m of the camera; any converged preimage where the surface
+ * folds).  The model is vertical hydrostatics only: no drag or added mass (the maps carry no water velocity), the column
+ * element stays vertical under rotation, and volumes are not rescaled by a non-rigid transform.
+ * density must be finite and > 0, counts non-negative, every body's range inside [0, num_points), and the sum of the bodies'
+ * num_points (the world points) at most INT32_MAX.  samples may be NULL, or receives the surface record of every world point
+ * ([sum of num_points], body-major, j increasing).  The bodies and map_scales are host arrays in both entry points (the poses
+ * come from the host's physics engine every tick); ocean_buoyancy takes host points, results and samples and is synchronous;
+ * ocean_buoyancy_device takes device pointers for them and is asynchronous on the generator's stream.  A call with world
+ * points launches 5 kernels (3 with max_iterations = 0). */
+typedef struct ocean_buoyancy_point {
+    float position[3];
+    float volume;
+    float half_height;
+} ocean_buoyancy_point;    /* 20 B */
+typedef struct ocean_buoyancy_body {
+    float transform[12];
+    int32_t first_point;
+    int32_t num_points;
+} ocean_buoyancy_body;     /* 56 B */
+typedef struct ocean_buoyancy_result {
+    float force[3];
+    float torque[3];
+    float submerged_volume;
+    float center_offset[3];
+    float max_residual;
+    uint32_t unconverged;
+} ocean_buoyancy_result;   /* 48 B */
+int ocean_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int num_points,
+                   const ocean_buoyancy_point* points_host, int num_cascades, const float* map_scales_host, float density,
+                   float tolerance, int max_iterations, ocean_buoyancy_result* results_host, ocean_surface_sample* samples_host);
+int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int num_points,
+                          const ocean_buoyancy_point* points_dev, int num_cascades, const float* map_scales_host, float density,
+                          float tolerance, int max_iterations, ocean_buoyancy_result* results_dev, ocean_surface_sample* samples_dev);
+
 /* Spray candidates -- the spawn test of the sea-spray particle shader as a stream-compaction op
  * (assets/shaders/spatial/sea_spray_particle.gdshader:80-94; the reference evaluates it for every particle of the emitter and
  * culls the inactive ones, README.md:29).  For each candidate START_POS.xz:

@@ -116,16 +116,17 @@ def run_spray(N, C, particles, reps, label):
     print(json.dumps(out), flush=True)
 
 
-run(256, 4, 2000, "cfg2 latency: one 256x256x4 set per launch (launch/latency-bound, L2-resident)")
-run(256, 4, 2000, "cfg2 latency, fused frames (ocean_update_frames: 64 frames per launch)", fused=True)
-run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, frame by frame")
-run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, fused frames (ocean_update_frames)", fused=True)
-run(1024, 8, 200, "cfg4 (1 GPU): 1024x1024x8")
-run(256, 4, 300, "cfg5: 256x256x4 wind/fetch sweep, one grid point per step, spectrum regenerated every step", regen=True)
-run_sweep_batch(256, 4, 50, "cfg5 batched: the 6x4 (U,F) grid = 24 sets x 4 cascades per step, all spectra regenerated every step")
-run(128, 1, 2000, "cfg1 shape on GPU: 128x128x1")
-run_spectrum(256, 128, 10, "spectrum generation alone: 128 cascades of 256x256, one launch")
-run_spray(256, 4, 1 << 20, 50, "spray candidates: 2^20 grid candidates x 4 cascades of 256x256")
+if "--buoyancy" not in sys.argv:       # --buoyancy runs run_buoyancy (defined below) alone
+    run(256, 4, 2000, "cfg2 latency: one 256x256x4 set per launch (launch/latency-bound, L2-resident)")
+    run(256, 4, 2000, "cfg2 latency, fused frames (ocean_update_frames: 64 frames per launch)", fused=True)
+    run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, frame by frame")
+    run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, fused frames (ocean_update_frames)", fused=True)
+    run(1024, 8, 200, "cfg4 (1 GPU): 1024x1024x8")
+    run(256, 4, 300, "cfg5: 256x256x4 wind/fetch sweep, one grid point per step, spectrum regenerated every step", regen=True)
+    run_sweep_batch(256, 4, 50, "cfg5 batched: the 6x4 (U,F) grid = 24 sets x 4 cascades per step, all spectra regenerated every step")
+    run(128, 1, 2000, "cfg1 shape on GPU: 128x128x1")
+    run_spectrum(256, 128, 10, "spectrum generation alone: 128 cascades of 256x256, one launch")
+    run_spray(256, 4, 1 << 20, 50, "spray candidates: 2^20 grid candidates x 4 cascades of 256x256")
 
 
 def run_query(N, C, n_points, reps, label):
@@ -204,6 +205,81 @@ def run_surface(N, C, n_points, reps, label, tolerance=1e-3, max_iterations=8):
     g.free()
     print(json.dumps(out), flush=True)
 
+
+def run_buoyancy(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_iterations=8):
+    """Buoyancy op (ocean_buoyancy_device) on device-resident hulls of `per_body` points per body: kernel time from CUDA
+    events, against ocean_query_surface_device on the same world points in the same run, in alternating windows.  The card's
+    name, power limit and max SM clock are read in the same run."""
+    import subprocess
+    import numpy as np
+    import torch
+    from godotoceanwaves_b200.native import load_library, check
+    from oracle import buoyancy as bu
+    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
+    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
+    for _ in range(2):
+        g.update_all(0.02, p)
+    scales = gow.WaveGenerator.map_scales(p)
+    rng = np.random.default_rng(1)
+    hull = np.zeros(n_bodies * per_body, bu.POINT)
+    hull["position"] = rng.uniform(-2.0, 2.0, (len(hull), 3))
+    hull["volume"] = rng.uniform(0.01, 0.1, len(hull))
+    hull["half_height"] = rng.uniform(0.05, 0.3, len(hull))
+    q = rng.standard_normal((n_bodies, 4))
+    q /= np.linalg.norm(q, axis=1, keepdims=True)
+    w, x, y, z = q.T
+    R = np.stack([1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y),
+                  2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x),
+                  2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)], 1).reshape(n_bodies, 3, 3)
+    t = np.stack([rng.uniform(-300, 300, n_bodies), rng.uniform(-1, 1, n_bodies), rng.uniform(-300, 300, n_bodies)], 1)
+    bodies = np.zeros(n_bodies, bu.BODY)
+    bodies["transform"] = np.concatenate([R, t[:, :, None]], 2).reshape(n_bodies, 12)
+    bodies["first_point"] = np.arange(n_bodies) * per_body
+    bodies["num_points"] = per_body
+    _, _, _, wp = bu.world_points(bodies, hull)
+    n_points = len(wp)
+    dev = torch.device("cuda", 0)
+    hull_d = torch.from_numpy(hull.view(np.uint8).copy()).to(dev)
+    pts_d = torch.from_numpy(np.ascontiguousarray(wp[:, [0, 2]])).to(dev)
+    res_d = torch.empty(n_bodies * 12, dtype=torch.int32, device=dev)           # ocean_buoyancy_result: 48 B
+    recs_d = torch.empty(n_points * 10, dtype=torch.int32, device=dev)          # ocean_surface_sample: 40 B
+    torch.cuda.synchronize()
+    lib = load_library()
+    buoy = lambda: check(lib.ocean_buoyancy_device(g.context, n_bodies, bodies.ctypes.data, len(hull), hull_d.data_ptr(), C, scales.ctypes.data,
+                                                   1025.0, tolerance, max_iterations, res_d.data_ptr(), None))
+    query = lambda: check(lib.ocean_query_surface_device(g.context, n_points, pts_d.data_ptr(), C, scales.ctypes.data, tolerance, max_iterations,
+                                                         recs_d.data_ptr()))
+
+    def timed(call):
+        for _ in range(3):
+            call()
+        g.synchronize()
+        g.timer_start()
+        for _ in range(reps):
+            call()
+        return g.timer_stop() / reps
+
+    t_b, t_q = [], []
+    for _ in range(3):                          # alternating windows: clock ramp-up and neighbours hit both alike
+        t_b.append(timed(buoy))
+        t_q.append(timed(query))
+    res = res_d.cpu().numpy().view(bu.RESULT)
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                         stdout=subprocess.PIPE, text=True).stdout.strip()
+    out = {"config": label, "gpu": torch.cuda.get_device_name(0), "power_limit_and_max_sm_clock": smi, "map_size": N, "cascades": C,
+           "bodies": n_bodies, "points_per_body": per_body, "world_points": n_points, "tolerance": tolerance, "max_iterations": max_iterations,
+           "buoyancy_us_per_call": [1e3 * v for v in t_b], "query_surface_us_per_call": [1e3 * v for v in t_q],
+           "overhead_over_query": min(t_b) / min(t_q) - 1.0, "mpoints_per_s": n_points / (min(t_b) * 1e-3) / 1e6,
+           "frac_bodies_afloat": float(np.mean(res["submerged_volume"] > 0)),
+           "frac_points_unconverged": float(res["unconverged"].sum()) / n_points}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
+if "--buoyancy" in sys.argv:
+    run_buoyancy(256, 4, 1 << 14, 64, 50, "buoyancy: 2^14 bodies x 64 points over 4 cascades of 256x256")
+    run_buoyancy(1024, 8, 1 << 14, 64, 20, "buoyancy: 2^14 bodies x 64 points over 8 cascades of 1024x1024")
+    sys.exit(0)
 
 if "--query" in sys.argv or os.environ.get("OCEAN_RUN_QUERY", "1") != "0":
     run_query(256, 4, 1 << 20, 50, "query op: 2^20 random points x 4 cascades of 256x256 (maps L2-resident)")
