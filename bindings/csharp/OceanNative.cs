@@ -160,6 +160,22 @@ namespace OceanB200
         internal static partial int ocean_buoyancy_device(IntPtr handle, int num_bodies, OceanBuoyancyBody* bodies, int num_points, void* points_dev,
                                                           int num_cascades, float* map_scales, float density, float tolerance, int max_iterations,
                                                           void* results_dev, void* samples_dev);
+        // velocity maps: d/dt of the displacement map, recomputed for the cascades whose maps changed; recomputed may be null
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_update_velocity(IntPtr handle, int* recomputed);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_get_velocity_map(IntPtr handle, IntPtr* velocity_dev, nuint* layer_bytes);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_copy_velocity_to_host(IntPtr handle, int first, int count, void* velocity);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_copy_f32_velocity_to_host(IntPtr handle, int cascade, float* velocity);
+        // water velocity at undisplaced points [n][2]; output [n][3]
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_sample_velocity(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,
+                                                          float* velocity);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_sample_velocity_device(IntPtr handle, int num_points, void* points_xz_dev, int num_cascades, float* map_scales,
+                                                                 void* velocity_dev);
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_get_info(IntPtr handle, OceanInfo* info);
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]

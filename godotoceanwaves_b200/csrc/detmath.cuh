@@ -72,7 +72,7 @@ __device__ __forceinline__ void sincos64(double x, double& s, double& c) {
 // ---- exp: clamp to [-110, 90]; n = rint(x*log2e); two-term ln2 reduction; Taylor to r^13 ----
 // (exp64 / log64 are real functions, not inlined: the spectrum kernel calls them a dozen times per texel quad and was an
 //  instruction-cache-bound 61 KB of straight-line code with every call expanded)
-__device__ __noinline__ double exp64(double x) {
+static __device__ __noinline__ double exp64(double x) {   // static: the header is compiled into more than one object
     if (x != x) return x;
     if (x < -110.0) x = -110.0;
     if (x > 90.0) x = 90.0;
@@ -97,7 +97,7 @@ __device__ __noinline__ double exp64(double x) {
 }
 
 // ---- log of a non-negative binary32 value widened to binary64 ----
-__device__ __noinline__ double log64(double x) {
+static __device__ __noinline__ double log64(double x) {
     if (x != x) return x;
     if (x < 0.0) return __longlong_as_double(0x7ff8000000000000LL);
     if (x == 0.0) return __longlong_as_double(0xfff0000000000000LL);

@@ -84,6 +84,13 @@ struct ocean_generator {
     size_t buoy_points_capacity = 0;
     ocean_buoyancy_result* buoy_results = nullptr;
     size_t buoy_results_capacity = 0;
+    // velocity maps, allocated by the first velocity call: row-pass scratch, the map, its binary32 tap while the taps are on
+    float4* vel_scratch = nullptr;                      // [num_cascades][N][N]
+    uint2* velocity = nullptr;                          // [num_cascades][N][N] 4 x half
+    float4* velocity_f32 = nullptr;                     // [num_cascades][N][N]
+    std::vector<ocean::VelocityDispatch> vel_source;    // [num_cascades] table slot and time of the update that built the current maps
+    std::vector<char> vel_has_source;                   // the cascade's maps were written at least once
+    std::vector<char> vel_stale;                        // its velocity layer does not describe its current maps yet
     ocean::CascadeDispatch* d_cascade = nullptr;        // [num_cascades] (two-kernel path only)
     ocean::SpectrumDispatch* d_spectrum = nullptr;      // [num_cascades]
     ocean::TableDispatch* d_tables = nullptr;           // [num_cascades]
@@ -202,6 +209,9 @@ void release(ocean_generator* g) {
     cudaFree(g->buoy_q);
     cudaFree(g->buoy_samples);
     cudaFree(g->buoy_points);
+    cudaFree(g->vel_scratch);
+    cudaFree(g->velocity);
+    cudaFree(g->velocity_f32);
     cudaFree(g->d_cascade);
     cudaFree(g->d_spectrum);
     cudaFree(g->d_queue);
@@ -320,6 +330,13 @@ int assign_table_slot(ocean_generator* g, int i, const ocean_cascade_params& p, 
     return pick;
 }
 
+// Every path that writes a cascade's maps records the dispatch it used: the velocity layer is recomputed from it on demand.
+void record_velocity_source(ocean_generator* g, const ocean::CascadeDispatch& d) {
+    g->vel_source[d.cascade] = ocean::VelocityDispatch{d.cascade, d.table_slot, d.time};
+    g->vel_has_source[d.cascade] = 1;
+    g->vel_stale[d.cascade] = 1;
+}
+
 // Runs WaveGenerator._update (wave_generator.gd:65-85) for the cascades listed in `indices`
 // (all of them in ONE batched launch sequence; cascades are independent).
 int run_cascades(ocean_generator* g, const int* indices, int n) {
@@ -415,6 +432,7 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
         const int i = indices[k];
         g->pass_parameters[i].should_generate_spectrum = 0;          // :72
         g->done_count[i] += per_update;
+        record_velocity_source(g, hc[k]);
     }
     if (two_kernel)
         RUN_CUDA(cudaMemcpyAsync(g->d_queue + 1, g->done_count.data(), sizeof(uint32_t) * g->done_count.size(), cudaMemcpyHostToDevice, g->stream));
@@ -530,6 +548,9 @@ int ocean_create(int device, int map_size, int num_cascades, ocean_generator** o
     g->slot_refs.assign(C, 0);
     g->cascade_slot.assign(C, -1);
     g->scratch_layer_of.resize(C);
+    g->vel_source.assign(C, ocean::VelocityDispatch{0, 0, 0.0f});
+    g->vel_has_source.assign(C, 0);
+    g->vel_stale.assign(C, 0);
     for (int i = 0; i < C; ++i) g->scratch_layer_of[i] = 2 * i;
     {
         const char* mode = std::getenv("OCEAN_PIPELINE");
@@ -723,7 +744,10 @@ int ocean_update_frames(ocean_generator* gen, double delta, ocean_cascade_params
             cudaMemcpy(gen->d_queue + 1, gen->done_count.data(), sizeof(uint32_t) * gen->done_count.size(), cudaMemcpyHostToDevice);
             return fail(OCEAN_ERR_CUDA, "multi-frame launch failed: %s", cudaGetErrorString(le));
         }
-        for (int i = 0; i < count; ++i) frame_protocol_commit(gen->done_count.data(), C, i, done, F, a_per, b_per);
+        for (int i = 0; i < count; ++i) {
+            frame_protocol_commit(gen->done_count.data(), C, i, done, F, a_per, b_per);
+            record_velocity_source(gen, rec[(size_t)(F - 1) * count + i]);     // the launch's last frame built the maps
+        }
         gen->kernel_launches += 1;
         gen->cascade_updates += (uint64_t)F * count;
         done += F;
@@ -908,6 +932,7 @@ int ocean_set_spectrum_amplitudes(ocean_generator* gen, int cascade, const float
         }
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     OCEAN_CUDA(cudaMemcpy(gen->buf.spectrum + (size_t)cascade * N * N, tex.data(), sizeof(float) * tex.size(), cudaMemcpyHostToDevice));
+    if (gen->vel_has_source[cascade]) gen->vel_stale[cascade] = 1;       // the velocity layer reads the spectrum as stored
     return OCEAN_OK;
 }
 
@@ -926,6 +951,11 @@ int ocean_enable_f32_taps(ocean_generator* gen, int enable) {
         cudaFree(gen->buf.normal_f32);
         gen->buf.displacement_f32 = gen->buf.normal_f32 = nullptr;
         gen->device_bytes -= 2 * sizeof(float4) * n;
+        if (gen->velocity_f32) {
+            cudaFree(gen->velocity_f32);
+            gen->velocity_f32 = nullptr;
+            gen->device_bytes -= sizeof(float4) * n;
+        }
     }
     return OCEAN_OK;
 }
@@ -1286,6 +1316,123 @@ int ocean_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_bo
     if (samples_host && world > 0)
         OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
                                    gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+// ---- velocity maps: the time derivative of the displacement map (ocean_velocity.cu; oracle_velocity_update) ----
+namespace {
+// Allocates the velocity buffers on first use, zeroed: a cascade whose maps were never written has a zero velocity layer.
+// A binary32 tap created while the taps are on is filled by recomputing every layer that has a source.
+int ensure_velocity(ocean_generator* gen) {
+    const size_t n = (size_t)gen->num_cascades * gen->map_size * gen->map_size;
+    if (!gen->vel_scratch) {
+        OCEAN_CUDA(dev_alloc(gen, &gen->vel_scratch, n));
+        OCEAN_CUDA(ocean::init_velocity_twiddles(gen->twiddles, gen->stream));
+    }
+    if (!gen->velocity) {
+        OCEAN_CUDA(dev_alloc(gen, &gen->velocity, n));
+        OCEAN_CUDA(cudaMemsetAsync(gen->velocity, 0, sizeof(uint2) * n, gen->stream));
+    }
+    if (gen->buf.displacement_f32 && !gen->velocity_f32) {
+        OCEAN_CUDA(dev_alloc(gen, &gen->velocity_f32, n));
+        OCEAN_CUDA(cudaMemsetAsync(gen->velocity_f32, 0, sizeof(float4) * n, gen->stream));
+        for (int i = 0; i < gen->num_cascades; ++i) gen->vel_stale[i] = gen->vel_has_source[i];
+    }
+    return OCEAN_OK;
+}
+
+// Recomputes every stale velocity layer in one launch sequence.
+int refresh_velocity(ocean_generator* gen, int* recomputed) {
+    int rc = ensure_velocity(gen);
+    if (rc) return rc;
+    std::vector<ocean::VelocityDispatch> jobs;
+    for (int i = 0; i < gen->num_cascades; ++i)
+        if (gen->vel_has_source[i] && gen->vel_stale[i]) jobs.push_back(gen->vel_source[i]);
+    if (!jobs.empty()) {
+        int launched = 0;
+        OCEAN_CUDA(ocean::launch_velocity(gen->buf, jobs.data(), (int)jobs.size(), gen->vel_scratch, gen->velocity, gen->velocity_f32,
+                                          gen->stream, &launched));
+        gen->kernel_launches += (uint64_t)launched;
+        for (const auto& j : jobs) gen->vel_stale[j.cascade] = 0;
+    }
+    if (recomputed) *recomputed = (int)jobs.size();
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_update_velocity(ocean_generator* gen, int* recomputed) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if (recomputed) *recomputed = 0;
+    return refresh_velocity(gen, recomputed);
+}
+
+int ocean_get_velocity_map(ocean_generator* gen, void** velocity_dev, size_t* layer_bytes) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = ensure_velocity(gen))) return rc;
+    if (velocity_dev) *velocity_dev = gen->velocity;
+    if (layer_bytes) *layer_bytes = sizeof(uint2) * (size_t)gen->map_size * gen->map_size;
+    return OCEAN_OK;
+}
+
+int ocean_copy_velocity_to_host(ocean_generator* gen, int first, int count, void* velocity_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if (first < 0 || count < 0 || first + count > gen->num_cascades)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "layer range [%d,%d) outside [0,%d)", first, first + count, gen->num_cascades);
+    if (count == 0) return OCEAN_OK;
+    if (!velocity_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "velocity_host is NULL");
+    if ((rc = refresh_velocity(gen, nullptr))) return rc;
+    const size_t layer = (size_t)gen->map_size * gen->map_size;
+    OCEAN_CUDA(cudaMemcpyAsync(velocity_host, gen->velocity + first * layer, sizeof(uint2) * layer * count, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+int ocean_copy_f32_velocity_to_host(ocean_generator* gen, int cascade, float* host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_cascade(gen, cascade))) return rc;
+    if (!host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "host is NULL");
+    if (!gen->buf.displacement_f32) return fail(OCEAN_ERR_STATE, "binary32 taps are disabled; call ocean_enable_f32_taps(gen, 1) first");
+    if ((rc = refresh_velocity(gen, nullptr))) return rc;
+    const size_t layer = (size_t)gen->map_size * gen->map_size;
+    OCEAN_CUDA(cudaMemcpyAsync(host, gen->velocity_f32 + cascade * layer, sizeof(float4) * layer, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+int ocean_sample_velocity_device(ocean_generator* gen, int num_points, const float* points_xz_dev, int num_cascades, const float* map_scales_host,
+                                 float* velocity_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
+    if (num_points == 0) return OCEAN_OK;
+    if (!points_xz_dev || !velocity_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // validates before anything is launched
+    if ((rc = refresh_velocity(gen, nullptr))) return rc;
+    OCEAN_CUDA(ocean::launch_sample_velocity(gen->velocity, gen->map_size, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_points,
+                                             gen->q_scales, velocity_dev, gen->stream));
+    gen->kernel_launches += 1;
+    return OCEAN_OK;
+}
+
+int ocean_sample_velocity(ocean_generator* gen, int num_points, const float* points_xz_host, int num_cascades, const float* map_scales_host,
+                          float* velocity_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
+    if (num_points == 0) return OCEAN_OK;
+    if (!points_xz_host || !velocity_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
+    const size_t n = (size_t)num_points;
+    if ((rc = grow_query_staging(gen, n))) return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(gen->q_points, points_xz_host, sizeof(float2) * n, cudaMemcpyHostToDevice, gen->stream));
+    if ((rc = ocean_sample_velocity_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points), num_cascades, map_scales_host,
+                                           gen->q_disp)))
+        return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(velocity_host, gen->q_disp, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }

@@ -134,6 +134,24 @@ cudaError_t launch_buoyancy_transform(const void* bodies_dev, const int* offsets
 cudaError_t launch_buoyancy_reduce(const void* bodies_dev, const int* offsets_dev, int num_bodies, const void* points_dev,
                                    const void* samples_dev, float rho_g, float tolerance, void* results_dev, cudaStream_t stream);
 
+// ocean_velocity.cu: velocity maps (oracle_velocity_update).  One record per cascade to recompute: the table slot and time of
+// the update that built the cascade's current maps.
+struct VelocityDispatch {
+    int32_t cascade;
+    int32_t table_slot;
+    float time;
+};
+constexpr int kMaxVelocityLaunch = 256;   // records per launch pair (they travel by value)
+// Copies the twiddle table into ocean_velocity.cu's constant bank (once per device before its first launch).
+cudaError_t init_velocity_twiddles(const float2* twiddles_dev, cudaStream_t stream);
+// Row pass into scratch_dev ([C][N][N] float4), column pass into velocity_dev ([C][N][N] 4 x half) and, when not null,
+// velocity_f32_dev ([C][N][N] float4).  *launched receives the number of kernels launched.
+cudaError_t launch_velocity(const DeviceBuffers& b, const VelocityDispatch* jobs_host, int count, float4* scratch_dev, uint2* velocity_dev,
+                            float4* velocity_f32_dev, cudaStream_t stream, int* launched);
+// ocean_sample.cu: the displacement half of launch_sample_maps on the velocity map: out_dev = [n][3] floats
+cudaError_t launch_sample_velocity(const uint2* velocity_dev, int map_size, int num_cascades, const float2* points_dev, int n,
+                                   const float4* scales_dev, float* out_dev, cudaStream_t stream);
+
 // ocean_spray.cu: spray candidates (sea_spray_particle.gdshader:80-94) as a stable stream compaction; counts_dev is
 // [spray_blocks(n) + 1] ints of scratch whose last element receives the number of active candidates
 int spray_blocks(int n);

@@ -50,6 +50,15 @@ __device__ __forceinline__ float4 texture_bicubic(const uint2* __restrict__ laye
                 mix4(texture_bilinear(layer, N, hy, hz), texture_bilinear(layer, N, hx, hz), wxx), wyy);
 }
 
+// Cascade c's term of the displacement sum of vertex() (:34-35), added to (dx, dy, dz).
+__device__ __forceinline__ void add_displacement(const uint2* __restrict__ layer, int N, float u, float v, float scale, float& dx, float& dy,
+                                                 float& dz) {
+    const float4 d = texture_bilinear(layer, N, u, v);
+    dx = dx + d.x * scale;
+    dy = dy + d.y * scale;
+    dz = dz + d.z * scale;
+}
+
 // The sampling contract at one point p: displacement (vertex(), :27-39) and gradient/foam (fragment(), :72-84).
 __device__ __forceinline__ void sample_point(const uint2* __restrict__ displacement, const uint2* __restrict__ normal, int N, int C, float2 p,
                                              const float4* __restrict__ scales, float3& disp, float3& grad) {
@@ -58,10 +67,7 @@ __device__ __forceinline__ void sample_point(const uint2* __restrict__ displacem
         const float4 s = __ldg(&scales[c]);
         const float u = p.x * s.x, v = p.y * s.y;
         const size_t layer = (size_t)c * N * N;
-        const float4 d = texture_bilinear(displacement + layer, N, u, v);                         // :34-35
-        dx = dx + d.x * s.z;
-        dy = dy + d.y * s.z;
-        dz = dz + d.z * s.z;
+        add_displacement(displacement + layer, N, u, v, s.z, dx, dy, dz);                           // :34-35
         const float ppm = (float)N * fminf(s.x, s.y);                                             // :80
         const float t = fminf(1.0f, ppm * 0.1f);
         const float4 m = mix4(texture_bicubic(normal + layer, N, u, v), texture_bilinear(normal + layer, N, u, v), t);   // :83
@@ -86,6 +92,23 @@ __global__ void __launch_bounds__(256) k_sample_maps(const uint2* __restrict__ d
     grad_out[3 * (size_t)i + 0] = g.x;
     grad_out[3 * (size_t)i + 1] = g.y;
     grad_out[3 * (size_t)i + 2] = g.z;
+}
+
+// The water velocity at undisplaced points: the displacement half of k_sample_maps on the velocity maps (v = dD/dt, so the
+// displacement scale applies).
+__global__ void __launch_bounds__(256) k_sample_velocity(const uint2* __restrict__ velocity, int N, int C, const float2* __restrict__ points, int n,
+                                                         const float4* __restrict__ scales, float* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float2 p = points[i];
+    float vx = 0.0f, vy = 0.0f, vz = 0.0f;
+    for (int c = 0; c < C; ++c) {
+        const float4 s = __ldg(&scales[c]);
+        add_displacement(velocity + (size_t)c * N * N, N, p.x * s.x, p.y * s.y, s.z, vx, vy, vz);
+    }
+    out[3 * (size_t)i + 0] = vx;
+    out[3 * (size_t)i + 1] = vy;
+    out[3 * (size_t)i + 2] = vz;
 }
 
 // ---- surface query: the surface at a world position (oracle/surface.py is the specification) ----
@@ -253,6 +276,13 @@ cudaError_t launch_sample_maps(const DeviceBuffers& b, int num_cascades, const f
     if (n <= 0) return cudaSuccess;
     k_sample_maps<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(b.displacement, b.normal, b.map_size, num_cascades, points_dev, n, scales_dev,
                                                                   disp_out_dev, grad_out_dev);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_sample_velocity(const uint2* velocity_dev, int map_size, int num_cascades, const float2* points_dev, int n,
+                                   const float4* scales_dev, float* out_dev, cudaStream_t stream) {
+    if (n <= 0) return cudaSuccess;
+    k_sample_velocity<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(velocity_dev, map_size, num_cascades, points_dev, n, scales_dev, out_dev);
     return cudaGetLastError();
 }
 

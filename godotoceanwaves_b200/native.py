@@ -93,6 +93,12 @@ SIGNATURES = {
                                  C.c_void_p, C.c_void_p]),
     "ocean_buoyancy_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int,
                                         C.c_void_p, C.c_void_p]),
+    "ocean_update_velocity": (C.c_int, [_H, _P(C.c_int)]),
+    "ocean_get_velocity_map": (C.c_int, [_H, _P(C.c_void_p), _P(C.c_size_t)]),
+    "ocean_copy_velocity_to_host": (C.c_int, [_H, C.c_int, C.c_int, C.c_void_p]),
+    "ocean_copy_f32_velocity_to_host": (C.c_int, [_H, C.c_int, C.c_void_p]),
+    "ocean_sample_velocity": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ocean_sample_velocity_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "ocean_spray_grid":(C.c_int, [C.c_int, C.c_void_p, C.c_void_p]),
     "ocean_extract_spray": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, _P(C.c_int)]),
     "ocean_extract_spray_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),

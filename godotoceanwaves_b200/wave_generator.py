@@ -230,6 +230,42 @@ class WaveGenerator:
                                                disp.ctypes.data, grad.ctypes.data))
         return disp, grad
 
+    # -- velocity maps: the time derivative of the displacement map (include/ocean.h, ocean_update_velocity) -----------
+    def update_velocity(self) -> int:
+        """Recomputes the velocity layers whose maps changed since their last computation (asynchronous); returns their number."""
+        self._require()
+        n = C.c_int(0)
+        check(load_library().ocean_update_velocity(self.context, C.byref(n)))
+        return n.value
+
+    def velocity_to_host(self, first: int = 0, count: int | None = None) -> np.ndarray:
+        """The velocity maps (vx, vy, vz, 0) as float16 [count, N, N, 4], brought up to date first."""
+        self._require()
+        count = self._num_cascades - first if count is None else count
+        N = self.map_size
+        v = np.empty((count, N, N, 4), np.float16)
+        check(load_library().ocean_copy_velocity_to_host(self.context, first, count, v.ctypes.data))
+        return v
+
+    def velocity_f32_to_host(self, cascade: int) -> np.ndarray:
+        """One velocity layer before the half conversion, float32 [N, N, 4] (needs enable_f32_taps)."""
+        self._require()
+        N = self.map_size
+        out = np.empty((N, N, 4), np.float32)
+        check(load_library().ocean_copy_f32_velocity_to_host(self.context, cascade, out.ctypes.data))
+        return out
+
+    def sample_velocity(self, points_xz, map_scales) -> np.ndarray:
+        """Water velocity [n][3] float32 at the UNDISPLACED points points_xz [n][2], summed over the len(map_scales) first
+        cascades like the displacement of sample().  For the velocity at a world position pass query_surface()'s source point."""
+        self._require()
+        pts = np.ascontiguousarray(points_xz, np.float32).reshape(-1, 2)
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        out = np.empty((pts.shape[0], 3), np.float32)
+        check(load_library().ocean_sample_velocity(self.context, pts.shape[0], pts.ctypes.data, sc.shape[0], sc.ctypes.data,
+                                                   out.ctypes.data))
+        return out
+
     # -- surface query: the surface at a world position (inverts the horizontal displacement, then samples) ----------
     SURFACE_SAMPLE = np.dtype([("source_x", np.float32), ("source_z", np.float32), ("displacement", np.float32, 3),
                                ("gradient_foam", np.float32, 3), ("residual", np.float32), ("iterations", np.uint32)])  # struct ocean_surface_sample

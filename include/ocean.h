@@ -233,8 +233,9 @@ int ocean_query_surface_device(ocean_generator* gen, int num_points, const float
  *   unconverged       points whose residual is not <= tolerance
  * A body with num_points = 0 gets an all-zero record.  num_cascades, map_scales, tolerance and max_iterations mean what they
  * mean for ocean_query_surface, whose limits carry over (within 150 m of the camera; any converged preimage where the surface
- * folds).  The model is vertical hydrostatics only: no drag or added mass (the maps carry no water velocity), the column
- * element stays vertical under rotation, and volumes are not rescaled by a non-rigid transform.
+ * folds).  The model is vertical hydrostatics only: no drag or added mass (the water velocity these need comes from
+ * ocean_sample_velocity, but the body table carries no body velocities, so neither is applied), the column element stays
+ * vertical under rotation, and volumes are not rescaled by a non-rigid transform.
  * density must be finite and > 0, counts non-negative, every body's range inside [0, num_points), and the sum of the bodies'
  * num_points (the world points) at most INT32_MAX.  samples may be NULL, or receives the surface record of every world point
  * ([sum of num_points], body-major, j increasing).  The bodies and map_scales are host arrays in both entry points (the poses
@@ -265,6 +266,40 @@ int ocean_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_bo
 int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int num_points,
                           const ocean_buoyancy_point* points_dev, int num_cascades, const float* map_scales_host, float density,
                           float tolerance, int max_iterations, ocean_buoyancy_result* results_dev, ocean_surface_sample* samples_dev);
+
+/* Velocity maps -- the water velocity: the time derivative of the displacement map, what drag, damping and floating debris
+ * need.  A cascade's velocity layer is (vx, vy, vz, 0) = d/dt of its displacement texel (hx, hy, hz, 0): same layout, same
+ * orientation (ocean_get_maps), RGBA16F, in m/s before the displacement scale.  It is computed exactly, as one more inverse
+ * FFT of the same spectrum (differences of two map sets would not work: the cascades of consecutive map sets are at
+ * different times, and the half quantisation swamps the difference).  Per texel, binary32, with every name as in
+ * spectrum_modulate.glsl and the update's FMA sites only in mul_complex:
+ *   w = sqrt(G * k * tanh(k * depth)) (the dispersion table's omega),  m = (cos(w*time), sin(w*time)),
+ *   pa = h0a * m,  pb = h0b * conj(m),  d = (pa.x - pb.x, pa.y - pb.y),  ht = (-(w*d.y), w*d.x),  hti = (-ht.y, ht.x),
+ *   vx = hti * k_unit.y,  vy = ht,  vz = hti * k_unit.x  (each product rounded on its own),
+ *   layer 0 = (vx.x - vy.y, vx.y + vy.x),  layer 1 = (vz.x, vz.y),
+ * then the update's row IFFT, transpose and row IFFT, and texel = (l0.re, l0.im, l1.re, 0) * sign_shift, half RTNE.
+ * oracle_velocity_update (oracle/velocity_oracle.c) is the specification, bit for bit.  `time` and the tile are those of the
+ * update that built the cascade's CURRENT maps (ocean_update_all, ocean_process, ocean_update_frames: its last frame); the
+ * spectrum is the texture as stored when the velocity is computed.
+ * Every map write marks the cascade's velocity layer stale.  ocean_update_velocity recomputes the stale layers in one launch
+ * sequence (asynchronous on the generator's stream) and reports their number in *recomputed (may be NULL); with one cascade
+ * per rendered frame (ocean_water_frame) that is usually one layer per tick.  The sample and copy entry points bring stale
+ * layers up to date first.  The buffers are allocated (zeroed) by the first velocity call, so generators that never ask
+ * pay no memory; a cascade whose maps were never written has a zero layer.  ocean_get_velocity_map returns the device map
+ * ([num_cascades][N][N] 4 x half, layer-major like the displacement map) without refreshing it.
+ * ocean_sample_velocity: velocity[p] = sum_i texture(velocity, vec3(xz * scales_i.xy, i)).xyz * scales_i.z, the displacement
+ * half of ocean_sample_maps (same filter, wrap and arguments, same validation) at UNDISPLACED points.  The velocity of the
+ * water at a world position Q: call ocean_query_surface for Q and pass its source point P (source_x, source_z) to
+ * ocean_sample_velocity.  With the binary32 taps on, ocean_copy_f32_velocity_to_host returns one layer before the half
+ * conversion ([N][N][4] float). */
+int ocean_update_velocity(ocean_generator* gen, int* recomputed);
+int ocean_get_velocity_map(ocean_generator* gen, void** velocity_dev, size_t* layer_bytes);
+int ocean_copy_velocity_to_host(ocean_generator* gen, int first, int count, void* velocity_host);
+int ocean_sample_velocity(ocean_generator* gen, int num_points, const float* points_xz_host, int num_cascades, const float* map_scales_host,
+                          float* velocity_host);
+int ocean_sample_velocity_device(ocean_generator* gen, int num_points, const float* points_xz_dev, int num_cascades, const float* map_scales_host,
+                                 float* velocity_dev);
+int ocean_copy_f32_velocity_to_host(ocean_generator* gen, int cascade, float* host);
 
 /* Spray candidates -- the spawn test of the sea-spray particle shader as a stream-compaction op
  * (assets/shaders/spatial/sea_spray_particle.gdshader:80-94; the reference evaluates it for every particle of the emitter and

@@ -116,7 +116,7 @@ def run_spray(N, C, particles, reps, label):
     print(json.dumps(out), flush=True)
 
 
-if "--buoyancy" not in sys.argv:       # --buoyancy runs run_buoyancy (defined below) alone
+if "--buoyancy" not in sys.argv and "--velocity" not in sys.argv:   # --buoyancy / --velocity run their op (defined below) alone
     run(256, 4, 2000, "cfg2 latency: one 256x256x4 set per launch (launch/latency-bound, L2-resident)")
     run(256, 4, 2000, "cfg2 latency, fused frames (ocean_update_frames: 64 frames per launch)", fused=True)
     run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, frame by frame")
@@ -275,6 +275,88 @@ def run_buoyancy(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_iter
     g.free()
     print(json.dumps(out), flush=True)
 
+
+def run_velocity(N, C, reps, label, sample_points=0):
+    """ocean_update_velocity with every layer stale against ocean_update_all of the same cascades: CUDA events (the C ABI's
+    device timer) around each call, in alternating windows of `reps` calls.  Every velocity call follows an update_all
+    (which marks every layer stale) that is already queued on the stream, so the velocity kernels start right behind it.
+    With sample_points, also one ocean_sample_velocity_device call against ocean_sample_maps_device on the same points.
+    The card's name, power limit and SM clocks are read in the same run."""
+    import subprocess
+    import torch
+    from godotoceanwaves_b200.native import load_library, check
+    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
+    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
+    for _ in range(3):
+        g.update_all(0.02, p)
+    assert g.update_velocity() == C
+    g.synchronize()
+
+    def window_update():
+        tot = 0.0
+        for _ in range(reps):
+            g.timer_start()
+            g.update_all(0.02, p)
+            tot += g.timer_stop()
+        return tot / reps
+
+    def window_velocity():
+        tot = 0.0
+        for _ in range(reps):
+            g.update_all(0.02, p)
+            g.timer_start()
+            n = g.update_velocity()
+            tot += g.timer_stop()
+            assert n == C
+        return tot / reps
+
+    t_u, t_v = [], []
+    for _ in range(3):                          # alternating windows: clock ramp-up and neighbours hit both alike
+        t_u.append(window_update())
+        t_v.append(window_velocity())
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                         stdout=subprocess.PIPE, text=True).stdout.strip()
+    texels = C * N * N
+    out = {"config": label, "gpu": torch.cuda.get_device_name(0), "power_limit_sm_clock_max_sm_clock": smi, "map_size": N, "cascades": C,
+           "velocity_us_per_call": [1e3 * v for v in t_v], "update_all_us_per_call": [1e3 * v for v in t_u],
+           "velocity_over_update": min(t_v) / min(t_u), "velocity_algorithmic_GBps": 24.0 * texels / (min(t_v) * 1e-3) / 1e9}
+    if sample_points:
+        dev = torch.device("cuda", 0)
+        pts = (torch.rand(sample_points, 2, device=dev, generator=torch.Generator(dev).manual_seed(1)) * 600.0 - 300.0).contiguous()
+        vel = torch.empty(sample_points, 3, device=dev)
+        disp = torch.empty(sample_points, 3, device=dev)
+        grad = torch.empty(sample_points, 3, device=dev)
+        scales = gow.WaveGenerator.map_scales(p)
+        torch.cuda.synchronize()
+        lib = load_library()
+        sv = lambda: check(lib.ocean_sample_velocity_device(g.context, sample_points, pts.data_ptr(), C, scales.ctypes.data, vel.data_ptr()))
+        sm = lambda: check(lib.ocean_sample_maps_device(g.context, sample_points, pts.data_ptr(), C, scales.ctypes.data, disp.data_ptr(),
+                                                        grad.data_ptr()))
+
+        def timed(call):
+            for _ in range(3):
+                call()
+            g.synchronize()
+            g.timer_start()
+            for _ in range(reps):
+                call()
+            return g.timer_stop() / reps
+
+        t_s, t_m = [], []
+        for _ in range(3):
+            t_s.append(timed(sv))
+            t_m.append(timed(sm))
+        out.update({"sample_points": sample_points, "sample_velocity_us_per_call": [1e3 * v for v in t_s],
+                    "sample_maps_us_per_call": [1e3 * v for v in t_m]})
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
+if "--velocity" in sys.argv:
+    run_velocity(256, 4, 200, "velocity: 4 cascades of 256x256, every layer stale", sample_points=1 << 20)
+    run_velocity(256, 128, 50, "velocity: the bench workload, 128 cascades of 256x256, every layer stale")
+    run_velocity(1024, 8, 20, "velocity: 8 cascades of 1024x1024, every layer stale")
+    sys.exit(0)
 
 if "--buoyancy" in sys.argv:
     run_buoyancy(256, 4, 1 << 14, 64, 50, "buoyancy: 2^14 bodies x 64 points over 4 cascades of 256x256")
