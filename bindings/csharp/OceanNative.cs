@@ -77,6 +77,22 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanBodyVelocity                          // struct ocean_body_velocity (24 B), world frame
+    {
+        public fixed float linear[3];                               // of the body ORIGIN: Godot's linear_velocity + angular x (t - com)
+        public fixed float angular[3];                              // rad/s
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanDragResult                            // struct ocean_drag_result (32 B)
+    {
+        public fixed float force[3];
+        public fixed float torque[3];                               // about the body origin
+        public float wetted_drag_area;                              // sum of f * C_d A (m^2)
+        public float max_relative_speed;                            // over the submerged points: for choosing sub-steps
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public struct OceanInfo
     {
         public int device, map_size, num_cascades, pending_cascades;
@@ -160,6 +176,18 @@ namespace OceanB200
         internal static partial int ocean_buoyancy_device(IntPtr handle, int num_bodies, OceanBuoyancyBody* bodies, int num_points, void* points_dev,
                                                           int num_cascades, float* map_scales, float density, float tolerance, int max_iterations,
                                                           void* results_dev, void* samples_dev);
+        // body forces: the buoyancy records plus quadratic drag against the water velocity, from one surface query;
+        // drag_areas [num_points] (C_d A per hull point); samples may be null
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_body_forces(IntPtr handle, int num_bodies, OceanBuoyancyBody* bodies, OceanBodyVelocity* velocities,
+                                                      int num_points, OceanBuoyancyPoint* points, float* drag_areas, int num_cascades,
+                                                      float* map_scales, float density, float tolerance, int max_iterations,
+                                                      OceanBuoyancyResult* hydrostatic, OceanDragResult* drag, OceanSurfaceSample* samples);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_body_forces_device(IntPtr handle, int num_bodies, OceanBuoyancyBody* bodies, OceanBodyVelocity* velocities,
+                                                             int num_points, void* points_dev, void* drag_areas_dev, int num_cascades,
+                                                             float* map_scales, float density, float tolerance, int max_iterations,
+                                                             void* hydrostatic_dev, void* drag_dev, void* samples_dev);
         // velocity maps: d/dt of the displacement map, recomputed for the cascades whose maps changed; recomputed may be null
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_update_velocity(IntPtr handle, int* recomputed);

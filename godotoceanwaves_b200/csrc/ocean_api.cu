@@ -84,6 +84,13 @@ struct ocean_generator {
     size_t buoy_points_capacity = 0;
     ocean_buoyancy_result* buoy_results = nullptr;
     size_t buoy_results_capacity = 0;
+    // body-forces staging, grown on demand: body velocities, and the host entry point's drag areas and drag results
+    ocean_body_velocity* drag_velocities = nullptr;
+    size_t drag_velocities_capacity = 0;
+    float* drag_areas = nullptr;
+    size_t drag_areas_capacity = 0;
+    ocean_drag_result* drag_results = nullptr;
+    size_t drag_results_capacity = 0;
     // velocity maps, allocated by the first velocity call: row-pass scratch, the map, its binary32 tap while the taps are on
     float4* vel_scratch = nullptr;                      // [num_cascades][N][N]
     uint2* velocity = nullptr;                          // [num_cascades][N][N] 4 x half
@@ -209,6 +216,9 @@ void release(ocean_generator* g) {
     cudaFree(g->buoy_q);
     cudaFree(g->buoy_samples);
     cudaFree(g->buoy_points);
+    cudaFree(g->drag_velocities);
+    cudaFree(g->drag_areas);
+    cudaFree(g->drag_results);
     cudaFree(g->vel_scratch);
     cudaFree(g->velocity);
     cudaFree(g->velocity_f32);
@@ -1258,18 +1268,14 @@ int check_buoyancy_args(int num_bodies, const ocean_buoyancy_body* bodies, int n
     *world = (int)total;
     return OCEAN_OK;
 }
-}  // namespace
 
-int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int num_points,
-                          const ocean_buoyancy_point* points_dev, int num_cascades, const float* map_scales_host, float density,
-                          float tolerance, int max_iterations, ocean_buoyancy_result* results_dev, ocean_surface_sample* samples_dev) {
-    OCEAN_ENTER(gen);
-    if (rc) return rc;
-    int world = 0;
-    if ((rc = check_buoyancy_args(num_bodies, bodies_host, num_points, density, tolerance, max_iterations, &world))) return rc;
-    if (num_bodies == 0) return OCEAN_OK;
-    if (!results_dev || (world > 0 && !points_dev)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
-    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
+// The buoyancy launch sequence on validated arguments (num_bodies > 0), with the map scales already in gen->q_scales: the body
+// table and offsets are uploaded to gen->buoy_bodies / gen->buoy_offsets, and *samples_used receives the surface records
+// (samples_dev, or the generator's staging when samples_dev is NULL) for a drag pass on the same points.
+int run_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int world, const ocean_buoyancy_point* points_dev,
+                 int num_cascades, float density, float tolerance, int max_iterations, ocean_buoyancy_result* results_dev,
+                 ocean_surface_sample* samples_dev, ocean_surface_sample** samples_used) {
+    int rc;
     const size_t B = (size_t)num_bodies;
     if ((rc = grow_buffer(gen, &gen->buoy_bodies, &gen->buoy_bodies_capacity, B))) return rc;
     if ((rc = grow_buffer(gen, &gen->buoy_offsets, &gen->buoy_offsets_capacity, B))) return rc;
@@ -1290,7 +1296,23 @@ int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoy
     OCEAN_CUDA(ocean::launch_buoyancy_reduce(gen->buoy_bodies, gen->buoy_offsets, num_bodies, points_dev, samples, rho_g, tolerance,
                                              results_dev, gen->stream));
     gen->kernel_launches += 1;
+    if (samples_used) *samples_used = samples;
     return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int num_points,
+                          const ocean_buoyancy_point* points_dev, int num_cascades, const float* map_scales_host, float density,
+                          float tolerance, int max_iterations, ocean_buoyancy_result* results_dev, ocean_surface_sample* samples_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_buoyancy_args(num_bodies, bodies_host, num_points, density, tolerance, max_iterations, &world))) return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (!results_dev || (world > 0 && !points_dev)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
+    return run_buoyancy(gen, num_bodies, bodies_host, world, points_dev, num_cascades, density, tolerance, max_iterations, results_dev,
+                        samples_dev, nullptr);
 }
 
 int ocean_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int num_points,
@@ -1433,6 +1455,86 @@ int ocean_sample_velocity(ocean_generator* gen, int num_points, const float* poi
                                            gen->q_disp)))
         return rc;
     OCEAN_CUDA(cudaMemcpyAsync(velocity_host, gen->q_disp, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+// ---- body forces: buoyancy plus quadratic drag against the water velocity, from one surface query (oracle/drag.py) ----
+static_assert(sizeof(ocean_body_velocity) == 24, "ocean_body_velocity layout");
+static_assert(sizeof(ocean_drag_result) == 32, "ocean_drag_result layout");
+
+namespace {
+// ocean_buoyancy's checks plus the body velocities and drag areas; *world as for check_buoyancy_args.
+int check_body_forces_args(int num_bodies, const ocean_buoyancy_body* bodies, const ocean_body_velocity* velocities, int num_points,
+                           const float* drag_areas, float density, float tolerance, int max_iterations, int* world) {
+    int rc = check_buoyancy_args(num_bodies, bodies, num_points, density, tolerance, max_iterations, world);
+    if (rc) return rc;
+    if (num_bodies > 0 && !velocities) return fail(OCEAN_ERR_INVALID_ARGUMENT, "velocities is NULL");
+    if (*world > 0 && !drag_areas) return fail(OCEAN_ERR_INVALID_ARGUMENT, "drag_areas is NULL");
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_body_forces_device(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host,
+                             const ocean_body_velocity* velocities_host, int num_points, const ocean_buoyancy_point* points_dev,
+                             const float* drag_areas_dev, int num_cascades, const float* map_scales_host, float density, float tolerance,
+                             int max_iterations, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
+                             ocean_surface_sample* samples_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_body_forces_args(num_bodies, bodies_host, velocities_host, num_points, drag_areas_dev, density, tolerance, max_iterations,
+                                     &world)))
+        return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (!hydrostatic_dev || !drag_dev || (world > 0 && !points_dev)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
+    if ((rc = refresh_velocity(gen, nullptr))) return rc;
+    const size_t B = (size_t)num_bodies;
+    if ((rc = grow_buffer(gen, &gen->drag_velocities, &gen->drag_velocities_capacity, B))) return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(gen->drag_velocities, velocities_host, sizeof(ocean_body_velocity) * B, cudaMemcpyHostToDevice, gen->stream));
+    ocean_surface_sample* samples = nullptr;
+    if ((rc = run_buoyancy(gen, num_bodies, bodies_host, world, points_dev, num_cascades, density, tolerance, max_iterations, hydrostatic_dev,
+                           samples_dev, &samples)))
+        return rc;
+    const float half_rho = 0.5f * density;
+    OCEAN_CUDA(ocean::launch_drag_reduce(gen->buoy_bodies, gen->drag_velocities, gen->buoy_offsets, num_bodies, points_dev, drag_areas_dev, samples,
+                                         gen->velocity, gen->map_size, num_cascades, gen->q_scales, half_rho, drag_dev, gen->stream));
+    gen->kernel_launches += 1;
+    return OCEAN_OK;
+}
+
+int ocean_body_forces(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, const ocean_body_velocity* velocities_host,
+                      int num_points, const ocean_buoyancy_point* points_host, const float* drag_areas_host, int num_cascades,
+                      const float* map_scales_host, float density, float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_host,
+                      ocean_drag_result* drag_host, ocean_surface_sample* samples_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_body_forces_args(num_bodies, bodies_host, velocities_host, num_points, drag_areas_host, density, tolerance, max_iterations,
+                                     &world)))
+        return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (!hydrostatic_host || !drag_host || (world > 0 && !points_host)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
+    if ((rc = grow_buffer(gen, &gen->buoy_results, &gen->buoy_results_capacity, (size_t)num_bodies))) return rc;
+    if ((rc = grow_buffer(gen, &gen->drag_results, &gen->drag_results_capacity, (size_t)num_bodies))) return rc;
+    if (world > 0) {
+        if ((rc = grow_buffer(gen, &gen->buoy_points, &gen->buoy_points_capacity, (size_t)num_points))) return rc;
+        if ((rc = grow_buffer(gen, &gen->drag_areas, &gen->drag_areas_capacity, (size_t)num_points))) return rc;
+        OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_points, points_host, sizeof(ocean_buoyancy_point) * (size_t)num_points, cudaMemcpyHostToDevice,
+                                   gen->stream));
+        OCEAN_CUDA(cudaMemcpyAsync(gen->drag_areas, drag_areas_host, sizeof(float) * (size_t)num_points, cudaMemcpyHostToDevice, gen->stream));
+    }
+    if ((rc = ocean_body_forces_device(gen, num_bodies, bodies_host, velocities_host, num_points, world > 0 ? gen->buoy_points : nullptr,
+                                       world > 0 ? gen->drag_areas : nullptr, num_cascades, map_scales_host, density, tolerance, max_iterations,
+                                       gen->buoy_results, gen->drag_results, nullptr)))
+        return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(hydrostatic_host, gen->buoy_results, sizeof(ocean_buoyancy_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost,
+                               gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(drag_host, gen->drag_results, sizeof(ocean_drag_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost, gen->stream));
+    if (samples_host && world > 0)
+        OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
+                                   gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }

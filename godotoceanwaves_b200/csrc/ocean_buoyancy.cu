@@ -10,9 +10,15 @@
 //                         sums v, v r.x, v r.y, v r.z in the specification's order -- each lane from +0 in increasing j, then
 //                         __shfl_down_sync with offsets 16, 8, 4, 2, 1 -- and lane 0 writes the body's record.
 // No shared memory and no atomics: a body of any size is a longer lane loop, and the result does not depend on the schedule.
+//
+// The body-forces op (ocean_body_forces; oracle/drag.py is the specification) runs the same three steps and then
+//   k_drag_reduce         one warp per body in the same lane order: recomputes r and f as k_buoyancy_reduce does; for a
+//                         submerged point (f > 0) gathers the velocity maps at the record's source point (4 texels per
+//                         cascade), and sums the quadratic drag force, its torque about the body origin and f * C_d A.
 // Numeric policy: binary32, the specification's operation order, no contraction (-fmad=false).
 #include "../../include/ocean.h"
 #include "ocean_kernels.cuh"
+#include "ocean_texture.cuh"
 
 namespace ocean {
 
@@ -25,6 +31,11 @@ __device__ __forceinline__ float3 rotate(const float* __restrict__ T, const floa
     r.y = (T[4] * p[0] + T[5] * p[1]) + T[6] * p[2];
     r.z = (T[8] * p[0] + T[9] * p[1]) + T[10] * p[2];
     return r;
+}
+
+// f of the specification: the submerged fraction of a column of half height h centred at height wy, under water height eta
+__device__ __forceinline__ float submerged_fraction(float eta, float wy, float h) {
+    return h > 0.0f ? fminf(fmaxf(__fdiv_rn(eta - (wy - h), h + h), 0.0f), 1.0f) : (wy <= eta ? 1.0f : 0.0f);
 }
 
 __global__ void __launch_bounds__(256) k_buoyancy_transform(const ocean_buoyancy_body* __restrict__ bodies, const int* __restrict__ offsets,
@@ -68,7 +79,7 @@ __global__ void __launch_bounds__(256) k_buoyancy_reduce(const ocean_buoyancy_bo
         const float h = hull[j].half_height;
         const float eta = rec[j].displacement[1];
         const float res = rec[j].residual;
-        const float f = h > 0.0f ? fminf(fmaxf(__fdiv_rn(eta - (wy - h), h + h), 0.0f), 1.0f) : (wy <= eta ? 1.0f : 0.0f);
+        const float f = submerged_fraction(eta, wy, h);
         const float v = f * hull[j].volume;
         s0 = s0 + v;
         sx = sx + v * r.x;
@@ -104,6 +115,79 @@ __global__ void __launch_bounds__(256) k_buoyancy_reduce(const ocean_buoyancy_bo
     out[body] = o;
 }
 
+// d = u - (v + w x r) per submerged point, F = ((f * cda) * |d|) d, T = r x F; per body half_rho * sum F, half_rho * sum T,
+// sum f * cda and the NaN-dropping max of |d| (from 0), each summed in k_buoyancy_reduce's order.
+__global__ void __launch_bounds__(256) k_drag_reduce(const ocean_buoyancy_body* __restrict__ bodies, const ocean_body_velocity* __restrict__ velocities,
+                                                     const int* __restrict__ offsets, int num_bodies, const ocean_buoyancy_point* __restrict__ points,
+                                                     const float* __restrict__ drag_areas, const ocean_surface_sample* __restrict__ samples,
+                                                     const uint2* __restrict__ velocity, int N, int C, const float4* __restrict__ scales,
+                                                     float half_rho, ocean_drag_result* __restrict__ out) {
+    const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (warp >= (size_t)num_bodies) return;        // whole warps: the shuffles below see all 32 lanes
+    const int body = (int)warp;
+    const int lane = threadIdx.x & 31;
+    const ocean_buoyancy_body& b = bodies[body];
+    const int count = b.num_points;
+    if (count == 0) {
+        if (lane == 0) out[body] = ocean_drag_result{};
+        return;
+    }
+    const ocean_buoyancy_point* hull = points + b.first_point;
+    const float* cda = drag_areas + b.first_point;
+    const ocean_surface_sample* rec = samples + offsets[body];
+    const ocean_body_velocity bv = velocities[body];
+    const float ty = b.transform[7];
+    float sfx = 0.0f, sfy = 0.0f, sfz = 0.0f, stx = 0.0f, sty = 0.0f, stz = 0.0f, sa = 0.0f, max_s = 0.0f;
+    for (int j = lane; j < count; j += 32) {
+        const float3 r = rotate(b.transform, hull[j].position);
+        const float f = submerged_fraction(rec[j].displacement[1], r.y + ty, hull[j].half_height);
+        if (!(f > 0.0f)) continue;                  // a dry point gathers nothing and adds nothing
+        const float px = rec[j].source_x, pz = rec[j].source_z;
+        float ux = 0.0f, uy = 0.0f, uz = 0.0f;
+        for (int c = 0; c < C; ++c) {
+            const float4 s = __ldg(&scales[c]);
+            add_displacement(velocity + (size_t)c * N * N, N, px * s.x, pz * s.y, s.z, ux, uy, uz);
+        }
+        const float dx = ux - (bv.linear[0] + (bv.angular[1] * r.z - bv.angular[2] * r.y));
+        const float dy = uy - (bv.linear[1] + (bv.angular[2] * r.x - bv.angular[0] * r.z));
+        const float dz = uz - (bv.linear[2] + (bv.angular[0] * r.y - bv.angular[1] * r.x));
+        const float speed = __fsqrt_rn((dx * dx + dy * dy) + dz * dz);
+        const float a = f * __ldg(&cda[j]);
+        const float k = a * speed;
+        const float Fx = k * dx, Fy = k * dy, Fz = k * dz;
+        sfx = sfx + Fx;
+        sfy = sfy + Fy;
+        sfz = sfz + Fz;
+        stx = stx + (r.y * Fz - r.z * Fy);
+        sty = sty + (r.z * Fx - r.x * Fz);
+        stz = stz + (r.x * Fy - r.y * Fx);
+        sa = sa + a;
+        max_s = fmaxf(max_s, speed);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {              // p[l] = p[l] + p[l + o]: the specification's tree
+        sfx = sfx + __shfl_down_sync(0xffffffffu, sfx, o);
+        sfy = sfy + __shfl_down_sync(0xffffffffu, sfy, o);
+        sfz = sfz + __shfl_down_sync(0xffffffffu, sfz, o);
+        stx = stx + __shfl_down_sync(0xffffffffu, stx, o);
+        sty = sty + __shfl_down_sync(0xffffffffu, sty, o);
+        stz = stz + __shfl_down_sync(0xffffffffu, stz, o);
+        sa = sa + __shfl_down_sync(0xffffffffu, sa, o);
+        max_s = fmaxf(max_s, __shfl_down_sync(0xffffffffu, max_s, o));
+    }
+    if (lane != 0) return;
+    ocean_drag_result o;
+    o.force[0] = half_rho * sfx;
+    o.force[1] = half_rho * sfy;
+    o.force[2] = half_rho * sfz;
+    o.torque[0] = half_rho * stx;
+    o.torque[1] = half_rho * sty;
+    o.torque[2] = half_rho * stz;
+    o.wetted_drag_area = sa;
+    o.max_relative_speed = max_s;
+    out[body] = o;
+}
+
 }  // namespace
 
 cudaError_t launch_buoyancy_transform(const void* bodies_dev, const int* offsets_dev, int num_bodies, const void* points_dev, int n,
@@ -122,6 +206,19 @@ cudaError_t launch_buoyancy_reduce(const void* bodies_dev, const int* offsets_de
                                                   static_cast<const ocean_buoyancy_point*>(points_dev),
                                                   static_cast<const ocean_surface_sample*>(samples_dev), rho_g, tolerance,
                                                   static_cast<ocean_buoyancy_result*>(results_dev));
+    return cudaGetLastError();
+}
+
+cudaError_t launch_drag_reduce(const void* bodies_dev, const void* velocities_dev, const int* offsets_dev, int num_bodies,
+                               const void* points_dev, const float* drag_areas_dev, const void* samples_dev, const uint2* velocity_dev,
+                               int map_size, int num_cascades, const float4* scales_dev, float half_rho, void* results_dev, cudaStream_t stream) {
+    if (num_bodies <= 0) return cudaSuccess;
+    const unsigned blocks = (unsigned)(((size_t)num_bodies * 32 + 255) / 256);      // 8 bodies per block
+    k_drag_reduce<<<blocks, 256, 0, stream>>>(static_cast<const ocean_buoyancy_body*>(bodies_dev),
+                                              static_cast<const ocean_body_velocity*>(velocities_dev), offsets_dev, num_bodies,
+                                              static_cast<const ocean_buoyancy_point*>(points_dev), drag_areas_dev,
+                                              static_cast<const ocean_surface_sample*>(samples_dev), velocity_dev, map_size, num_cascades,
+                                              scales_dev, half_rho, static_cast<ocean_drag_result*>(results_dev));
     return cudaGetLastError();
 }
 

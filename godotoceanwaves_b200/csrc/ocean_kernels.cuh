@@ -133,6 +133,12 @@ cudaError_t launch_buoyancy_transform(const void* bodies_dev, const int* offsets
                                       float2* q_dev, cudaStream_t stream);
 cudaError_t launch_buoyancy_reduce(const void* bodies_dev, const int* offsets_dev, int num_bodies, const void* points_dev,
                                    const void* samples_dev, float rho_g, float tolerance, void* results_dev, cudaStream_t stream);
+// The drag half of the body-forces op (oracle/drag.py), on the same bodies, offsets, points and surface records:
+// velocities_dev = ocean_body_velocity[num_bodies], drag_areas_dev = [num_points] C_d A parallel to points_dev, velocity_dev =
+// the velocity maps ([num_cascades used][map_size^2] 4 x half), results_dev = ocean_drag_result[num_bodies]
+cudaError_t launch_drag_reduce(const void* bodies_dev, const void* velocities_dev, const int* offsets_dev, int num_bodies,
+                               const void* points_dev, const float* drag_areas_dev, const void* samples_dev, const uint2* velocity_dev,
+                               int map_size, int num_cascades, const float4* scales_dev, float half_rho, void* results_dev, cudaStream_t stream);
 
 // ocean_velocity.cu: velocity maps (oracle_velocity_update).  One record per cascade to recompute: the table slot and time of
 // the update that built the cascade's current maps.

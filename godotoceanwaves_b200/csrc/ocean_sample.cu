@@ -50,15 +50,6 @@ __device__ __forceinline__ float4 texture_bicubic(const uint2* __restrict__ laye
                 mix4(texture_bilinear(layer, N, hy, hz), texture_bilinear(layer, N, hx, hz), wxx), wyy);
 }
 
-// Cascade c's term of the displacement sum of vertex() (:34-35), added to (dx, dy, dz).
-__device__ __forceinline__ void add_displacement(const uint2* __restrict__ layer, int N, float u, float v, float scale, float& dx, float& dy,
-                                                 float& dz) {
-    const float4 d = texture_bilinear(layer, N, u, v);
-    dx = dx + d.x * scale;
-    dy = dy + d.y * scale;
-    dz = dz + d.z * scale;
-}
-
 // The sampling contract at one point p: displacement (vertex(), :27-39) and gradient/foam (fragment(), :72-84).
 __device__ __forceinline__ void sample_point(const uint2* __restrict__ displacement, const uint2* __restrict__ normal, int N, int C, float2 p,
                                              const float4* __restrict__ scales, float3& disp, float3& grad) {

@@ -1,6 +1,7 @@
 // ocean_texture.cuh -- texture() of the reference's spatial shaders on the generator's RGBA16F maps: exact-weight bilinear
 // filter with REPEAT addressing, binary32, round to nearest, no contraction (oracle/sampling.py is the specification).
-// Shared by the map-query and surface-query ops (ocean_sample.cu) and the spray-candidate op (ocean_spray.cu).
+// Shared by the map-query, surface-query and velocity-query ops (ocean_sample.cu), the spray-candidate op (ocean_spray.cu)
+// and the drag reduction of the body-forces op (ocean_buoyancy.cu).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -59,6 +60,16 @@ __device__ __forceinline__ float4 texture_bilinear_slopes(const uint2* __restric
     du = make_float4(su.x * n, su.y * n, su.z * n, su.w * n);
     dv = make_float4(sv.x * n, sv.y * n, sv.z * n, sv.w * n);
     return mix4(mix4(t00, t10, fx), mix4(t01, t11, fx), fy);
+}
+
+// Cascade c's term of the displacement sum of the water shader's vertex() (water.gdshader:34-35), added to (dx, dy, dz).
+// On the velocity maps (v = dD/dt, so the displacement scale applies) it is the cascade's term of the water velocity.
+__device__ __forceinline__ void add_displacement(const uint2* __restrict__ layer, int N, float u, float v, float scale, float& dx, float& dy,
+                                                 float& dz) {
+    const float4 d = texture_bilinear(layer, N, u, v);
+    dx = dx + d.x * scale;
+    dy = dy + d.y * scale;
+    dz = dz + d.z * scale;
 }
 
 }  // namespace

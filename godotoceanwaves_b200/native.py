@@ -51,6 +51,16 @@ class BuoyancyResultC(C.Structure):
                 ("center_offset", C.c_float * 3), ("max_residual", C.c_float), ("unconverged", C.c_uint32)]
 
 
+class BodyVelocityC(C.Structure):
+    """struct ocean_body_velocity (include/ocean.h), 24 B: world-frame velocity of the body origin (m/s), angular velocity (rad/s)"""
+    _fields_ = [("linear", C.c_float * 3), ("angular", C.c_float * 3)]
+
+
+class DragResultC(C.Structure):
+    """struct ocean_drag_result (include/ocean.h), 32 B"""
+    _fields_ = [("force", C.c_float * 3), ("torque", C.c_float * 3), ("wetted_drag_area", C.c_float), ("max_relative_speed", C.c_float)]
+
+
 # every symbol include/ocean.h declares: name -> (restype, argtypes)
 _H = C.c_void_p
 _P = C.POINTER
@@ -93,6 +103,10 @@ SIGNATURES = {
                                  C.c_void_p, C.c_void_p]),
     "ocean_buoyancy_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int,
                                         C.c_void_p, C.c_void_p]),
+    "ocean_body_forces": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_float,
+                                    C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ocean_body_forces_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                           C.c_float, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ocean_update_velocity": (C.c_int, [_H, _P(C.c_int)]),
     "ocean_get_velocity_map": (C.c_int, [_H, _P(C.c_void_p), _P(C.c_size_t)]),
     "ocean_copy_velocity_to_host": (C.c_int, [_H, C.c_int, C.c_int, C.c_void_p]),

@@ -307,6 +307,34 @@ class WaveGenerator:
                                             None if samples is None else samples.ctypes.data))
         return (out, samples) if return_samples else out
 
+    # -- body forces: buoyancy plus quadratic drag against the water velocity, from one surface query ---------------
+    BODY_VELOCITY = np.dtype([("linear", np.float32, 3), ("angular", np.float32, 3)])   # struct ocean_body_velocity
+    DRAG_RESULT = np.dtype([("force", np.float32, 3), ("torque", np.float32, 3), ("wetted_drag_area", np.float32),
+                            ("max_relative_speed", np.float32)])                      # struct ocean_drag_result
+
+    def body_forces(self, bodies, velocities, points, drag_areas, map_scales, density: float = 1025.0, tolerance: float = 1e-3,
+                    max_iterations: int = 8, return_samples: bool = False):
+        """(BUOYANCY_RESULT rows, DRAG_RESULT rows), one each per BUOYANCY_BODY row of `bodies`: the records buoyancy() returns,
+        and the quadratic drag against the water velocity (include/ocean.h, ocean_body_forces).  `velocities` holds one
+        BODY_VELOCITY row per body (world frame; `linear` is the velocity of the body ORIGIN), `drag_areas` one C_d A (m^2)
+        per BUOYANCY_POINT row of `points`.  With return_samples, also the SURFACE_SAMPLE of every world point."""
+        self._require()
+        b = np.ascontiguousarray(bodies, self.BUOYANCY_BODY).reshape(-1)
+        v = np.ascontiguousarray(velocities, self.BODY_VELOCITY).reshape(-1)
+        p = np.ascontiguousarray(points, self.BUOYANCY_POINT).reshape(-1)
+        a = np.ascontiguousarray(drag_areas, np.float32).reshape(-1)
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        if len(v) != len(b) or len(a) != len(p):
+            raise ValueError(f"{len(v)} velocities for {len(b)} bodies, or {len(a)} drag areas for {len(p)} points")
+        hydro = np.zeros(len(b), self.BUOYANCY_RESULT)
+        drag = np.zeros(len(b), self.DRAG_RESULT)
+        world = int(np.maximum(b["num_points"], 0).astype(np.int64).sum())
+        samples = np.zeros(world, self.SURFACE_SAMPLE) if return_samples else None
+        check(load_library().ocean_body_forces(self.context, len(b), b.ctypes.data, v.ctypes.data, len(p), p.ctypes.data, a.ctypes.data,
+                                               sc.shape[0], sc.ctypes.data, float(density), float(tolerance), int(max_iterations),
+                                               hydro.ctypes.data, drag.ctypes.data, None if samples is None else samples.ctypes.data))
+        return (hydro, drag, samples) if return_samples else (hydro, drag)
+
     # -- spray candidates: the spawn test of sea_spray_particle.gdshader:80-94 as a stream compaction --------------
     SPRAY_RECORD = np.dtype([("index", np.uint32), ("start_x", np.float32), ("start_z", np.float32), ("scale_factor", np.float32),
                              ("particle_scale", np.float32, 3), ("foam", np.float32)])     # struct ocean_spray_record

@@ -233,9 +233,9 @@ int ocean_query_surface_device(ocean_generator* gen, int num_points, const float
  *   unconverged       points whose residual is not <= tolerance
  * A body with num_points = 0 gets an all-zero record.  num_cascades, map_scales, tolerance and max_iterations mean what they
  * mean for ocean_query_surface, whose limits carry over (within 150 m of the camera; any converged preimage where the surface
- * folds).  The model is vertical hydrostatics only: no drag or added mass (the water velocity these need comes from
- * ocean_sample_velocity, but the body table carries no body velocities, so neither is applied), the column element stays
- * vertical under rotation, and volumes are not rescaled by a non-rigid transform.
+ * folds).  The model is vertical hydrostatics only: no drag (ocean_body_forces below returns this record together with a
+ * drag record, from one surface query) and no added mass, the column element stays vertical under rotation, and volumes
+ * are not rescaled by a non-rigid transform.
  * density must be finite and > 0, counts non-negative, every body's range inside [0, num_points), and the sum of the bodies'
  * num_points (the world points) at most INT32_MAX.  samples may be NULL, or receives the surface record of every world point
  * ([sum of num_points], body-major, j increasing).  The bodies and map_scales are host arrays in both entry points (the poses
@@ -266,6 +266,54 @@ int ocean_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_bo
 int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int num_points,
                           const ocean_buoyancy_point* points_dev, int num_cascades, const float* map_scales_host, float density,
                           float tolerance, int max_iterations, ocean_buoyancy_result* results_dev, ocean_surface_sample* samples_dev);
+
+/* Body forces -- buoyancy plus quadratic drag against the water velocity, per body, from one surface query.
+ * The bodies, hull points, num_cascades, map_scales, density, tolerance and max_iterations are those of ocean_buoyancy, and
+ * `hydrostatic` receives exactly the records ocean_buoyancy returns for them.  Each body also has a velocity (world frame):
+ * `linear` is the velocity of the body ORIGIN t, `angular` its angular velocity in rad/s.  Godot's linear_velocity is that
+ * of the centre of mass: pass v_com + angular x (t - com).  drag_areas[num_points] runs parallel to the hull points: C_d A in
+ * m^2 per hull point, so bodies that share a hull share its areas.  For world point j of a body, with r, w, the surface
+ * record and f as in ocean_buoyancy, a point with f > 0 contributes
+ *   u  = sum_i texture(velocity, vec3((source_x, source_z) * scales_i.xy, i)).xyz * scales_i.z   (ocean_sample_velocity at
+ *        the record's source point: the water velocity at w)
+ *   vb = linear + (a.y r.z - a.z r.y, a.z r.x - a.x r.z, a.x r.y - a.y r.x)   (a = angular; each bracket rounded as written)
+ *   d  = u - vb,  s = sqrt((d.x d.x + d.y d.y) + d.z d.z),  k = (f * cda) * s,  F = k d,  T = r x F (component order as vb's)
+ * and a point with f = 0 contributes nothing.  Per body, in ocean_buoyancy's summation order, with half_rho = 0.5f * density:
+ *   force               half_rho * sum F
+ *   torque              half_rho * sum T, about the body origin t (like ocean_buoyancy's)
+ *   wetted_drag_area    sum f * cda (m^2)
+ *   max_relative_speed  NaN-dropping max of s over the points with f > 0, from 0 (0 when there are none)
+ * oracle/drag.py is the specification, bit for bit.  A body with num_points = 0 gets an all-zero record.  The model's limits:
+ * it uses the SURFACE water velocity at every submerged point, while the orbital velocity of a wave decays as e^(-k z) with
+ * depth z (at 1 m of draft this overstates the longest wave of a 16 m tile about 1.5 times, shorter waves more); there is no
+ * added mass, radiation or wave-making damping, skin friction, or separate normal and tangential coefficients; nothing is
+ * written back into the maps (no wake or foam).  Quadratic drag is stiff for light bodies under explicit integration: the op
+ * does not integrate, and max_relative_speed lets a host choose sub-steps.
+ * The call first brings stale velocity layers up to date (as ocean_sample_velocity does; the velocity buffers are allocated
+ * on first use).  Validation is ocean_buoyancy's, plus velocities and drag_areas non-NULL where a count needs them and both
+ * outputs non-NULL; an invalid call launches nothing.  samples may be NULL, as for ocean_buoyancy.  The bodies, velocities
+ * and map_scales are host arrays in both entry points; ocean_body_forces takes host points, areas and outputs and is
+ * synchronous; ocean_body_forces_device takes device pointers for them and is asynchronous on the generator's stream.  With
+ * no stale velocity layer, a call with world points launches 6 kernels (4 with max_iterations = 0). */
+typedef struct ocean_body_velocity {
+    float linear[3];       /* velocity of the body origin t (m/s) */
+    float angular[3];      /* rad/s */
+} ocean_body_velocity;     /* 24 B */
+typedef struct ocean_drag_result {
+    float force[3];
+    float torque[3];       /* about the body origin t */
+    float wetted_drag_area;
+    float max_relative_speed;
+} ocean_drag_result;       /* 32 B */
+int ocean_body_forces(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, const ocean_body_velocity* velocities_host,
+                      int num_points, const ocean_buoyancy_point* points_host, const float* drag_areas_host, int num_cascades,
+                      const float* map_scales_host, float density, float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_host,
+                      ocean_drag_result* drag_host, ocean_surface_sample* samples_host);
+int ocean_body_forces_device(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host,
+                             const ocean_body_velocity* velocities_host, int num_points, const ocean_buoyancy_point* points_dev,
+                             const float* drag_areas_dev, int num_cascades, const float* map_scales_host, float density, float tolerance,
+                             int max_iterations, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
+                             ocean_surface_sample* samples_dev);
 
 /* Velocity maps -- the water velocity: the time derivative of the displacement map, what drag, damping and floating debris
  * need.  A cascade's velocity layer is (vx, vy, vz, 0) = d/dt of its displacement texel (hx, hy, hz, 0): same layout, same

@@ -116,7 +116,7 @@ def run_spray(N, C, particles, reps, label):
     print(json.dumps(out), flush=True)
 
 
-if "--buoyancy" not in sys.argv and "--velocity" not in sys.argv:   # --buoyancy / --velocity run their op (defined below) alone
+if not {"--buoyancy", "--velocity", "--drag"} & set(sys.argv):    # --buoyancy / --velocity / --drag run their op (defined below) alone
     run(256, 4, 2000, "cfg2 latency: one 256x256x4 set per launch (launch/latency-bound, L2-resident)")
     run(256, 4, 2000, "cfg2 latency, fused frames (ocean_update_frames: 64 frames per launch)", fused=True)
     run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, frame by frame")
@@ -206,20 +206,11 @@ def run_surface(N, C, n_points, reps, label, tolerance=1e-3, max_iterations=8):
     print(json.dumps(out), flush=True)
 
 
-def run_buoyancy(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_iterations=8):
-    """Buoyancy op (ocean_buoyancy_device) on device-resident hulls of `per_body` points per body: kernel time from CUDA
-    events, against ocean_query_surface_device on the same world points in the same run, in alternating windows.  The card's
-    name, power limit and max SM clock are read in the same run."""
-    import subprocess
+def _buoyancy_scene(n_bodies, per_body):
+    """n_bodies bodies of per_body hull points each (points in [-2, 2]^3 m), random rotations, positions in [-300, 300] m
+    around the surface: (bodies, hull) in the layouts of oracle/buoyancy.py."""
     import numpy as np
-    import torch
-    from godotoceanwaves_b200.native import load_library, check
     from oracle import buoyancy as bu
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for _ in range(2):
-        g.update_all(0.02, p)
-    scales = gow.WaveGenerator.map_scales(p)
     rng = np.random.default_rng(1)
     hull = np.zeros(n_bodies * per_body, bu.POINT)
     hull["position"] = rng.uniform(-2.0, 2.0, (len(hull), 3))
@@ -236,6 +227,24 @@ def run_buoyancy(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_iter
     bodies["transform"] = np.concatenate([R, t[:, :, None]], 2).reshape(n_bodies, 12)
     bodies["first_point"] = np.arange(n_bodies) * per_body
     bodies["num_points"] = per_body
+    return bodies, hull
+
+
+def run_buoyancy(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_iterations=8):
+    """Buoyancy op (ocean_buoyancy_device) on device-resident hulls of `per_body` points per body: kernel time from CUDA
+    events, against ocean_query_surface_device on the same world points in the same run, in alternating windows.  The card's
+    name, power limit and max SM clock are read in the same run."""
+    import subprocess
+    import numpy as np
+    import torch
+    from godotoceanwaves_b200.native import load_library, check
+    from oracle import buoyancy as bu
+    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
+    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
+    for _ in range(2):
+        g.update_all(0.02, p)
+    scales = gow.WaveGenerator.map_scales(p)
+    bodies, hull = _buoyancy_scene(n_bodies, per_body)
     _, _, _, wp = bu.world_points(bodies, hull)
     n_points = len(wp)
     dev = torch.device("cuda", 0)
@@ -272,6 +281,69 @@ def run_buoyancy(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_iter
            "overhead_over_query": min(t_b) / min(t_q) - 1.0, "mpoints_per_s": n_points / (min(t_b) * 1e-3) / 1e6,
            "frac_bodies_afloat": float(np.mean(res["submerged_volume"] > 0)),
            "frac_points_unconverged": float(res["unconverged"].sum()) / n_points}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
+def run_body_forces(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_iterations=8):
+    """Body-forces op (ocean_body_forces_device: buoyancy plus drag) against ocean_buoyancy_device on the same bodies and
+    device-resident hulls: CUDA events around each call, in alternating windows.  No velocity layer is stale inside the
+    windows (the warm-up calls refresh them).  Reports both times, the overhead of the drag pass, and the fraction of world
+    points that are submerged.  The card's name, power limit and max SM clock are read in the same run."""
+    import subprocess
+    import numpy as np
+    import torch
+    from godotoceanwaves_b200.native import load_library, check
+    from oracle import buoyancy as bu
+    from oracle import drag as dr
+    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
+    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
+    for _ in range(2):
+        g.update_all(0.02, p)
+    scales = gow.WaveGenerator.map_scales(p)
+    bodies, hull = _buoyancy_scene(n_bodies, per_body)
+    rng = np.random.default_rng(2)
+    vel = np.zeros(n_bodies, dr.VELOCITY)
+    vel["linear"] = rng.uniform(-2.0, 2.0, (n_bodies, 3))
+    vel["angular"] = rng.uniform(-1.0, 1.0, (n_bodies, 3))
+    cda = rng.uniform(0.01, 0.2, len(hull)).astype(np.float32)
+    n_points = n_bodies * per_body
+    dev = torch.device("cuda", 0)
+    hull_d = torch.from_numpy(hull.view(np.uint8).copy()).to(dev)
+    cda_d = torch.from_numpy(cda).to(dev)
+    hyd_d = torch.empty(n_bodies * 12, dtype=torch.int32, device=dev)           # ocean_buoyancy_result: 48 B
+    drag_d = torch.empty(n_bodies * 8, dtype=torch.int32, device=dev)           # ocean_drag_result: 32 B
+    torch.cuda.synchronize()
+    lib = load_library()
+    forces = lambda: check(lib.ocean_body_forces_device(g.context, n_bodies, bodies.ctypes.data, vel.ctypes.data, len(hull), hull_d.data_ptr(),
+                                                        cda_d.data_ptr(), C, scales.ctypes.data, 1025.0, tolerance, max_iterations,
+                                                        hyd_d.data_ptr(), drag_d.data_ptr(), None))
+    buoy = lambda: check(lib.ocean_buoyancy_device(g.context, n_bodies, bodies.ctypes.data, len(hull), hull_d.data_ptr(), C, scales.ctypes.data,
+                                                   1025.0, tolerance, max_iterations, hyd_d.data_ptr(), None))
+
+    def timed(call):
+        for _ in range(3):
+            call()
+        g.synchronize()
+        g.timer_start()
+        for _ in range(reps):
+            call()
+        return g.timer_stop() / reps
+
+    t_f, t_b = [], []
+    for _ in range(3):                          # alternating windows: clock ramp-up and neighbours hit both alike
+        t_f.append(timed(forces))
+        t_b.append(timed(buoy))
+    _, drag, smp = g.body_forces(bodies, vel, hull, cda, scales, 1025.0, tolerance, max_iterations, return_samples=True)
+    body, j, _, wp = bu.world_points(bodies, hull)
+    f = bu.submerged_fraction(smp["displacement"][:, 1], wp[:, 1], hull["half_height"][bodies["first_point"][body] + j])
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                         stdout=subprocess.PIPE, text=True).stdout.strip()
+    out = {"config": label, "gpu": torch.cuda.get_device_name(0), "power_limit_and_max_sm_clock": smi, "map_size": N, "cascades": C,
+           "bodies": n_bodies, "points_per_body": per_body, "world_points": n_points, "tolerance": tolerance, "max_iterations": max_iterations,
+           "body_forces_us_per_call": [1e3 * v for v in t_f], "buoyancy_us_per_call": [1e3 * v for v in t_b],
+           "overhead_over_buoyancy": min(t_f) / min(t_b) - 1.0, "frac_points_submerged": float(np.mean(f > 0)),
+           "frac_bodies_with_drag": float(np.mean(drag["wetted_drag_area"] > 0))}
     g.free()
     print(json.dumps(out), flush=True)
 
@@ -361,6 +433,11 @@ if "--velocity" in sys.argv:
 if "--buoyancy" in sys.argv:
     run_buoyancy(256, 4, 1 << 14, 64, 50, "buoyancy: 2^14 bodies x 64 points over 4 cascades of 256x256")
     run_buoyancy(1024, 8, 1 << 14, 64, 20, "buoyancy: 2^14 bodies x 64 points over 8 cascades of 1024x1024")
+    sys.exit(0)
+
+if "--drag" in sys.argv:
+    run_body_forces(256, 4, 1 << 14, 64, 50, "body forces: 2^14 bodies x 64 points over 4 cascades of 256x256")
+    run_body_forces(1024, 8, 1 << 14, 64, 20, "body forces: 2^14 bodies x 64 points over 8 cascades of 1024x1024")
     sys.exit(0)
 
 if "--query" in sys.argv or os.environ.get("OCEAN_RUN_QUERY", "1") != "0":
