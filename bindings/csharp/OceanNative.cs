@@ -93,6 +93,28 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanRay                                   // struct ocean_ray (28 B)
+    {
+        public fixed float origin[3];
+        public fixed float direction[3];                            // need not be unit; t is in units of |direction|
+        public float t_max;                                         // +inf allowed
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanRayHit                                // struct ocean_ray_hit (72 B)
+    {
+        public float t;
+        public fixed float position[3];
+        public float source_x, source_z;
+        public fixed float displacement[3];
+        public fixed float gradient_foam[3];
+        public float gap;                                           // position.y - water height there
+        public float residual;
+        public uint status;                                         // OCEAN_RAY_*: 0 miss, 1 hit from above, 2 from below, 3 truncated, 4 invalid
+        public uint evaluations, iterations, unconverged;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public struct OceanInfo
     {
         public int device, map_size, num_cascades, pending_cascades;
@@ -167,6 +189,13 @@ namespace OceanB200
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,
                                                         float tolerance, int max_iterations, OceanSurfaceSample* samples);
+        // ray cast: the first crossing of each ray with the displaced surface (step = horizontal sample spacing in metres)
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_raycast(IntPtr handle, int num_rays, OceanRay* rays, int num_cascades, float* map_scales, float step,
+                                                  int max_samples, float tolerance, int max_iterations, OceanRayHit* hits);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_raycast_device(IntPtr handle, int num_rays, void* rays_dev, int num_cascades, float* map_scales, float step,
+                                                         int max_samples, float tolerance, int max_iterations, void* hits_dev);
         // buoyancy: per-body force and torque from hull points on the surface; samples may be null
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_buoyancy(IntPtr handle, int num_bodies, OceanBuoyancyBody* bodies, int num_points, OceanBuoyancyPoint* points,

@@ -129,6 +129,11 @@ struct ocean_generator {
     uint64_t kernel_launches = 0;
     uint64_t cascade_updates = 0;
     uint64_t device_bytes = 0;
+    unsigned* ray_bounds = nullptr;                     // ray cast scratch: [3 * num_cascades] per-layer bounds (first use)
+    ocean_ray* ray_in = nullptr;                        // ray cast staging for the host entry point, grown on demand
+    size_t ray_in_capacity = 0;
+    ocean_ray_hit* ray_out = nullptr;
+    size_t ray_out_capacity = 0;
 };
 
 namespace {
@@ -210,6 +215,9 @@ void release(ocean_generator* g) {
     cudaFree(g->spray_records);
     cudaFree(g->surf_scratch);
     cudaFree(g->surf_records);
+    cudaFree(g->ray_bounds);
+    cudaFree(g->ray_in);
+    cudaFree(g->ray_out);
     cudaFree(g->buoy_bodies);
     cudaFree(g->buoy_offsets);
     cudaFree(g->buoy_results);
@@ -1238,6 +1246,54 @@ int ocean_query_surface(ocean_generator* gen, int num_points, const float* point
                                          tolerance, max_iterations, gen->surf_records)))
         return rc;
     OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->surf_records, sizeof(ocean_surface_sample) * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+// ---- ray cast: the first crossing of each ray with the displaced surface (slab bounds, then one thread per ray) ----
+static_assert(sizeof(ocean_ray) == 28, "ocean_ray layout");
+static_assert(sizeof(ocean_ray_hit) == 72, "ocean_ray_hit layout");
+
+namespace {
+int check_raycast_args(int num_rays, float step, int max_samples, float tolerance, int max_iterations) {
+    int rc = check_surface_args(num_rays, tolerance, max_iterations);
+    if (rc) return rc;
+    if (!(step > 0.0f) || !std::isfinite(step)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "step %g is not finite and > 0", step);
+    if (max_samples < 2 || max_samples > (1 << 20)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "max_samples %d outside [2, 2^20]", max_samples);
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_raycast_device(ocean_generator* gen, int num_rays, const ocean_ray* rays_dev, int num_cascades, const float* map_scales_host,
+                         float step, int max_samples, float tolerance, int max_iterations, ocean_ray_hit* out_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_raycast_args(num_rays, step, max_samples, tolerance, max_iterations))) return rc;
+    if (num_rays == 0) return OCEAN_OK;
+    if (!rays_dev || !out_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
+    if (!gen->ray_bounds) OCEAN_CUDA(dev_alloc(gen, &gen->ray_bounds, 3 * (size_t)gen->num_cascades));
+    OCEAN_CUDA(ocean::launch_raycast(gen->buf, num_cascades, rays_dev, num_rays, gen->q_scales, step, max_samples, tolerance, max_iterations,
+                                     gen->ray_bounds, out_dev, gen->stream));
+    gen->kernel_launches += 2;
+    return OCEAN_OK;
+}
+
+int ocean_raycast(ocean_generator* gen, int num_rays, const ocean_ray* rays_host, int num_cascades, const float* map_scales_host,
+                  float step, int max_samples, float tolerance, int max_iterations, ocean_ray_hit* out_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_raycast_args(num_rays, step, max_samples, tolerance, max_iterations))) return rc;
+    if (num_rays == 0) return OCEAN_OK;
+    if (!rays_host || !out_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
+    const size_t n = (size_t)num_rays;
+    if ((rc = grow_buffer(gen, &gen->ray_in, &gen->ray_in_capacity, n))) return rc;
+    if ((rc = grow_buffer(gen, &gen->ray_out, &gen->ray_out_capacity, n))) return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(gen->ray_in, rays_host, sizeof(ocean_ray) * n, cudaMemcpyHostToDevice, gen->stream));
+    if ((rc = ocean_raycast_device(gen, num_rays, gen->ray_in, num_cascades, map_scales_host, step, max_samples, tolerance, max_iterations,
+                                   gen->ray_out)))
+        return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->ray_out, sizeof(ocean_ray_hit) * n, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }

@@ -125,6 +125,10 @@ cudaError_t launch_sample_maps(const DeviceBuffers& b, int num_cascades, const f
 size_t surface_scratch_ints(int num_cascades, int n);
 cudaError_t launch_query_surface(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
                                  float tolerance, int max_iterations, void* out_dev, int* scratch_dev, cudaStream_t stream);
+// ocean_sample.cu: ray cast against the displaced surface (oracle/raycast.py); rays_dev = ocean_ray[n], out_dev = ocean_ray_hit[n],
+// bounds_dev = [3 * num_cascades] unsigned of scratch (the per-layer height and displacement bounds)
+cudaError_t launch_raycast(const DeviceBuffers& b, int num_cascades, const void* rays_dev, int n, const float4* scales_dev, float step,
+                           int max_samples, float tolerance, int max_iterations, unsigned* bounds_dev, void* out_dev, cudaStream_t stream);
 
 // ocean_buoyancy.cu: buoyancy (oracle/buoyancy.py).  bodies_dev = ocean_buoyancy_body[num_bodies], offsets_dev = the exclusive
 // prefix of their num_points (body-major world points), points_dev = ocean_buoyancy_point[], q_dev / samples_dev = [n] world

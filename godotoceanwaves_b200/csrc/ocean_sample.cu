@@ -16,6 +16,8 @@
 // The surface query (ocean_query_surface; oracle/surface.py is the specification) inverts the horizontal displacement
 // first: for a world position Q it solves P + D_xz(P) = Q by damped Newton steps (four displacement texels per cascade and
 // trial give D and its exact bilinear Jacobian), then samples the maps at P with the same per-point body as k_sample_maps.
+// The ray cast (ocean_raycast; oracle/raycast.py is the specification) marches each ray through the height slab of the maps
+// with the same inversion, warm-started from sample to sample, and refines the first crossing.
 #include "ocean_kernels.cuh"
 #include "ocean_texture.cuh"
 
@@ -260,6 +262,240 @@ __global__ void __launch_bounds__(kRestartBlock, 8) k_surface_restart(const uint
     }
 }
 
+// ---- ray cast: the first crossing of each ray with the displaced surface (oracle/raycast.py is the specification) ----
+
+struct Ray {                 // == ocean_ray (include/ocean.h), 28 bytes
+    float ox, oy, oz, dx, dy, dz, t_max;
+};
+
+struct RayHit {              // == ocean_ray_hit (include/ocean.h), 72 bytes
+    float t;
+    float position[3];
+    float source_x, source_z;
+    float displacement[3];
+    float gradient_foam[3];
+    float gap;
+    float residual;
+    uint32_t status, evaluations, iterations, unconverged;
+};
+constexpr uint32_t kRayMiss = 0, kRayFromAbove = 1, kRayFromBelow = 2, kRayTruncated = 3, kRayInvalid = 4;
+constexpr int kRayRefineSteps = 32;
+
+// Signed floats as unsigned keys in the same order (atomicMax over signed values).
+__device__ __forceinline__ unsigned order_key(float f) {
+    const unsigned b = __float_as_uint(f);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float order_value(unsigned k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+
+// Per layer, three maxima over the texels (NaN-dropping): [0] y, [1] -y (as order_key), [2] max(|x|, |z|) from 0 (bits, as
+// k_surface_bound).  bounds must be zero on entry.
+__global__ void __launch_bounds__(256) k_raycast_bound(const uint2* __restrict__ displacement, int N, unsigned* __restrict__ bounds) {
+    const size_t texels = (size_t)N * N;
+    const uint2* layer = displacement + blockIdx.y * texels;
+    float hi = -INFINITY, nlo = -INFINITY, m = 0.0f;
+    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < texels; t += (size_t)gridDim.x * blockDim.x) {
+        const float4 v = texel(layer, N, (int)t, 0);
+        hi = fmaxf(hi, v.y);
+        nlo = fmaxf(nlo, -v.y);
+        m = fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.z)));
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+        nlo = fmaxf(nlo, __shfl_xor_sync(0xffffffffu, nlo, o));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    }
+    if ((threadIdx.x & 31) == 0) {
+        atomicMax(&bounds[3 * blockIdx.y + 0], order_key(hi));
+        atomicMax(&bounds[3 * blockIdx.y + 1], order_key(nlo));
+        atomicMax(&bounds[3 * blockIdx.y + 2], __float_as_uint(m));
+    }
+}
+
+// An evaluated point of a ray: parameter, position, source point P, inversion residual, gap.
+struct RayPoint {
+    float t, x, y, z, px, pz, r, g;
+};
+
+// One gap evaluation at parameter t, started at Q or (warm) from the evaluated point `base` shifted by the ray's horizontal
+// advance since it, with the surface query's restarts when that start does not converge.
+__device__ __forceinline__ RayPoint ray_gap(const uint2* __restrict__ displacement, int N, int C, const float4* __restrict__ scales,
+                                            const Ray& ray, float t, bool warm, float base_x, float base_z, float base_px, float base_pz,
+                                            float tol, int max_iterations, float rho, uint32_t& iterations, uint32_t& unconverged) {
+    RayPoint e;
+    e.t = t;
+    e.x = ray.ox + t * ray.dx;
+    e.y = ray.oy + t * ray.dy;
+    e.z = ray.oz + t * ray.dz;
+    const float2 q = make_float2(e.x, e.z);
+    float px = q.x, pz = q.y;
+    if (warm && max_iterations > 0) {
+        px = base_px + (e.x - base_x);
+        pz = base_pz + (e.z - base_z);
+    }
+    // start -1 is the first (from Q or warm); starts 0..4 are k_surface_restart's seeds, in its order.  One solve site keeps
+    // the solve inlined.
+    float r = 0.0f;
+    int total = 0;
+    SurfaceEval eq;
+    for (int s = -1; s < 5; ++s) {
+        float sx = px, sz = pz;
+        if (s >= 0) {
+            if (s == 0) eq = surface_eval(displacement, N, C, scales, q.x, q.y);
+            sx = q.x; sz = q.y;
+            switch (s) {
+                case 0: sx = q.x - eq.dx; sz = q.y - eq.dz; break;
+                case 1: sx = q.x + rho; break;
+                case 2: sz = q.y + rho; break;
+                case 3: sx = q.x - rho; break;
+                default: sz = q.y - rho; break;
+            }
+        }
+        int steps;
+        const float rs = surface_solve(displacement, N, C, scales, q, sx, sz, tol, max_iterations, steps);
+        total += steps;
+        if (s < 0) {
+            r = rs;
+            px = sx; pz = sz;
+            if (r <= tol || max_iterations == 0) break;
+        } else {
+            if (rs < r) { px = sx; pz = sz; r = rs; }
+            if (rs <= tol) break;
+        }
+    }
+    float hx = 0.0f, eta = 0.0f, hz = 0.0f;
+    for (int c = 0; c < C; ++c) {
+        const float4 s = __ldg(&scales[c]);
+        add_displacement(displacement + (size_t)c * N * N, N, px * s.x, pz * s.y, s.z, hx, eta, hz);
+    }
+    e.px = px;
+    e.pz = pz;
+    e.r = r;
+    e.g = e.y - eta;
+    iterations += (uint32_t)total;
+    unconverged += (r <= tol) ? 0u : 1u;
+    return e;
+}
+
+// One thread per ray: slab clip, march, Illinois refinement, and the map sample at the reported point.  bounds = the
+// per-layer maxima of k_raycast_bound.  (128, 4) lets ptxas keep the ray's state in registers (no spill).
+__global__ void __launch_bounds__(128, 4) k_raycast(const uint2* __restrict__ displacement, const uint2* __restrict__ normal, int N, int C,
+                                                 const Ray* __restrict__ rays, int n, const float4* __restrict__ scales, float step,
+                                                 int max_samples, float tol, int max_iterations, const unsigned* __restrict__ bounds,
+                                                 RayHit* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Ray ray = rays[i];
+    RayHit hit = {};
+    const bool finite = isfinite(ray.ox) && isfinite(ray.oy) && isfinite(ray.oz) && isfinite(ray.dx) && isfinite(ray.dy) && isfinite(ray.dz);
+    if (!finite || (ray.dx == 0.0f && ray.dy == 0.0f && ray.dz == 0.0f) || !(ray.t_max >= 0.0f)) {
+        hit.status = kRayInvalid;
+        out[i] = hit;
+        return;
+    }
+    // height slab and rho
+    float y_lo = 0.0f, y_hi = 0.0f, acc = 0.0f, rho = 0.0f;
+    for (int c = 0; c < C; ++c) {
+        const float s = __ldg(&scales[c]).z;
+        const float ymax = order_value(bounds[3 * c + 0]), ymin = -order_value(bounds[3 * c + 1]);
+        const float a = s * ymin, b = s * ymax;
+        y_lo = y_lo + fminf(a, b);
+        y_hi = y_hi + fmaxf(a, b);
+        acc = acc + fabsf(s) * fmaxf(fabsf(ymin), fabsf(ymax));
+        rho = rho + fabsf(s) * __uint_as_float(bounds[3 * c + 2]);
+    }
+    rho = rho * 0.5f;
+    const float pad = tol + acc * 0x1p-13f;
+    const float lo = y_lo - pad, hi = y_hi + pad;
+    float t_in, t_out;
+    bool enters;
+    if (ray.dy == 0.0f) {
+        t_in = 0.0f;
+        t_out = ray.t_max;
+        enters = lo <= ray.oy && ray.oy <= hi;
+    } else {
+        const float ta = __fdiv_rn(lo - ray.oy, ray.dy), tb = __fdiv_rn(hi - ray.oy, ray.dy);
+        const float tn = ta < tb ? ta : tb, tf = ta < tb ? tb : ta;
+        t_in = tn > 0.0f ? tn : 0.0f;
+        t_out = tf < ray.t_max ? tf : ray.t_max;
+        enters = t_in <= t_out && isfinite(t_in);
+    }
+    if (!enters) {
+        hit.status = kRayMiss;
+        hit.position[0] = ray.ox; hit.position[1] = ray.oy; hit.position[2] = ray.oz;
+        out[i] = hit;
+        return;
+    }
+    const float h = __fdiv_rn(step, __fsqrt_rn(ray.dx * ray.dx + ray.dz * ray.dz));
+    uint32_t evaluations = 0, iterations = 0, unconverged = 0, status = kRayMiss;
+    // One evaluation per trip, so that ray_gap is inlined once.  March: a = the previous sample.  Refinement: [a, b] is the
+    // bracket, wa / wb its Illinois weights, last = 1 (2) when the previous step replaced a (b).
+    RayPoint a = {}, b = {}, rep = {};
+    bool above = false, refining = false;
+    float t = t_in, base_x = 0.0f, base_z = 0.0f, base_px = 0.0f, base_pz = 0.0f, wa = 0.0f, wb = 0.0f;
+    int k = 0, steps = 0, last = 0;
+    for (;;) {
+        const RayPoint e = ray_gap(displacement, N, C, scales, ray, t, evaluations > 0, base_x, base_z, base_px, base_pz, tol, max_iterations,
+                                   rho, iterations, unconverged);
+        ++evaluations;
+        if (isnan(e.g)) { status = kRayInvalid; rep = e; break; }
+        if (!refining) {
+            const bool side = e.g > 0.0f;
+            if (k == 0) above = side;
+            if (k == 0 || side == above) {
+                rep = e;
+                if (t == t_out) break;                                      // MISS
+                if (evaluations == (uint32_t)max_samples) { status = kRayTruncated; break; }
+                ++k;
+                float tn = t_in + (float)k * h;
+                if (!(tn < t_out)) tn = t_out;
+                if (!isfinite(tn)) break;                                   // MISS
+                a = e;
+                t = tn;
+                base_x = e.x; base_z = e.z; base_px = e.px; base_pz = e.pz;
+                continue;
+            }
+            refining = true;
+            b = e;
+            wa = a.g;
+            wb = b.g;
+            status = above ? kRayFromAbove : kRayFromBelow;
+        } else {
+            ++steps;
+            if ((e.g > 0.0f) == above) {
+                if (last == 1) wb = wb * 0.5f;
+                a = e; wa = e.g; last = 1;
+            } else {
+                if (last == 2) wa = wa * 0.5f;
+                b = e; wb = e.g; last = 2;
+            }
+        }
+        rep = fabsf(a.g) <= fabsf(b.g) ? a : b;
+        if (steps == kRayRefineSteps || fabsf(a.g) <= tol || fabsf(b.g) <= tol) break;
+        const float w = __fdiv_rn(wa, wa - wb);
+        const float tn = a.t + w * (b.t - a.t);
+        if (!(tn > a.t && tn < b.t)) break;
+        const bool near_a = (tn - a.t) <= (b.t - tn);
+        base_x = near_a ? a.x : b.x; base_z = near_a ? a.z : b.z; base_px = near_a ? a.px : b.px; base_pz = near_a ? a.pz : b.pz;
+        t = tn;
+    }
+    float3 d, g;
+    sample_point(displacement, normal, N, C, make_float2(rep.px, rep.pz), scales, d, g);
+    hit.t = rep.t;
+    hit.position[0] = rep.x; hit.position[1] = rep.y; hit.position[2] = rep.z;
+    hit.source_x = rep.px;
+    hit.source_z = rep.pz;
+    hit.displacement[0] = d.x; hit.displacement[1] = d.y; hit.displacement[2] = d.z;
+    hit.gradient_foam[0] = g.x; hit.gradient_foam[1] = g.y; hit.gradient_foam[2] = g.z;
+    hit.gap = rep.g;
+    hit.residual = rep.r;
+    hit.status = status;
+    hit.evaluations = evaluations;
+    hit.iterations = iterations;
+    hit.unconverged = unconverged;
+    out[i] = hit;
+}
+
 }  // namespace
 
 cudaError_t launch_sample_maps(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
@@ -301,6 +537,22 @@ cudaError_t launch_query_surface(const DeviceBuffers& b, int num_cascades, const
     const int restart_blocks = (n + kRestartBlock - 1) / kRestartBlock < 2048 ? (n + kRestartBlock - 1) / kRestartBlock : 2048;
     k_surface_restart<<<restart_blocks, kRestartBlock, 0, stream>>>(b.displacement, b.normal, N, num_cascades, points_dev, scales_dev, tolerance,
                                                                    max_iterations, out, count, pending, layer_max);
+    return cudaGetLastError();
+}
+
+// bounds_dev: [3 * num_cascades] unsigned, cleared here, then filled by k_raycast_bound; k_raycast reads them.
+cudaError_t launch_raycast(const DeviceBuffers& b, int num_cascades, const void* rays_dev, int n, const float4* scales_dev, float step,
+                           int max_samples, float tolerance, int max_iterations, unsigned* bounds_dev, void* out_dev, cudaStream_t stream) {
+    if (n <= 0) return cudaSuccess;
+    const int N = b.map_size;
+    cudaError_t e = cudaMemsetAsync(bounds_dev, 0, sizeof(unsigned) * 3 * (size_t)num_cascades, stream);
+    if (e != cudaSuccess) return e;
+    const unsigned bound_blocks = (unsigned)(((size_t)N * N + 4095) / 4096);     // 16 texels per thread
+    k_raycast_bound<<<dim3(bound_blocks, (unsigned)num_cascades), 256, 0, stream>>>(b.displacement, N, bounds_dev);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    k_raycast<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(b.displacement, b.normal, N, num_cascades, static_cast<const Ray*>(rays_dev), n,
+                                                              scales_dev, step, max_samples, tolerance, max_iterations, bounds_dev,
+                                                              static_cast<RayHit*>(out_dev));
     return cudaGetLastError();
 }
 

@@ -35,6 +35,18 @@ class InfoC(C.Structure):
                 ("cascade_updates", C.c_uint64), ("device_bytes", C.c_uint64)]
 
 
+class RayC(C.Structure):
+    """struct ocean_ray (include/ocean.h), 28 B: origin, direction (need not be unit), t_max (+inf allowed)"""
+    _fields_ = [("origin", C.c_float * 3), ("direction", C.c_float * 3), ("t_max", C.c_float)]
+
+
+class RayHitC(C.Structure):
+    """struct ocean_ray_hit (include/ocean.h), 72 B"""
+    _fields_ = [("t", C.c_float), ("position", C.c_float * 3), ("source_x", C.c_float), ("source_z", C.c_float),
+                ("displacement", C.c_float * 3), ("gradient_foam", C.c_float * 3), ("gap", C.c_float), ("residual", C.c_float),
+                ("status", C.c_uint32), ("evaluations", C.c_uint32), ("iterations", C.c_uint32), ("unconverged", C.c_uint32)]
+
+
 class BuoyancyPointC(C.Structure):
     """struct ocean_buoyancy_point (include/ocean.h), 20 B: body-local position, volume (m^3), half height (m)"""
     _fields_ = [("position", C.c_float * 3), ("volume", C.c_float), ("half_height", C.c_float)]
@@ -99,6 +111,8 @@ SIGNATURES = {
     "ocean_sample_maps_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ocean_query_surface": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_int, C.c_void_p]),
     "ocean_query_surface_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_int, C.c_void_p]),
+    "ocean_raycast": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_int, C.c_void_p]),
+    "ocean_raycast_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_int, C.c_void_p]),
     "ocean_buoyancy": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int,
                                  C.c_void_p, C.c_void_p]),
     "ocean_buoyancy_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int,

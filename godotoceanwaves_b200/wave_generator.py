@@ -282,6 +282,27 @@ class WaveGenerator:
                                                  float(tolerance), int(max_iterations), out.ctypes.data))
         return out
 
+    # -- ray cast: the first crossing of each ray with the displaced surface ------------------------------------------
+    RAY = np.dtype([("origin", np.float32, 3), ("direction", np.float32, 3), ("t_max", np.float32)])   # struct ocean_ray
+    RAY_HIT = np.dtype([("t", np.float32), ("position", np.float32, 3), ("source_x", np.float32), ("source_z", np.float32),
+                        ("displacement", np.float32, 3), ("gradient_foam", np.float32, 3), ("gap", np.float32), ("residual", np.float32),
+                        ("status", np.uint32), ("evaluations", np.uint32), ("iterations", np.uint32),
+                        ("unconverged", np.uint32)])                                         # struct ocean_ray_hit
+    RAY_MISS, RAY_HIT_FROM_ABOVE, RAY_HIT_FROM_BELOW, RAY_TRUNCATED, RAY_INVALID = range(5)  # OCEAN_RAY_*
+
+    def raycast(self, rays, map_scales, step: float = 0.5, max_samples: int = 1024, tolerance: float = 1e-3,
+                max_iterations: int = 8) -> np.ndarray:
+        """RAY_HIT rows, one per RAY row of `rays`: the first crossing of origin + t * direction, t in [0, t_max], with the
+        displaced surface (include/ocean.h, ocean_raycast).  `step` is the horizontal sample spacing in metres; status is
+        one of the RAY_* constants, and a hit has |gap| <= tolerance when its refinement converged."""
+        self._require()
+        r = np.ascontiguousarray(rays, self.RAY).reshape(-1)
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        out = np.zeros(len(r), self.RAY_HIT)
+        check(load_library().ocean_raycast(self.context, len(r), r.ctypes.data, sc.shape[0], sc.ctypes.data, float(step), int(max_samples),
+                                           float(tolerance), int(max_iterations), out.ctypes.data))
+        return out
+
     # -- buoyancy: per-body hydrostatic force and torque from hull points on the displaced surface -------------------
     BUOYANCY_POINT = np.dtype([("position", np.float32, 3), ("volume", np.float32), ("half_height", np.float32)])   # struct ocean_buoyancy_point
     BUOYANCY_BODY = np.dtype([("transform", np.float32, 12), ("first_point", np.int32), ("num_points", np.int32)])  # struct ocean_buoyancy_body

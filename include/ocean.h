@@ -214,6 +214,69 @@ int ocean_query_surface(ocean_generator* gen, int num_points, const float* point
 int ocean_query_surface_device(ocean_generator* gen, int num_points, const float* points_xz_dev, int num_cascades, const float* map_scales_host,
                                float tolerance, int max_iterations, ocean_surface_sample* out_dev);
 
+/* Ray cast -- the first crossing of each ray with the displaced water surface: where a projectile enters the water, what
+ * the crosshair points at, whether a line of sight crosses a crest, where an underwater camera ray leaves the water.
+ * The surface is the one ocean_query_surface describes.  Along the ray r(t) = origin + t * direction the gap is
+ * g(t) = r.y - eta(r.x, r.z), eta the water height from the surface query's inversion; a point is above iff g > 0.
+ *   slab        the call bounds the heights of the maps per layer (y min and max, scaled and summed over the cascades,
+ *               padded by tolerance plus 2^-13 of the summed magnitudes) and clips [0, t_max] to that slab.  A ray that
+ *               never enters it is a MISS with 0 evaluations, t = 0 and position = origin (every other field 0).
+ *   march       a sample every `step` metres of horizontal travel from the slab entry (ray parameter step / |direction.xz|;
+ *               a vertical ray is sampled at entry and exit only), plus one at the slab exit.  Each sample inverts the
+ *               horizontal displacement at r.xz, warm-started from the previous sample's source point (the first one from
+ *               r.xz, so sample 0 is the surface query at the ray's entry point), with the surface query's restarts.
+ *               max_iterations = 0 uses the map height at r.xz: a plain height-field march.
+ *   refinement  the first sample on the other side of the surface than sample 0 brackets a crossing with the previous one;
+ *               Illinois regula falsi refines it until |g| <= tolerance, the new parameter is not strictly inside the
+ *               bracket, or 32 steps have run.  The bracket end with the smaller |g| is reported (the earlier on ties).
+ * The record (ocean_ray_hit) describes the reported point: its parameter t, position, source point, the map sample at the
+ * source (as ocean_query_surface's displacement and gradient_foam), gap and inversion residual.  status:
+ *   OCEAN_RAY_MISS             the segment [0, t_max] ends without a crossing (the last sample's record)
+ *   OCEAN_RAY_HIT_FROM_ABOVE   a crossing, sample 0 above the water;  OCEAN_RAY_HIT_FROM_BELOW  sample 0 below it (an
+ *                              underwater origin);  |gap| <= tolerance when the refinement converged
+ *   OCEAN_RAY_TRUNCATED        max_samples samples without a crossing (the last sample's record): near-horizontal rays in the
+ *                              slab, t_max = +inf
+ *   OCEAN_RAY_INVALID          a non-finite origin or direction component, a zero direction, or t_max NaN or negative (0
+ *                              evaluations, every other field 0); or an evaluation whose gap is NaN (that evaluation's record)
+ * evaluations counts march samples plus refinement evaluations, iterations the Newton steps over all of them, unconverged
+ * the evaluations whose inversion residual is not <= tolerance.  A bad ray never fails the call nor affects other rays.
+ * oracle/raycast.py is the specification (binary32, bit-exact, every operation written out).
+ * Limits: the surface as rendered within 150 m of the camera (distance_factor, as for ocean_query_surface); crests thinner
+ * than `step` along the ray can be missed; where the surface folds, any crossing may be found; binary32 resolution of the
+ * positions falls with distance from the origin (tolerance must exceed a few ulps of the coordinates).
+ * direction need not be unit: t is in units of |direction|, and scaling direction by 2^k scales t by 2^-k and changes no
+ * other field.  step must be finite and > 0, max_samples in [2, 2^20]; tolerance, max_iterations, num_cascades and
+ * map_scales as for ocean_query_surface; an invalid call launches nothing.  map_scales is a host array in both entry points;
+ * ocean_raycast takes host rays and records and is synchronous; ocean_raycast_device takes device pointers for them and is
+ * asynchronous on the generator's stream.  A call with rays launches 2 kernels. */
+#define OCEAN_RAY_MISS 0
+#define OCEAN_RAY_HIT_FROM_ABOVE 1
+#define OCEAN_RAY_HIT_FROM_BELOW 2
+#define OCEAN_RAY_TRUNCATED 3
+#define OCEAN_RAY_INVALID 4
+typedef struct ocean_ray {
+    float origin[3];
+    float direction[3];         /* need not be unit; t is in units of |direction| */
+    float t_max;                /* in [0, +inf]; +inf allowed */
+} ocean_ray;                    /* 28 B */
+typedef struct ocean_ray_hit {
+    float t;                    /* ray parameter of the reported point */
+    float position[3];          /* origin + t * direction, each component rounded as written */
+    float source_x, source_z;   /* undisplaced point P whose surface point is under / over `position` */
+    float displacement[3];      /* the map sample at P, as ocean_query_surface's record */
+    float gradient_foam[3];
+    float gap;                  /* position.y - water height there (|gap| <= tolerance for a resolved hit) */
+    float residual;             /* horizontal inversion residual at P */
+    uint32_t status;            /* OCEAN_RAY_* */
+    uint32_t evaluations;       /* gap evaluations: march samples + refinement */
+    uint32_t iterations;        /* Newton steps over all evaluations */
+    uint32_t unconverged;       /* evaluations whose inversion residual is not <= tolerance */
+} ocean_ray_hit;                /* 72 B */
+int ocean_raycast(ocean_generator* gen, int num_rays, const ocean_ray* rays_host, int num_cascades, const float* map_scales_host,
+                  float step, int max_samples, float tolerance, int max_iterations, ocean_ray_hit* out_host);
+int ocean_raycast_device(ocean_generator* gen, int num_rays, const ocean_ray* rays_dev, int num_cascades, const float* map_scales_host,
+                         float step, int max_samples, float tolerance, int max_iterations, ocean_ray_hit* out_dev);
+
 /* Buoyancy -- per-body hydrostatic force and torque for this physics tick, from hull sample points on the displaced surface.
  * A hull point (body-local position, volume in m^3, half_height in m) stands for a vertical column element of that volume,
  * centred on the point and reaching half_height above and below it.  A body is a 3 x 4 row-major body-to-world matrix [R | t]

@@ -116,7 +116,7 @@ def run_spray(N, C, particles, reps, label):
     print(json.dumps(out), flush=True)
 
 
-if not {"--buoyancy", "--velocity", "--drag"} & set(sys.argv):    # --buoyancy / --velocity / --drag run their op (defined below) alone
+if not {"--buoyancy", "--velocity", "--drag", "--raycast"} & set(sys.argv):    # --buoyancy / --velocity / --drag / --raycast run their op (defined below) alone
     run(256, 4, 2000, "cfg2 latency: one 256x256x4 set per launch (launch/latency-bound, L2-resident)")
     run(256, 4, 2000, "cfg2 latency, fused frames (ocean_update_frames: 64 frames per launch)", fused=True)
     run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, frame by frame")
@@ -438,6 +438,104 @@ if "--buoyancy" in sys.argv:
 if "--drag" in sys.argv:
     run_body_forces(256, 4, 1 << 14, 64, 50, "body forces: 2^14 bodies x 64 points over 4 cascades of 256x256")
     run_body_forces(1024, 8, 1 << 14, 64, 20, "body forces: 2^14 bodies x 64 points over 8 cascades of 1024x1024")
+    sys.exit(0)
+
+def _picking_rays(side, y=12.0, fov_deg=90.0, pitch_deg=-20.0):
+    """side x side camera rays from (0, y, 0) through a square image plane of fov_deg pitched pitch_deg: (RAY array)."""
+    import numpy as np
+    from oracle import raycast as rc
+    f = np.tan(np.radians(fov_deg) / 2.0)
+    u = (np.arange(side) + 0.5) / side * 2.0 - 1.0
+    U, V = np.meshgrid(u * f, u * f)
+    p = np.radians(pitch_deg)
+    fwd = np.array([0.0, np.sin(p), np.cos(p)]); up = np.array([0.0, np.cos(p), -np.sin(p)]); right = np.array([1.0, 0.0, 0.0])
+    d = fwd[None, :] + U.reshape(-1, 1) * right[None, :] + V.reshape(-1, 1) * up[None, :]
+    r = np.zeros(side * side, rc.RAY)
+    r["origin"] = [0.0, y, 0.0]
+    r["direction"] = d / np.linalg.norm(d, axis=1, keepdims=True)
+    r["t_max"] = np.inf
+    return r
+
+
+def _projectile_rays(n, seed=1):
+    """n rays 30 to 90 degrees down from 5 to 50 m over [-300, 300]^2 m"""
+    import numpy as np
+    from oracle import raycast as rc
+    rng = np.random.default_rng(seed)
+    p = np.radians(rng.uniform(-90.0, -30.0, n))
+    yaw = rng.uniform(0.0, 2.0 * np.pi, n)
+    r = np.zeros(n, rc.RAY)
+    r["origin"] = np.stack([rng.uniform(-300, 300, n), rng.uniform(5.0, 50.0, n), rng.uniform(-300, 300, n)], 1)
+    r["direction"] = np.stack([np.cos(p) * np.cos(yaw), np.sin(p), np.cos(p) * np.sin(yaw)], 1)
+    r["t_max"] = np.inf
+    return r
+
+
+def run_raycast(N, C, reps, label, step=0.5, max_samples=1024, tolerance=1e-3, max_iterations=8):
+    """Ray cast (ocean_raycast_device) on device-resident rays, two scenes: (a) 2^20 picking rays from a camera 12 m up
+    through a 1024 x 1024 grid over a 90 degree field of view pitched 20 degrees down, (b) 2^16 projectile rays 30 to 90
+    degrees down from 5 to 50 m.  CUDA events around each call, best of three windows alternating with
+    ocean_query_surface_device on 2^20 points.  The card's name, power limit and max SM clock are read in the same run."""
+    import subprocess
+    import numpy as np
+    import torch
+    from godotoceanwaves_b200.native import load_library, check
+    from oracle import raycast as rc
+    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
+    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
+    for _ in range(2):
+        g.update_all(0.02, p)
+    scales = gow.WaveGenerator.map_scales(p)
+    dev = torch.device("cuda", 0)
+    lib = load_library()
+    n_pts = 1 << 20
+    pts = (torch.rand(n_pts, 2, device=dev, generator=torch.Generator(dev).manual_seed(1)) * 600.0 - 300.0).contiguous()
+    recs = torch.empty(n_pts * 10, dtype=torch.int32, device=dev)
+    query = lambda: check(lib.ocean_query_surface_device(g.context, n_pts, pts.data_ptr(), C, scales.ctypes.data, tolerance, max_iterations,
+                                                         recs.data_ptr()))
+
+    def timed(call):
+        for _ in range(2):
+            call()
+        g.synchronize()
+        g.timer_start()
+        for _ in range(reps):
+            call()
+        return g.timer_stop() / reps
+
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                         stdout=subprocess.PIPE, text=True).stdout.strip()
+    for scene, rays in (("picking: 2^20 rays, camera 12 m up, 90 deg fov pitched 20 deg down", _picking_rays(1024)),
+                        ("projectiles: 2^16 rays 30-90 deg down from 5-50 m", _projectile_rays(1 << 16))):
+        n = len(rays)
+        rays_d = torch.from_numpy(rays.view(np.uint8).copy()).to(dev)
+        out_d = torch.empty(n * 18, dtype=torch.int32, device=dev)
+        cast = lambda: check(lib.ocean_raycast_device(g.context, n, rays_d.data_ptr(), C, scales.ctypes.data, step, max_samples, tolerance,
+                                                      max_iterations, out_d.data_ptr()))
+        t_r, t_q = [], []
+        for _ in range(3):                      # alternating windows: clock ramp-up and neighbours hit both alike
+            t_r.append(timed(cast))
+            t_q.append(timed(query))
+        hit = out_d.cpu().numpy().view(rc.HIT)
+        st = hit["status"]
+        ev = np.maximum(hit["evaluations"], 1)
+        out = {"config": label, "scene": scene, "gpu": torch.cuda.get_device_name(0), "power_limit_and_max_sm_clock": smi, "map_size": N,
+               "cascades": C, "rays": n, "step": step, "max_samples": max_samples, "tolerance": tolerance, "max_iterations": max_iterations,
+               "raycast_us_per_call": [1e3 * v for v in t_r], "best_us": 1e3 * min(t_r), "mrays_per_s": n / (min(t_r) * 1e-3) / 1e6,
+               "query_surface_2e20_us_per_call": [1e3 * v for v in t_q], "mean_evaluations": float(hit["evaluations"].mean()),
+               "mean_newton_steps": float(hit["iterations"].mean()),
+               "frac_hit": float(np.mean((st == rc.HIT_FROM_ABOVE) | (st == rc.HIT_FROM_BELOW))),
+               "frac_truncated": float(np.mean(st == rc.TRUNCATED)), "frac_miss": float(np.mean(st == rc.MISS)),
+               "frac_invalid": float(np.mean(st == rc.INVALID)),
+               "frac_rays_with_unconverged": float(np.mean(hit["unconverged"] > 0)),
+               "frac_evaluations_unconverged": float(hit["unconverged"].sum() / max(1, hit["evaluations"].sum()))}
+        print(json.dumps(out), flush=True)
+    g.free()
+
+
+if "--raycast" in sys.argv:
+    run_raycast(256, 4, 20, "ray cast over 4 cascades of 256x256")
+    run_raycast(1024, 8, 10, "ray cast over 8 cascades of 1024x1024")
     sys.exit(0)
 
 if "--query" in sys.argv or os.environ.get("OCEAN_RUN_QUERY", "1") != "0":
