@@ -93,6 +93,23 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanFloatingBody                          // struct ocean_floating_body (24 B)
+    {
+        public float mass;                                          // kg, finite and > 0
+        public fixed float inertia[3];                              // principal moments about the centre of mass (kg m^2), hull axes
+        public int first_point, num_points;                         // range into the hull points and drag areas
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanBodyState                             // struct ocean_body_state (52 B)
+    {
+        public fixed float position[3];                             // the centre of mass: global_position + basis * center_of_mass
+        public fixed float orientation[4];                          // unit quaternion x, y, z, w (Godot's Quaternion order), body -> world
+        public fixed float linear_velocity[3];                      // of the centre of mass (RigidBody3D.LinearVelocity)
+        public fixed float angular_velocity[3];                     // world frame, rad/s (RigidBody3D.AngularVelocity)
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public unsafe struct OceanRay                                   // struct ocean_ray (28 B)
     {
         public fixed float origin[3];
@@ -217,6 +234,19 @@ namespace OceanB200
                                                              int num_points, void* points_dev, void* drag_areas_dev, int num_cascades,
                                                              float* map_scales, float density, float tolerance, int max_iterations,
                                                              void* hydrostatic_dev, void* drag_dev, void* samples_dev);
+        // floating bodies: substeps sub-steps of dt / substeps with the states advanced in place; the records are the last
+        // sub-step's and transforms [num_bodies][12] is [R | position] row-major (a MultiMesh TRANSFORM_3D buffer); each may be null
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_simulate_bodies(IntPtr handle, int num_bodies, OceanFloatingBody* bodies, OceanBodyState* states,
+                                                          int num_points, OceanBuoyancyPoint* points, float* drag_areas, int num_cascades,
+                                                          float* map_scales, float density, float dt, int substeps, float tolerance,
+                                                          int max_iterations, OceanBuoyancyResult* hydrostatic, OceanDragResult* drag,
+                                                          float* transforms);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_simulate_bodies_device(IntPtr handle, int num_bodies, OceanFloatingBody* bodies, void* states_dev,
+                                                                 int num_points, void* points_dev, void* drag_areas_dev, int num_cascades,
+                                                                 float* map_scales, float density, float dt, int substeps, float tolerance,
+                                                                 int max_iterations, void* hydrostatic_dev, void* drag_dev, void* transforms_dev);
         // velocity maps: d/dt of the displacement map, recomputed for the cascades whose maps changed; recomputed may be null
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_update_velocity(IntPtr handle, int* recomputed);

@@ -91,6 +91,16 @@ struct ocean_generator {
     size_t drag_areas_capacity = 0;
     ocean_drag_result* drag_results = nullptr;
     size_t drag_results_capacity = 0;
+    // floating-body staging, grown on demand: the body table, max |p|^2 per hull, and the host entry point's states and
+    // transforms (the pose and velocity tables are buoy_bodies and drag_velocities)
+    ocean_floating_body* sim_bodies = nullptr;
+    size_t sim_bodies_capacity = 0;
+    float* sim_r2 = nullptr;
+    size_t sim_r2_capacity = 0;
+    ocean_body_state* sim_states = nullptr;
+    size_t sim_states_capacity = 0;
+    float* sim_transforms = nullptr;
+    size_t sim_transforms_capacity = 0;
     // velocity maps, allocated by the first velocity call: row-pass scratch, the map, its binary32 tap while the taps are on
     float4* vel_scratch = nullptr;                      // [num_cascades][N][N]
     uint2* velocity = nullptr;                          // [num_cascades][N][N] 4 x half
@@ -227,6 +237,10 @@ void release(ocean_generator* g) {
     cudaFree(g->drag_velocities);
     cudaFree(g->drag_areas);
     cudaFree(g->drag_results);
+    cudaFree(g->sim_bodies);
+    cudaFree(g->sim_r2);
+    cudaFree(g->sim_states);
+    cudaFree(g->sim_transforms);
     cudaFree(g->vel_scratch);
     cudaFree(g->velocity);
     cudaFree(g->velocity_f32);
@@ -1304,14 +1318,10 @@ static_assert(sizeof(ocean_buoyancy_body) == 56, "ocean_buoyancy_body layout");
 static_assert(sizeof(ocean_buoyancy_result) == 48, "ocean_buoyancy_result layout");
 
 namespace {
-// The checks both entry points make; *world receives the number of world points, the sum of the bodies' num_points.
-int check_buoyancy_args(int num_bodies, const ocean_buoyancy_body* bodies, int num_points, float density, float tolerance,
-                        int max_iterations, int* world) {
-    int rc = check_surface_args(num_points, tolerance, max_iterations);
-    if (rc) return rc;
-    if (num_bodies < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_bodies %d is negative", num_bodies);
-    if (!(density > 0.0f) || !std::isfinite(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
-    if (num_bodies > 0 && !bodies) return fail(OCEAN_ERR_INVALID_ARGUMENT, "bodies is NULL");
+// The bodies' ranges into the hull points, in 64-bit; *world receives the number of world points, the sum of their num_points.
+// (The templates here, over ocean_buoyancy_body and ocean_floating_body, need C++ linkage inside this extern "C" block.)
+extern "C++" template <typename Body>
+int check_point_ranges(int num_bodies, const Body* bodies, int num_points, int* world) {
     long long total = 0;
     for (int b = 0; b < num_bodies; ++b) {
         const long long first = bodies[b].first_point, n = bodies[b].num_points;
@@ -1322,6 +1332,47 @@ int check_buoyancy_args(int num_bodies, const ocean_buoyancy_body* bodies, int n
     }
     if (total > INT32_MAX) return fail(OCEAN_ERR_INVALID_ARGUMENT, "%lld world points exceed INT32_MAX", total);
     *world = (int)total;
+    return OCEAN_OK;
+}
+
+// The checks both entry points make; *world receives the number of world points, the sum of the bodies' num_points.
+int check_buoyancy_args(int num_bodies, const ocean_buoyancy_body* bodies, int num_points, float density, float tolerance,
+                        int max_iterations, int* world) {
+    int rc = check_surface_args(num_points, tolerance, max_iterations);
+    if (rc) return rc;
+    if (num_bodies < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_bodies %d is negative", num_bodies);
+    if (!(density > 0.0f) || !std::isfinite(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
+    if (num_bodies > 0 && !bodies) return fail(OCEAN_ERR_INVALID_ARGUMENT, "bodies is NULL");
+    return check_point_ranges(num_bodies, bodies, num_points, world);
+}
+
+// The exclusive prefix of the bodies' num_points into gen->buoy_offsets_host (kept in the generator: the upload of it is
+// asynchronous), uploaded to gen->buoy_offsets (grown by the caller).
+extern "C++" template <typename Body>
+int upload_offsets(ocean_generator* gen, int num_bodies, const Body* bodies_host) {
+    const size_t B = (size_t)num_bodies;
+    std::vector<int>& offsets = gen->buoy_offsets_host;
+    offsets.resize(B);
+    for (size_t b = 0, start = 0; b < B; start += (size_t)bodies_host[b].num_points, ++b) offsets[b] = (int)start;
+    OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_offsets, offsets.data(), sizeof(int) * B, cudaMemcpyHostToDevice, gen->stream));
+    return OCEAN_OK;
+}
+
+// The buoyancy launches on a body table and offsets already in device memory (bodies_dev may be written by earlier kernels on
+// the stream), with the map scales in gen->q_scales and gen->buoy_q grown to `world`: samples receives the surface records.
+int launch_buoyancy_sequence(ocean_generator* gen, const ocean_buoyancy_body* bodies_dev, const int* offsets_dev, int num_bodies, int world,
+                             const ocean_buoyancy_point* points_dev, int num_cascades, float density, float tolerance, int max_iterations,
+                             ocean_buoyancy_result* results_dev, ocean_surface_sample* samples) {
+    int rc;
+    if (world > 0) {
+        OCEAN_CUDA(ocean::launch_buoyancy_transform(bodies_dev, offsets_dev, num_bodies, points_dev, world, gen->buoy_q, gen->stream));
+        gen->kernel_launches += 1;
+        if ((rc = run_query_surface(gen, world, gen->buoy_q, num_cascades, tolerance, max_iterations, samples))) return rc;
+    }
+    const float rho_g = density * 9.81f;                                 // G, wave_generator.gd:5, in binary32
+    OCEAN_CUDA(ocean::launch_buoyancy_reduce(bodies_dev, offsets_dev, num_bodies, points_dev, samples, rho_g, tolerance, results_dev,
+                                             gen->stream));
+    gen->kernel_launches += 1;
     return OCEAN_OK;
 }
 
@@ -1338,20 +1389,11 @@ int run_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body
     if ((rc = grow_buffer(gen, &gen->buoy_q, &gen->buoy_q_capacity, (size_t)world))) return rc;
     if (!samples_dev && (rc = grow_buffer(gen, &gen->buoy_samples, &gen->buoy_samples_capacity, (size_t)world))) return rc;
     ocean_surface_sample* samples = samples_dev ? samples_dev : gen->buoy_samples;
-    std::vector<int>& offsets = gen->buoy_offsets_host;              // kept in the generator: the copy below is asynchronous
-    offsets.resize(B);
-    for (size_t b = 0, start = 0; b < B; start += (size_t)bodies_host[b].num_points, ++b) offsets[b] = (int)start;
     OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_bodies, bodies_host, sizeof(ocean_buoyancy_body) * B, cudaMemcpyHostToDevice, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_offsets, offsets.data(), sizeof(int) * B, cudaMemcpyHostToDevice, gen->stream));
-    if (world > 0) {
-        OCEAN_CUDA(ocean::launch_buoyancy_transform(gen->buoy_bodies, gen->buoy_offsets, num_bodies, points_dev, world, gen->buoy_q, gen->stream));
-        gen->kernel_launches += 1;
-        if ((rc = run_query_surface(gen, world, gen->buoy_q, num_cascades, tolerance, max_iterations, samples))) return rc;
-    }
-    const float rho_g = density * 9.81f;                                 // G, wave_generator.gd:5, in binary32
-    OCEAN_CUDA(ocean::launch_buoyancy_reduce(gen->buoy_bodies, gen->buoy_offsets, num_bodies, points_dev, samples, rho_g, tolerance,
-                                             results_dev, gen->stream));
-    gen->kernel_launches += 1;
+    if ((rc = upload_offsets(gen, num_bodies, bodies_host))) return rc;
+    if ((rc = launch_buoyancy_sequence(gen, gen->buoy_bodies, gen->buoy_offsets, num_bodies, world, points_dev, num_cascades, density, tolerance,
+                                       max_iterations, results_dev, samples)))
+        return rc;
     if (samples_used) *samples_used = samples;
     return OCEAN_OK;
 }
@@ -1591,6 +1633,129 @@ int ocean_body_forces(ocean_generator* gen, int num_bodies, const ocean_buoyancy
     if (samples_host && world > 0)
         OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
                                    gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+// ---- floating bodies: sub-stepped buoyancy and drag with the body state on the device (ocean_bodies.cu; oracle/bodies.py) ----
+static_assert(sizeof(ocean_floating_body) == 24, "ocean_floating_body layout");
+static_assert(sizeof(ocean_body_state) == 52, "ocean_body_state layout");
+
+namespace {
+bool finite_positive(float x) { return x > 0.0f && std::isfinite(x); }
+
+// ocean_body_forces' checks on the floating bodies, plus mass, inertia, dt, substeps and the states; *world as for
+// check_buoyancy_args.
+int check_simulate_args(int num_bodies, const ocean_floating_body* bodies, const ocean_body_state* states, int num_points,
+                        const float* drag_areas, float density, float dt, int substeps, float tolerance, int max_iterations, int* world) {
+    int rc = check_surface_args(num_points, tolerance, max_iterations);
+    if (rc) return rc;
+    if (num_bodies < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_bodies %d is negative", num_bodies);
+    if (!finite_positive(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
+    if (!finite_positive(dt)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "dt %g is not finite and > 0", dt);
+    if (substeps < 1 || substeps > 64) return fail(OCEAN_ERR_INVALID_ARGUMENT, "substeps %d outside [1, 64]", substeps);
+    if (num_bodies > 0 && !bodies) return fail(OCEAN_ERR_INVALID_ARGUMENT, "bodies is NULL");
+    if (num_bodies > 0 && !states) return fail(OCEAN_ERR_INVALID_ARGUMENT, "states is NULL");
+    for (int b = 0; b < num_bodies; ++b) {
+        const ocean_floating_body& fb = bodies[b];
+        if (!finite_positive(fb.mass)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: mass %g is not finite and > 0", b, fb.mass);
+        for (int k = 0; k < 3; ++k)
+            if (!finite_positive(fb.inertia[k]))
+                return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: inertia[%d] %g is not finite and > 0", b, k, fb.inertia[k]);
+    }
+    if ((rc = check_point_ranges(num_bodies, bodies, num_points, world))) return rc;
+    if (*world > 0 && !drag_areas) return fail(OCEAN_ERR_INVALID_ARGUMENT, "drag_areas is NULL");
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_dev,
+                                 int num_points, const ocean_buoyancy_point* points_dev, const float* drag_areas_dev, int num_cascades,
+                                 const float* map_scales_host, float density, float dt, int substeps, float tolerance, int max_iterations,
+                                 ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev, float* transforms_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_simulate_args(num_bodies, bodies_host, states_dev, num_points, drag_areas_dev, density, dt, substeps, tolerance,
+                                  max_iterations, &world)))
+        return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (world > 0 && !points_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
+    if ((rc = refresh_velocity(gen, nullptr))) return rc;
+    const size_t B = (size_t)num_bodies;
+    if ((rc = grow_buffer(gen, &gen->sim_bodies, &gen->sim_bodies_capacity, B))) return rc;
+    if ((rc = grow_buffer(gen, &gen->sim_r2, &gen->sim_r2_capacity, B))) return rc;
+    if ((rc = grow_buffer(gen, &gen->buoy_bodies, &gen->buoy_bodies_capacity, B))) return rc;
+    if ((rc = grow_buffer(gen, &gen->buoy_offsets, &gen->buoy_offsets_capacity, B))) return rc;
+    if ((rc = grow_buffer(gen, &gen->drag_velocities, &gen->drag_velocities_capacity, B))) return rc;
+    if ((rc = grow_buffer(gen, &gen->buoy_q, &gen->buoy_q_capacity, (size_t)world))) return rc;
+    if ((rc = grow_buffer(gen, &gen->buoy_samples, &gen->buoy_samples_capacity, (size_t)world))) return rc;
+    if (!hydrostatic_dev) {
+        if ((rc = grow_buffer(gen, &gen->buoy_results, &gen->buoy_results_capacity, B))) return rc;
+        hydrostatic_dev = gen->buoy_results;
+    }
+    if (!drag_dev) {
+        if ((rc = grow_buffer(gen, &gen->drag_results, &gen->drag_results_capacity, B))) return rc;
+        drag_dev = gen->drag_results;
+    }
+    OCEAN_CUDA(cudaMemcpyAsync(gen->sim_bodies, bodies_host, sizeof(ocean_floating_body) * B, cudaMemcpyHostToDevice, gen->stream));
+    if ((rc = upload_offsets(gen, num_bodies, bodies_host))) return rc;
+    OCEAN_CUDA(ocean::launch_bodies_prepare(gen->sim_bodies, states_dev, num_bodies, points_dev, gen->sim_r2, gen->buoy_bodies,
+                                            gen->drag_velocities, gen->stream));
+    gen->kernel_launches += 1;
+    const float h = dt / (float)substeps;
+    const float half_rho = 0.5f * density;
+    for (int s = 0; s < substeps; ++s) {
+        if ((rc = launch_buoyancy_sequence(gen, gen->buoy_bodies, gen->buoy_offsets, num_bodies, world, points_dev, num_cascades, density,
+                                           tolerance, max_iterations, hydrostatic_dev, gen->buoy_samples)))
+            return rc;
+        OCEAN_CUDA(ocean::launch_drag_reduce(gen->buoy_bodies, gen->drag_velocities, gen->buoy_offsets, num_bodies, points_dev, drag_areas_dev,
+                                             gen->buoy_samples, gen->velocity, gen->map_size, num_cascades, gen->q_scales, half_rho, drag_dev,
+                                             gen->stream));
+        OCEAN_CUDA(ocean::launch_bodies_integrate(gen->sim_bodies, gen->sim_r2, num_bodies, hydrostatic_dev, drag_dev, density, h, states_dev,
+                                                  gen->buoy_bodies, gen->drag_velocities, s == substeps - 1 ? transforms_dev : nullptr,
+                                                  gen->stream));
+        gen->kernel_launches += 2;
+    }
+    return OCEAN_OK;
+}
+
+int ocean_simulate_bodies(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_host,
+                          int num_points, const ocean_buoyancy_point* points_host, const float* drag_areas_host, int num_cascades,
+                          const float* map_scales_host, float density, float dt, int substeps, float tolerance, int max_iterations,
+                          ocean_buoyancy_result* hydrostatic_host, ocean_drag_result* drag_host, float* transforms_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_simulate_args(num_bodies, bodies_host, states_host, num_points, drag_areas_host, density, dt, substeps, tolerance,
+                                  max_iterations, &world)))
+        return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (world > 0 && !points_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
+    const size_t B = (size_t)num_bodies;
+    if ((rc = grow_buffer(gen, &gen->sim_states, &gen->sim_states_capacity, B))) return rc;
+    if ((rc = grow_buffer(gen, &gen->buoy_results, &gen->buoy_results_capacity, B))) return rc;
+    if ((rc = grow_buffer(gen, &gen->drag_results, &gen->drag_results_capacity, B))) return rc;
+    if (transforms_host && (rc = grow_buffer(gen, &gen->sim_transforms, &gen->sim_transforms_capacity, 12 * B))) return rc;
+    if (world > 0) {
+        if ((rc = grow_buffer(gen, &gen->buoy_points, &gen->buoy_points_capacity, (size_t)num_points))) return rc;
+        if ((rc = grow_buffer(gen, &gen->drag_areas, &gen->drag_areas_capacity, (size_t)num_points))) return rc;
+        OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_points, points_host, sizeof(ocean_buoyancy_point) * (size_t)num_points, cudaMemcpyHostToDevice,
+                                   gen->stream));
+        OCEAN_CUDA(cudaMemcpyAsync(gen->drag_areas, drag_areas_host, sizeof(float) * (size_t)num_points, cudaMemcpyHostToDevice, gen->stream));
+    }
+    OCEAN_CUDA(cudaMemcpyAsync(gen->sim_states, states_host, sizeof(ocean_body_state) * B, cudaMemcpyHostToDevice, gen->stream));
+    if ((rc = ocean_simulate_bodies_device(gen, num_bodies, bodies_host, gen->sim_states, num_points, world > 0 ? gen->buoy_points : nullptr,
+                                           world > 0 ? gen->drag_areas : nullptr, num_cascades, map_scales_host, density, dt, substeps, tolerance,
+                                           max_iterations, gen->buoy_results, gen->drag_results, transforms_host ? gen->sim_transforms : nullptr)))
+        return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(states_host, gen->sim_states, sizeof(ocean_body_state) * B, cudaMemcpyDeviceToHost, gen->stream));
+    if (hydrostatic_host)
+        OCEAN_CUDA(cudaMemcpyAsync(hydrostatic_host, gen->buoy_results, sizeof(ocean_buoyancy_result) * B, cudaMemcpyDeviceToHost, gen->stream));
+    if (drag_host) OCEAN_CUDA(cudaMemcpyAsync(drag_host, gen->drag_results, sizeof(ocean_drag_result) * B, cudaMemcpyDeviceToHost, gen->stream));
+    if (transforms_host)
+        OCEAN_CUDA(cudaMemcpyAsync(transforms_host, gen->sim_transforms, sizeof(float) * 12 * B, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }

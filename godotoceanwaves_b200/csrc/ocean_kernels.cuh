@@ -144,6 +144,17 @@ cudaError_t launch_drag_reduce(const void* bodies_dev, const void* velocities_de
                                const void* points_dev, const float* drag_areas_dev, const void* samples_dev, const uint2* velocity_dev,
                                int map_size, int num_cascades, const float4* scales_dev, float half_rho, void* results_dev, cudaStream_t stream);
 
+// ocean_bodies.cu: the floating-body integrator (oracle/bodies.py).  bodies_dev = ocean_floating_body[num_bodies], states_dev =
+// ocean_body_state[num_bodies], r2_dev = [num_bodies] max |p|^2 over each hull, pose_dev / velocities_dev = the
+// ocean_buoyancy_body / ocean_body_velocity tables the body-forces kernels read.  prepare fills r2 and the first sub-step's
+// tables; integrate takes one sub-step of h from the records of the tables' pose and writes the next sub-step's tables, and
+// the 3 x 4 transforms ([num_bodies][12]) when transforms_dev is not null.
+cudaError_t launch_bodies_prepare(const void* bodies_dev, const void* states_dev, int num_bodies, const void* points_dev, float* r2_dev,
+                                  void* pose_dev, void* velocities_dev, cudaStream_t stream);
+cudaError_t launch_bodies_integrate(const void* bodies_dev, const float* r2_dev, int num_bodies, const void* hydrostatic_dev, const void* drag_dev,
+                                    float density, float h, void* states_dev, void* pose_dev, void* velocities_dev, float* transforms_dev,
+                                    cudaStream_t stream);
+
 // ocean_velocity.cu: velocity maps (oracle_velocity_update).  One record per cascade to recompute: the table slot and time of
 // the update that built the cascade's current maps.
 struct VelocityDispatch {

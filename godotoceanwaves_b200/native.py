@@ -73,6 +73,17 @@ class DragResultC(C.Structure):
     _fields_ = [("force", C.c_float * 3), ("torque", C.c_float * 3), ("wetted_drag_area", C.c_float), ("max_relative_speed", C.c_float)]
 
 
+class FloatingBodyC(C.Structure):
+    """struct ocean_floating_body (include/ocean.h), 24 B: mass (kg), principal inertia (kg m^2), range into the hull points"""
+    _fields_ = [("mass", C.c_float), ("inertia", C.c_float * 3), ("first_point", C.c_int32), ("num_points", C.c_int32)]
+
+
+class BodyStateC(C.Structure):
+    """struct ocean_body_state (include/ocean.h), 52 B: centre of mass, unit quaternion (x, y, z, w), world-frame velocities"""
+    _fields_ = [("position", C.c_float * 3), ("orientation", C.c_float * 4), ("linear_velocity", C.c_float * 3),
+                ("angular_velocity", C.c_float * 3)]
+
+
 # every symbol include/ocean.h declares: name -> (restype, argtypes)
 _H = C.c_void_p
 _P = C.POINTER
@@ -121,6 +132,10 @@ SIGNATURES = {
                                     C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ocean_body_forces_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                            C.c_float, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ocean_simulate_bodies": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                        C.c_float, C.c_float, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ocean_simulate_bodies_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                               C.c_float, C.c_float, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ocean_update_velocity": (C.c_int, [_H, _P(C.c_int)]),
     "ocean_get_velocity_map": (C.c_int, [_H, _P(C.c_void_p), _P(C.c_size_t)]),
     "ocean_copy_velocity_to_host": (C.c_int, [_H, C.c_int, C.c_int, C.c_void_p]),

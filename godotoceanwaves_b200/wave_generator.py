@@ -356,6 +356,43 @@ class WaveGenerator:
                                                hydro.ctypes.data, drag.ctypes.data, None if samples is None else samples.ctypes.data))
         return (hydro, drag, samples) if return_samples else (hydro, drag)
 
+    # -- floating bodies: sub-stepped buoyancy and drag, the body state advanced on the device ----------------------
+    FLOATING_BODY = np.dtype([("mass", np.float32), ("inertia", np.float32, 3), ("first_point", np.int32),
+                              ("num_points", np.int32)])                                     # struct ocean_floating_body
+    BODY_STATE = np.dtype([("position", np.float32, 3), ("orientation", np.float32, 4), ("linear_velocity", np.float32, 3),
+                           ("angular_velocity", np.float32, 3)])                            # struct ocean_body_state
+
+    def simulate_bodies(self, bodies, states, points, drag_areas, map_scales, dt: float, substeps: int = 1, density: float = 1025.0,
+                        tolerance: float = 1e-3, max_iterations: int = 8, return_records: bool = False,
+                        return_transforms: bool = False):
+        """The BODY_STATE rows of `states` advanced by `substeps` sub-steps of dt / substeps (include/ocean.h,
+        ocean_simulate_bodies): buoyancy, drag and gravity on each FLOATING_BODY row of `bodies` (mass, principal inertia,
+        a range of the BUOYANCY_POINT rows of `points` and of `drag_areas`).  The state's origin is the centre of mass and its
+        orientation a unit quaternion (x, y, z, w).  Returns the new states (a new array); with return_records also the
+        (BUOYANCY_RESULT, DRAG_RESULT) rows of the last sub-step, with return_transforms also the [n][12] float32 3 x 4
+        row-major [R | position] of each new state."""
+        self._require()
+        b = np.ascontiguousarray(bodies, self.FLOATING_BODY).reshape(-1)
+        s = np.array(states, self.BODY_STATE, copy=True).reshape(-1)
+        p = np.ascontiguousarray(points, self.BUOYANCY_POINT).reshape(-1)
+        a = np.ascontiguousarray(drag_areas, np.float32).reshape(-1)
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        if len(s) != len(b) or len(a) != len(p):
+            raise ValueError(f"{len(s)} states for {len(b)} bodies, or {len(a)} drag areas for {len(p)} points")
+        hydro = np.zeros(len(b), self.BUOYANCY_RESULT) if return_records else None
+        drag = np.zeros(len(b), self.DRAG_RESULT) if return_records else None
+        transforms = np.zeros((len(b), 12), np.float32) if return_transforms else None
+        ptr = lambda x: None if x is None else x.ctypes.data  # noqa: E731
+        check(load_library().ocean_simulate_bodies(self.context, len(b), b.ctypes.data, s.ctypes.data, len(p), p.ctypes.data, a.ctypes.data,
+                                                   sc.shape[0], sc.ctypes.data, float(density), float(dt), int(substeps), float(tolerance),
+                                                   int(max_iterations), ptr(hydro), ptr(drag), ptr(transforms)))
+        out = (s,)
+        if return_records:
+            out += (hydro, drag)
+        if return_transforms:
+            out += (transforms,)
+        return out if len(out) > 1 else s
+
     # -- spray candidates: the spawn test of sea_spray_particle.gdshader:80-94 as a stream compaction --------------
     SPRAY_RECORD = np.dtype([("index", np.uint32), ("start_x", np.float32), ("start_z", np.float32), ("scale_factor", np.float32),
                              ("particle_scale", np.float32, 3), ("foam", np.float32)])     # struct ocean_spray_record

@@ -351,7 +351,8 @@ int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoy
  * depth z (at 1 m of draft this overstates the longest wave of a 16 m tile about 1.5 times, shorter waves more); there is no
  * added mass, radiation or wave-making damping, skin friction, or separate normal and tangential coefficients; nothing is
  * written back into the maps (no wake or foam).  Quadratic drag is stiff for light bodies under explicit integration: the op
- * does not integrate, and max_relative_speed lets a host choose sub-steps.
+ * does not integrate, and max_relative_speed lets a host choose sub-steps (ocean_simulate_bodies below integrates on the
+ * device with a step that stays stable under it).
  * The call first brings stale velocity layers up to date (as ocean_sample_velocity does; the velocity buffers are allocated
  * on first use).  Validation is ocean_buoyancy's, plus velocities and drag_areas non-NULL where a count needs them and both
  * outputs non-NULL; an invalid call launches nothing.  samples may be NULL, as for ocean_buoyancy.  The bodies, velocities
@@ -377,6 +378,62 @@ int ocean_body_forces_device(ocean_generator* gen, int num_bodies, const ocean_b
                              const float* drag_areas_dev, int num_cascades, const float* map_scales_host, float density, float tolerance,
                              int max_iterations, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
                              ocean_surface_sample* samples_dev);
+
+/* Floating bodies -- advance rigid bodies on the water by `substeps` sub-steps of h = dt / substeps (binary32), with the
+ * body state kept in device memory.  A floating body is a mass (kg), principal moments of inertia about its centre of mass
+ * (kg m^2, body axes = hull axes) and a range into the hull points and drag areas, as ocean_buoyancy_body's.  The body ORIGIN
+ * is its centre of mass and its hull axes are its principal axes: a Godot host whose RigidBody3D has a custom center_of_mass
+ * c shifts its hull points by -c once (p - c) and keeps position = global_position + basis * c.  A state is the world
+ * position of the origin, a unit quaternion (x, y, z, w) from body to world, and the world-frame linear velocity of the
+ * centre of mass and angular velocity (Godot's linear_velocity and angular_velocity).  One sub-step, per body
+ * (oracle/bodies.py is the specification, bit for bit):
+ *   pose    R = R(q), the standard unit-quaternion rotation (R00 = 1 - 2 (yy + zz), R01 = 2 (xy - wz), R02 = 2 (xz + wy),
+ *           R10 = 2 (xy + wz), R11 = 1 - 2 (xx + zz), R12 = 2 (yz - wx), R20 = 2 (xz - wy), R21 = 2 (yz + wx),
+ *           R22 = 1 - 2 (xx + yy)); transform = [R | position]; the origin's velocity is (linear, angular).
+ *   forces  hyd and drg = ocean_body_forces' two records for that transform and velocity, through the same kernels.
+ *   step    c_v = (density * drg.wetted_drag_area) * drg.max_relative_speed   (bounds |dF_drag/dv|)
+ *           c_w = c_v * r2, r2 = max |p|^2 over the body's hull points          (bounds |dT_drag/dw|)
+ *           F = hyd.force + drg.force, F.y = F.y - mass * 9.81f;   v' = v + (h / (mass + h c_v)) F
+ *           tau = hyd.torque + drg.torque; tau_b = R^T tau, w_b = R^T w;  w_b' = w_b + (h tau_b) / (inertia + h c_w) per
+ *           axis;  w' = R w_b'
+ *           position' = position + h v';   q' = normalize(q + (h / 2) (w' (x) q))
+ * A semi-implicit Euler step whose drag Jacobian is bounded by the scalars c_v and c_w: for the linearised drag it never
+ * overshoots and is stable at any h, so light bodies with large drag areas do not blow up at 60 Hz; as h -> 0 it is explicit
+ * Euler on the true forces.  A body with num_points = 0 is ballistic (all-zero records).  A NaN or infinite state affects
+ * only its own body.  hydrostatic and drag (may be NULL) receive the records of the LAST sub-step (the forces at the pose that
+ * sub-step started from); transforms (may be NULL) receives the 3 x 4 row-major [R | position] of each final state, the
+ * layout of ocean_buoyancy_body.transform and of a Godot 4 MultiMesh transform buffer (RenderingServer.multimesh_set_buffer
+ * with TRANSFORM_3D, no colours or custom data: 12 floats per instance).  The model's limits: no added mass (the heave period
+ * is shorter than a real body's); no gyroscopic term; no contacts between bodies; the surface water velocity at every depth
+ * (ocean_body_forces'); every sub-step of a call sees the same maps; the hydrostatic spring is explicit in position, so h must
+ * stay below T_heave / pi with T_heave = 2 pi sqrt(mass / (density * 9.81 * A_waterplane)).
+ * The bodies and map_scales are host arrays in both entry points: the call validates the bodies, computes the world-point
+ * offsets and uploads both once.  Validation is ocean_body_forces' (without its velocities and outputs), plus mass and every
+ * inertia finite and > 0, dt finite and > 0, substeps in [1, 64] and states non-NULL when num_bodies > 0; an invalid call
+ * launches nothing and refreshes nothing.  The call brings stale velocity layers up to date once, then launches 1 + 7 S
+ * kernels (1 + 5 S with max_iterations = 0, 1 + 3 S when no body has hull points).  ocean_simulate_bodies takes host
+ * states, points, areas and outputs and is synchronous; ocean_simulate_bodies_device takes device pointers for them and is
+ * asynchronous on the generator's stream. */
+typedef struct ocean_floating_body {
+    float mass;                 /* kg, finite and > 0 */
+    float inertia[3];           /* principal moments about the centre of mass, body axes = hull axes (kg m^2), finite and > 0 */
+    int32_t first_point;        /* range into the hull points and drag areas, as ocean_buoyancy_body's */
+    int32_t num_points;
+} ocean_floating_body;          /* 24 B */
+typedef struct ocean_body_state {
+    float position[3];          /* world position of the body origin = its centre of mass */
+    float orientation[4];       /* unit quaternion (x, y, z, w), body -> world */
+    float linear_velocity[3];   /* of the centre of mass, m/s (Godot's linear_velocity) */
+    float angular_velocity[3];  /* world frame, rad/s (Godot's angular_velocity) */
+} ocean_body_state;             /* 52 B */
+int ocean_simulate_bodies(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_host,
+                          int num_points, const ocean_buoyancy_point* points_host, const float* drag_areas_host, int num_cascades,
+                          const float* map_scales_host, float density, float dt, int substeps, float tolerance, int max_iterations,
+                          ocean_buoyancy_result* hydrostatic_host, ocean_drag_result* drag_host, float* transforms_host);
+int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_dev,
+                                 int num_points, const ocean_buoyancy_point* points_dev, const float* drag_areas_dev, int num_cascades,
+                                 const float* map_scales_host, float density, float dt, int substeps, float tolerance, int max_iterations,
+                                 ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev, float* transforms_dev);
 
 /* Velocity maps -- the water velocity: the time derivative of the displacement map, what drag, damping and floating debris
  * need.  A cascade's velocity layer is (vx, vy, vz, 0) = d/dt of its displacement texel (hx, hy, hz, 0): same layout, same

@@ -116,7 +116,7 @@ def run_spray(N, C, particles, reps, label):
     print(json.dumps(out), flush=True)
 
 
-if not {"--buoyancy", "--velocity", "--drag", "--raycast"} & set(sys.argv):    # --buoyancy / --velocity / --drag / --raycast run their op (defined below) alone
+if not {"--buoyancy", "--velocity", "--drag", "--bodies", "--raycast"} & set(sys.argv):    # each of these runs its op (defined below) alone
     run(256, 4, 2000, "cfg2 latency: one 256x256x4 set per launch (launch/latency-bound, L2-resident)")
     run(256, 4, 2000, "cfg2 latency, fused frames (ocean_update_frames: 64 frames per launch)", fused=True)
     run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, frame by frame")
@@ -438,6 +438,109 @@ if "--buoyancy" in sys.argv:
 if "--drag" in sys.argv:
     run_body_forces(256, 4, 1 << 14, 64, 50, "body forces: 2^14 bodies x 64 points over 4 cascades of 256x256")
     run_body_forces(1024, 8, 1 << 14, 64, 20, "body forces: 2^14 bodies x 64 points over 8 cascades of 1024x1024")
+    sys.exit(0)
+
+
+def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, tolerance=1e-3, max_iterations=8):
+    """Floating-body integrator (ocean_simulate_bodies_device, S sub-steps per call, states in device memory) against
+    S x ocean_body_forces_device on the same bodies and device-resident hulls (the integrator's own overhead), and against
+    a host loop of S rounds of ocean_body_forces_device, read-back of the records and the numpy step of oracle/bodies.py
+    (what the op saves a host).  Device times from CUDA events, the host loop from the wall clock after a synchronise; the
+    states are restored before each window; alternating windows.  The card's name, power limit and max SM clock are read
+    in the same run."""
+    import subprocess
+    import time
+    import numpy as np
+    import torch
+    from godotoceanwaves_b200.native import load_library, check
+    from oracle import bodies as ob
+    from oracle import buoyancy as bu
+    from oracle import drag as dr
+    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
+    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
+    for _ in range(2):
+        g.update_all(0.02, p)
+    scales = gow.WaveGenerator.map_scales(p)
+    table, hull = _buoyancy_scene(n_bodies, per_body)
+    rng = np.random.default_rng(3)
+    bodies = np.zeros(n_bodies, ob.BODY)
+    bodies["first_point"], bodies["num_points"] = table["first_point"], table["num_points"]
+    bodies["mass"] = hull["volume"].reshape(n_bodies, per_body).sum(1) * rng.uniform(200.0, 900.0, n_bodies)
+    bodies["inertia"] = bodies["mass"][:, None] * rng.uniform(0.5, 3.0, (n_bodies, 3))
+    states = np.zeros(n_bodies, ob.STATE)
+    states["position"] = table["transform"][:, [3, 7, 11]]
+    q = rng.standard_normal((n_bodies, 4))
+    states["orientation"] = q / np.linalg.norm(q, axis=1, keepdims=True)
+    states["linear_velocity"] = rng.uniform(-2.0, 2.0, (n_bodies, 3))
+    states["angular_velocity"] = rng.uniform(-1.0, 1.0, (n_bodies, 3))
+    cda = rng.uniform(0.01, 0.2, len(hull)).astype(np.float32)
+    pose, vel = ob.pose(bodies, states)
+    dev = torch.device("cuda", 0)
+    hull_d = torch.from_numpy(hull.view(np.uint8).copy()).to(dev)
+    cda_d = torch.from_numpy(cda).to(dev)
+    st0_d = torch.from_numpy(states.view(np.uint8).copy()).to(dev)
+    st_d = st0_d.clone()
+    hyd_d = torch.empty(n_bodies * 12, dtype=torch.int32, device=dev)           # ocean_buoyancy_result: 48 B
+    drag_d = torch.empty(n_bodies * 8, dtype=torch.int32, device=dev)           # ocean_drag_result: 32 B
+    torch.cuda.synchronize()
+    lib = load_library()
+    h = np.float32(dt) / np.float32(substeps)
+    r2 = ob.radius2(bodies, hull)
+    sim = lambda: check(lib.ocean_simulate_bodies_device(g.context, n_bodies, bodies.ctypes.data, st_d.data_ptr(), len(hull), hull_d.data_ptr(),
+                                                         cda_d.data_ptr(), C, scales.ctypes.data, 1025.0, dt, substeps, tolerance,
+                                                         max_iterations, hyd_d.data_ptr(), drag_d.data_ptr(), None))
+    forces_once = lambda tbl, v: check(lib.ocean_body_forces_device(g.context, n_bodies, tbl.ctypes.data, v.ctypes.data, len(hull),
+                                                                    hull_d.data_ptr(), cda_d.data_ptr(), C, scales.ctypes.data, 1025.0,
+                                                                    tolerance, max_iterations, hyd_d.data_ptr(), drag_d.data_ptr(), None))
+
+    def forces():
+        for _ in range(substeps):
+            forces_once(pose, vel)
+
+    def timed(call):
+        st_d.copy_(st0_d)
+        for _ in range(3):
+            call()
+        g.synchronize()
+        g.timer_start()
+        for _ in range(reps):
+            call()
+        return g.timer_stop() / reps
+
+    def host_loop():
+        s = states
+        g.synchronize()
+        t0 = time.perf_counter()
+        for _ in range(max(1, reps // 10)):
+            for _ in range(substeps):
+                tbl, v = ob.pose(bodies, s)
+                forces_once(tbl, v)
+                g.synchronize()                 # the records come from the generator's stream, not torch's
+                hyd = hyd_d.cpu().numpy().view(bu.RESULT)
+                drg = drag_d.cpu().numpy().view(dr.RESULT)
+                s = ob.step(bodies, s, r2, hyd, drg, 1025.0, h)
+        return (time.perf_counter() - t0) * 1e3 / max(1, reps // 10)
+
+    t_s, t_f, t_h = [], [], []
+    for _ in range(3):                          # alternating windows: clock ramp-up and neighbours hit both alike
+        t_s.append(timed(sim))
+        t_f.append(timed(forces))
+        t_h.append(host_loop())
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                         stdout=subprocess.PIPE, text=True).stdout.strip()
+    out = {"config": label, "gpu": torch.cuda.get_device_name(0), "power_limit_and_max_sm_clock": smi, "map_size": N, "cascades": C,
+           "bodies": n_bodies, "points_per_body": per_body, "substeps": substeps, "dt": dt, "max_iterations": max_iterations,
+           "simulate_us_per_call": [1e3 * v for v in t_s], "S_x_body_forces_us": [1e3 * v for v in t_f],
+           "host_loop_us_per_call": [1e3 * v for v in t_h], "overhead_over_S_x_body_forces": min(t_s) / min(t_f) - 1.0,
+           "host_loop_over_simulate": min(t_h) / min(t_s)}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
+if "--bodies" in sys.argv:
+    for S in (1, 4):
+        run_bodies(256, 4, 1 << 14, 64, S, 50, f"floating bodies: 2^14 bodies x 64 points, {S} sub-step(s) of 1/60 s, 4 cascades of 256x256")
+        run_bodies(1024, 8, 1 << 14, 64, S, 20, f"floating bodies: 2^14 bodies x 64 points, {S} sub-step(s) of 1/60 s, 8 cascades of 1024x1024")
     sys.exit(0)
 
 def _picking_rays(side, y=12.0, fov_deg=90.0, pitch_deg=-20.0):
