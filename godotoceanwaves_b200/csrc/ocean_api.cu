@@ -43,74 +43,81 @@ constexpr int kRing = 8;          // pinned staging slots for dispatch records
 
 }  // namespace
 
+struct ocean_generator;
+
+namespace {
+// A device block of `capacity` elements of T owned by one generator and counted in its device_bytes while it lives.
+template <typename T>
+struct DeviceArray {
+    T* ptr = nullptr;
+    size_t capacity = 0;
+    ocean_generator* owner = nullptr;                   // whose device_bytes count the block
+
+    DeviceArray() = default;
+    DeviceArray(const DeviceArray&) = delete;
+    DeviceArray& operator=(const DeviceArray&) = delete;
+    ~DeviceArray() { release(); }
+    cudaError_t grow(ocean_generator* g, size_t n);
+    cudaError_t upload(ocean_generator* g, const void* host, size_t n);
+    void release();
+};
+}  // namespace
+
 struct ocean_generator {
     int device = 0;
     int map_size = 0;
     int num_cascades = 0;
+    uint64_t device_bytes = 0;                          // declared before the DeviceArrays: their destructors update it
     cudaStream_t stream = nullptr;
     cudaStream_t copy_stream = nullptr;                 // snapshot hand-off: device->host copies that overlap the next update
     cudaEvent_t snap_ready = nullptr, snap_free = nullptr;
-    uint2* snap_disp = nullptr;                         // [num_cascades][N][N] snapshot of the maps (lazy)
-    uint2* snap_normal = nullptr;
+    DeviceArray<uint2> snap_disp, snap_normal;          // [num_cascades][N][N] snapshot of the maps (lazy)
     bool snap_busy = false;
+    // the maps, scratch and tables of ocean_create; `buf` is the view of them (and of the taps) that the kernels take
+    DeviceArray<float4> spectrum, rowpass, disp_table;
+    DeviceArray<uint2> displacement, normal;
+    DeviceArray<float4> displacement_f32, normal_f32;   // binary32 taps, while they are on
+    DeviceArray<float> disp_kvy;
+    DeviceArray<float2> twiddles;
     ocean::DeviceBuffers buf{};
-    float2* twiddles = nullptr;
-    float2* export_buf = nullptr;                       // rowpass export scratch (lazy)
-    float2* q_points = nullptr;                         // query staging (lazy, grown on demand): points, outputs, scales
-    float* q_disp = nullptr;
-    float* q_grad = nullptr;
-    float4* q_scales = nullptr;
-    size_t q_capacity = 0;
-    int* spray_counts = nullptr;                        // spray op scratch: block counts / offsets (+ total), grown on demand
-    int spray_count_capacity = 0;
-    void* spray_records = nullptr;                      // spray op staging for the host entry point
-    size_t spray_record_capacity = 0;
-    int* surf_scratch = nullptr;                        // surface query scratch: pending count, layer maxima, pending list
-    size_t surf_scratch_capacity = 0;                   // (ints), grown on demand
-    ocean_surface_sample* surf_records = nullptr;       // surface query staging for the host entry point
-    size_t surf_record_capacity = 0;
-    // buoyancy staging, each grown on demand: body table and world-point offsets, query positions, surface records (when the
-    // caller wants none), and the host entry point's hull points and results
-    ocean_buoyancy_body* buoy_bodies = nullptr;
-    size_t buoy_bodies_capacity = 0;
-    int* buoy_offsets = nullptr;
-    size_t buoy_offsets_capacity = 0;
+    DeviceArray<float2> export_buf;                     // rowpass export scratch (lazy)
+    // query staging, grown on demand: points and map-query outputs for the host entry points, map scales
+    DeviceArray<float2> q_points;
+    DeviceArray<float> q_disp, q_grad;
+    DeviceArray<float4> q_scales;
+    DeviceArray<int> spray_counts;                      // spray op scratch: block counts / offsets (+ total)
+    DeviceArray<ocean_spray_record> spray_records;      // spray op staging for the host entry point (+ one slot for the count)
+    DeviceArray<int> surf_scratch;                      // surface query scratch: pending count, layer maxima, pending list
+    DeviceArray<ocean_surface_sample> surf_records;     // surface query staging for the host entry point
+    // buoyancy staging: body table and world-point offsets, query positions, surface records (when the caller wants none),
+    // and the host entry point's hull points and results
+    DeviceArray<ocean_buoyancy_body> buoy_bodies;
+    DeviceArray<int> buoy_offsets;
     std::vector<int> buoy_offsets_host;
-    float2* buoy_q = nullptr;
-    size_t buoy_q_capacity = 0;
-    ocean_surface_sample* buoy_samples = nullptr;
-    size_t buoy_samples_capacity = 0;
-    ocean_buoyancy_point* buoy_points = nullptr;
-    size_t buoy_points_capacity = 0;
-    ocean_buoyancy_result* buoy_results = nullptr;
-    size_t buoy_results_capacity = 0;
-    // body-forces staging, grown on demand: body velocities, and the host entry point's drag areas and drag results
-    ocean_body_velocity* drag_velocities = nullptr;
-    size_t drag_velocities_capacity = 0;
-    float* drag_areas = nullptr;
-    size_t drag_areas_capacity = 0;
-    ocean_drag_result* drag_results = nullptr;
-    size_t drag_results_capacity = 0;
-    // floating-body staging, grown on demand: the body table, max |p|^2 per hull, and the host entry point's states and
-    // transforms (the pose and velocity tables are buoy_bodies and drag_velocities)
-    ocean_floating_body* sim_bodies = nullptr;
-    size_t sim_bodies_capacity = 0;
-    float* sim_r2 = nullptr;
-    size_t sim_r2_capacity = 0;
-    ocean_body_state* sim_states = nullptr;
-    size_t sim_states_capacity = 0;
-    float* sim_transforms = nullptr;
-    size_t sim_transforms_capacity = 0;
+    DeviceArray<float2> buoy_q;
+    DeviceArray<ocean_surface_sample> buoy_samples;
+    DeviceArray<ocean_buoyancy_point> buoy_points;
+    DeviceArray<ocean_buoyancy_result> buoy_results;
+    // body-forces staging: body velocities, and the host entry point's drag areas and drag results
+    DeviceArray<ocean_body_velocity> drag_velocities;
+    DeviceArray<float> drag_areas;
+    DeviceArray<ocean_drag_result> drag_results;
+    // floating-body staging: the body table, max |p|^2 per hull, and the host entry point's states and transforms (the pose
+    // and velocity tables are buoy_bodies and drag_velocities)
+    DeviceArray<ocean_floating_body> sim_bodies;
+    DeviceArray<float> sim_r2;
+    DeviceArray<ocean_body_state> sim_states;
+    DeviceArray<float> sim_transforms;
     // velocity maps, allocated by the first velocity call: row-pass scratch, the map, its binary32 tap while the taps are on
-    float4* vel_scratch = nullptr;                      // [num_cascades][N][N]
-    uint2* velocity = nullptr;                          // [num_cascades][N][N] 4 x half
-    float4* velocity_f32 = nullptr;                     // [num_cascades][N][N]
+    DeviceArray<float4> vel_scratch;                    // [num_cascades][N][N]
+    DeviceArray<uint2> velocity;                        // [num_cascades][N][N] 4 x half
+    DeviceArray<float4> velocity_f32;                   // [num_cascades][N][N]
     std::vector<ocean::VelocityDispatch> vel_source;    // [num_cascades] table slot and time of the update that built the current maps
     std::vector<char> vel_has_source;                   // the cascade's maps were written at least once
     std::vector<char> vel_stale;                        // its velocity layer does not describe its current maps yet
-    ocean::CascadeDispatch* d_cascade = nullptr;        // [num_cascades] (two-kernel path only)
-    ocean::SpectrumDispatch* d_spectrum = nullptr;      // [num_cascades]
-    ocean::TableDispatch* d_tables = nullptr;           // [num_cascades]
+    DeviceArray<ocean::CascadeDispatch> d_cascade;      // [num_cascades] (two-kernel path only)
+    DeviceArray<ocean::SpectrumDispatch> d_spectrum;    // [num_cascades]
+    DeviceArray<ocean::TableDispatch> d_tables;         // [num_cascades]
     ocean::CascadeDispatch* h_cascade = nullptr;        // pinned [kRing][num_cascades]
     ocean::SpectrumDispatch* h_spectrum = nullptr;      // pinned [kRing][num_cascades]
     ocean::TableDispatch* h_tables = nullptr;           // pinned [kRing][num_cascades]
@@ -128,22 +135,19 @@ struct ocean_generator {
     int prof_chunk = 0;                                 // cascades in the profiled first chunk
     bool profiling = false;
     bool prof_valid = false, prof_had_gen = false;
-    int* d_queue = nullptr;                             // [1 + 3 * num_cascades] work counter + completion counters
+    DeviceArray<int> d_queue;                           // [1 + 3 * num_cascades] work counter + completion counters
     std::vector<uint32_t> done_count;                   // host mirror of the completion counters (modulo 2^32)
     int resident_ctas = 0;
-    std::map<int, std::pair<int*, int>> item_tables;    // cascades per launch -> (device item table, item count)
-    std::map<std::pair<int, int>, std::pair<int*, int>> frame_tables;   // (cascades, frames per launch) -> same, multi-frame order
+    std::map<int, DeviceArray<int>> item_tables;        // cascades per launch -> item table (capacity = item count)
+    std::map<std::pair<int, int>, DeviceArray<int>> frame_tables;   // (cascades, frames per launch) -> same, multi-frame order
     bool persistent = true;                             // OCEAN_PIPELINE=split selects the two-kernel path
     std::vector<ocean_cascade_params> pass_parameters;  // wave_generator.gd:14
     int pass_num_cascades_remaining = 0;                // wave_generator.gd:15
     uint64_t kernel_launches = 0;
     uint64_t cascade_updates = 0;
-    uint64_t device_bytes = 0;
-    unsigned* ray_bounds = nullptr;                     // ray cast scratch: [3 * num_cascades] per-layer bounds (first use)
-    ocean_ray* ray_in = nullptr;                        // ray cast staging for the host entry point, grown on demand
-    size_t ray_in_capacity = 0;
-    ocean_ray_hit* ray_out = nullptr;
-    size_t ray_out_capacity = 0;
+    DeviceArray<unsigned> ray_bounds;                   // ray cast scratch: [3 * num_cascades] per-layer bounds (first use)
+    DeviceArray<ocean_ray> ray_in;                      // ray cast staging for the host entry point
+    DeviceArray<ocean_ray_hit> ray_out;
 };
 
 namespace {
@@ -174,81 +178,52 @@ int enter_gen(ocean_generator* g, DeviceScope& scope) {
     DeviceScope device_scope__;          \
     int rc = enter_gen(gen, device_scope__)
 
+// At least n elements; the contents are not kept.
 template <typename T>
-cudaError_t dev_alloc(ocean_generator* g, T** p, size_t count) {
-    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(T));
-    if (e == cudaSuccess) g->device_bytes += count * sizeof(T);
-    return e;
+cudaError_t DeviceArray<T>::grow(ocean_generator* g, size_t n) {
+    if (n <= capacity) return cudaSuccess;
+    if (ptr) {
+        cudaError_t e = cudaStreamSynchronize(g->stream);    // an earlier call may still read the old block
+        if (e != cudaSuccess) return e;
+        release();
+    }
+    T* p = nullptr;
+    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&p), n * sizeof(T));
+    if (e != cudaSuccess) return e;
+    ptr = p;
+    capacity = n;
+    owner = g;
+    g->device_bytes += n * sizeof(T);
+    return cudaSuccess;
 }
 
-// A staging buffer of at least n elements (grown on demand; its contents are not kept).
+// grow(g, n), then the copy of n elements from host memory, enqueued on the generator's stream.
 template <typename T>
-int grow_buffer(ocean_generator* g, T** p, size_t* capacity, size_t n) {
-    if (n <= *capacity) return OCEAN_OK;
-    OCEAN_CUDA(cudaStreamSynchronize(g->stream));        // an earlier call may still read it
-    cudaFree(*p);
-    *p = nullptr;
-    g->device_bytes -= *capacity * sizeof(T);
-    *capacity = 0;
-    OCEAN_CUDA(dev_alloc(g, p, n));
-    *capacity = n;
-    return OCEAN_OK;
+cudaError_t DeviceArray<T>::upload(ocean_generator* g, const void* host, size_t n) {
+    cudaError_t e = grow(g, n);
+    if (e != cudaSuccess) return e;
+    return cudaMemcpyAsync(ptr, host, n * sizeof(T), cudaMemcpyHostToDevice, g->stream);
 }
 
+template <typename T>
+void DeviceArray<T>::release() {
+    if (!ptr) return;
+    cudaFree(ptr);
+    owner->device_bytes -= capacity * sizeof(T);
+    ptr = nullptr;
+    capacity = 0;
+}
+
+// Device memory is released by the generator's DeviceArrays; the rest is released here.
 void release(ocean_generator* g) {
     if (!g) return;
     DeviceScope scope;
     scope.enter(g->device);
     if (g->stream) cudaStreamSynchronize(g->stream);
-    cudaFree(g->buf.disp_table);
-    cudaFree(g->buf.disp_kvy);
-    cudaFree(g->d_tables);
     if (g->h_tables) cudaFreeHost(g->h_tables);
-    cudaFree(g->buf.spectrum);
-    cudaFree(g->buf.rowpass);
-    cudaFree(g->buf.displacement);
-    cudaFree(g->buf.normal);
-    cudaFree(g->buf.displacement_f32);
-    cudaFree(g->buf.normal_f32);
-    cudaFree(g->twiddles);
-    cudaFree(g->export_buf);
-    cudaFree(g->q_points);
-    cudaFree(g->q_disp);
-    cudaFree(g->q_grad);
-    cudaFree(g->q_scales);
-    cudaFree(g->snap_disp);
-    cudaFree(g->snap_normal);
     if (g->copy_stream) { cudaStreamSynchronize(g->copy_stream); cudaStreamDestroy(g->copy_stream); }
     if (g->snap_ready) cudaEventDestroy(g->snap_ready);
     if (g->snap_free) cudaEventDestroy(g->snap_free);
-    cudaFree(g->spray_counts);
-    cudaFree(g->spray_records);
-    cudaFree(g->surf_scratch);
-    cudaFree(g->surf_records);
-    cudaFree(g->ray_bounds);
-    cudaFree(g->ray_in);
-    cudaFree(g->ray_out);
-    cudaFree(g->buoy_bodies);
-    cudaFree(g->buoy_offsets);
-    cudaFree(g->buoy_results);
-    cudaFree(g->buoy_q);
-    cudaFree(g->buoy_samples);
-    cudaFree(g->buoy_points);
-    cudaFree(g->drag_velocities);
-    cudaFree(g->drag_areas);
-    cudaFree(g->drag_results);
-    cudaFree(g->sim_bodies);
-    cudaFree(g->sim_r2);
-    cudaFree(g->sim_states);
-    cudaFree(g->sim_transforms);
-    cudaFree(g->vel_scratch);
-    cudaFree(g->velocity);
-    cudaFree(g->velocity_f32);
-    cudaFree(g->d_cascade);
-    cudaFree(g->d_spectrum);
-    cudaFree(g->d_queue);
-    for (auto& kv : g->item_tables) cudaFree(kv.second.first);
-    for (auto& kv : g->frame_tables) cudaFree(kv.second.first);
     if (g->h_cascade) cudaFreeHost(g->h_cascade);
     if (g->h_spectrum) cudaFreeHost(g->h_spectrum);
     for (auto& ev : g->ring_done)
@@ -259,6 +234,26 @@ void release(ocean_generator* g) {
         if (ev) cudaEventDestroy(ev);
     if (g->stream) cudaStreamDestroy(g->stream);
     delete g;
+}
+
+// The persistent kernel's work-item table cached under `key`.  On first use build(out) makes it on the host (it returns
+// the item count, and fills `out` unless that is NULL) and it is uploaded; the table's capacity is its item count.
+template <typename Key, typename Build>
+cudaError_t item_table(ocean_generator* g, std::map<Key, DeviceArray<int>>& cache, const Key& key, Build build,
+                       const DeviceArray<int>** table) {
+    auto slot = cache.try_emplace(key);
+    if (slot.second) {
+        std::vector<int> host((size_t)build(nullptr));
+        build(host.data());
+        cudaError_t e = slot.first->second.upload(g, host.data(), host.size());
+        if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);        // host vector goes out of scope
+        if (e != cudaSuccess) {
+            cache.erase(slot.first);
+            return e;
+        }
+    }
+    *table = &slot.first->second;
+    return cudaSuccess;
 }
 
 // Push constants of wave_generator.gd:69-71 (spectrum_compute) with the binary64 -> binary32
@@ -397,7 +392,7 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
     auto fail_resync = [&](int code) {
         if (counters_touched) {
             cudaStreamSynchronize(g->stream);
-            cudaMemcpy(g->d_queue + 1, g->done_count.data(), sizeof(uint32_t) * g->done_count.size(), cudaMemcpyHostToDevice);
+            cudaMemcpy(g->d_queue.ptr + 1, g->done_count.data(), sizeof(uint32_t) * g->done_count.size(), cudaMemcpyHostToDevice);
         }
         return code;
     };
@@ -409,16 +404,16 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
     } while (0)
     if (g->profiling) RUN_CUDA(cudaEventRecord(g->prof[0], g->stream));
     if (n_dirty) {
-        RUN_CUDA(cudaMemcpyAsync(g->d_spectrum, hs, sizeof(ocean::SpectrumDispatch) * n_dirty, cudaMemcpyHostToDevice, g->stream));
-        RUN_CUDA(ocean::launch_spectrum_compute(g->buf, g->d_spectrum, n_dirty, g->stream));
+        RUN_CUDA(cudaMemcpyAsync(g->d_spectrum.ptr, hs, sizeof(ocean::SpectrumDispatch) * n_dirty, cudaMemcpyHostToDevice, g->stream));
+        RUN_CUDA(ocean::launch_spectrum_compute(g->buf, g->d_spectrum.ptr, n_dirty, g->stream));
     }
     if (n_tables) {
-        RUN_CUDA(cudaMemcpyAsync(g->d_tables, ht, sizeof(ocean::TableDispatch) * n_tables, cudaMemcpyHostToDevice, g->stream));
-        RUN_CUDA(ocean::launch_dispersion_tables(g->buf, g->d_tables, n_tables, g->stream));
+        RUN_CUDA(cudaMemcpyAsync(g->d_tables.ptr, ht, sizeof(ocean::TableDispatch) * n_tables, cudaMemcpyHostToDevice, g->stream));
+        RUN_CUDA(ocean::launch_dispersion_tables(g->buf, g->d_tables.ptr, n_tables, g->stream));
     }
     const bool two_kernel = !(g->persistent && !g->profiling);
     if (two_kernel)   // the persistent launch takes its dispatch records by value
-        RUN_CUDA(cudaMemcpyAsync(g->d_cascade, hc, sizeof(ocean::CascadeDispatch) * n, cudaMemcpyHostToDevice, g->stream));
+        RUN_CUDA(cudaMemcpyAsync(g->d_cascade.ptr, hc, sizeof(ocean::CascadeDispatch) * n, cudaMemcpyHostToDevice, g->stream));
     RUN_CUDA(cudaEventRecord(g->ring_done[slot], g->stream));
     int launched = 0;
     if (g->profiling) RUN_CUDA(cudaEventRecord(g->prof[1], g->stream));
@@ -426,29 +421,18 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
         // one persistent launch per <= kMaxPersistentCascades cascades (their dispatch records travel by value)
         for (int first = 0; first < n; first += ocean::kMaxPersistentCascades) {
             const int m = (n - first < ocean::kMaxPersistentCascades) ? n - first : ocean::kMaxPersistentCascades;
-            auto it = g->item_tables.find(m);
-            if (it == g->item_tables.end()) {
-                const int group = ocean::persistent_group(g->map_size), lag = ocean::persistent_lag(g->map_size);
-                const int total = ocean::build_item_table(g->map_size, m, group, lag, nullptr);
-                std::vector<int> host((size_t)total);
-                ocean::build_item_table(g->map_size, m, group, lag, host.data());
-                int* dev = nullptr;
-                RUN_CUDA(dev_alloc(g, &dev, (size_t)total));
-                cudaError_t ce = cudaMemcpyAsync(dev, host.data(), sizeof(int) * (size_t)total, cudaMemcpyHostToDevice, g->stream);
-                if (ce == cudaSuccess) ce = cudaStreamSynchronize(g->stream);        // host vector goes out of scope
-                if (ce != cudaSuccess) {
-                    cudaFree(dev);
-                    RUN_CUDA(ce);
-                }
-                it = g->item_tables.emplace(m, std::make_pair(dev, total)).first;
-            }
+            auto build = [&](int* out) {
+                return ocean::build_item_table(g->map_size, m, ocean::persistent_group(g->map_size), ocean::persistent_lag(g->map_size), out);
+            };
+            const DeviceArray<int>* table = nullptr;
+            RUN_CUDA(item_table(g, g->item_tables, m, build, &table));
             counters_touched = true;
-            RUN_CUDA(ocean::launch_cascade_update_persistent(g->buf, hc + first, m, g->stream, g->d_queue, it->second.first,
-                                                             it->second.second, g->resident_ctas));
+            RUN_CUDA(ocean::launch_cascade_update_persistent(g->buf, hc + first, m, g->stream, g->d_queue.ptr, table->ptr,
+                                                             (int)table->capacity, g->resident_ctas));
             launched += 1;
         }
     } else {
-        RUN_CUDA(ocean::launch_cascade_update(g->buf, g->d_cascade, n, g->stream, &launched, g->profiling ? g->prof[2] : nullptr,
+        RUN_CUDA(ocean::launch_cascade_update(g->buf, g->d_cascade.ptr, n, g->stream, &launched, g->profiling ? g->prof[2] : nullptr,
                                               g->profiling ? g->prof[4] : nullptr));
         // (the device-side completion counters are brought in step with the host mirror at the commit below)
     }
@@ -467,7 +451,7 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
         record_velocity_source(g, hc[k]);
     }
     if (two_kernel)
-        RUN_CUDA(cudaMemcpyAsync(g->d_queue + 1, g->done_count.data(), sizeof(uint32_t) * g->done_count.size(), cudaMemcpyHostToDevice, g->stream));
+        RUN_CUDA(cudaMemcpyAsync(g->d_queue.ptr + 1, g->done_count.data(), sizeof(uint32_t) * g->done_count.size(), cudaMemcpyHostToDevice, g->stream));
 #undef RUN_CUDA
     g->ring_next = (g->ring_next + 1) % kRing;
     g->kernel_launches += (uint64_t)launched + (n_dirty ? 1 : 0) + (n_tables ? 1 : 0);
@@ -562,18 +546,25 @@ int ocean_create(int device, int map_size, int num_cascades, ocean_generator** o
         }                                                                                                        \
     } while (0)
     CREATE_CUDA(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
-    CREATE_CUDA(dev_alloc(g, &g->buf.spectrum, C * NN));                  // wave_generator.gd:31
-    CREATE_CUDA(dev_alloc(g, &g->buf.rowpass, ocean::kScratchHalves * C * 2 * NN));               // replaces fft_buffer, :33
-    CREATE_CUDA(dev_alloc(g, &g->buf.displacement, C * NN));              // :34
-    CREATE_CUDA(dev_alloc(g, &g->buf.normal, C * NN));                    // :35
-    CREATE_CUDA(dev_alloc(g, &g->twiddles, (size_t)ocean::kTwiddleCount + 1));   // :32
-    CREATE_CUDA(dev_alloc(g, &g->buf.disp_table, C * (size_t)(map_size / 2 + 1) * map_size));   // one slot per cascade at most
-    CREATE_CUDA(dev_alloc(g, &g->buf.disp_kvy, C * (size_t)map_size));
-    CREATE_CUDA(dev_alloc(g, &g->d_cascade, C));
-    CREATE_CUDA(dev_alloc(g, &g->d_spectrum, C));
-    CREATE_CUDA(dev_alloc(g, &g->d_tables, C));
-    CREATE_CUDA(dev_alloc(g, &g->d_queue, 3 * C + 1));
-    CREATE_CUDA(cudaMemsetAsync(g->d_queue, 0, sizeof(int) * (3 * C + 1), g->stream));
+    CREATE_CUDA(g->spectrum.grow(g, C * NN));                             // wave_generator.gd:31
+    CREATE_CUDA(g->rowpass.grow(g, ocean::kScratchHalves * C * 2 * NN));  // replaces fft_buffer, :33
+    CREATE_CUDA(g->displacement.grow(g, C * NN));                         // :34
+    CREATE_CUDA(g->normal.grow(g, C * NN));                               // :35
+    CREATE_CUDA(g->twiddles.grow(g, (size_t)ocean::kTwiddleCount + 1));   // :32
+    CREATE_CUDA(g->disp_table.grow(g, C * (size_t)(map_size / 2 + 1) * map_size));   // one slot per cascade at most
+    CREATE_CUDA(g->disp_kvy.grow(g, C * (size_t)map_size));
+    CREATE_CUDA(g->d_cascade.grow(g, C));
+    CREATE_CUDA(g->d_spectrum.grow(g, C));
+    CREATE_CUDA(g->d_tables.grow(g, C));
+    CREATE_CUDA(g->d_queue.grow(g, 3 * C + 1));
+    g->buf.spectrum = g->spectrum.ptr;
+    g->buf.rowpass = g->rowpass.ptr;
+    g->buf.displacement = g->displacement.ptr;
+    g->buf.normal = g->normal.ptr;
+    g->buf.twiddles = g->twiddles.ptr;
+    g->buf.disp_table = g->disp_table.ptr;
+    g->buf.disp_kvy = g->disp_kvy.ptr;
+    CREATE_CUDA(cudaMemsetAsync(g->d_queue.ptr, 0, sizeof(int) * (3 * C + 1), g->stream));
     g->done_count.assign(3 * C, 0u);                  // [0, C): row-pass counters (scratch half 0), [C, 2C): column pass, [2C, 3C): row pass, half 1
     g->slot_key.assign(C, ocean_generator::TableKey{0.f, 0.f, 0.f});
     g->slot_valid.assign(C, 0);
@@ -602,11 +593,10 @@ int ocean_create(int device, int map_size, int num_cascades, ocean_generator** o
     CREATE_CUDA(cudaMemsetAsync(g->buf.normal, 0, sizeof(uint2) * C * NN, g->stream));
     g->buf.map_size = map_size;
     g->buf.num_cascades = num_cascades;
-    g->buf.twiddles = g->twiddles;
     CREATE_CUDA(ocean::make_rowpass_tensor_map(g->buf.rowpass, map_size, num_cascades, &g->buf.rowpass_tmap));
     CREATE_CUDA(ocean::configure_kernels(map_size));
     CREATE_CUDA(ocean::persistent_grid_size(map_size, &g->resident_ctas));
-    CREATE_CUDA(ocean::init_twiddles(g->twiddles, g->stream));            // fft_butterfly once, :52-54
+    CREATE_CUDA(ocean::init_twiddles(g->twiddles.ptr, g->stream));        // fft_butterfly once, :52-54
     g->kernel_launches += 1;
     CREATE_CUDA(cudaStreamSynchronize(g->stream));
 #undef CREATE_CUDA
@@ -753,27 +743,14 @@ int ocean_update_frames(ocean_generator* gen, double delta, ocean_cascade_params
                 rec[(size_t)f * count + i] = d;
             }
         }
-        auto key = std::make_pair(count, F);
-        auto it = gen->frame_tables.find(key);
-        if (it == gen->frame_tables.end()) {
-            const int total = ocean::build_item_table_frames(gen->map_size, count, F, nullptr);
-            std::vector<int> host((size_t)total);
-            ocean::build_item_table_frames(gen->map_size, count, F, host.data());
-            int* dev = nullptr;
-            OCEAN_CUDA(dev_alloc(gen, &dev, (size_t)total));
-            cudaError_t ce = cudaMemcpyAsync(dev, host.data(), sizeof(int) * (size_t)total, cudaMemcpyHostToDevice, gen->stream);
-            if (ce == cudaSuccess) ce = cudaStreamSynchronize(gen->stream);
-            if (ce != cudaSuccess) {
-                cudaFree(dev);
-                return fail(OCEAN_ERR_CUDA, "item table upload failed: %s", cudaGetErrorString(ce));
-            }
-            it = gen->frame_tables.emplace(key, std::make_pair(dev, total)).first;
-        }
-        cudaError_t le = ocean::launch_cascade_update_persistent(gen->buf, rec.data(), F * count, gen->stream, gen->d_queue, it->second.first,
-                                                                 it->second.second, gen->resident_ctas, true);
+        auto build = [&](int* out) { return ocean::build_item_table_frames(gen->map_size, count, F, out); };
+        const DeviceArray<int>* table = nullptr;
+        OCEAN_CUDA(item_table(gen, gen->frame_tables, std::make_pair(count, F), build, &table));
+        cudaError_t le = ocean::launch_cascade_update_persistent(gen->buf, rec.data(), F * count, gen->stream, gen->d_queue.ptr, table->ptr,
+                                                                 (int)table->capacity, gen->resident_ctas, true);
         if (le != cudaSuccess) {
             cudaStreamSynchronize(gen->stream);
-            cudaMemcpy(gen->d_queue + 1, gen->done_count.data(), sizeof(uint32_t) * gen->done_count.size(), cudaMemcpyHostToDevice);
+            cudaMemcpy(gen->d_queue.ptr + 1, gen->done_count.data(), sizeof(uint32_t) * gen->done_count.size(), cudaMemcpyHostToDevice);
             return fail(OCEAN_ERR_CUDA, "multi-frame launch failed: %s", cudaGetErrorString(le));
         }
         for (int i = 0; i < count; ++i) {
@@ -881,24 +858,24 @@ int ocean_snapshot_maps_to_host_async(ocean_generator* gen, int first, int count
         OCEAN_CUDA(cudaStreamCreateWithFlags(&gen->copy_stream, cudaStreamNonBlocking));
         OCEAN_CUDA(cudaEventCreateWithFlags(&gen->snap_ready, cudaEventDisableTiming));
         OCEAN_CUDA(cudaEventCreateWithFlags(&gen->snap_free, cudaEventDisableTiming));
-        OCEAN_CUDA(dev_alloc(gen, &gen->snap_disp, (size_t)gen->num_cascades * layer));
-        OCEAN_CUDA(dev_alloc(gen, &gen->snap_normal, (size_t)gen->num_cascades * layer));
     }
+    OCEAN_CUDA(gen->snap_disp.grow(gen, (size_t)gen->num_cascades * layer));
+    OCEAN_CUDA(gen->snap_normal.grow(gen, (size_t)gen->num_cascades * layer));
     // the snapshot buffers are free again once the previous hand-off has left the device
     if (gen->snap_busy) OCEAN_CUDA(cudaStreamWaitEvent(gen->stream, gen->snap_free, 0));
     if (displacement_host)
-        OCEAN_CUDA(cudaMemcpyAsync(gen->snap_disp + first * layer, gen->buf.displacement + first * layer, sizeof(uint2) * layer * count,
+        OCEAN_CUDA(cudaMemcpyAsync(gen->snap_disp.ptr + first * layer, gen->buf.displacement + first * layer, sizeof(uint2) * layer * count,
                                    cudaMemcpyDeviceToDevice, gen->stream));
     if (normal_host)
-        OCEAN_CUDA(cudaMemcpyAsync(gen->snap_normal + first * layer, gen->buf.normal + first * layer, sizeof(uint2) * layer * count,
+        OCEAN_CUDA(cudaMemcpyAsync(gen->snap_normal.ptr + first * layer, gen->buf.normal + first * layer, sizeof(uint2) * layer * count,
                                    cudaMemcpyDeviceToDevice, gen->stream));
     OCEAN_CUDA(cudaEventRecord(gen->snap_ready, gen->stream));
     OCEAN_CUDA(cudaStreamWaitEvent(gen->copy_stream, gen->snap_ready, 0));
     if (displacement_host)
-        OCEAN_CUDA(cudaMemcpyAsync(displacement_host, gen->snap_disp + first * layer, sizeof(uint2) * layer * count, cudaMemcpyDeviceToHost,
+        OCEAN_CUDA(cudaMemcpyAsync(displacement_host, gen->snap_disp.ptr + first * layer, sizeof(uint2) * layer * count, cudaMemcpyDeviceToHost,
                                    gen->copy_stream));
     if (normal_host)
-        OCEAN_CUDA(cudaMemcpyAsync(normal_host, gen->snap_normal + first * layer, sizeof(uint2) * layer * count, cudaMemcpyDeviceToHost,
+        OCEAN_CUDA(cudaMemcpyAsync(normal_host, gen->snap_normal.ptr + first * layer, sizeof(uint2) * layer * count, cudaMemcpyDeviceToHost,
                                    gen->copy_stream));
     OCEAN_CUDA(cudaEventRecord(gen->snap_free, gen->copy_stream));
     gen->snap_busy = true;
@@ -974,20 +951,18 @@ int ocean_enable_f32_taps(ocean_generator* gen, int enable) {
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     const size_t n = (size_t)gen->num_cascades * gen->map_size * gen->map_size;
     if (enable && !gen->buf.displacement_f32) {
-        OCEAN_CUDA(dev_alloc(gen, &gen->buf.displacement_f32, n));
-        OCEAN_CUDA(dev_alloc(gen, &gen->buf.normal_f32, n));
-        OCEAN_CUDA(cudaMemset(gen->buf.displacement_f32, 0, sizeof(float4) * n));
-        OCEAN_CUDA(cudaMemset(gen->buf.normal_f32, 0, sizeof(float4) * n));
+        // both maps exist and are cleared before the kernels see either
+        OCEAN_CUDA(gen->displacement_f32.grow(gen, n));
+        OCEAN_CUDA(gen->normal_f32.grow(gen, n));
+        OCEAN_CUDA(cudaMemset(gen->displacement_f32.ptr, 0, sizeof(float4) * n));
+        OCEAN_CUDA(cudaMemset(gen->normal_f32.ptr, 0, sizeof(float4) * n));
+        gen->buf.displacement_f32 = gen->displacement_f32.ptr;
+        gen->buf.normal_f32 = gen->normal_f32.ptr;
     } else if (!enable && gen->buf.displacement_f32) {
-        cudaFree(gen->buf.displacement_f32);
-        cudaFree(gen->buf.normal_f32);
         gen->buf.displacement_f32 = gen->buf.normal_f32 = nullptr;
-        gen->device_bytes -= 2 * sizeof(float4) * n;
-        if (gen->velocity_f32) {
-            cudaFree(gen->velocity_f32);
-            gen->velocity_f32 = nullptr;
-            gen->device_bytes -= sizeof(float4) * n;
-        }
+        gen->displacement_f32.release();
+        gen->normal_f32.release();
+        gen->velocity_f32.release();
     }
     return OCEAN_OK;
 }
@@ -1014,10 +989,10 @@ int ocean_copy_rowpass_to_host(ocean_generator* gen, int cascade, float* host) {
     // without the taps the column pass drops the scratch lines from L2 once it has consumed them (no DRAM write-back)
     if (!gen->buf.displacement_f32) return fail(OCEAN_ERR_STATE, "the row-pass scratch is only kept while the taps are on; call ocean_enable_f32_taps(gen, 1) before the update");
     const size_t layer = (size_t)gen->map_size * gen->map_size;
-    if (!gen->export_buf) OCEAN_CUDA(dev_alloc(gen, &gen->export_buf, 4 * layer));
-    OCEAN_CUDA(ocean::launch_rowpass_export(gen->buf, gen->scratch_layer_of[cascade], gen->export_buf, gen->stream));
+    OCEAN_CUDA(gen->export_buf.grow(gen, 4 * layer));
+    OCEAN_CUDA(ocean::launch_rowpass_export(gen->buf, gen->scratch_layer_of[cascade], gen->export_buf.ptr, gen->stream));
     gen->kernel_launches += 1;
-    OCEAN_CUDA(cudaMemcpyAsync(host, gen->export_buf, sizeof(float2) * 4 * layer, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(host, gen->export_buf.ptr, sizeof(float2) * 4 * layer, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1048,21 +1023,8 @@ int upload_scales(ocean_generator* gen, int num_cascades, const float* map_scale
     if (num_cascades < 1 || num_cascades > gen->num_cascades)
         return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_cascades %d outside [1, %d]", num_cascades, gen->num_cascades);
     if (!map_scales_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "map_scales is NULL");
-    if (!gen->q_scales) OCEAN_CUDA(dev_alloc(gen, &gen->q_scales, (size_t)gen->num_cascades));
-    OCEAN_CUDA(cudaMemcpyAsync(gen->q_scales, map_scales_host, sizeof(float4) * (size_t)num_cascades, cudaMemcpyHostToDevice, gen->stream));
-    return OCEAN_OK;
-}
-
-// The host-side query entry points stage their points (and the map-query outputs) in buffers they share, grown on demand.
-int grow_query_staging(ocean_generator* gen, size_t n) {
-    if (n <= gen->q_capacity) return OCEAN_OK;
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    cudaFree(gen->q_points); cudaFree(gen->q_disp); cudaFree(gen->q_grad);
-    gen->q_points = nullptr; gen->q_disp = gen->q_grad = nullptr; gen->q_capacity = 0;
-    OCEAN_CUDA(dev_alloc(gen, &gen->q_points, n));
-    OCEAN_CUDA(dev_alloc(gen, &gen->q_disp, 3 * n));
-    OCEAN_CUDA(dev_alloc(gen, &gen->q_grad, 3 * n));
-    gen->q_capacity = n;
+    OCEAN_CUDA(gen->q_scales.grow(gen, (size_t)gen->num_cascades));
+    OCEAN_CUDA(cudaMemcpyAsync(gen->q_scales.ptr, map_scales_host, sizeof(float4) * (size_t)num_cascades, cudaMemcpyHostToDevice, gen->stream));
     return OCEAN_OK;
 }
 }  // namespace
@@ -1075,7 +1037,7 @@ int ocean_sample_maps_device(ocean_generator* gen, int num_points, const float* 
     if (num_points == 0) return OCEAN_OK;
     if (!points_xz_dev || !displacement_dev || !gradient_foam_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
-    OCEAN_CUDA(ocean::launch_sample_maps(gen->buf, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_points, gen->q_scales,
+    OCEAN_CUDA(ocean::launch_sample_maps(gen->buf, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_points, gen->q_scales.ptr,
                                          displacement_dev, gradient_foam_dev, gen->stream));
     gen->kernel_launches += 1;
     return OCEAN_OK;
@@ -1089,13 +1051,14 @@ int ocean_sample_maps(ocean_generator* gen, int num_points, const float* points_
     if (num_points == 0) return OCEAN_OK;
     if (!points_xz_host || !displacement_host || !gradient_foam_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
     const size_t n = (size_t)num_points;
-    if ((rc = grow_query_staging(gen, n))) return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(gen->q_points, points_xz_host, sizeof(float2) * n, cudaMemcpyHostToDevice, gen->stream));
-    if ((rc = ocean_sample_maps_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points), num_cascades, map_scales_host,
-                                       gen->q_disp, gen->q_grad)))
+    OCEAN_CUDA(gen->q_disp.grow(gen, 3 * n));
+    OCEAN_CUDA(gen->q_grad.grow(gen, 3 * n));
+    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, n));
+    if ((rc = ocean_sample_maps_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points.ptr), num_cascades, map_scales_host,
+                                       gen->q_disp.ptr, gen->q_grad.ptr)))
         return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(displacement_host, gen->q_disp, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(gradient_foam_host, gen->q_grad, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(displacement_host, gen->q_disp.ptr, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(gradient_foam_host, gen->q_grad.ptr, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1143,19 +1106,12 @@ int ocean_extract_spray_device(ocean_generator* gen, int num_candidates, const f
     if (!points_xz_dev || !particle_scale || (max_records > 0 && !records_dev)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
     const int blocks = ocean::spray_blocks(num_candidates);
-    if (blocks + 1 > gen->spray_count_capacity) {
-        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-        cudaFree(gen->spray_counts);
-        gen->spray_counts = nullptr;
-        gen->spray_count_capacity = 0;
-        OCEAN_CUDA(dev_alloc(gen, &gen->spray_counts, (size_t)blocks + 1));
-        gen->spray_count_capacity = blocks + 1;
-    }
-    OCEAN_CUDA(ocean::launch_extract_spray(gen->buf, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_candidates, gen->q_scales,
-                                           make_float3(particle_scale[0], particle_scale[1], particle_scale[2]), gen->spray_counts, records_dev,
-                                           max_records, gen->stream));
+    OCEAN_CUDA(gen->spray_counts.grow(gen, (size_t)blocks + 1));
+    OCEAN_CUDA(ocean::launch_extract_spray(gen->buf, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_candidates,
+                                           gen->q_scales.ptr, make_float3(particle_scale[0], particle_scale[1], particle_scale[2]),
+                                           gen->spray_counts.ptr, records_dev, max_records, gen->stream));
     gen->kernel_launches += 3;
-    OCEAN_CUDA(cudaMemcpyAsync(num_active_dev, gen->spray_counts + blocks, sizeof(int), cudaMemcpyDeviceToDevice, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(num_active_dev, gen->spray_counts.ptr + blocks, sizeof(int), cudaMemcpyDeviceToDevice, gen->stream));
     return OCEAN_OK;
 }
 
@@ -1169,22 +1125,11 @@ int ocean_extract_spray(ocean_generator* gen, int num_candidates, const float* p
     *num_active = 0;
     if (num_candidates == 0) return OCEAN_OK;
     if (!points_xz_host || (max_records > 0 && !records_host)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    const size_t n = (size_t)num_candidates;
-    if ((rc = grow_query_staging(gen, n))) return rc;
-    const size_t rec_bytes = ((size_t)max_records + 1) * sizeof(ocean_spray_record);    // + one slot for the count
-    if (rec_bytes > gen->spray_record_capacity) {
-        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-        cudaFree(gen->spray_records);
-        gen->spray_records = nullptr;
-        gen->spray_record_capacity = 0;
-        OCEAN_CUDA(cudaMalloc(&gen->spray_records, rec_bytes));
-        gen->device_bytes += rec_bytes;
-        gen->spray_record_capacity = rec_bytes;
-    }
-    ocean_spray_record* recs = static_cast<ocean_spray_record*>(gen->spray_records);
+    OCEAN_CUDA(gen->spray_records.grow(gen, (size_t)max_records + 1));                 // + one slot for the count
+    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, (size_t)num_candidates));
+    ocean_spray_record* recs = gen->spray_records.ptr;
     int* count_dev = reinterpret_cast<int*>(recs + max_records);
-    OCEAN_CUDA(cudaMemcpyAsync(gen->q_points, points_xz_host, sizeof(float2) * n, cudaMemcpyHostToDevice, gen->stream));
-    if ((rc = ocean_extract_spray_device(gen, num_candidates, reinterpret_cast<const float*>(gen->q_points), num_cascades, map_scales_host,
+    if ((rc = ocean_extract_spray_device(gen, num_candidates, reinterpret_cast<const float*>(gen->q_points.ptr), num_cascades, map_scales_host,
                                          particle_scale, max_records, recs, count_dev)))
         return rc;
     int count = 0;
@@ -1211,17 +1156,9 @@ int check_surface_args(int num_points, float tolerance, int max_iterations) {
 // ocean_buoyancy_device).
 int run_query_surface(ocean_generator* gen, int num_points, const float2* points_xz_dev, int num_cascades, float tolerance,
                       int max_iterations, ocean_surface_sample* out_dev) {
-    const size_t ints = ocean::surface_scratch_ints(gen->num_cascades, num_points);
-    if (ints > gen->surf_scratch_capacity) {
-        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-        cudaFree(gen->surf_scratch);
-        gen->surf_scratch = nullptr;
-        gen->surf_scratch_capacity = 0;
-        OCEAN_CUDA(dev_alloc(gen, &gen->surf_scratch, ints));
-        gen->surf_scratch_capacity = ints;
-    }
-    OCEAN_CUDA(ocean::launch_query_surface(gen->buf, num_cascades, points_xz_dev, num_points, gen->q_scales, tolerance, max_iterations,
-                                           out_dev, gen->surf_scratch, gen->stream));
+    OCEAN_CUDA(gen->surf_scratch.grow(gen, ocean::surface_scratch_ints(gen->num_cascades, num_points)));
+    OCEAN_CUDA(ocean::launch_query_surface(gen->buf, num_cascades, points_xz_dev, num_points, gen->q_scales.ptr, tolerance, max_iterations,
+                                           out_dev, gen->surf_scratch.ptr, gen->stream));
     gen->kernel_launches += max_iterations > 0 ? 3 : 1;
     return OCEAN_OK;
 }
@@ -1246,20 +1183,12 @@ int ocean_query_surface(ocean_generator* gen, int num_points, const float* point
     if (num_points == 0) return OCEAN_OK;
     if (!points_xz_host || !out_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
     const size_t n = (size_t)num_points;
-    if ((rc = grow_query_staging(gen, n))) return rc;
-    if (n > gen->surf_record_capacity) {
-        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-        cudaFree(gen->surf_records);
-        gen->surf_records = nullptr;
-        gen->surf_record_capacity = 0;
-        OCEAN_CUDA(dev_alloc(gen, &gen->surf_records, n));
-        gen->surf_record_capacity = n;
-    }
-    OCEAN_CUDA(cudaMemcpyAsync(gen->q_points, points_xz_host, sizeof(float2) * n, cudaMemcpyHostToDevice, gen->stream));
-    if ((rc = ocean_query_surface_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points), num_cascades, map_scales_host,
-                                         tolerance, max_iterations, gen->surf_records)))
+    OCEAN_CUDA(gen->surf_records.grow(gen, n));
+    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, n));
+    if ((rc = ocean_query_surface_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points.ptr), num_cascades, map_scales_host,
+                                         tolerance, max_iterations, gen->surf_records.ptr)))
         return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->surf_records, sizeof(ocean_surface_sample) * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->surf_records.ptr, sizeof(ocean_surface_sample) * n, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1286,9 +1215,9 @@ int ocean_raycast_device(ocean_generator* gen, int num_rays, const ocean_ray* ra
     if (num_rays == 0) return OCEAN_OK;
     if (!rays_dev || !out_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
-    if (!gen->ray_bounds) OCEAN_CUDA(dev_alloc(gen, &gen->ray_bounds, 3 * (size_t)gen->num_cascades));
-    OCEAN_CUDA(ocean::launch_raycast(gen->buf, num_cascades, rays_dev, num_rays, gen->q_scales, step, max_samples, tolerance, max_iterations,
-                                     gen->ray_bounds, out_dev, gen->stream));
+    OCEAN_CUDA(gen->ray_bounds.grow(gen, 3 * (size_t)gen->num_cascades));
+    OCEAN_CUDA(ocean::launch_raycast(gen->buf, num_cascades, rays_dev, num_rays, gen->q_scales.ptr, step, max_samples, tolerance, max_iterations,
+                                     gen->ray_bounds.ptr, out_dev, gen->stream));
     gen->kernel_launches += 2;
     return OCEAN_OK;
 }
@@ -1301,13 +1230,12 @@ int ocean_raycast(ocean_generator* gen, int num_rays, const ocean_ray* rays_host
     if (num_rays == 0) return OCEAN_OK;
     if (!rays_host || !out_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
     const size_t n = (size_t)num_rays;
-    if ((rc = grow_buffer(gen, &gen->ray_in, &gen->ray_in_capacity, n))) return rc;
-    if ((rc = grow_buffer(gen, &gen->ray_out, &gen->ray_out_capacity, n))) return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(gen->ray_in, rays_host, sizeof(ocean_ray) * n, cudaMemcpyHostToDevice, gen->stream));
-    if ((rc = ocean_raycast_device(gen, num_rays, gen->ray_in, num_cascades, map_scales_host, step, max_samples, tolerance, max_iterations,
-                                   gen->ray_out)))
+    OCEAN_CUDA(gen->ray_out.grow(gen, n));
+    OCEAN_CUDA(gen->ray_in.upload(gen, rays_host, n));
+    if ((rc = ocean_raycast_device(gen, num_rays, gen->ray_in.ptr, num_cascades, map_scales_host, step, max_samples, tolerance, max_iterations,
+                                   gen->ray_out.ptr)))
         return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->ray_out, sizeof(ocean_ray_hit) * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->ray_out.ptr, sizeof(ocean_ray_hit) * n, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1347,14 +1275,14 @@ int check_buoyancy_args(int num_bodies, const ocean_buoyancy_body* bodies, int n
 }
 
 // The exclusive prefix of the bodies' num_points into gen->buoy_offsets_host (kept in the generator: the upload of it is
-// asynchronous), uploaded to gen->buoy_offsets (grown by the caller).
+// asynchronous), uploaded to gen->buoy_offsets.
 extern "C++" template <typename Body>
 int upload_offsets(ocean_generator* gen, int num_bodies, const Body* bodies_host) {
     const size_t B = (size_t)num_bodies;
     std::vector<int>& offsets = gen->buoy_offsets_host;
     offsets.resize(B);
     for (size_t b = 0, start = 0; b < B; start += (size_t)bodies_host[b].num_points, ++b) offsets[b] = (int)start;
-    OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_offsets, offsets.data(), sizeof(int) * B, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(gen->buoy_offsets.upload(gen, offsets.data(), B));
     return OCEAN_OK;
 }
 
@@ -1365,9 +1293,9 @@ int launch_buoyancy_sequence(ocean_generator* gen, const ocean_buoyancy_body* bo
                              ocean_buoyancy_result* results_dev, ocean_surface_sample* samples) {
     int rc;
     if (world > 0) {
-        OCEAN_CUDA(ocean::launch_buoyancy_transform(bodies_dev, offsets_dev, num_bodies, points_dev, world, gen->buoy_q, gen->stream));
+        OCEAN_CUDA(ocean::launch_buoyancy_transform(bodies_dev, offsets_dev, num_bodies, points_dev, world, gen->buoy_q.ptr, gen->stream));
         gen->kernel_launches += 1;
-        if ((rc = run_query_surface(gen, world, gen->buoy_q, num_cascades, tolerance, max_iterations, samples))) return rc;
+        if ((rc = run_query_surface(gen, world, gen->buoy_q.ptr, num_cascades, tolerance, max_iterations, samples))) return rc;
     }
     const float rho_g = density * 9.81f;                                 // G, wave_generator.gd:5, in binary32
     OCEAN_CUDA(ocean::launch_buoyancy_reduce(bodies_dev, offsets_dev, num_bodies, points_dev, samples, rho_g, tolerance, results_dev,
@@ -1383,16 +1311,13 @@ int run_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body
                  int num_cascades, float density, float tolerance, int max_iterations, ocean_buoyancy_result* results_dev,
                  ocean_surface_sample* samples_dev, ocean_surface_sample** samples_used) {
     int rc;
-    const size_t B = (size_t)num_bodies;
-    if ((rc = grow_buffer(gen, &gen->buoy_bodies, &gen->buoy_bodies_capacity, B))) return rc;
-    if ((rc = grow_buffer(gen, &gen->buoy_offsets, &gen->buoy_offsets_capacity, B))) return rc;
-    if ((rc = grow_buffer(gen, &gen->buoy_q, &gen->buoy_q_capacity, (size_t)world))) return rc;
-    if (!samples_dev && (rc = grow_buffer(gen, &gen->buoy_samples, &gen->buoy_samples_capacity, (size_t)world))) return rc;
-    ocean_surface_sample* samples = samples_dev ? samples_dev : gen->buoy_samples;
-    OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_bodies, bodies_host, sizeof(ocean_buoyancy_body) * B, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(gen->buoy_q.grow(gen, (size_t)world));
+    if (!samples_dev) OCEAN_CUDA(gen->buoy_samples.grow(gen, (size_t)world));
+    ocean_surface_sample* samples = samples_dev ? samples_dev : gen->buoy_samples.ptr;
+    OCEAN_CUDA(gen->buoy_bodies.upload(gen, bodies_host, (size_t)num_bodies));
     if ((rc = upload_offsets(gen, num_bodies, bodies_host))) return rc;
-    if ((rc = launch_buoyancy_sequence(gen, gen->buoy_bodies, gen->buoy_offsets, num_bodies, world, points_dev, num_cascades, density, tolerance,
-                                       max_iterations, results_dev, samples)))
+    if ((rc = launch_buoyancy_sequence(gen, gen->buoy_bodies.ptr, gen->buoy_offsets.ptr, num_bodies, world, points_dev, num_cascades, density,
+                                       tolerance, max_iterations, results_dev, samples)))
         return rc;
     if (samples_used) *samples_used = samples;
     return OCEAN_OK;
@@ -1422,19 +1347,15 @@ int ocean_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_bo
     if ((rc = check_buoyancy_args(num_bodies, bodies_host, num_points, density, tolerance, max_iterations, &world))) return rc;
     if (num_bodies == 0) return OCEAN_OK;
     if (!results_host || (world > 0 && !points_host)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    if ((rc = grow_buffer(gen, &gen->buoy_results, &gen->buoy_results_capacity, (size_t)num_bodies))) return rc;
-    if (world > 0) {
-        if ((rc = grow_buffer(gen, &gen->buoy_points, &gen->buoy_points_capacity, (size_t)num_points))) return rc;
-        OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_points, points_host, sizeof(ocean_buoyancy_point) * (size_t)num_points, cudaMemcpyHostToDevice,
-                                   gen->stream));
-    }
-    if ((rc = ocean_buoyancy_device(gen, num_bodies, bodies_host, num_points, world > 0 ? gen->buoy_points : nullptr, num_cascades,
-                                    map_scales_host, density, tolerance, max_iterations, gen->buoy_results, nullptr)))
+    OCEAN_CUDA(gen->buoy_results.grow(gen, (size_t)num_bodies));
+    if (world > 0) OCEAN_CUDA(gen->buoy_points.upload(gen, points_host, (size_t)num_points));
+    if ((rc = ocean_buoyancy_device(gen, num_bodies, bodies_host, num_points, world > 0 ? gen->buoy_points.ptr : nullptr, num_cascades,
+                                    map_scales_host, density, tolerance, max_iterations, gen->buoy_results.ptr, nullptr)))
         return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(results_host, gen->buoy_results, sizeof(ocean_buoyancy_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost,
+    OCEAN_CUDA(cudaMemcpyAsync(results_host, gen->buoy_results.ptr, sizeof(ocean_buoyancy_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost,
                                gen->stream));
     if (samples_host && world > 0)
-        OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
+        OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples.ptr, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
                                    gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
@@ -1446,17 +1367,17 @@ namespace {
 // A binary32 tap created while the taps are on is filled by recomputing every layer that has a source.
 int ensure_velocity(ocean_generator* gen) {
     const size_t n = (size_t)gen->num_cascades * gen->map_size * gen->map_size;
-    if (!gen->vel_scratch) {
-        OCEAN_CUDA(dev_alloc(gen, &gen->vel_scratch, n));
-        OCEAN_CUDA(ocean::init_velocity_twiddles(gen->twiddles, gen->stream));
+    if (!gen->vel_scratch.ptr) {
+        OCEAN_CUDA(gen->vel_scratch.grow(gen, n));
+        OCEAN_CUDA(ocean::init_velocity_twiddles(gen->twiddles.ptr, gen->stream));
     }
-    if (!gen->velocity) {
-        OCEAN_CUDA(dev_alloc(gen, &gen->velocity, n));
-        OCEAN_CUDA(cudaMemsetAsync(gen->velocity, 0, sizeof(uint2) * n, gen->stream));
+    if (!gen->velocity.ptr) {
+        OCEAN_CUDA(gen->velocity.grow(gen, n));
+        OCEAN_CUDA(cudaMemsetAsync(gen->velocity.ptr, 0, sizeof(uint2) * n, gen->stream));
     }
-    if (gen->buf.displacement_f32 && !gen->velocity_f32) {
-        OCEAN_CUDA(dev_alloc(gen, &gen->velocity_f32, n));
-        OCEAN_CUDA(cudaMemsetAsync(gen->velocity_f32, 0, sizeof(float4) * n, gen->stream));
+    if (gen->buf.displacement_f32 && !gen->velocity_f32.ptr) {
+        OCEAN_CUDA(gen->velocity_f32.grow(gen, n));
+        OCEAN_CUDA(cudaMemsetAsync(gen->velocity_f32.ptr, 0, sizeof(float4) * n, gen->stream));
         for (int i = 0; i < gen->num_cascades; ++i) gen->vel_stale[i] = gen->vel_has_source[i];
     }
     return OCEAN_OK;
@@ -1471,8 +1392,8 @@ int refresh_velocity(ocean_generator* gen, int* recomputed) {
         if (gen->vel_has_source[i] && gen->vel_stale[i]) jobs.push_back(gen->vel_source[i]);
     if (!jobs.empty()) {
         int launched = 0;
-        OCEAN_CUDA(ocean::launch_velocity(gen->buf, jobs.data(), (int)jobs.size(), gen->vel_scratch, gen->velocity, gen->velocity_f32,
-                                          gen->stream, &launched));
+        OCEAN_CUDA(ocean::launch_velocity(gen->buf, jobs.data(), (int)jobs.size(), gen->vel_scratch.ptr, gen->velocity.ptr,
+                                          gen->velocity_f32.ptr, gen->stream, &launched));
         gen->kernel_launches += (uint64_t)launched;
         for (const auto& j : jobs) gen->vel_stale[j.cascade] = 0;
     }
@@ -1492,7 +1413,7 @@ int ocean_get_velocity_map(ocean_generator* gen, void** velocity_dev, size_t* la
     OCEAN_ENTER(gen);
     if (rc) return rc;
     if ((rc = ensure_velocity(gen))) return rc;
-    if (velocity_dev) *velocity_dev = gen->velocity;
+    if (velocity_dev) *velocity_dev = gen->velocity.ptr;
     if (layer_bytes) *layer_bytes = sizeof(uint2) * (size_t)gen->map_size * gen->map_size;
     return OCEAN_OK;
 }
@@ -1506,7 +1427,7 @@ int ocean_copy_velocity_to_host(ocean_generator* gen, int first, int count, void
     if (!velocity_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "velocity_host is NULL");
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
     const size_t layer = (size_t)gen->map_size * gen->map_size;
-    OCEAN_CUDA(cudaMemcpyAsync(velocity_host, gen->velocity + first * layer, sizeof(uint2) * layer * count, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(velocity_host, gen->velocity.ptr + first * layer, sizeof(uint2) * layer * count, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1519,7 +1440,7 @@ int ocean_copy_f32_velocity_to_host(ocean_generator* gen, int cascade, float* ho
     if (!gen->buf.displacement_f32) return fail(OCEAN_ERR_STATE, "binary32 taps are disabled; call ocean_enable_f32_taps(gen, 1) first");
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
     const size_t layer = (size_t)gen->map_size * gen->map_size;
-    OCEAN_CUDA(cudaMemcpyAsync(host, gen->velocity_f32 + cascade * layer, sizeof(float4) * layer, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(host, gen->velocity_f32.ptr + cascade * layer, sizeof(float4) * layer, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1533,8 +1454,8 @@ int ocean_sample_velocity_device(ocean_generator* gen, int num_points, const flo
     if (!points_xz_dev || !velocity_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // validates before anything is launched
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
-    OCEAN_CUDA(ocean::launch_sample_velocity(gen->velocity, gen->map_size, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_points,
-                                             gen->q_scales, velocity_dev, gen->stream));
+    OCEAN_CUDA(ocean::launch_sample_velocity(gen->velocity.ptr, gen->map_size, num_cascades, reinterpret_cast<const float2*>(points_xz_dev),
+                                             num_points, gen->q_scales.ptr, velocity_dev, gen->stream));
     gen->kernel_launches += 1;
     return OCEAN_OK;
 }
@@ -1547,12 +1468,12 @@ int ocean_sample_velocity(ocean_generator* gen, int num_points, const float* poi
     if (num_points == 0) return OCEAN_OK;
     if (!points_xz_host || !velocity_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
     const size_t n = (size_t)num_points;
-    if ((rc = grow_query_staging(gen, n))) return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(gen->q_points, points_xz_host, sizeof(float2) * n, cudaMemcpyHostToDevice, gen->stream));
-    if ((rc = ocean_sample_velocity_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points), num_cascades, map_scales_host,
-                                           gen->q_disp)))
+    OCEAN_CUDA(gen->q_disp.grow(gen, 3 * n));
+    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, n));
+    if ((rc = ocean_sample_velocity_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points.ptr), num_cascades, map_scales_host,
+                                           gen->q_disp.ptr)))
         return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(velocity_host, gen->q_disp, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(velocity_host, gen->q_disp.ptr, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1588,16 +1509,15 @@ int ocean_body_forces_device(ocean_generator* gen, int num_bodies, const ocean_b
     if (!hydrostatic_dev || !drag_dev || (world > 0 && !points_dev)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
-    const size_t B = (size_t)num_bodies;
-    if ((rc = grow_buffer(gen, &gen->drag_velocities, &gen->drag_velocities_capacity, B))) return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(gen->drag_velocities, velocities_host, sizeof(ocean_body_velocity) * B, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(gen->drag_velocities.upload(gen, velocities_host, (size_t)num_bodies));
     ocean_surface_sample* samples = nullptr;
     if ((rc = run_buoyancy(gen, num_bodies, bodies_host, world, points_dev, num_cascades, density, tolerance, max_iterations, hydrostatic_dev,
                            samples_dev, &samples)))
         return rc;
     const float half_rho = 0.5f * density;
-    OCEAN_CUDA(ocean::launch_drag_reduce(gen->buoy_bodies, gen->drag_velocities, gen->buoy_offsets, num_bodies, points_dev, drag_areas_dev, samples,
-                                         gen->velocity, gen->map_size, num_cascades, gen->q_scales, half_rho, drag_dev, gen->stream));
+    OCEAN_CUDA(ocean::launch_drag_reduce(gen->buoy_bodies.ptr, gen->drag_velocities.ptr, gen->buoy_offsets.ptr, num_bodies, points_dev,
+                                         drag_areas_dev, samples, gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, half_rho,
+                                         drag_dev, gen->stream));
     gen->kernel_launches += 1;
     return OCEAN_OK;
 }
@@ -1614,24 +1534,22 @@ int ocean_body_forces(ocean_generator* gen, int num_bodies, const ocean_buoyancy
         return rc;
     if (num_bodies == 0) return OCEAN_OK;
     if (!hydrostatic_host || !drag_host || (world > 0 && !points_host)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    if ((rc = grow_buffer(gen, &gen->buoy_results, &gen->buoy_results_capacity, (size_t)num_bodies))) return rc;
-    if ((rc = grow_buffer(gen, &gen->drag_results, &gen->drag_results_capacity, (size_t)num_bodies))) return rc;
+    OCEAN_CUDA(gen->buoy_results.grow(gen, (size_t)num_bodies));
+    OCEAN_CUDA(gen->drag_results.grow(gen, (size_t)num_bodies));
     if (world > 0) {
-        if ((rc = grow_buffer(gen, &gen->buoy_points, &gen->buoy_points_capacity, (size_t)num_points))) return rc;
-        if ((rc = grow_buffer(gen, &gen->drag_areas, &gen->drag_areas_capacity, (size_t)num_points))) return rc;
-        OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_points, points_host, sizeof(ocean_buoyancy_point) * (size_t)num_points, cudaMemcpyHostToDevice,
-                                   gen->stream));
-        OCEAN_CUDA(cudaMemcpyAsync(gen->drag_areas, drag_areas_host, sizeof(float) * (size_t)num_points, cudaMemcpyHostToDevice, gen->stream));
+        OCEAN_CUDA(gen->buoy_points.upload(gen, points_host, (size_t)num_points));
+        OCEAN_CUDA(gen->drag_areas.upload(gen, drag_areas_host, (size_t)num_points));
     }
-    if ((rc = ocean_body_forces_device(gen, num_bodies, bodies_host, velocities_host, num_points, world > 0 ? gen->buoy_points : nullptr,
-                                       world > 0 ? gen->drag_areas : nullptr, num_cascades, map_scales_host, density, tolerance, max_iterations,
-                                       gen->buoy_results, gen->drag_results, nullptr)))
+    if ((rc = ocean_body_forces_device(gen, num_bodies, bodies_host, velocities_host, num_points, world > 0 ? gen->buoy_points.ptr : nullptr,
+                                       world > 0 ? gen->drag_areas.ptr : nullptr, num_cascades, map_scales_host, density, tolerance,
+                                       max_iterations, gen->buoy_results.ptr, gen->drag_results.ptr, nullptr)))
         return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(hydrostatic_host, gen->buoy_results, sizeof(ocean_buoyancy_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost,
+    OCEAN_CUDA(cudaMemcpyAsync(hydrostatic_host, gen->buoy_results.ptr, sizeof(ocean_buoyancy_result) * (size_t)num_bodies,
+                               cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(drag_host, gen->drag_results.ptr, sizeof(ocean_drag_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost,
                                gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(drag_host, gen->drag_results, sizeof(ocean_drag_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost, gen->stream));
     if (samples_host && world > 0)
-        OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
+        OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples.ptr, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
                                    gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
@@ -1684,38 +1602,37 @@ int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const oce
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
     const size_t B = (size_t)num_bodies;
-    if ((rc = grow_buffer(gen, &gen->sim_bodies, &gen->sim_bodies_capacity, B))) return rc;
-    if ((rc = grow_buffer(gen, &gen->sim_r2, &gen->sim_r2_capacity, B))) return rc;
-    if ((rc = grow_buffer(gen, &gen->buoy_bodies, &gen->buoy_bodies_capacity, B))) return rc;
-    if ((rc = grow_buffer(gen, &gen->buoy_offsets, &gen->buoy_offsets_capacity, B))) return rc;
-    if ((rc = grow_buffer(gen, &gen->drag_velocities, &gen->drag_velocities_capacity, B))) return rc;
-    if ((rc = grow_buffer(gen, &gen->buoy_q, &gen->buoy_q_capacity, (size_t)world))) return rc;
-    if ((rc = grow_buffer(gen, &gen->buoy_samples, &gen->buoy_samples_capacity, (size_t)world))) return rc;
+    OCEAN_CUDA(gen->sim_r2.grow(gen, B));
+    OCEAN_CUDA(gen->buoy_bodies.grow(gen, B));
+    OCEAN_CUDA(gen->drag_velocities.grow(gen, B));
+    OCEAN_CUDA(gen->buoy_q.grow(gen, (size_t)world));
+    OCEAN_CUDA(gen->buoy_samples.grow(gen, (size_t)world));
     if (!hydrostatic_dev) {
-        if ((rc = grow_buffer(gen, &gen->buoy_results, &gen->buoy_results_capacity, B))) return rc;
-        hydrostatic_dev = gen->buoy_results;
+        OCEAN_CUDA(gen->buoy_results.grow(gen, B));
+        hydrostatic_dev = gen->buoy_results.ptr;
     }
     if (!drag_dev) {
-        if ((rc = grow_buffer(gen, &gen->drag_results, &gen->drag_results_capacity, B))) return rc;
-        drag_dev = gen->drag_results;
+        OCEAN_CUDA(gen->drag_results.grow(gen, B));
+        drag_dev = gen->drag_results.ptr;
     }
-    OCEAN_CUDA(cudaMemcpyAsync(gen->sim_bodies, bodies_host, sizeof(ocean_floating_body) * B, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(gen->sim_bodies.upload(gen, bodies_host, B));
     if ((rc = upload_offsets(gen, num_bodies, bodies_host))) return rc;
-    OCEAN_CUDA(ocean::launch_bodies_prepare(gen->sim_bodies, states_dev, num_bodies, points_dev, gen->sim_r2, gen->buoy_bodies,
-                                            gen->drag_velocities, gen->stream));
+    ocean_floating_body* bodies = gen->sim_bodies.ptr;
+    ocean_buoyancy_body* poses = gen->buoy_bodies.ptr;
+    ocean_body_velocity* velocities = gen->drag_velocities.ptr;
+    OCEAN_CUDA(ocean::launch_bodies_prepare(bodies, states_dev, num_bodies, points_dev, gen->sim_r2.ptr, poses, velocities, gen->stream));
     gen->kernel_launches += 1;
     const float h = dt / (float)substeps;
     const float half_rho = 0.5f * density;
     for (int s = 0; s < substeps; ++s) {
-        if ((rc = launch_buoyancy_sequence(gen, gen->buoy_bodies, gen->buoy_offsets, num_bodies, world, points_dev, num_cascades, density,
-                                           tolerance, max_iterations, hydrostatic_dev, gen->buoy_samples)))
+        if ((rc = launch_buoyancy_sequence(gen, poses, gen->buoy_offsets.ptr, num_bodies, world, points_dev, num_cascades, density, tolerance,
+                                           max_iterations, hydrostatic_dev, gen->buoy_samples.ptr)))
             return rc;
-        OCEAN_CUDA(ocean::launch_drag_reduce(gen->buoy_bodies, gen->drag_velocities, gen->buoy_offsets, num_bodies, points_dev, drag_areas_dev,
-                                             gen->buoy_samples, gen->velocity, gen->map_size, num_cascades, gen->q_scales, half_rho, drag_dev,
-                                             gen->stream));
-        OCEAN_CUDA(ocean::launch_bodies_integrate(gen->sim_bodies, gen->sim_r2, num_bodies, hydrostatic_dev, drag_dev, density, h, states_dev,
-                                                  gen->buoy_bodies, gen->drag_velocities, s == substeps - 1 ? transforms_dev : nullptr,
-                                                  gen->stream));
+        OCEAN_CUDA(ocean::launch_drag_reduce(poses, velocities, gen->buoy_offsets.ptr, num_bodies, points_dev, drag_areas_dev,
+                                             gen->buoy_samples.ptr, gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, half_rho,
+                                             drag_dev, gen->stream));
+        OCEAN_CUDA(ocean::launch_bodies_integrate(bodies, gen->sim_r2.ptr, num_bodies, hydrostatic_dev, drag_dev, density, h, states_dev, poses,
+                                                  velocities, s == substeps - 1 ? transforms_dev : nullptr, gen->stream));
         gen->kernel_launches += 2;
     }
     return OCEAN_OK;
@@ -1734,28 +1651,27 @@ int ocean_simulate_bodies(ocean_generator* gen, int num_bodies, const ocean_floa
     if (num_bodies == 0) return OCEAN_OK;
     if (world > 0 && !points_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
     const size_t B = (size_t)num_bodies;
-    if ((rc = grow_buffer(gen, &gen->sim_states, &gen->sim_states_capacity, B))) return rc;
-    if ((rc = grow_buffer(gen, &gen->buoy_results, &gen->buoy_results_capacity, B))) return rc;
-    if ((rc = grow_buffer(gen, &gen->drag_results, &gen->drag_results_capacity, B))) return rc;
-    if (transforms_host && (rc = grow_buffer(gen, &gen->sim_transforms, &gen->sim_transforms_capacity, 12 * B))) return rc;
+    OCEAN_CUDA(gen->buoy_results.grow(gen, B));
+    OCEAN_CUDA(gen->drag_results.grow(gen, B));
+    if (transforms_host) OCEAN_CUDA(gen->sim_transforms.grow(gen, 12 * B));
     if (world > 0) {
-        if ((rc = grow_buffer(gen, &gen->buoy_points, &gen->buoy_points_capacity, (size_t)num_points))) return rc;
-        if ((rc = grow_buffer(gen, &gen->drag_areas, &gen->drag_areas_capacity, (size_t)num_points))) return rc;
-        OCEAN_CUDA(cudaMemcpyAsync(gen->buoy_points, points_host, sizeof(ocean_buoyancy_point) * (size_t)num_points, cudaMemcpyHostToDevice,
-                                   gen->stream));
-        OCEAN_CUDA(cudaMemcpyAsync(gen->drag_areas, drag_areas_host, sizeof(float) * (size_t)num_points, cudaMemcpyHostToDevice, gen->stream));
+        OCEAN_CUDA(gen->buoy_points.upload(gen, points_host, (size_t)num_points));
+        OCEAN_CUDA(gen->drag_areas.upload(gen, drag_areas_host, (size_t)num_points));
     }
-    OCEAN_CUDA(cudaMemcpyAsync(gen->sim_states, states_host, sizeof(ocean_body_state) * B, cudaMemcpyHostToDevice, gen->stream));
-    if ((rc = ocean_simulate_bodies_device(gen, num_bodies, bodies_host, gen->sim_states, num_points, world > 0 ? gen->buoy_points : nullptr,
-                                           world > 0 ? gen->drag_areas : nullptr, num_cascades, map_scales_host, density, dt, substeps, tolerance,
-                                           max_iterations, gen->buoy_results, gen->drag_results, transforms_host ? gen->sim_transforms : nullptr)))
+    OCEAN_CUDA(gen->sim_states.upload(gen, states_host, B));
+    if ((rc = ocean_simulate_bodies_device(gen, num_bodies, bodies_host, gen->sim_states.ptr, num_points, world > 0 ? gen->buoy_points.ptr : nullptr,
+                                           world > 0 ? gen->drag_areas.ptr : nullptr, num_cascades, map_scales_host, density, dt, substeps,
+                                           tolerance, max_iterations, gen->buoy_results.ptr, gen->drag_results.ptr,
+                                           transforms_host ? gen->sim_transforms.ptr : nullptr)))
         return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(states_host, gen->sim_states, sizeof(ocean_body_state) * B, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(states_host, gen->sim_states.ptr, sizeof(ocean_body_state) * B, cudaMemcpyDeviceToHost, gen->stream));
     if (hydrostatic_host)
-        OCEAN_CUDA(cudaMemcpyAsync(hydrostatic_host, gen->buoy_results, sizeof(ocean_buoyancy_result) * B, cudaMemcpyDeviceToHost, gen->stream));
-    if (drag_host) OCEAN_CUDA(cudaMemcpyAsync(drag_host, gen->drag_results, sizeof(ocean_drag_result) * B, cudaMemcpyDeviceToHost, gen->stream));
+        OCEAN_CUDA(cudaMemcpyAsync(hydrostatic_host, gen->buoy_results.ptr, sizeof(ocean_buoyancy_result) * B, cudaMemcpyDeviceToHost,
+                                   gen->stream));
+    if (drag_host)
+        OCEAN_CUDA(cudaMemcpyAsync(drag_host, gen->drag_results.ptr, sizeof(ocean_drag_result) * B, cudaMemcpyDeviceToHost, gen->stream));
     if (transforms_host)
-        OCEAN_CUDA(cudaMemcpyAsync(transforms_host, gen->sim_transforms, sizeof(float) * 12 * B, cudaMemcpyDeviceToHost, gen->stream));
+        OCEAN_CUDA(cudaMemcpyAsync(transforms_host, gen->sim_transforms.ptr, sizeof(float) * 12 * B, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1764,7 +1680,7 @@ int ocean_copy_twiddles_to_host(ocean_generator* gen, float* host) {
     OCEAN_ENTER(gen);
     if (rc) return rc;
     if (!host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "host is NULL");
-    OCEAN_CUDA(cudaMemcpyAsync(host, gen->twiddles, sizeof(float2) * (gen->map_size - 1), cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(host, gen->twiddles.ptr, sizeof(float2) * (gen->map_size - 1), cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1835,15 +1751,14 @@ int ocean_selftest_math(ocean_generator* gen, uint64_t* failures, uint64_t* test
     OCEAN_ENTER(gen);
     if (rc) return rc;
     if (!failures || !tested) return fail(OCEAN_ERR_INVALID_ARGUMENT, "NULL argument");
-    unsigned long long* d = nullptr;
-    OCEAN_CUDA(cudaMalloc(reinterpret_cast<void**>(&d), 2 * sizeof(unsigned long long)));
-    OCEAN_CUDA(cudaMemsetAsync(d, 0, 2 * sizeof(unsigned long long), gen->stream));
-    OCEAN_CUDA(ocean::launch_selftest_math(d, d + 1, gen->stream));
+    DeviceArray<unsigned long long> d;                  // freed and uncounted on every return
+    OCEAN_CUDA(d.grow(gen, 2));
+    OCEAN_CUDA(cudaMemsetAsync(d.ptr, 0, 2 * sizeof(unsigned long long), gen->stream));
+    OCEAN_CUDA(ocean::launch_selftest_math(d.ptr, d.ptr + 1, gen->stream));
     gen->kernel_launches += 1;
     unsigned long long h[2] = {0, 0};
-    OCEAN_CUDA(cudaMemcpyAsync(h, d, sizeof h, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(h, d.ptr, sizeof h, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    cudaFree(d);
     *failures = h[0];
     *tested = h[1];
     return OCEAN_OK;
@@ -1857,12 +1772,13 @@ int ocean_debug_device_math(ocean_generator* gen, int fn, int n, const float* a_
     if (n == 0) return OCEAN_OK;
     if (!a_host || !b_host || !out_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "NULL argument");
     // the query staging buffers: a and b in the first 2n floats of q_disp, the results in q_points
-    if ((rc = grow_query_staging(gen, (size_t)n))) return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(gen->q_disp, a_host, sizeof(float) * n, cudaMemcpyHostToDevice, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(gen->q_disp + n, b_host, sizeof(float) * n, cudaMemcpyHostToDevice, gen->stream));
-    OCEAN_CUDA(ocean::launch_debug_device_math(fn, n, gen->q_disp, gen->q_disp + n, gen->q_points, gen->stream));
+    OCEAN_CUDA(gen->q_points.grow(gen, (size_t)n));
+    OCEAN_CUDA(gen->q_disp.grow(gen, 2 * (size_t)n));
+    OCEAN_CUDA(cudaMemcpyAsync(gen->q_disp.ptr, a_host, sizeof(float) * n, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(gen->q_disp.ptr + n, b_host, sizeof(float) * n, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(ocean::launch_debug_device_math(fn, n, gen->q_disp.ptr, gen->q_disp.ptr + n, gen->q_points.ptr, gen->stream));
     gen->kernel_launches += 1;
-    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->q_points, sizeof(float2) * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->q_points.ptr, sizeof(float2) * n, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
