@@ -1,15 +1,101 @@
-"""Times the BASELINE.json configs beyond the bench default (GPU).  Prints one JSON object per config."""
-import json, math, os, sys, time
+"""Times the BASELINE.json configs beyond the bench default, and the consumer ops, on the GPU.  Prints one JSON object per
+config.
+
+    python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast]
+
+Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
+--query.  An unknown argument exits before anything touches the GPU."""
+import json
+import os
+import subprocess
+import sys
+import time
+from functools import partial
+
+import numpy as np
+import torch
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import godotoceanwaves_b200 as gow
 from bench import synth_params
+from godotoceanwaves_b200.native import check, load_library
+from oracle import bodies as ob
+from oracle import buoyancy as bu
+from oracle import drag as dr
+from oracle import raycast as rc
+
+DEV = torch.device("cuda", 0)
+
+
+def warmed_generator(N, C, updates, configure=None):
+    """A generator of C cascades of N x N after `updates` calls of update_all(0.02): (generator, parameters, map scales).
+    configure(parameters), when given, edits the parameters before the first update."""
+    g = gow.WaveGenerator()
+    g.map_size = N
+    g.init_gpu(max(2, C))
+    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
+    if configure:
+        configure(p)
+    for _ in range(updates):
+        g.update_all(0.02, p)
+    return g, p, gow.WaveGenerator.map_scales(p)
+
+
+def records(n, dtype):
+    """A device buffer for n records of the numpy `dtype`; read it back with .cpu().numpy().view(dtype)."""
+    return torch.empty(n * dtype.itemsize, dtype=torch.uint8, device=DEV)
+
+
+def upload(a):
+    """A numpy record array as a device buffer of its bytes."""
+    return torch.from_numpy(a.view(np.uint8).copy()).to(DEV)
+
+
+def seeded_points(n):
+    """n device-resident points (x, z) in [-300, 300]^2 m, from seed 1."""
+    return (torch.rand(n, 2, device=DEV, generator=torch.Generator(DEV).manual_seed(1)) * 600.0 - 300.0).contiguous()
+
+
+def timed(g, call, reps, warmup, setup=None):
+    """Milliseconds per call: setup(), `warmup` calls, a synchronise, then the generator's CUDA events around `reps` calls."""
+    if setup:
+        setup()
+    for _ in range(warmup):
+        call()
+    g.synchronize()
+    g.timer_start()
+    for _ in range(reps):
+        call()
+    return g.timer_stop() / reps
+
+
+def alternate(*windows, rounds=3):
+    """Runs the windows (callables returning milliseconds per call) in turn for `rounds` rounds, so that clock ramp-up and
+    neighbours hit each alike: one list of times per window."""
+    times = [[] for _ in windows]
+    for _ in range(rounds):
+        for window, t in zip(windows, times):
+            t.append(window())
+    return times
+
+
+def card(key="power_limit_and_max_sm_clock", fields="power.limit,clocks.max.sm"):
+    """The card's name and its current `fields` (a --query-gpu list), as the "gpu" and `key` entries of a result line."""
+    smi = subprocess.run(["nvidia-smi", f"--query-gpu={fields}", "--format=csv,noheader", "-i", "0"],
+                         stdout=subprocess.PIPE, text=True).stdout.strip()
+    return {"gpu": torch.cuda.get_device_name(0), key: smi}
+
+
+def update_result(label, N, C, frames, ms, bytes_per_texel):
+    texels = C * N * N * frames
+    return {"config": label, "map_size": N, "cascades": C, "frames": frames, "ms_total": ms, "us_per_frame": 1e3 * ms / frames,
+            "cascades_per_s": C * frames / (ms * 1e-3), "gtexels_per_s": texels / (ms * 1e-3) / 1e9,
+            "algorithmic_GBps": bytes_per_texel * texels / (ms * 1e-3) / 1e9}
+
 
 def run(N, C, frames, label, regen=False, fused=False):
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for _ in range(3):
-        g.update_all(0.02, p)
+    g, p, _ = warmed_generator(N, C, 3)
     if fused:
         g.update_frames(0.02, p, 70)    # item tables of the fused launches
     g.synchronize()
@@ -24,26 +110,22 @@ def run(N, C, frames, label, regen=False, fused=False):
                 q.wind_speed = U; q.fetch_length = F
         g.update_all(0.02, p)
     ms = g.timer_stop()
-    texels = C * N * N * frames
-    bytes_per_texel = 56.0 if regen else 40.0
-    out = {"config": label, "map_size": N, "cascades": C, "frames": frames, "ms_total": ms, "us_per_frame": 1e3 * ms / frames,
-           "cascades_per_s": C * frames / (ms * 1e-3), "gtexels_per_s": texels / (ms * 1e-3) / 1e9,
-           "algorithmic_GBps": bytes_per_texel * texels / (ms * 1e-3) / 1e9}
     g.free()
-    print(json.dumps(out), flush=True)
+    print(json.dumps(update_result(label, N, C, frames, ms, 56.0 if regen else 40.0)), flush=True)
+
 
 def run_sweep_batch(N, per_set, reps, label):
     """cfg5 as ONE batch: the 6 x 4 (U, F) grid points are 24 cascade sets of one generator; every step regenerates all 96
     spectra (one spectrum launch) and updates all maps (one persistent launch)."""
     grid = [(u, f) for u in (5.0, 10.0, 15.0, 20.0, 25.0, 30.0) for f in (1.0, 10.0, 100.0, 1000.0)]
     C = len(grid) * per_set
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(C)
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for s, (u, f) in enumerate(grid):
-        for c in range(per_set):
-            p[s * per_set + c].wind_speed = u; p[s * per_set + c].fetch_length = f
-    for _ in range(3):
-        g.update_all(0.02, p)
+
+    def configure(p):
+        for s, (u, f) in enumerate(grid):
+            for c in range(per_set):
+                p[s * per_set + c].wind_speed = u; p[s * per_set + c].fetch_length = f
+
+    g, p, _ = warmed_generator(N, C, 3, configure)
     g.synchronize()
     g.timer_start()
     for r in range(reps):
@@ -51,20 +133,14 @@ def run_sweep_batch(N, per_set, reps, label):
             q.should_generate_spectrum = True
         g.update_all(0.02, p)
     ms = g.timer_stop()
-    texels = C * N * N * reps
-    out = {"config": label, "map_size": N, "cascades": C, "frames": reps, "ms_total": ms, "us_per_frame": 1e3 * ms / reps,
-           "cascades_per_s": C * reps / (ms * 1e-3), "gtexels_per_s": texels / (ms * 1e-3) / 1e9,
-           "algorithmic_GBps": 56.0 * texels / (ms * 1e-3) / 1e9}
     g.free()
-    print(json.dumps(out), flush=True)
+    print(json.dumps(update_result(label, N, C, reps, ms, 56.0)), flush=True)
 
 
 def run_spectrum(N, C, reps, label):
     """k_spectrum_compute alone (spectrum_compute.glsl, a4): CUDA events around the launch (ocean_set_profiling), all C
     cascades dirty.  Algorithmic bytes: 16 B/texel written; the kernel is bound by the binary64 pipe (DETMATH), not by HBM."""
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(C)
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    g.update_all(0.02, p)
+    g, p, _ = warmed_generator(N, C, 1)
     g.set_profiling(True)
     tot = 0.0
     for _ in range(reps):
@@ -84,77 +160,35 @@ def run_spectrum(N, C, reps, label):
 
 def run_spray(N, C, particles, reps, label):
     """Spray-candidate op (sea_spray_particle.gdshader:80-94) on device-resident candidates: count + scan + write kernels."""
-    import ctypes
-    import numpy as np
-    import torch
-    from godotoceanwaves_b200.native import load_library, check
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for q in p:
-        q.whitecap = 0.9; q.foam_amount = 10.0
-    for _ in range(25):
-        g.update_all(0.02, p)
-    scales = gow.WaveGenerator.map_scales(p)
-    dev = torch.device("cuda", 0)
-    pts = torch.from_numpy(gow.WaveGenerator.spray_grid(particles, np.array([[40, 0, 0, 0], [0, 1, 0, 0], [0, 0, 40, 0]], np.float32))).to(dev)
-    recs = torch.empty(particles * 8, dtype=torch.float32, device=dev)
-    count = torch.zeros(1, dtype=torch.int32, device=dev)
+    def configure(p):
+        for q in p:
+            q.whitecap = 0.9; q.foam_amount = 10.0
+
+    g, _, scales = warmed_generator(N, C, 25, configure)
+    pts = torch.from_numpy(gow.WaveGenerator.spray_grid(particles, np.array([[40, 0, 0, 0], [0, 1, 0, 0], [0, 0, 40, 0]], np.float32))).to(DEV)
+    recs = records(particles, gow.WaveGenerator.SPRAY_RECORD)
+    count = torch.zeros(1, dtype=torch.int32, device=DEV)
     ps = np.array([1, 1, 1], np.float32)
     lib = load_library()
     call = lambda: check(lib.ocean_extract_spray_device(g.context, particles, pts.data_ptr(), C, scales.ctypes.data, ps.ctypes.data, particles,
                                                         recs.data_ptr(), count.data_ptr()))
-    for _ in range(3):
-        call()
-    g.synchronize()
-    g.timer_start()
-    for _ in range(reps):
-        call()
-    ms = g.timer_stop()
-    out = {"config": label, "map_size": N, "cascades": C, "candidates": particles, "active": int(count.item()), "us_per_call": 1e3 * ms / reps,
-           "mcandidates_per_s": particles / (ms / reps * 1e-3) / 1e6}
+    per = timed(g, call, reps, 3)
+    out = {"config": label, "map_size": N, "cascades": C, "candidates": particles, "active": int(count.item()), "us_per_call": 1e3 * per,
+           "mcandidates_per_s": particles / (per * 1e-3) / 1e6}
     g.free()
     print(json.dumps(out), flush=True)
 
 
-if not {"--buoyancy", "--velocity", "--drag", "--bodies", "--raycast"} & set(sys.argv):    # each of these runs its op (defined below) alone
-    run(256, 4, 2000, "cfg2 latency: one 256x256x4 set per launch (launch/latency-bound, L2-resident)")
-    run(256, 4, 2000, "cfg2 latency, fused frames (ocean_update_frames: 64 frames per launch)", fused=True)
-    run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, frame by frame")
-    run(512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, fused frames (ocean_update_frames)", fused=True)
-    run(1024, 8, 200, "cfg4 (1 GPU): 1024x1024x8")
-    run(256, 4, 300, "cfg5: 256x256x4 wind/fetch sweep, one grid point per step, spectrum regenerated every step", regen=True)
-    run_sweep_batch(256, 4, 50, "cfg5 batched: the 6x4 (U,F) grid = 24 sets x 4 cascades per step, all spectra regenerated every step")
-    run(128, 1, 2000, "cfg1 shape on GPU: 128x128x1")
-    run_spectrum(256, 128, 10, "spectrum generation alone: 128 cascades of 256x256, one launch")
-    run_spray(256, 4, 1 << 20, 50, "spray candidates: 2^20 grid candidates x 4 cascades of 256x256")
-
-
 def run_query(N, C, n_points, reps, label):
     """Map-query op (water.gdshader sampling contract) on device-resident points: kernel time only."""
-    import ctypes
-    import numpy as np
-    import torch
-    from godotoceanwaves_b200.native import load_library, check
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for _ in range(2):
-        g.update_all(0.02, p)
-    scales = gow.WaveGenerator.map_scales(p)
-    dev = torch.device("cuda", 0)
-    pts = (torch.rand(n_points, 2, device=dev) * 1000.0 - 500.0).contiguous()
-    disp = torch.empty(n_points, 3, device=dev)
-    grad = torch.empty(n_points, 3, device=dev)
+    g, _, scales = warmed_generator(N, C, 2)
+    pts = (torch.rand(n_points, 2, device=DEV) * 1000.0 - 500.0).contiguous()
+    disp = torch.empty(n_points, 3, device=DEV)
+    grad = torch.empty(n_points, 3, device=DEV)
     torch.cuda.synchronize()
     lib = load_library()
     call = lambda: check(lib.ocean_sample_maps_device(g.context, n_points, pts.data_ptr(), C, scales.ctypes.data, disp.data_ptr(), grad.data_ptr()))
-    for _ in range(3):
-        call()
-    g.synchronize()
-    g.timer_start()
-    for _ in range(reps):
-        call()
-    ms = g.timer_stop()
-    per = ms / reps
+    per = timed(g, call, reps, 3)
     gathered = n_points * C * 24 * 8           # 4 + 16 + 4 texel reads of 8 B per cascade and point
     out = {"config": label, "map_size": N, "cascades": C, "points": n_points, "us_per_call": 1e3 * per,
            "mpoints_per_s": n_points / (per * 1e-3) / 1e6, "gathered_GBps": gathered / (per * 1e-3) / 1e9,
@@ -167,36 +201,18 @@ def run_surface(N, C, n_points, reps, label, tolerance=1e-3, max_iterations=8):
     """Surface-query op (ocean_query_surface_device) on device-resident points: kernel time from CUDA events, against
     ocean_sample_maps_device on the same points in the same run.  restarted = points that took more than max_iterations
     steps, i.e. ran the restart kernel (a first start that stalls early and then converges on a restart is not counted)."""
-    import numpy as np
-    import torch
-    from godotoceanwaves_b200.native import load_library, check
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for _ in range(2):
-        g.update_all(0.02, p)
-    scales = gow.WaveGenerator.map_scales(p)
-    dev = torch.device("cuda", 0)
-    pts = (torch.rand(n_points, 2, device=dev, generator=torch.Generator(dev).manual_seed(1)) * 600.0 - 300.0).contiguous()
-    recs = torch.empty(n_points * 10, dtype=torch.int32, device=dev)        # ocean_surface_sample: 40 B
-    disp = torch.empty(n_points, 3, device=dev)
-    grad = torch.empty(n_points, 3, device=dev)
+    g, _, scales = warmed_generator(N, C, 2)
+    pts = seeded_points(n_points)
+    recs = records(n_points, gow.WaveGenerator.SURFACE_SAMPLE)
+    disp = torch.empty(n_points, 3, device=DEV)
+    grad = torch.empty(n_points, 3, device=DEV)
     torch.cuda.synchronize()
     lib = load_library()
     query = lambda: check(lib.ocean_query_surface_device(g.context, n_points, pts.data_ptr(), C, scales.ctypes.data, tolerance, max_iterations,
                                                          recs.data_ptr()))
     sample = lambda: check(lib.ocean_sample_maps_device(g.context, n_points, pts.data_ptr(), C, scales.ctypes.data, disp.data_ptr(), grad.data_ptr()))
-
-    def timed(call):
-        for _ in range(3):
-            call()
-        g.synchronize()
-        g.timer_start()
-        for _ in range(reps):
-            call()
-        return g.timer_stop() / reps
-
-    t_query, t_sample = timed(query), timed(sample)
-    t_query = min(t_query, timed(query))        # alternate: the first window also absorbs clock ramp-up
+    t_query, t_sample = timed(g, query, reps, 3), timed(g, sample, reps, 3)
+    t_query = min(t_query, timed(g, query, reps, 3))        # alternate: the first window also absorbs clock ramp-up
     rec = recs.cpu().numpy().view(gow.WaveGenerator.SURFACE_SAMPLE)
     out = {"config": label, "map_size": N, "cascades": C, "points": n_points, "tolerance": tolerance, "max_iterations": max_iterations,
            "us_per_call": 1e3 * t_query, "mpoints_per_s": n_points / (t_query * 1e-3) / 1e6, "sample_maps_us_per_call": 1e3 * t_sample,
@@ -209,8 +225,6 @@ def run_surface(N, C, n_points, reps, label, tolerance=1e-3, max_iterations=8):
 def _buoyancy_scene(n_bodies, per_body):
     """n_bodies bodies of per_body hull points each (points in [-2, 2]^3 m), random rotations, positions in [-300, 300] m
     around the surface: (bodies, hull) in the layouts of oracle/buoyancy.py."""
-    import numpy as np
-    from oracle import buoyancy as bu
     rng = np.random.default_rng(1)
     hull = np.zeros(n_bodies * per_body, bu.POINT)
     hull["position"] = rng.uniform(-2.0, 2.0, (len(hull), 3))
@@ -234,48 +248,23 @@ def run_buoyancy(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_iter
     """Buoyancy op (ocean_buoyancy_device) on device-resident hulls of `per_body` points per body: kernel time from CUDA
     events, against ocean_query_surface_device on the same world points in the same run, in alternating windows.  The card's
     name, power limit and max SM clock are read in the same run."""
-    import subprocess
-    import numpy as np
-    import torch
-    from godotoceanwaves_b200.native import load_library, check
-    from oracle import buoyancy as bu
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for _ in range(2):
-        g.update_all(0.02, p)
-    scales = gow.WaveGenerator.map_scales(p)
+    g, _, scales = warmed_generator(N, C, 2)
     bodies, hull = _buoyancy_scene(n_bodies, per_body)
     _, _, _, wp = bu.world_points(bodies, hull)
     n_points = len(wp)
-    dev = torch.device("cuda", 0)
-    hull_d = torch.from_numpy(hull.view(np.uint8).copy()).to(dev)
-    pts_d = torch.from_numpy(np.ascontiguousarray(wp[:, [0, 2]])).to(dev)
-    res_d = torch.empty(n_bodies * 12, dtype=torch.int32, device=dev)           # ocean_buoyancy_result: 48 B
-    recs_d = torch.empty(n_points * 10, dtype=torch.int32, device=dev)          # ocean_surface_sample: 40 B
+    hull_d = upload(hull)
+    pts_d = torch.from_numpy(np.ascontiguousarray(wp[:, [0, 2]])).to(DEV)
+    res_d = records(n_bodies, bu.RESULT)
+    recs_d = records(n_points, gow.WaveGenerator.SURFACE_SAMPLE)
     torch.cuda.synchronize()
     lib = load_library()
     buoy = lambda: check(lib.ocean_buoyancy_device(g.context, n_bodies, bodies.ctypes.data, len(hull), hull_d.data_ptr(), C, scales.ctypes.data,
                                                    1025.0, tolerance, max_iterations, res_d.data_ptr(), None))
     query = lambda: check(lib.ocean_query_surface_device(g.context, n_points, pts_d.data_ptr(), C, scales.ctypes.data, tolerance, max_iterations,
                                                          recs_d.data_ptr()))
-
-    def timed(call):
-        for _ in range(3):
-            call()
-        g.synchronize()
-        g.timer_start()
-        for _ in range(reps):
-            call()
-        return g.timer_stop() / reps
-
-    t_b, t_q = [], []
-    for _ in range(3):                          # alternating windows: clock ramp-up and neighbours hit both alike
-        t_b.append(timed(buoy))
-        t_q.append(timed(query))
+    t_b, t_q = alternate(lambda: timed(g, buoy, reps, 3), lambda: timed(g, query, reps, 3))
     res = res_d.cpu().numpy().view(bu.RESULT)
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                         stdout=subprocess.PIPE, text=True).stdout.strip()
-    out = {"config": label, "gpu": torch.cuda.get_device_name(0), "power_limit_and_max_sm_clock": smi, "map_size": N, "cascades": C,
+    out = {"config": label, **card(), "map_size": N, "cascades": C,
            "bodies": n_bodies, "points_per_body": per_body, "world_points": n_points, "tolerance": tolerance, "max_iterations": max_iterations,
            "buoyancy_us_per_call": [1e3 * v for v in t_b], "query_surface_us_per_call": [1e3 * v for v in t_q],
            "overhead_over_query": min(t_b) / min(t_q) - 1.0, "mpoints_per_s": n_points / (min(t_b) * 1e-3) / 1e6,
@@ -290,17 +279,7 @@ def run_body_forces(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_i
     device-resident hulls: CUDA events around each call, in alternating windows.  No velocity layer is stale inside the
     windows (the warm-up calls refresh them).  Reports both times, the overhead of the drag pass, and the fraction of world
     points that are submerged.  The card's name, power limit and max SM clock are read in the same run."""
-    import subprocess
-    import numpy as np
-    import torch
-    from godotoceanwaves_b200.native import load_library, check
-    from oracle import buoyancy as bu
-    from oracle import drag as dr
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for _ in range(2):
-        g.update_all(0.02, p)
-    scales = gow.WaveGenerator.map_scales(p)
+    g, _, scales = warmed_generator(N, C, 2)
     bodies, hull = _buoyancy_scene(n_bodies, per_body)
     rng = np.random.default_rng(2)
     vel = np.zeros(n_bodies, dr.VELOCITY)
@@ -308,11 +287,10 @@ def run_body_forces(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_i
     vel["angular"] = rng.uniform(-1.0, 1.0, (n_bodies, 3))
     cda = rng.uniform(0.01, 0.2, len(hull)).astype(np.float32)
     n_points = n_bodies * per_body
-    dev = torch.device("cuda", 0)
-    hull_d = torch.from_numpy(hull.view(np.uint8).copy()).to(dev)
-    cda_d = torch.from_numpy(cda).to(dev)
-    hyd_d = torch.empty(n_bodies * 12, dtype=torch.int32, device=dev)           # ocean_buoyancy_result: 48 B
-    drag_d = torch.empty(n_bodies * 8, dtype=torch.int32, device=dev)           # ocean_drag_result: 32 B
+    hull_d = upload(hull)
+    cda_d = torch.from_numpy(cda).to(DEV)
+    hyd_d = records(n_bodies, bu.RESULT)
+    drag_d = records(n_bodies, dr.RESULT)
     torch.cuda.synchronize()
     lib = load_library()
     forces = lambda: check(lib.ocean_body_forces_device(g.context, n_bodies, bodies.ctypes.data, vel.ctypes.data, len(hull), hull_d.data_ptr(),
@@ -320,26 +298,11 @@ def run_body_forces(N, C, n_bodies, per_body, reps, label, tolerance=1e-3, max_i
                                                         hyd_d.data_ptr(), drag_d.data_ptr(), None))
     buoy = lambda: check(lib.ocean_buoyancy_device(g.context, n_bodies, bodies.ctypes.data, len(hull), hull_d.data_ptr(), C, scales.ctypes.data,
                                                    1025.0, tolerance, max_iterations, hyd_d.data_ptr(), None))
-
-    def timed(call):
-        for _ in range(3):
-            call()
-        g.synchronize()
-        g.timer_start()
-        for _ in range(reps):
-            call()
-        return g.timer_stop() / reps
-
-    t_f, t_b = [], []
-    for _ in range(3):                          # alternating windows: clock ramp-up and neighbours hit both alike
-        t_f.append(timed(forces))
-        t_b.append(timed(buoy))
+    t_f, t_b = alternate(lambda: timed(g, forces, reps, 3), lambda: timed(g, buoy, reps, 3))
     _, drag, smp = g.body_forces(bodies, vel, hull, cda, scales, 1025.0, tolerance, max_iterations, return_samples=True)
     body, j, _, wp = bu.world_points(bodies, hull)
     f = bu.submerged_fraction(smp["displacement"][:, 1], wp[:, 1], hull["half_height"][bodies["first_point"][body] + j])
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                         stdout=subprocess.PIPE, text=True).stdout.strip()
-    out = {"config": label, "gpu": torch.cuda.get_device_name(0), "power_limit_and_max_sm_clock": smi, "map_size": N, "cascades": C,
+    out = {"config": label, **card(), "map_size": N, "cascades": C,
            "bodies": n_bodies, "points_per_body": per_body, "world_points": n_points, "tolerance": tolerance, "max_iterations": max_iterations,
            "body_forces_us_per_call": [1e3 * v for v in t_f], "buoyancy_us_per_call": [1e3 * v for v in t_b],
            "overhead_over_buoyancy": min(t_f) / min(t_b) - 1.0, "frac_points_submerged": float(np.mean(f > 0)),
@@ -354,13 +317,7 @@ def run_velocity(N, C, reps, label, sample_points=0):
     (which marks every layer stale) that is already queued on the stream, so the velocity kernels start right behind it.
     With sample_points, also one ocean_sample_velocity_device call against ocean_sample_maps_device on the same points.
     The card's name, power limit and SM clocks are read in the same run."""
-    import subprocess
-    import torch
-    from godotoceanwaves_b200.native import load_library, check
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for _ in range(3):
-        g.update_all(0.02, p)
+    g, p, scales = warmed_generator(N, C, 3)
     assert g.update_velocity() == C
     g.synchronize()
 
@@ -382,63 +339,26 @@ def run_velocity(N, C, reps, label, sample_points=0):
             assert n == C
         return tot / reps
 
-    t_u, t_v = [], []
-    for _ in range(3):                          # alternating windows: clock ramp-up and neighbours hit both alike
-        t_u.append(window_update())
-        t_v.append(window_velocity())
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                         stdout=subprocess.PIPE, text=True).stdout.strip()
+    t_u, t_v = alternate(window_update, window_velocity)
     texels = C * N * N
-    out = {"config": label, "gpu": torch.cuda.get_device_name(0), "power_limit_sm_clock_max_sm_clock": smi, "map_size": N, "cascades": C,
+    out = {"config": label, **card("power_limit_sm_clock_max_sm_clock", "power.limit,clocks.sm,clocks.max.sm"), "map_size": N, "cascades": C,
            "velocity_us_per_call": [1e3 * v for v in t_v], "update_all_us_per_call": [1e3 * v for v in t_u],
            "velocity_over_update": min(t_v) / min(t_u), "velocity_algorithmic_GBps": 24.0 * texels / (min(t_v) * 1e-3) / 1e9}
     if sample_points:
-        dev = torch.device("cuda", 0)
-        pts = (torch.rand(sample_points, 2, device=dev, generator=torch.Generator(dev).manual_seed(1)) * 600.0 - 300.0).contiguous()
-        vel = torch.empty(sample_points, 3, device=dev)
-        disp = torch.empty(sample_points, 3, device=dev)
-        grad = torch.empty(sample_points, 3, device=dev)
-        scales = gow.WaveGenerator.map_scales(p)
+        pts = seeded_points(sample_points)
+        vel = torch.empty(sample_points, 3, device=DEV)
+        disp = torch.empty(sample_points, 3, device=DEV)
+        grad = torch.empty(sample_points, 3, device=DEV)
         torch.cuda.synchronize()
         lib = load_library()
         sv = lambda: check(lib.ocean_sample_velocity_device(g.context, sample_points, pts.data_ptr(), C, scales.ctypes.data, vel.data_ptr()))
         sm = lambda: check(lib.ocean_sample_maps_device(g.context, sample_points, pts.data_ptr(), C, scales.ctypes.data, disp.data_ptr(),
                                                         grad.data_ptr()))
-
-        def timed(call):
-            for _ in range(3):
-                call()
-            g.synchronize()
-            g.timer_start()
-            for _ in range(reps):
-                call()
-            return g.timer_stop() / reps
-
-        t_s, t_m = [], []
-        for _ in range(3):
-            t_s.append(timed(sv))
-            t_m.append(timed(sm))
+        t_s, t_m = alternate(lambda: timed(g, sv, reps, 3), lambda: timed(g, sm, reps, 3))
         out.update({"sample_points": sample_points, "sample_velocity_us_per_call": [1e3 * v for v in t_s],
                     "sample_maps_us_per_call": [1e3 * v for v in t_m]})
     g.free()
     print(json.dumps(out), flush=True)
-
-
-if "--velocity" in sys.argv:
-    run_velocity(256, 4, 200, "velocity: 4 cascades of 256x256, every layer stale", sample_points=1 << 20)
-    run_velocity(256, 128, 50, "velocity: the bench workload, 128 cascades of 256x256, every layer stale")
-    run_velocity(1024, 8, 20, "velocity: 8 cascades of 1024x1024, every layer stale")
-    sys.exit(0)
-
-if "--buoyancy" in sys.argv:
-    run_buoyancy(256, 4, 1 << 14, 64, 50, "buoyancy: 2^14 bodies x 64 points over 4 cascades of 256x256")
-    run_buoyancy(1024, 8, 1 << 14, 64, 20, "buoyancy: 2^14 bodies x 64 points over 8 cascades of 1024x1024")
-    sys.exit(0)
-
-if "--drag" in sys.argv:
-    run_body_forces(256, 4, 1 << 14, 64, 50, "body forces: 2^14 bodies x 64 points over 4 cascades of 256x256")
-    run_body_forces(1024, 8, 1 << 14, 64, 20, "body forces: 2^14 bodies x 64 points over 8 cascades of 1024x1024")
-    sys.exit(0)
 
 
 def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, tolerance=1e-3, max_iterations=8):
@@ -448,19 +368,7 @@ def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, t
     (what the op saves a host).  Device times from CUDA events, the host loop from the wall clock after a synchronise; the
     states are restored before each window; alternating windows.  The card's name, power limit and max SM clock are read
     in the same run."""
-    import subprocess
-    import time
-    import numpy as np
-    import torch
-    from godotoceanwaves_b200.native import load_library, check
-    from oracle import bodies as ob
-    from oracle import buoyancy as bu
-    from oracle import drag as dr
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for _ in range(2):
-        g.update_all(0.02, p)
-    scales = gow.WaveGenerator.map_scales(p)
+    g, _, scales = warmed_generator(N, C, 2)
     table, hull = _buoyancy_scene(n_bodies, per_body)
     rng = np.random.default_rng(3)
     bodies = np.zeros(n_bodies, ob.BODY)
@@ -475,13 +383,12 @@ def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, t
     states["angular_velocity"] = rng.uniform(-1.0, 1.0, (n_bodies, 3))
     cda = rng.uniform(0.01, 0.2, len(hull)).astype(np.float32)
     pose, vel = ob.pose(bodies, states)
-    dev = torch.device("cuda", 0)
-    hull_d = torch.from_numpy(hull.view(np.uint8).copy()).to(dev)
-    cda_d = torch.from_numpy(cda).to(dev)
-    st0_d = torch.from_numpy(states.view(np.uint8).copy()).to(dev)
+    hull_d = upload(hull)
+    cda_d = torch.from_numpy(cda).to(DEV)
+    st0_d = upload(states)
     st_d = st0_d.clone()
-    hyd_d = torch.empty(n_bodies * 12, dtype=torch.int32, device=dev)           # ocean_buoyancy_result: 48 B
-    drag_d = torch.empty(n_bodies * 8, dtype=torch.int32, device=dev)           # ocean_drag_result: 32 B
+    hyd_d = records(n_bodies, bu.RESULT)
+    drag_d = records(n_bodies, dr.RESULT)
     torch.cuda.synchronize()
     lib = load_library()
     h = np.float32(dt) / np.float32(substeps)
@@ -497,16 +404,6 @@ def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, t
         for _ in range(substeps):
             forces_once(pose, vel)
 
-    def timed(call):
-        st_d.copy_(st0_d)
-        for _ in range(3):
-            call()
-        g.synchronize()
-        g.timer_start()
-        for _ in range(reps):
-            call()
-        return g.timer_stop() / reps
-
     def host_loop():
         s = states
         g.synchronize()
@@ -521,14 +418,9 @@ def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, t
                 s = ob.step(bodies, s, r2, hyd, drg, 1025.0, h)
         return (time.perf_counter() - t0) * 1e3 / max(1, reps // 10)
 
-    t_s, t_f, t_h = [], [], []
-    for _ in range(3):                          # alternating windows: clock ramp-up and neighbours hit both alike
-        t_s.append(timed(sim))
-        t_f.append(timed(forces))
-        t_h.append(host_loop())
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                         stdout=subprocess.PIPE, text=True).stdout.strip()
-    out = {"config": label, "gpu": torch.cuda.get_device_name(0), "power_limit_and_max_sm_clock": smi, "map_size": N, "cascades": C,
+    restore = lambda: st_d.copy_(st0_d)
+    t_s, t_f, t_h = alternate(lambda: timed(g, sim, reps, 3, restore), lambda: timed(g, forces, reps, 3, restore), host_loop)
+    out = {"config": label, **card(), "map_size": N, "cascades": C,
            "bodies": n_bodies, "points_per_body": per_body, "substeps": substeps, "dt": dt, "max_iterations": max_iterations,
            "simulate_us_per_call": [1e3 * v for v in t_s], "S_x_body_forces_us": [1e3 * v for v in t_f],
            "host_loop_us_per_call": [1e3 * v for v in t_h], "overhead_over_S_x_body_forces": min(t_s) / min(t_f) - 1.0,
@@ -537,16 +429,8 @@ def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, t
     print(json.dumps(out), flush=True)
 
 
-if "--bodies" in sys.argv:
-    for S in (1, 4):
-        run_bodies(256, 4, 1 << 14, 64, S, 50, f"floating bodies: 2^14 bodies x 64 points, {S} sub-step(s) of 1/60 s, 4 cascades of 256x256")
-        run_bodies(1024, 8, 1 << 14, 64, S, 20, f"floating bodies: 2^14 bodies x 64 points, {S} sub-step(s) of 1/60 s, 8 cascades of 1024x1024")
-    sys.exit(0)
-
 def _picking_rays(side, y=12.0, fov_deg=90.0, pitch_deg=-20.0):
     """side x side camera rays from (0, y, 0) through a square image plane of fov_deg pitched pitch_deg: (RAY array)."""
-    import numpy as np
-    from oracle import raycast as rc
     f = np.tan(np.radians(fov_deg) / 2.0)
     u = (np.arange(side) + 0.5) / side * 2.0 - 1.0
     U, V = np.meshgrid(u * f, u * f)
@@ -562,8 +446,6 @@ def _picking_rays(side, y=12.0, fov_deg=90.0, pitch_deg=-20.0):
 
 def _projectile_rays(n, seed=1):
     """n rays 30 to 90 degrees down from 5 to 50 m over [-300, 300]^2 m"""
-    import numpy as np
-    from oracle import raycast as rc
     rng = np.random.default_rng(seed)
     p = np.radians(rng.uniform(-90.0, -30.0, n))
     yaw = rng.uniform(0.0, 2.0 * np.pi, n)
@@ -579,50 +461,25 @@ def run_raycast(N, C, reps, label, step=0.5, max_samples=1024, tolerance=1e-3, m
     through a 1024 x 1024 grid over a 90 degree field of view pitched 20 degrees down, (b) 2^16 projectile rays 30 to 90
     degrees down from 5 to 50 m.  CUDA events around each call, best of three windows alternating with
     ocean_query_surface_device on 2^20 points.  The card's name, power limit and max SM clock are read in the same run."""
-    import subprocess
-    import numpy as np
-    import torch
-    from godotoceanwaves_b200.native import load_library, check
-    from oracle import raycast as rc
-    g = gow.WaveGenerator(); g.map_size = N; g.init_gpu(max(2, C))
-    p = [synth_params(gow.WaveCascadeParameters, c) for c in range(C)]
-    for _ in range(2):
-        g.update_all(0.02, p)
-    scales = gow.WaveGenerator.map_scales(p)
-    dev = torch.device("cuda", 0)
+    g, _, scales = warmed_generator(N, C, 2)
     lib = load_library()
     n_pts = 1 << 20
-    pts = (torch.rand(n_pts, 2, device=dev, generator=torch.Generator(dev).manual_seed(1)) * 600.0 - 300.0).contiguous()
-    recs = torch.empty(n_pts * 10, dtype=torch.int32, device=dev)
+    pts = seeded_points(n_pts)
+    recs = records(n_pts, gow.WaveGenerator.SURFACE_SAMPLE)
     query = lambda: check(lib.ocean_query_surface_device(g.context, n_pts, pts.data_ptr(), C, scales.ctypes.data, tolerance, max_iterations,
                                                          recs.data_ptr()))
-
-    def timed(call):
-        for _ in range(2):
-            call()
-        g.synchronize()
-        g.timer_start()
-        for _ in range(reps):
-            call()
-        return g.timer_stop() / reps
-
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                         stdout=subprocess.PIPE, text=True).stdout.strip()
+    gpu = card()
     for scene, rays in (("picking: 2^20 rays, camera 12 m up, 90 deg fov pitched 20 deg down", _picking_rays(1024)),
                         ("projectiles: 2^16 rays 30-90 deg down from 5-50 m", _projectile_rays(1 << 16))):
         n = len(rays)
-        rays_d = torch.from_numpy(rays.view(np.uint8).copy()).to(dev)
-        out_d = torch.empty(n * 18, dtype=torch.int32, device=dev)
+        rays_d = upload(rays)
+        out_d = records(n, rc.HIT)
         cast = lambda: check(lib.ocean_raycast_device(g.context, n, rays_d.data_ptr(), C, scales.ctypes.data, step, max_samples, tolerance,
                                                       max_iterations, out_d.data_ptr()))
-        t_r, t_q = [], []
-        for _ in range(3):                      # alternating windows: clock ramp-up and neighbours hit both alike
-            t_r.append(timed(cast))
-            t_q.append(timed(query))
+        t_r, t_q = alternate(lambda: timed(g, cast, reps, 2), lambda: timed(g, query, reps, 2))
         hit = out_d.cpu().numpy().view(rc.HIT)
         st = hit["status"]
-        ev = np.maximum(hit["evaluations"], 1)
-        out = {"config": label, "scene": scene, "gpu": torch.cuda.get_device_name(0), "power_limit_and_max_sm_clock": smi, "map_size": N,
+        out = {"config": label, "scene": scene, **gpu, "map_size": N,
                "cascades": C, "rays": n, "step": step, "max_samples": max_samples, "tolerance": tolerance, "max_iterations": max_iterations,
                "raycast_us_per_call": [1e3 * v for v in t_r], "best_us": 1e3 * min(t_r), "mrays_per_s": n / (min(t_r) * 1e-3) / 1e6,
                "query_surface_2e20_us_per_call": [1e3 * v for v in t_q], "mean_evaluations": float(hit["evaluations"].mean()),
@@ -636,13 +493,61 @@ def run_raycast(N, C, reps, label, step=0.5, max_samples=1024, tolerance=1e-3, m
     g.free()
 
 
-if "--raycast" in sys.argv:
-    run_raycast(256, 4, 20, "ray cast over 4 cascades of 256x256")
-    run_raycast(1024, 8, 10, "ray cast over 8 cascades of 1024x1024")
-    sys.exit(0)
+GROUPS = {          # flag: its configs, in the order they run
+    "--updates": [
+        partial(run, 256, 4, 2000, "cfg2 latency: one 256x256x4 set per launch (launch/latency-bound, L2-resident)"),
+        partial(run, 256, 4, 2000, "cfg2 latency, fused frames (ocean_update_frames: 64 frames per launch)", fused=True),
+        partial(run, 512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, frame by frame"),
+        partial(run, 512, 4, 1000, "cfg3: 512x512x4, 1000-frame foam accumulate/decay loop, fused frames (ocean_update_frames)", fused=True),
+        partial(run, 1024, 8, 200, "cfg4 (1 GPU): 1024x1024x8"),
+        partial(run, 256, 4, 300, "cfg5: 256x256x4 wind/fetch sweep, one grid point per step, spectrum regenerated every step", regen=True),
+        partial(run_sweep_batch, 256, 4, 50, "cfg5 batched: the 6x4 (U,F) grid = 24 sets x 4 cascades per step, all spectra regenerated every step"),
+        partial(run, 128, 1, 2000, "cfg1 shape on GPU: 128x128x1"),
+        partial(run_spectrum, 256, 128, 10, "spectrum generation alone: 128 cascades of 256x256, one launch"),
+        partial(run_spray, 256, 4, 1 << 20, 50, "spray candidates: 2^20 grid candidates x 4 cascades of 256x256"),
+    ],
+    "--query": [
+        partial(run_query, 256, 4, 1 << 20, 50, "query op: 2^20 random points x 4 cascades of 256x256 (maps L2-resident)"),
+        partial(run_query, 1024, 8, 1 << 20, 20, "query op: 2^20 random points x 8 cascades of 1024x1024 (maps 128 MiB)"),
+        partial(run_surface, 256, 4, 1 << 20, 50, "surface query: 2^20 points in [-300, 300]^2 m x 4 cascades of 256x256"),
+        partial(run_surface, 1024, 8, 1 << 20, 20, "surface query: 2^20 points in [-300, 300]^2 m x 8 cascades of 1024x1024"),
+    ],
+    "--velocity": [
+        partial(run_velocity, 256, 4, 200, "velocity: 4 cascades of 256x256, every layer stale", sample_points=1 << 20),
+        partial(run_velocity, 256, 128, 50, "velocity: the bench workload, 128 cascades of 256x256, every layer stale"),
+        partial(run_velocity, 1024, 8, 20, "velocity: 8 cascades of 1024x1024, every layer stale"),
+    ],
+    "--buoyancy": [
+        partial(run_buoyancy, 256, 4, 1 << 14, 64, 50, "buoyancy: 2^14 bodies x 64 points over 4 cascades of 256x256"),
+        partial(run_buoyancy, 1024, 8, 1 << 14, 64, 20, "buoyancy: 2^14 bodies x 64 points over 8 cascades of 1024x1024"),
+    ],
+    "--drag": [
+        partial(run_body_forces, 256, 4, 1 << 14, 64, 50, "body forces: 2^14 bodies x 64 points over 4 cascades of 256x256"),
+        partial(run_body_forces, 1024, 8, 1 << 14, 64, 20, "body forces: 2^14 bodies x 64 points over 8 cascades of 1024x1024"),
+    ],
+    "--bodies": [
+        partial(run_bodies, N, C, 1 << 14, 64, S, reps,
+                f"floating bodies: 2^14 bodies x 64 points, {S} sub-step(s) of 1/60 s, {C} cascades of {N}x{N}")
+        for S in (1, 4) for N, C, reps in ((256, 4, 50), (1024, 8, 20))
+    ],
+    "--raycast": [
+        partial(run_raycast, 256, 4, 20, "ray cast over 4 cascades of 256x256"),
+        partial(run_raycast, 1024, 8, 10, "ray cast over 8 cascades of 1024x1024"),
+    ],
+}
+DEFAULT = ("--updates", "--query")
 
-if "--query" in sys.argv or os.environ.get("OCEAN_RUN_QUERY", "1") != "0":
-    run_query(256, 4, 1 << 20, 50, "query op: 2^20 random points x 4 cascades of 256x256 (maps L2-resident)")
-    run_query(1024, 8, 1 << 20, 20, "query op: 2^20 random points x 8 cascades of 1024x1024 (maps 128 MiB)")
-    run_surface(256, 4, 1 << 20, 50, "surface query: 2^20 points in [-300, 300]^2 m x 4 cascades of 256x256")
-    run_surface(1024, 8, 1 << 20, 20, "surface query: 2^20 points in [-300, 300]^2 m x 8 cascades of 1024x1024")
+
+def main(args):
+    unknown = [a for a in args if a not in GROUPS]
+    if unknown:
+        sys.exit(f"{os.path.basename(__file__)}: unknown argument(s) {' '.join(unknown)}; the flags are {' '.join(GROUPS)}")
+    chosen = set(args or DEFAULT)
+    for flag, configs in GROUPS.items():
+        if flag in chosen:
+            for config in configs:
+                config()
+
+
+if __name__ == "__main__":
+    main(sys.argv[1:])
