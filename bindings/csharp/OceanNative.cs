@@ -41,6 +41,29 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanSprayEmitter                          // struct ocean_spray_emitter (88 B) <- main.tscn:133-140
+    {
+        public int amount;                                          // GPUParticles3D.amount
+        public int num_particles;                                   // the shader's num_particles uniform (grid side sqrt)
+        public fixed float emission_transform[12];                  // 3 x 4 row-major, basis columns then origin
+        public fixed float particle_scale[3];
+        public float lifetime, lifetime_randomness;
+        public uint random_seed;
+        public double emitter_lifetime;                             // GPUParticles3D.lifetime (LIFETIME)
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanSprayParticle                         // struct ocean_spray_particle (120 B); all zero = never emitted
+    {
+        public fixed float transform[12];                           // 3 x 4 row-major like the instances
+        public fixed float custom[4];
+        public fixed float userdata1[4];                            // START_POS, START_TIME
+        public fixed float userdata2[4];                            // PARTICLE_SCALE, PARTICLE_LIFETIME
+        public fixed float userdata3[4];                            // .z SCALE_FACTOR, .w HAS_STARTED
+        public uint number, flags;                                  // flags: 1 ACTIVE, 2 EMITTED
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public unsafe struct OceanSurfaceSample                         // struct ocean_surface_sample (40 B) <- water.gdshader:28,37 inverted
     {
         public float source_x, source_z;
@@ -202,6 +225,17 @@ namespace OceanB200
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_extract_spray(IntPtr handle, int num_candidates, float* points_xz, int num_cascades, float* map_scales,
                                                         float* particle_scale, int max_records, OceanSprayRecord* records, int* num_active);
+        // spray particles: one particle-process frame [t0, t1) of the emitter; instances [num_live][16] for multimesh_set_buffer
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_default_spray_emitter(OceanSprayEmitter* emitter);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_spray_particles(IntPtr handle, OceanSprayEmitter* emitter, double t0, double t1, int num_cascades,
+                                                          float* map_scales, OceanSprayParticle* states, int max_instances, float* instances,
+                                                          int* num_live);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_spray_particles_device(IntPtr handle, OceanSprayEmitter* emitter, double t0, double t1, int num_cascades,
+                                                                 float* map_scales, void* states_dev, int max_instances, void* instances_dev,
+                                                                 void* num_live_dev);
         // surface query: the surface at world positions points [n][2] (P + D_xz(P) = Q solved for P, then the map query at P)
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,

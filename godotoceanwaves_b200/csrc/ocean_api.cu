@@ -87,6 +87,8 @@ struct ocean_generator {
     DeviceArray<float4> q_scales;
     DeviceArray<int> spray_counts;                      // spray op scratch: block counts / offsets (+ total)
     DeviceArray<ocean_spray_record> spray_records;      // spray op staging for the host entry point (+ one slot for the count)
+    DeviceArray<ocean_spray_particle> spray_states;     // spray particle staging for the host entry point: states
+    DeviceArray<float> spray_instances;                 // and instances (+ one slot for the count); block counts in spray_counts
     DeviceArray<int> surf_scratch;                      // surface query scratch: pending count, layer maxima, pending list
     DeviceArray<ocean_surface_sample> surf_records;     // surface query staging for the host entry point
     // buoyancy staging: body table and world-point offsets, query positions, surface records (when the caller wants none),
@@ -1138,6 +1140,103 @@ int ocean_extract_spray(ocean_generator* gen, int num_candidates, const float* p
     const int kept = count < max_records ? count : max_records;
     if (kept > 0) OCEAN_CUDA(cudaMemcpy(records_host, recs, sizeof(ocean_spray_record) * (size_t)kept, cudaMemcpyDeviceToHost));
     *num_active = count;
+    return OCEAN_OK;
+}
+
+// ---- spray particles: one particle-process frame of a spray emitter ----
+static_assert(sizeof(ocean_spray_emitter) == 88, "ocean_spray_emitter layout");
+static_assert(sizeof(ocean_spray_particle) == 120, "ocean_spray_particle layout");
+
+int ocean_default_spray_emitter(ocean_spray_emitter* out) {
+    if (!out) return fail(OCEAN_ERR_INVALID_ARGUMENT, "out is NULL");
+    *out = ocean_spray_emitter{};
+    out->amount = 32768;                                // main.tscn:137
+    out->num_particles = 32768;
+    for (int r = 0; r < 3; ++r) out->emission_transform[5 * r] = 15.0f;     // main.tscn:134
+    out->particle_scale[0] = 20.0f;
+    out->particle_scale[1] = 8.5f;
+    out->particle_scale[2] = 20.0f;
+    out->lifetime = 3.0f;                               // sea_spray_particle.gdshader:22-23
+    out->lifetime_randomness = 0.25f;
+    out->random_seed = 0;
+    out->emitter_lifetime = 6.0;                        // main.tscn:138
+    return OCEAN_OK;
+}
+
+namespace {
+int check_spray_particles_args(ocean_generator* gen, const ocean_spray_emitter* e, double t0, double t1, int num_cascades,
+                               const float* map_scales, const void* states, int max_instances, const void* instances, const void* num_live) {
+    if (!e) return fail(OCEAN_ERR_INVALID_ARGUMENT, "emitter is NULL");
+    if (e->amount < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "amount %d is negative", e->amount);
+    if (e->num_particles < 1) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_particles %d is below 1", e->num_particles);
+    if (!(e->lifetime > 0.0f) || !std::isfinite(e->lifetime))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "lifetime %g is not finite and > 0", e->lifetime);
+    if (!(e->emitter_lifetime > 0.0) || !std::isfinite(e->emitter_lifetime))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "emitter_lifetime %g is not finite and > 0", e->emitter_lifetime);
+    if (!(e->lifetime_randomness >= 0.0f && e->lifetime_randomness <= 1.0f))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "lifetime_randomness %g outside [0, 1]", e->lifetime_randomness);
+    if (!std::isfinite(t0) || !std::isfinite(t1) || !(0.0 <= t0 && t0 <= t1))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "frame [%g, %g) is not 0 <= t0 <= t1, finite", t0, t1);
+    if (!((float)t1 < 4294967296.0f) || !(t1 / e->emitter_lifetime < 4294967296.0))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "t1 %g: (float)t1 and t1 / emitter_lifetime must be below 2^32", t1);
+    if (num_cascades < 1 || num_cascades > gen->num_cascades)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_cascades %d outside [1, %d]", num_cascades, gen->num_cascades);
+    if (!map_scales) return fail(OCEAN_ERR_INVALID_ARGUMENT, "map_scales is NULL");
+    if (max_instances < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "max_instances %d is negative", max_instances);
+    if (e->amount > 0 && !states) return fail(OCEAN_ERR_INVALID_ARGUMENT, "states is NULL");
+    if (max_instances > 0 && !instances) return fail(OCEAN_ERR_INVALID_ARGUMENT, "instances is NULL");
+    if (!num_live) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_live is NULL");
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter* emitter, double t0, double t1, int num_cascades,
+                                 const float* map_scales_host, ocean_spray_particle* states_dev, int max_instances, float* instances_dev,
+                                 int* num_live_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_spray_particles_args(gen, emitter, t0, t1, num_cascades, map_scales_host, states_dev, max_instances, instances_dev,
+                                         num_live_dev)))
+        return rc;
+    if (emitter->amount == 0) {
+        OCEAN_CUDA(cudaMemsetAsync(num_live_dev, 0, sizeof(int), gen->stream));
+        return OCEAN_OK;
+    }
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
+    const int blocks = ocean::spray_blocks(emitter->amount);
+    OCEAN_CUDA(gen->spray_counts.grow(gen, (size_t)blocks + 1));
+    OCEAN_CUDA(ocean::launch_spray_particles(gen->buf, num_cascades, gen->q_scales.ptr, emitter, t0, t1, states_dev, gen->spray_counts.ptr,
+                                             instances_dev, max_instances, gen->stream));
+    gen->kernel_launches += 3;
+    OCEAN_CUDA(cudaMemcpyAsync(num_live_dev, gen->spray_counts.ptr + blocks, sizeof(int), cudaMemcpyDeviceToDevice, gen->stream));
+    return OCEAN_OK;
+}
+
+int ocean_spray_particles(ocean_generator* gen, const ocean_spray_emitter* emitter, double t0, double t1, int num_cascades,
+                          const float* map_scales_host, ocean_spray_particle* states_host, int max_instances, float* instances_host,
+                          int* num_live) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_spray_particles_args(gen, emitter, t0, t1, num_cascades, map_scales_host, states_host, max_instances, instances_host,
+                                         num_live)))
+        return rc;
+    *num_live = 0;
+    if (emitter->amount == 0) return OCEAN_OK;
+    const size_t n = (size_t)emitter->amount;
+    OCEAN_CUDA(gen->spray_instances.grow(gen, 16 * (size_t)max_instances + 1));          // + one slot for the count
+    OCEAN_CUDA(gen->spray_states.upload(gen, states_host, n));
+    float* inst = gen->spray_instances.ptr;
+    int* count_dev = reinterpret_cast<int*>(inst + 16 * (size_t)max_instances);
+    if ((rc = ocean_spray_particles_device(gen, emitter, t0, t1, num_cascades, map_scales_host, gen->spray_states.ptr, max_instances, inst,
+                                           count_dev)))
+        return rc;
+    int count = 0;
+    OCEAN_CUDA(cudaMemcpyAsync(states_host, gen->spray_states.ptr, sizeof(ocean_spray_particle) * n, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(&count, count_dev, sizeof(int), cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    const int kept = count < max_instances ? count : max_instances;
+    if (kept > 0) OCEAN_CUDA(cudaMemcpy(instances_host, inst, sizeof(float) * 16 * (size_t)kept, cudaMemcpyDeviceToHost));
+    *num_live = count;
     return OCEAN_OK;
 }
 

@@ -178,5 +178,11 @@ cudaError_t launch_sample_velocity(const uint2* velocity_dev, int map_size, int 
 int spray_blocks(int n);
 cudaError_t launch_extract_spray(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
                                  float3 particle_scale, int* counts_dev, void* records_dev, int max_records, cudaStream_t stream);
+// ocean_spray.cu: one particle-process frame [t0, t1) of a spray emitter (oracle/spray_particles.py), three launches when
+// amount > 0.  emitter_host = ocean_spray_emitter, states_dev = ocean_spray_particle[amount] (updated in place), counts_dev =
+// [spray_blocks(amount) + 1] ints of scratch whose last element receives the number of live particles, instances_dev =
+// [max_instances][16] floats
+cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const void* emitter_host, double t0,
+                                   double t1, void* states_dev, int* counts_dev, float* instances_dev, int max_instances, cudaStream_t stream);
 
 }  // namespace ocean

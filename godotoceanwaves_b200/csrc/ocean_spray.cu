@@ -12,8 +12,18 @@
 //   pass 2  evaluate again (four texel gathers per cascade, L2-resident) and write the record at its final position
 //           (block offset + rank inside the block from warp ballots) -- a STABLE compaction, deterministic output.
 // Numeric policy: oracle/spray.py is the specification (binary32, shader operation order, no contraction, -fmad=false).
+//
+// The particle op (ocean_spray_particles, oracle/spray_particles.py) runs the same shader's start() and process() on an
+// emitter's particle states, kept in device memory, and writes the live particles as MultiMesh instances:
+//   update  one thread per particle: the restart schedule (binary64), start(), process() and the state write; the live
+//           particles are counted per block of 256
+//   scan    k_spray_scan on the block counts
+//   write   the instances of the live particles at block offset + rank (warp ballots): a stable compaction in INDEX order
 #include "ocean_kernels.cuh"
 #include "ocean_texture.cuh"
+#include "detmath.cuh"
+
+#include <cstring>
 
 namespace ocean {
 
@@ -24,8 +34,13 @@ struct SprayEval {
     float scale_factor, psx, psy, psz, foam;
 };
 
-__device__ __forceinline__ SprayEval spray_eval(const uint2* __restrict__ normal, int N, int C, float2 p, const float4* __restrict__ scales,
-                                                float3 particle_scale) {
+struct SprayFactors {
+    float normal_factor, foam_factor, foam;
+};
+
+// :80-87: the gradient and foam at START_POS.xz, and the two factors
+__device__ __forceinline__ SprayFactors spray_factors(const uint2* __restrict__ normal, int N, int C, float2 p,
+                                                      const float4* __restrict__ scales) {
     float gx = 0.0f, gy = 0.0f, gf = 0.0f;
     for (int c = 0; c < C; ++c) {
         const float4 s = __ldg(&scales[c]);
@@ -36,8 +51,17 @@ __device__ __forceinline__ SprayEval spray_eval(const uint2* __restrict__ normal
     }
     const float nx = -gx, nz = -gy;
     const float ny = __fdiv_rn(1.0f, __fsqrt_rn((nx * nx + 1.0f * 1.0f) + nz * nz));               // normalize(...).y  :84
-    const float nf = mixf(0.25f, 1.0f, fminf(__fdiv_rn(ny - 0.92f, 0.99f - 0.92f), 1.0f));          // :86
-    const float ff = mixf(0.25f, 1.0f, fminf(__fdiv_rn(gf - 0.9f, 1.0f - 0.9f), 1.0f));             // :87
+    SprayFactors f;
+    f.normal_factor = mixf(0.25f, 1.0f, fminf(__fdiv_rn(ny - 0.92f, 0.99f - 0.92f), 1.0f));        // :86
+    f.foam_factor = mixf(0.25f, 1.0f, fminf(__fdiv_rn(gf - 0.9f, 1.0f - 0.9f), 1.0f));             // :87
+    f.foam = gf;
+    return f;
+}
+
+__device__ __forceinline__ SprayEval spray_eval(const uint2* __restrict__ normal, int N, int C, float2 p, const float4* __restrict__ scales,
+                                                float3 particle_scale) {
+    const SprayFactors f = spray_factors(normal, N, C, p, scales);
+    const float nf = f.normal_factor, ff = f.foam_factor, gf = f.foam;
     SprayEval e;
     e.active = nf >= 0.0f && nf <= 1.0f && gf > 0.9f;                                               // :89
     e.scale_factor = nf * ff;                                                                       // :90
@@ -137,6 +161,200 @@ __global__ void __launch_bounds__(kSprayBlock) k_spray_write(const uint2* __rest
     }
 }
 
+// ---- the particle op ----
+struct SprayEmitter {       // == ocean_spray_emitter (include/ocean.h), 88 bytes
+    int32_t amount, num_particles;
+    float emission_transform[12];
+    float particle_scale[3];
+    float lifetime, lifetime_randomness;
+    uint32_t random_seed;
+    double emitter_lifetime;
+};
+
+struct SprayParticle {      // == ocean_spray_particle (include/ocean.h), 120 bytes
+    float transform[12];    // 3 x 4 row-major: basis x, basis y, basis z, origin
+    float custom[4];
+    float userdata1[4];     // START_POS, START_TIME
+    float userdata2[4];     // PARTICLE_SCALE, PARTICLE_LIFETIME
+    float userdata3[4];     // .z SCALE_FACTOR, .w HAS_STARTED
+    uint32_t number, flags;
+};
+constexpr uint32_t kParticleActive = 1u, kParticleEmitted = 2u;
+
+// :32-38
+__device__ __forceinline__ float3 spray_hash32(uint32_t px, uint32_t py) {
+    const uint32_t M = 1103515245u;
+    const uint32_t x = M * ((px >> 1) ^ py), y = M * ((py >> 1) ^ px);
+    const uint32_t h = M * (x ^ (y >> 3));
+    const uint32_t n = h ^ (h >> 16);
+    const float d = 2147483648.0f;                       // float(0x7FFFFFFF)
+    return make_float3(__fdiv_rn(__uint2float_rn(n >> 1), d), __fdiv_rn(__uint2float_rn((n * 16807u) >> 1), d),
+                       __fdiv_rn(__uint2float_rn((n * 48271u) >> 1), d));
+}
+
+// :39-43: basis column c = normalize(column c) * s_c
+__device__ __forceinline__ void spray_set_scale(float* T, float sx, float sy, float sz) {
+    const float s[3] = {sx, sy, sz};
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float x = T[c], y = T[4 + c], z = T[8 + c];
+        const float n = __fsqrt_rn((x * x + y * y) + z * z);
+        T[c] = __fdiv_rn(x, n) * s[c];
+        T[4 + c] = __fdiv_rn(y, n) * s[c];
+        T[8 + c] = __fdiv_rn(z, n) * s[c];
+    }
+}
+
+// :69-72
+__device__ __forceinline__ float exp_impulse(float x, float k) {
+    const float h = k * x;
+    return h * detmath::expf_det(1.0f - h);
+}
+
+// r_k = L * ((double)k + (double)i / (double)amount)
+__device__ __forceinline__ double restart_time(double L, long long k, double f) { return __dmul_rn(L, __dadd_rn((double)k, f)); }
+
+// The cycle k of particle i's restart in [t0, t1), -1 for none: the largest k >= 0 with t0 <= r_k < t1.  r_k does not
+// decrease with k, so the largest k with r_k < t1 is reached from an estimate by unit steps (t1 / L < 2^32 is validated).
+__device__ __forceinline__ long long restart_cycle(double L, double f, double t0, double t1) {
+    long long k = (long long)fmax(floor(__dadd_rn(__ddiv_rn(t1, L), -f)), -1.0);
+    while (restart_time(L, k + 1, f) < t1) ++k;
+    while (k >= 0 && restart_time(L, k, f) >= t1) --k;
+    return (k >= 0 && restart_time(L, k, f) >= t0) ? k : -1;
+}
+
+// start() :45-66, after the restart's reset of TRANSFORM and CUSTOM
+__device__ __forceinline__ void spray_start(SprayParticle& p, const SprayEmitter& e, uint32_t index, float time) {
+    const uint32_t u = __float2uint_rz(time);
+    const float3 rand = spray_hash32(p.number + u + e.random_seed, 1u + u + e.random_seed);
+    const uint32_t t = __float2uint_rz(__fsqrt_rn(__uint2float_rn((uint32_t)e.num_particles)));
+    const float tm1 = __uint2float_rn(t) - 1.0f;
+    const float cx = (__fdiv_rn(__uint2float_rn(index / t), tm1) - 0.5f) * 10.0f;
+    const float cz = (__fdiv_rn(__uint2float_rn(index % t), tm1) - 0.5f) * 10.0f;
+    // TRANSFORM = EMISSION_TRANSFORM * TRANSFORM, the identity basis with origin (cx, 0, cz), as sums in index order
+    const float* E = e.emission_transform;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        const float e0 = E[4 * r], e1 = E[4 * r + 1], e2 = E[4 * r + 2], e3 = E[4 * r + 3];
+        p.transform[4 * r + 0] = ((e0 * 1.0f + e1 * 0.0f) + e2 * 0.0f) + e3 * 0.0f;
+        p.transform[4 * r + 1] = ((e0 * 0.0f + e1 * 1.0f) + e2 * 0.0f) + e3 * 0.0f;
+        p.transform[4 * r + 2] = ((e0 * 0.0f + e1 * 0.0f) + e2 * 1.0f) + e3 * 0.0f;
+        p.transform[4 * r + 3] = ((e0 * cx + e1 * 0.0f) + e2 * cz) + e3 * 1.0f;
+    }
+    p.custom[2] = rand.x;
+    const float pl = e.lifetime - (e.lifetime * e.lifetime_randomness) * rand.y;
+    p.userdata2[3] = pl;
+    p.userdata1[0] = p.transform[3];
+    p.userdata1[1] = p.transform[7];
+    p.userdata1[2] = p.transform[11];
+    p.userdata1[3] = time + rand.z * ((float)e.emitter_lifetime - pl);
+    p.userdata3[3] = 0.0f;
+    p.transform[3] = 0.0f;
+    p.transform[7] = -1e10f;
+    p.transform[11] = 0.0f;
+    spray_set_scale(p.transform, 1e-3f, 1e-3f, 1e-3f);
+}
+
+// process() :74-126 of an ACTIVE particle
+__device__ __forceinline__ void spray_process(SprayParticle& p, const SprayEmitter& e, float time, const uint2* __restrict__ disp,
+                                              const uint2* __restrict__ normal, int N, int C, const float4* __restrict__ scales) {
+    const float st = p.userdata1[3], pl = p.userdata2[3];
+    if (time > st + pl) {
+        p.flags &= ~kParticleActive;
+        return;
+    }
+    if (!(time >= st)) return;
+    const float2 sp = make_float2(p.userdata1[0], p.userdata1[2]);
+    if (p.userdata3[3] == 0.0f) {                                                                  // :78-96
+        const SprayFactors f = spray_factors(normal, N, C, sp, scales);
+        const float nf = f.normal_factor, ff = f.foam_factor;
+        const bool active = nf >= 0.0f && nf <= 1.0f && f.foam > 0.9f;
+        p.flags = active ? (p.flags | kParticleActive) : (p.flags & ~kParticleActive);
+        p.userdata3[2] = nf * ff;
+        const float s0 = ff * ((active ? 1.0f : 0.0f) + 1e-3f);
+        p.userdata2[0] = (s0 * 1.0f) * e.particle_scale[0];
+        p.userdata2[1] = (s0 * nf) * e.particle_scale[1];
+        p.userdata2[2] = (s0 * 1.0f) * e.particle_scale[2];
+        p.userdata3[3] = 1.0f;
+    }
+    if (!(p.flags & kParticleActive)) return;
+    const float t = __fdiv_rn(time - st, pl);                                                      // :99
+    p.custom[3] = exp_impulse(t, 10.0f);
+    float dx = 0.0f, dy = 0.0f, dz = 0.0f;
+    for (int c = 0; c < C; ++c) {                                                                  // :105-108
+        const float4 s = __ldg(&scales[c]);
+        add_displacement(disp + (size_t)c * N * N, N, sp.x * s.x, sp.y * s.y, s.z, dx, dy, dz);
+    }
+    dx = dx * 0.75f;                                                                               // :111
+    dy = dy * 1.0f;
+    dz = dz * 0.75f;
+    const float a = 2.5f * t - 0.45f;                                                              // :114, pow(a, 2) = a * a
+    dx = dx + 0.0f;
+    dy = dy + ((-5.0f * (a * a)) * p.userdata3[2] + 0.5f);
+    dz = dz + 0.0f;
+    p.transform[3] = sp.x + dx;                                                                    // :115
+    p.transform[7] = p.userdata1[1] + dy;
+    p.transform[11] = sp.y + dz;
+    const float size = __fdiv_rn(pl, e.lifetime);                                                  // :118-123
+    const float m = size * size;
+    const float my = m * exp_impulse(t, 3.0f);
+    const float lg = detmath::logf_det(1.0f + t);
+    const float mx = m * lg, mz = m * lg;
+    spray_set_scale(p.transform, p.userdata2[0] * mx, p.userdata2[1] * my, p.userdata2[2] * mz);
+}
+
+__device__ __forceinline__ bool spray_live(const SprayParticle& p) { return (p.flags & kParticleActive) && p.userdata3[3] != 0.0f; }
+
+__global__ void __launch_bounds__(kSprayBlock) k_spray_particles_update(const SprayEmitter e, double t0, double t1, float time,
+                                                                        const uint2* __restrict__ disp, const uint2* __restrict__ normal,
+                                                                        int N, int C, const float4* __restrict__ scales,
+                                                                        SprayParticle* __restrict__ states, int* __restrict__ block_counts) {
+    const int i = blockIdx.x * kSprayBlock + threadIdx.x;
+    bool live = false;
+    if (i < e.amount) {
+        SprayParticle p = states[i];
+        const double f = __ddiv_rn((double)i, (double)e.amount);
+        const long long k = restart_cycle(e.emitter_lifetime, f, t0, t1);
+        if (k >= 0) {
+            p.number = (uint32_t)k * (uint32_t)e.amount + (uint32_t)i;
+#pragma unroll
+            for (int j = 0; j < 12; ++j) p.transform[j] = (j % 5 == 0) ? 1.0f : 0.0f;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) p.custom[j] = 0.0f;
+            p.flags |= kParticleActive | kParticleEmitted;
+            spray_start(p, e, (uint32_t)i, time);
+        }
+        if (p.flags & kParticleActive) spray_process(p, e, time, disp, normal, N, C, scales);
+        states[i] = p;
+        live = spray_live(p);
+    }
+    const int total = __syncthreads_count(live);
+    if (threadIdx.x == 0) block_counts[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(kSprayBlock) k_spray_particles_write(const SprayParticle* __restrict__ states, int n,
+                                                                       const int* __restrict__ block_offsets, float* __restrict__ instances,
+                                                                       int max_instances) {
+    __shared__ int s_warp[kSprayBlock / 32];
+    const int i = blockIdx.x * kSprayBlock + threadIdx.x;
+    const bool live = i < n && spray_live(states[i]);
+    const unsigned ballot = __ballot_sync(0xffffffffu, live);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) s_warp[warp] = __popc(ballot);
+    __syncthreads();
+    int off = block_offsets[blockIdx.x];
+    for (int w = 0; w < warp; ++w) off += s_warp[w];
+    off += __popc(ballot & ((1u << lane) - 1u));
+    if (live && off < max_instances) {
+        const SprayParticle& p = states[i];
+        float* o = instances + (size_t)off * 16;
+#pragma unroll
+        for (int j = 0; j < 12; ++j) o[j] = p.transform[j];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) o[12 + j] = p.custom[j];
+    }
+}
+
 }  // namespace
 
 int spray_blocks(int n) { return (n + kSprayBlock - 1) / kSprayBlock; }
@@ -155,6 +373,27 @@ cudaError_t launch_extract_spray(const DeviceBuffers& b, int num_cascades, const
     if (e != cudaSuccess) return e;
     k_spray_write<<<blocks, kSprayBlock, 0, stream>>>(b.normal, b.map_size, num_cascades, points_dev, n, scales_dev, particle_scale, counts_dev,
                                                       static_cast<SprayRecord*>(records_dev), max_records);
+    return cudaGetLastError();
+}
+
+// counts_dev: [spray_blocks(amount) + 1] ints of scratch; on completion counts_dev[spray_blocks(amount)] = number of live
+// particles (which may exceed max_instances: the instances beyond it are dropped, the count is not clamped).
+cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const void* emitter_host, double t0,
+                                   double t1, void* states_dev, int* counts_dev, float* instances_dev, int max_instances, cudaStream_t stream) {
+    static_assert(sizeof(SprayEmitter) == 88 && sizeof(SprayParticle) == 120, "spray particle op layouts");
+    SprayEmitter e;
+    memcpy(&e, emitter_host, sizeof e);
+    if (e.amount <= 0) return cudaSuccess;
+    const int blocks = spray_blocks(e.amount);
+    SprayParticle* states = static_cast<SprayParticle*>(states_dev);
+    k_spray_particles_update<<<blocks, kSprayBlock, 0, stream>>>(e, t0, t1, (float)t1, b.displacement, b.normal, b.map_size, num_cascades,
+                                                                 scales_dev, states, counts_dev);
+    cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) return err;
+    k_spray_scan<<<1, 1024, 0, stream>>>(counts_dev, blocks);
+    err = cudaGetLastError();
+    if (err != cudaSuccess) return err;
+    k_spray_particles_write<<<blocks, kSprayBlock, 0, stream>>>(states, e.amount, counts_dev, instances_dev, max_instances);
     return cudaGetLastError();
 }
 

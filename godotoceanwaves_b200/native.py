@@ -84,6 +84,22 @@ class BodyStateC(C.Structure):
                 ("angular_velocity", C.c_float * 3)]
 
 
+class SprayEmitterC(C.Structure):
+    """struct ocean_spray_emitter (include/ocean.h), 88 B"""
+    _fields_ = [("amount", C.c_int32), ("num_particles", C.c_int32), ("emission_transform", C.c_float * 12),
+                ("particle_scale", C.c_float * 3), ("lifetime", C.c_float), ("lifetime_randomness", C.c_float),
+                ("random_seed", C.c_uint32), ("emitter_lifetime", C.c_double)]
+
+
+class SprayParticleC(C.Structure):
+    """struct ocean_spray_particle (include/ocean.h), 120 B: TRANSFORM (3 x 4 row-major), CUSTOM, USERDATA1..3, NUMBER, flags"""
+    _fields_ = [("transform", C.c_float * 12), ("custom", C.c_float * 4), ("userdata1", C.c_float * 4), ("userdata2", C.c_float * 4),
+                ("userdata3", C.c_float * 4), ("number", C.c_uint32), ("flags", C.c_uint32)]
+
+
+assert C.sizeof(SprayEmitterC) == 88 and SprayEmitterC.emitter_lifetime.offset == 80
+assert C.sizeof(SprayParticleC) == 120 and SprayParticleC.flags.offset == 116
+
 # every symbol include/ocean.h declares: name -> (restype, argtypes)
 _H = C.c_void_p
 _P = C.POINTER
@@ -145,6 +161,11 @@ SIGNATURES = {
     "ocean_spray_grid":(C.c_int, [C.c_int, C.c_void_p, C.c_void_p]),
     "ocean_extract_spray": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, _P(C.c_int)]),
     "ocean_extract_spray_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ocean_default_spray_emitter": (C.c_int, [_P(SprayEmitterC)]),
+    "ocean_spray_particles": (C.c_int, [_H, _P(SprayEmitterC), C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                        C.c_void_p, _P(C.c_int)]),
+    "ocean_spray_particles_device": (C.c_int, [_H, _P(SprayEmitterC), C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                               C.c_void_p, C.c_void_p]),
     "ocean_get_foam_state": (C.c_int, [_H, C.c_int, C.c_void_p]),
     "ocean_set_foam_state": (C.c_int, [_H, C.c_int, C.c_void_p]),
     "ocean_jonswap_alpha": (C.c_double, [C.c_double, C.c_double]),

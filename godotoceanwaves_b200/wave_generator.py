@@ -420,6 +420,41 @@ class WaveGenerator:
                                                  recs.ctypes.data, C.byref(count)))
         return recs[:min(count.value, cap)], count.value
 
+    # -- spray particles: one particle-process frame of the spray emitter, with the live particles as instances ------
+    SPRAY_EMITTER = np.dtype([("amount", np.int32), ("num_particles", np.int32), ("emission_transform", np.float32, 12),
+                              ("particle_scale", np.float32, 3), ("lifetime", np.float32), ("lifetime_randomness", np.float32),
+                              ("random_seed", np.uint32), ("emitter_lifetime", np.float64)])        # struct ocean_spray_emitter
+    SPRAY_PARTICLE = np.dtype([("transform", np.float32, 12), ("custom", np.float32, 4), ("userdata1", np.float32, 4),
+                               ("userdata2", np.float32, 4), ("userdata3", np.float32, 4), ("number", np.uint32),
+                               ("flags", np.uint32)])                                              # struct ocean_spray_particle
+
+    @staticmethod
+    def default_spray_emitter() -> np.ndarray:
+        """The reference scene's emitter (ocean_default_spray_emitter) as a 0-d SPRAY_EMITTER array."""
+        e = native.SprayEmitterC()
+        check(load_library().ocean_default_spray_emitter(C.byref(e)))
+        return np.frombuffer(C.string_at(C.addressof(e), C.sizeof(e)), WaveGenerator.SPRAY_EMITTER).reshape(()).copy()
+
+    def spray_particles(self, emitter, states, t0: float, t1: float, map_scales, max_instances: int | None = None):
+        """One particle-process frame [t0, t1) of the emitter (include/ocean.h, ocean_spray_particles): the restarts, start()
+        and process() of sea_spray_particle.gdshader on the SPRAY_PARTICLE rows of `states` (None = amount never-emitted
+        particles).  Returns (new states, instances [n][16] float32 of the live particles in INDEX order, number of live
+        particles), where n = min(count, max_instances)."""
+        self._require()
+        e = np.array(emitter, self.SPRAY_EMITTER).reshape(())
+        ec = native.SprayEmitterC.from_buffer_copy(e.tobytes())
+        amount = max(int(e["amount"]), 0)
+        s = np.zeros(amount, self.SPRAY_PARTICLE) if states is None else np.array(states, self.SPRAY_PARTICLE, copy=True).reshape(-1)
+        if len(s) != amount:
+            raise ValueError(f"{len(s)} states for an emitter of {amount} particles")
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        cap = amount if max_instances is None else int(max_instances)
+        inst = np.zeros((max(cap, 0), 16), np.float32)
+        count = C.c_int(0)
+        check(load_library().ocean_spray_particles(self.context, C.byref(ec), float(t0), float(t1), sc.shape[0], sc.ctypes.data,
+                                                   s.ctypes.data, cap, inst.ctypes.data, C.byref(count)))
+        return s, inst[:min(count.value, cap)], count.value
+
     def twiddles_to_host(self) -> np.ndarray:
         self._require()
         out = np.empty((self.map_size - 1, 2), np.float32)

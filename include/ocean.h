@@ -496,6 +496,69 @@ int ocean_extract_spray_device(ocean_generator* gen, int num_candidates, const f
                                const float* map_scales_host, const float* particle_scale, int max_records,
                                ocean_spray_record* records_dev, int* num_active_dev);
 
+/* Spray particles -- one particle-process frame of a sea-spray emitter: the restarts, start() and process() of
+ * sea_spray_particle.gdshader (:45-66, :74-126) on particle states kept in caller-owned memory, and the live particles as
+ * render-ready MultiMesh instances, for hosts that do not run Godot's GPUParticles3D (or want only the live particles drawn).
+ * The reference does not contain Godot's particle engine: the emitter cycle below is this library's statement of it, for a
+ * GPUParticles3D with explosiveness 0, randomness 0, local_coords = false, one_shot = false and disable_velocity
+ * (main.tscn:133-140).  oracle/spray_particles.py is the specification, bit for bit.  One call is the frame [t0, t1) of
+ * emitter time, with TIME = (float)t1 and L = emitter_lifetime:
+ *   restart   particle i (INDEX) restarts when some k >= 0 has t0 <= r_k < t1, r_k = L * ((double)k + (double)i / (double)amount)
+ *             in binary64; the largest such k is taken, and NUMBER = k * amount + i (mod 2^32).  A restart sets TRANSFORM to
+ *             the identity and CUSTOM to 0, sets ACTIVE and EMITTED, and runs start() literally, including
+ *             hash32(uvec2(NUMBER, 1U) + uint(TIME) + RANDOM_SEED) in uint32 arithmetic.
+ *   process   process() runs on every ACTIVE particle (an inactive one keeps its state until its next restart), literally:
+ *             the spawn test of ocean_extract_spray on the first frame at or after START_TIME, then the displacement
+ *             sum texture(displacements, START_POS.xz * map_scales[i].xy, i).xyz * map_scales[i].z, * (0.75, 1, 0.75), the
+ *             parabola, the exp_impulse and log(1 + t) scale shaping and set_scale on the previous frame's basis.
+ *   live      ACTIVE and HAS_STARTED != 0 after the frame (a restarted particle waiting for its START_TIME sits at
+ *             y = -1e10 with scale 1e-3 in Godot; it is not an instance).
+ *   instance  16 floats per live particle, in INDEX order: TRANSFORM as basis.x.x, basis.y.x, basis.z.x, origin.x, ... (the
+ *             transforms of ocean_simulate_bodies; a MultiMesh TRANSFORM_3D instance with custom data and no colours), then
+ *             CUSTOM.xyzw (sea_spray.gdshader reads .z and .w through INSTANCE_CUSTOM).  *num_live receives the number of
+ *             live particles even when it exceeds max_instances (instances beyond max_instances are dropped).
+ * Numeric policy (as ocean_extract_spray): binary32 in the shader's operation order, no contraction, IEEE division and sqrt;
+ * normalize(v) = v / sqrt(dot(v, v)); mat4 products as sums in index order; exp and log are DETMATH's; pow(a, 2.0) is taken
+ * as a * a (GLSL leaves pow undefined for a < 0, and 2.5t - 0.45 < 0 for the first 18 % of every particle's life); min(NaN, 1)
+ * is 1 (IEEE minNum).
+ * ocean_default_spray_emitter fills the reference scene's emitter (32768 particles, 15 * I, particle_scale (20, 8.5, 20),
+ * lifetime 3, randomness 0.25, emitter lifetime 6, seed 0).  Validation: amount >= 0, num_particles >= 1, lifetime and
+ * emitter_lifetime finite and > 0, lifetime_randomness in [0, 1], 0 <= t0 <= t1 finite with (float)t1 < 2^32 and
+ * t1 / emitter_lifetime < 2^32, num_cascades in [1, num_cascades of the generator], max_instances >= 0, and no NULL except
+ * states when amount = 0 and instances when max_instances = 0.  An invalid call returns OCEAN_ERR_INVALID_ARGUMENT, launches
+ * nothing and leaves the states untouched.  A valid call with amount > 0 launches three kernels (update, scan, write).
+ * ocean_spray_particles takes host states (updated in place), instances and count and is synchronous;
+ * ocean_spray_particles_device takes device pointers for them and is asynchronous on the generator's stream.  A zero-filled
+ * state is a particle that was never emitted. */
+typedef struct ocean_spray_emitter {
+    int32_t amount;                 /* particles of the emitter (GPUParticles3D.amount), >= 0 */
+    int32_t num_particles;          /* the shader's num_particles uniform: grid side uint(sqrt(float(num_particles))), >= 1 */
+    float emission_transform[12];   /* EMISSION_TRANSFORM, 3 x 4 row-major (basis columns, origin), ocean_spray_grid's layout */
+    float particle_scale[3];        /* uniforms of the particle shader */
+    float lifetime;
+    float lifetime_randomness;
+    uint32_t random_seed;           /* RANDOM_SEED */
+    double emitter_lifetime;        /* LIFETIME (GPUParticles3D.lifetime), s */
+} ocean_spray_emitter;              /* 88 B */
+#define OCEAN_SPRAY_ACTIVE 1u
+#define OCEAN_SPRAY_EMITTED 2u
+typedef struct ocean_spray_particle {
+    float transform[12];            /* TRANSFORM, 3 x 4 row-major like the instances */
+    float custom[4];                /* CUSTOM */
+    float userdata1[4];             /* START_POS, START_TIME */
+    float userdata2[4];             /* PARTICLE_SCALE, PARTICLE_LIFETIME */
+    float userdata3[4];             /* .z SCALE_FACTOR, .w HAS_STARTED */
+    uint32_t number;                /* NUMBER */
+    uint32_t flags;                 /* OCEAN_SPRAY_ACTIVE | OCEAN_SPRAY_EMITTED */
+} ocean_spray_particle;             /* 120 B */
+int ocean_default_spray_emitter(ocean_spray_emitter* out);
+int ocean_spray_particles(ocean_generator* gen, const ocean_spray_emitter* emitter, double t0, double t1, int num_cascades,
+                          const float* map_scales_host, ocean_spray_particle* states_host, int max_instances, float* instances_host,
+                          int* num_live);
+int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter* emitter, double t0, double t1, int num_cascades,
+                                 const float* map_scales_host, ocean_spray_particle* states_dev, int max_instances, float* instances_dev,
+                                 int* num_live_dev);
+
 /* Parity/debug taps (not timed): binary32 maps before the half conversion, the row-pass output
  * ([4][N][N][2] float, == fft_buffer half 1 after the first fft_compute, wave_generator.gd:79) and
  * the twiddle table ([N-1][2] float: stage s, index j at (1<<s)-1+j; fft_butterfly.glsl:27).

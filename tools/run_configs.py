@@ -1,10 +1,11 @@
 """Times the BASELINE.json configs beyond the bench default, and the consumer ops, on the GPU.  Prints one JSON object per
 config.
 
-    python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast]
+    python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast] [--spray-particles]
 
 Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
 --query.  An unknown argument exits before anything touches the GPU."""
+import ctypes
 import json
 import os
 import subprocess
@@ -19,7 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import godotoceanwaves_b200 as gow
 from bench import synth_params
-from godotoceanwaves_b200.native import check, load_library
+from godotoceanwaves_b200.native import SprayEmitterC, check, load_library
 from oracle import bodies as ob
 from oracle import buoyancy as bu
 from oracle import drag as dr
@@ -175,6 +176,37 @@ def run_spray(N, C, particles, reps, label):
     per = timed(g, call, reps, 3)
     out = {"config": label, "map_size": N, "cascades": C, "candidates": particles, "active": int(count.item()), "us_per_call": 1e3 * per,
            "mcandidates_per_s": particles / (per * 1e-3) / 1e6}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
+def run_spray_particles(N, C, amount, reps, label):
+    """Spray-particle op (sea_spray_particle.gdshader start() and process()) on device-resident states: one 30 Hz
+    particle-process frame per call (update + scan + write kernels), timed after 6 s of emitter time so that every
+    particle has been emitted."""
+    def configure(p):
+        for q in p:
+            q.whitecap = 0.9; q.foam_amount = 10.0
+
+    g, _, scales = warmed_generator(N, C, 25, configure)
+    e = gow.WaveGenerator.default_spray_emitter()
+    e["amount"] = e["num_particles"] = amount
+    ec = SprayEmitterC.from_buffer_copy(e.tobytes())
+    states = torch.zeros(amount * gow.WaveGenerator.SPRAY_PARTICLE.itemsize, dtype=torch.uint8, device=DEV)
+    inst = torch.empty(amount * 16, dtype=torch.float32, device=DEV)
+    count = torch.zeros(1, dtype=torch.int32, device=DEV)
+    lib = load_library()
+    clock = [0.0]
+
+    def call():
+        t0 = clock[0]
+        clock[0] = t0 + 1.0 / 30.0
+        check(lib.ocean_spray_particles_device(g.context, ctypes.byref(ec), t0, clock[0], C, scales.ctypes.data, states.data_ptr(), amount, inst.data_ptr(),
+                                               count.data_ptr()))
+
+    per = alternate(lambda: timed(g, call, reps, 180 if clock[0] == 0.0 else 3))[0]
+    out = {"config": label, **card(), "map_size": N, "cascades": C, "particles": amount, "live": int(count.item()),
+           "us_per_call": [1e3 * v for v in per], "best_us": 1e3 * min(per), "mparticles_per_s": amount / (min(per) * 1e-3) / 1e6}
     g.free()
     print(json.dumps(out), flush=True)
 
@@ -533,6 +565,10 @@ GROUPS = {          # flag: its configs, in the order they run
     "--raycast": [
         partial(run_raycast, 256, 4, 20, "ray cast over 4 cascades of 256x256"),
         partial(run_raycast, 1024, 8, 10, "ray cast over 8 cascades of 1024x1024"),
+    ],
+    "--spray-particles": [
+        partial(run_spray_particles, 256, 4, 32768, 100, "spray particles: the reference emitter (32768 particles) over 4 cascades of 256x256"),
+        partial(run_spray_particles, 256, 4, 1 << 20, 50, "spray particles: 2^20 particles over 4 cascades of 256x256"),
     ],
 }
 DEFAULT = ("--updates", "--query")
