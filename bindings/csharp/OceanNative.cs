@@ -64,6 +64,24 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public struct OceanWakeParams                                   // struct ocean_wake_params (20 B); size 0 releases the layer
+    {
+        public int size;                                            // N: a power of two in [128, 2048]
+        public int sponge_cells;                                    // [0, 64], <= size / 2
+        public float cell_size;                                     // dx, m
+        public float damping, sponge_damping;                       // alpha in the interior and at the edge, 1/s
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public struct OceanWakeSource                                   // struct ocean_wake_source (28 B)
+    {
+        public float x, z, vx, vz;                                  // position at the start of the call (offset from the body when body >= 0), m/s
+        public float radius;                                        // m, > 0
+        public float head;                                          // pressure head p / (rho g), m
+        public int body;                                            // index into the body states, or -1
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public unsafe struct OceanSurfaceSample                         // struct ocean_surface_sample (40 B) <- water.gdshader:28,37 inverted
     {
         public float source_x, source_z;
@@ -236,6 +254,27 @@ namespace OceanB200
         internal static partial int ocean_spray_particles_device(IntPtr handle, OceanSprayEmitter* emitter, double t0, double t1, int num_cascades,
                                                                  float* map_scales, void* states_dev, int max_instances, void* instances_dev,
                                                                  void* num_live_dev);
+        // wake layer: a local height field driven by moving sources and floating bodies (include/ocean.h, "Wake layer")
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_kernel_taps(float* taps);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_init(IntPtr handle, OceanWakeParams* parameters);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_step(IntPtr handle, double dt, int substeps, long origin_x, long origin_z, int num_sources,
+                                                    OceanWakeSource* sources, int num_states, OceanBodyState* states);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_step_device(IntPtr handle, double dt, int substeps, long origin_x, long origin_z, int num_sources,
+                                                           void* sources_dev, int num_states, void* states_dev);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_render_map(IntPtr handle, void* map_dev, float* world_rect);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_sample_wake(IntPtr handle, int num_points, float* points_xz, float* output);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_sample_wake_device(IntPtr handle, int num_points, void* points_xz_dev, void* output_dev);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_get_state(IntPtr handle, float* h, float* h_prev, long* origin_xz);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_set_state(IntPtr handle, float* h, float* h_prev, long origin_x, long origin_z);
         // surface query: the surface at world positions points [n][2] (P + D_xz(P) = Q solved for P, then the map query at P)
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,

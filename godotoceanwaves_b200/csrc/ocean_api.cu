@@ -150,6 +150,15 @@ struct ocean_generator {
     DeviceArray<unsigned> ray_bounds;                   // ray cast scratch: [3 * num_cascades] per-layer bounds (first use)
     DeviceArray<ocean_ray> ray_in;                      // ray cast staging for the host entry point
     DeviceArray<ocean_ray_hit> ray_out;
+    // wake layer (ocean_wake_init): four [size][size] fields -- h, h_prev and the two a sub-step writes -- and the host
+    // entry points' staging
+    DeviceArray<float> wake_fields;
+    DeviceArray<ocean_wake_source> wake_sources;
+    DeviceArray<ocean_body_state> wake_states;
+    DeviceArray<float> wake_samples;
+    ocean_wake_params wake{};                           // size 0: no layer
+    int wake_h = 0, wake_hp = 1;                        // which fields hold h and h_prev
+    int64_t wake_origin[2] = {0, 0};
 };
 
 namespace {
@@ -1879,6 +1888,235 @@ int ocean_debug_device_math(ocean_generator* gen, int fn, int n, const float* a_
     gen->kernel_launches += 1;
     OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->q_points.ptr, sizeof(float2) * n, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+// ---- wake layer: a local height field driven by moving sources (oracle/wake.py) ----
+static_assert(sizeof(ocean_wake_params) == 20, "ocean_wake_params layout");
+static_assert(sizeof(ocean_wake_source) == 28, "ocean_wake_source layout");
+
+int ocean_wake_kernel_taps(float* taps_host) {
+    if (!taps_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "taps_host is NULL");
+    ocean::wake_kernel_taps(taps_host);
+    return OCEAN_OK;
+}
+
+namespace {
+constexpr double kWakeCap = 4.0;                        // max Ghat of the stencil (tools/fit_wake_kernel.py)
+
+float* wake_field(ocean_generator* g, int k) { return g->wake_fields.ptr + (size_t)k * g->wake.size * g->wake.size; }
+
+int check_wake_layer(ocean_generator* g) {
+    if (g->wake.size == 0) return fail(OCEAN_ERR_STATE, "the generator has no wake layer (ocean_wake_init)");
+    return OCEAN_OK;
+}
+
+// The call's sub-step and per-ring coefficients, or an error for an invalid step.
+int wake_step_args(ocean_generator* g, double dt, int substeps, int num_sources, const void* sources, int num_states, const void* states,
+                   ocean::WakeStepArgs* a, float* h_sub) {
+    if (!(dt > 0.0) || !std::isfinite(dt)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "dt %g is not finite and > 0", dt);
+    if (substeps < 1 || substeps > 256) return fail(OCEAN_ERR_INVALID_ARGUMENT, "substeps %d outside [1, 256]", substeps);
+    if (num_sources < 0 || num_states < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "negative source or state count");
+    if ((num_sources > 0 && !sources) || (num_states > 0 && !states)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "sources or states is NULL");
+    const ocean_wake_params& p = g->wake;
+    const float hf = (float)(dt / substeps);
+    const double h = hf, dx = p.cell_size;
+    if (kG * h * h / dx * kWakeCap > 4.0)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "sub-step %g s above the stable bound sqrt(dx / g) = %g s", h, std::sqrt(dx / kG));
+    *a = ocean::WakeStepArgs{};
+    for (int r = 0; r <= p.sponge_cells; ++r) {
+        double alpha = p.damping;
+        if (r < p.sponge_cells) {
+            const double t = (double)(p.sponge_cells - r) / p.sponge_cells;
+            alpha = (double)p.damping + ((double)p.sponge_damping - (double)p.damping) * (t * t);
+        }
+        const double ah = alpha * h;
+        a->a1[r] = (float)((2.0 - ah) / (1.0 + ah));
+        a->a2[r] = (float)(1.0 / (1.0 + ah));
+        a->a3[r] = (float)(kG * h * h / (dx * (1.0 + ah)));
+    }
+    a->sources = sources;
+    a->states = states;
+    a->num_sources = num_sources;
+    a->num_states = num_states;
+    a->n = p.size;
+    a->sponge_cells = p.sponge_cells;
+    a->cell = p.cell_size;
+    *h_sub = hf;
+    return OCEAN_OK;
+}
+
+// (float)((double)origin * dx), the window's world corner
+float wake_corner(int64_t origin, float cell) { return (float)((double)origin * (double)cell); }
+
+int check_wake_points(int num_points, const void* points, const void* out) {
+    if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
+    if (num_points > 0 && (!points || !out)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "points or out is NULL");
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if (!params) return fail(OCEAN_ERR_INVALID_ARGUMENT, "params is NULL");
+    const ocean_wake_params p = *params;
+    if (p.size == 0) {
+        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+        gen->wake_fields.release();
+        gen->wake_sources.release();
+        gen->wake_states.release();
+        gen->wake_samples.release();
+        gen->wake = ocean_wake_params{};
+        return OCEAN_OK;
+    }
+    if (p.size < 128 || p.size > 2048 || (p.size & (p.size - 1)))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "size %d is not 0 or a power of two in [128, 2048]", p.size);
+    if (!(p.cell_size > 0.0f) || !std::isfinite(p.cell_size)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "cell_size %g is not finite and > 0", p.cell_size);
+    if (!(p.damping >= 0.0f) || !std::isfinite(p.damping) || !(p.sponge_damping >= 0.0f) || !std::isfinite(p.sponge_damping))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "damping %g / sponge_damping %g not finite and >= 0", p.damping, p.sponge_damping);
+    if (p.sponge_cells < 0 || p.sponge_cells > ocean::kWakeMaxSponge || 2 * p.sponge_cells > p.size)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "sponge_cells %d outside [0, min(64, size / 2)]", p.sponge_cells);
+    const size_t cells = 4 * (size_t)p.size * p.size;  // h, h_prev and two fields a scrolled sub-step writes
+    gen->wake = ocean_wake_params{};                    // no layer until the fields below are allocated and cleared
+    if (gen->wake_fields.capacity != cells) {
+        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+        gen->wake_fields.release();
+    }
+    OCEAN_CUDA(gen->wake_fields.grow(gen, cells));
+    OCEAN_CUDA(cudaMemsetAsync(gen->wake_fields.ptr, 0, cells * sizeof(float), gen->stream));
+    gen->wake = p;
+    gen->wake_h = 0;
+    gen->wake_hp = 1;
+    gen->wake_origin[0] = gen->wake_origin[1] = 0;
+    return OCEAN_OK;
+}
+
+int ocean_wake_step_device(ocean_generator* gen, double dt, int substeps, int64_t origin_x, int64_t origin_z, int num_sources,
+                           const ocean_wake_source* sources_dev, int num_states, const ocean_body_state* states_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    ocean::WakeStepArgs a;
+    float h = 0.0f;
+    if ((rc = wake_step_args(gen, dt, substeps, num_sources, sources_dev, num_states, states_dev, &a, &h))) return rc;
+    const int n = gen->wake.size;
+    // the scroll, clamped to [-n, n] per axis (a move of n cells or more reads nothing but zeros)
+    auto shift = [n](int64_t to, int64_t from) -> int {
+        const __int128 d = (__int128)to - (__int128)from;
+        return d > n ? n : d < -n ? -n : (int)d;
+    };
+    a.di = shift(origin_x, gen->wake_origin[0]);
+    a.dj = shift(origin_z, gen->wake_origin[1]);
+    a.x0 = wake_corner(origin_x, gen->wake.cell_size);
+    a.z0 = wake_corner(origin_z, gen->wake.cell_size);
+    for (int k = 0; k < substeps; ++k) {
+        int spare[2], m = 0;
+        for (int b = 0; b < 4 && m < 2; ++b)
+            if (b != gen->wake_h && b != gen->wake_hp) spare[m++] = b;
+        const bool scrolled = a.di != 0 || a.dj != 0;
+        a.h = wake_field(gen, gen->wake_h);
+        a.h_prev = wake_field(gen, gen->wake_hp);
+        a.out_h = wake_field(gen, spare[0]);
+        a.out_h_prev = scrolled ? wake_field(gen, spare[1]) : nullptr;
+        a.tau = (float)k * h;
+        OCEAN_CUDA(ocean::launch_wake_step(a, gen->stream));
+        gen->kernel_launches += 1;
+        gen->wake_hp = scrolled ? spare[1] : gen->wake_h;
+        gen->wake_h = spare[0];
+        // the fields are now those of the new origin: record it at once, so a later failed launch leaves them consistent
+        gen->wake_origin[0] = origin_x;
+        gen->wake_origin[1] = origin_z;
+        a.di = a.dj = 0;
+    }
+    return OCEAN_OK;
+}
+
+int ocean_wake_step(ocean_generator* gen, double dt, int substeps, int64_t origin_x, int64_t origin_z, int num_sources,
+                    const ocean_wake_source* sources_host, int num_states, const ocean_body_state* states_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    ocean::WakeStepArgs a;
+    float h = 0.0f;
+    if ((rc = wake_step_args(gen, dt, substeps, num_sources, sources_host, num_states, states_host, &a, &h))) return rc;
+    for (int k = 0; k < num_sources; ++k)
+        if (sources_host[k].body >= num_states)
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "source %d: body %d is not below num_states %d", k, sources_host[k].body, num_states);
+    if (num_sources > 0) OCEAN_CUDA(gen->wake_sources.upload(gen, sources_host, (size_t)num_sources));
+    if (num_states > 0) OCEAN_CUDA(gen->wake_states.upload(gen, states_host, (size_t)num_states));
+    return ocean_wake_step_device(gen, dt, substeps, origin_x, origin_z, num_sources, gen->wake_sources.ptr, num_states, gen->wake_states.ptr);
+}
+
+int ocean_wake_render_map(ocean_generator* gen, void* map_dev, float* world_rect) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (!map_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "map_dev is NULL");
+    const ocean_wake_params& p = gen->wake;
+    OCEAN_CUDA(ocean::launch_wake_map(wake_field(gen, gen->wake_h), p.size, p.cell_size, map_dev, gen->stream));
+    gen->kernel_launches += 1;
+    if (world_rect) {
+        world_rect[0] = wake_corner(gen->wake_origin[0], p.cell_size);
+        world_rect[1] = wake_corner(gen->wake_origin[1], p.cell_size);
+        world_rect[2] = world_rect[3] = (float)p.size * p.cell_size;
+    }
+    return OCEAN_OK;
+}
+
+int ocean_sample_wake_device(ocean_generator* gen, int num_points, const float* points_xz_dev, float* out_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if ((rc = check_wake_points(num_points, points_xz_dev, out_dev))) return rc;
+    if (num_points == 0) return OCEAN_OK;
+    const ocean_wake_params& p = gen->wake;
+    OCEAN_CUDA(ocean::launch_wake_sample(wake_field(gen, gen->wake_h), p.size, p.cell_size, wake_corner(gen->wake_origin[0], p.cell_size),
+                                         wake_corner(gen->wake_origin[1], p.cell_size), reinterpret_cast<const float2*>(points_xz_dev),
+                                         num_points, out_dev, gen->stream));
+    gen->kernel_launches += 1;
+    return OCEAN_OK;
+}
+
+int ocean_sample_wake(ocean_generator* gen, int num_points, const float* points_xz_host, float* out_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if ((rc = check_wake_points(num_points, points_xz_host, out_host))) return rc;
+    if (num_points == 0) return OCEAN_OK;
+    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, (size_t)num_points));
+    OCEAN_CUDA(gen->wake_samples.grow(gen, 3 * (size_t)num_points));
+    if ((rc = ocean_sample_wake_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points.ptr), gen->wake_samples.ptr))) return rc;
+    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->wake_samples.ptr, sizeof(float) * 3 * (size_t)num_points, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+int ocean_wake_get_state(ocean_generator* gen, float* h_host, float* h_prev_host, int64_t* origin_xz) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (!h_host || !h_prev_host || !origin_xz) return fail(OCEAN_ERR_INVALID_ARGUMENT, "NULL argument");
+    const size_t bytes = sizeof(float) * gen->wake.size * gen->wake.size;
+    OCEAN_CUDA(cudaMemcpyAsync(h_host, wake_field(gen, gen->wake_h), bytes, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(h_prev_host, wake_field(gen, gen->wake_hp), bytes, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    origin_xz[0] = gen->wake_origin[0];
+    origin_xz[1] = gen->wake_origin[1];
+    return OCEAN_OK;
+}
+
+int ocean_wake_set_state(ocean_generator* gen, const float* h_host, const float* h_prev_host, int64_t origin_x, int64_t origin_z) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (!h_host || !h_prev_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "NULL argument");
+    const size_t bytes = sizeof(float) * gen->wake.size * gen->wake.size;
+    OCEAN_CUDA(cudaMemcpyAsync(wake_field(gen, gen->wake_h), h_host, bytes, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(wake_field(gen, gen->wake_hp), h_prev_host, bytes, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    gen->wake_origin[0] = origin_x;
+    gen->wake_origin[1] = origin_z;
     return OCEAN_OK;
 }
 

@@ -185,4 +185,27 @@ cudaError_t launch_extract_spray(const DeviceBuffers& b, int num_cascades, const
 cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const void* emitter_host, double t0,
                                    double t1, void* states_dev, int* counts_dev, float* instances_dev, int max_instances, cudaStream_t stream);
 
+// ocean_wake.cu: the wake layer (oracle/wake.py).  One sub-step of the layer: h / h_prev ([n][n], read at (i + di, j + dj),
+// 0 outside: the scroll folded into the reads) to out_h, and, when out_h_prev is not null, the scrolled h to out_h_prev.
+// a1..a3 are the per-ring coefficients, index min(cells to the window edge, sponge_cells).
+constexpr int kWakeMaxSponge = 64;
+struct WakeStepArgs {
+    const float* h;
+    const float* h_prev;
+    float* out_h;
+    float* out_h_prev;
+    const void* sources;                            // ocean_wake_source[num_sources]
+    const void* states;                             // ocean_body_state[num_states]
+    int num_sources, num_states;
+    int n, di, dj, sponge_cells;
+    float cell, x0, z0, tau;
+    float a1[kWakeMaxSponge + 1], a2[kWakeMaxSponge + 1], a3[kWakeMaxSponge + 1];
+};
+void wake_kernel_taps(float* out);                  // host: the 28 taps in the specification's order
+cudaError_t launch_wake_step(const WakeStepArgs& args, cudaStream_t stream);
+// map_dev = [n][n][4] half (h, dh/dx, dh/dz, 0); out_dev = [count][3] floats
+cudaError_t launch_wake_map(const float* h_dev, int n, float cell, void* map_dev, cudaStream_t stream);
+cudaError_t launch_wake_sample(const float* h_dev, int n, float cell, float x0, float z0, const float2* xz_dev, int count, float* out_dev,
+                               cudaStream_t stream);
+
 }  // namespace ocean

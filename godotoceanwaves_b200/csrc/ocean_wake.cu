@@ -1,0 +1,281 @@
+// ocean_wake.cu -- the wake layer (include/ocean.h, "Wake layer"; oracle/wake.py is the specification, bit for bit): a
+// local N x N height field advanced by sub-steps of the iWave scheme with a radius-6 stencil for sqrt(-laplacian), forced
+// by the pressure head of moving sources.
+//
+//   k_wake_step     one sub-step; one CTA per 32 x 32 output tile (256 threads, 4 cells each).  The CTA culls the sources
+//                   against its tile plus the 6-cell halo, 256 at a time, with a warp ballot and a prefix over the warps
+//                   (index order is kept), and accumulates phi over its 44 x 44 halo cells in registers; then it stores
+//                   s = h + phi (0 outside the window) in shared memory and each thread takes the 28-class symmetric
+//                   convolution of its four cells from there.  The scroll is folded into the reads: h and h_prev are read at
+//                   (i + di, j + dj), 0 outside, and on a scrolled sub-step the scrolled h is written as the new h_prev.
+//   k_wake_map      one thread per cell: (h, dh/dx, dh/dz, 0) as half, central differences.
+//   k_wake_sample   one thread per point: bilinear h and central differences.
+// No atomics.  Numeric policy: binary32 in the specification's order with explicit _rn operations, no contraction
+// (-fmad=false), IEEE division.
+#include "../../include/ocean.h"
+#include "ocean_kernels.cuh"
+
+#include <cuda_fp16.h>
+
+namespace ocean {
+
+namespace {
+
+constexpr int kR = 6;
+constexpr int kTile = 32;
+constexpr int kHalo = kTile + 2 * kR;           // 44
+constexpr int kHaloCells = kHalo * kHalo;       // 1936
+constexpr int kThreads = 256;
+constexpr int kCellsPerThread = (kHaloCells + kThreads - 1) / kThreads;    // 8
+
+// the 28 taps G[a][b], 0 <= b <= a <= 6, in the specification's order (tools/fit_wake_kernel.py)
+__host__ __device__ constexpr float wake_tap(int t) {
+    constexpr float k[28] = {
+        0x1.cb69a8p+0f,   // G[0][0]
+        -0x1.1ee9ap-4f,   // G[1][0]
+        -0x1.0ffeap-3f,   // G[1][1]
+        -0x1.43e97p-2f,   // G[2][0]
+        -0x1.6504p-6f,    // G[2][1]
+        0x1.7312ep-4f,    // G[2][2]
+        0x1.1a2cp-2f,     // G[3][0]
+        0x1.ad1f8p-6f,    // G[3][1]
+        -0x1.142dp-4f,    // G[3][2]
+        0x1.1c418p-6f,    // G[3][3]
+        -0x1.b34d6p-3f,   // G[4][0]
+        -0x1.97ccp-6f,    // G[4][1]
+        0x1.228p-8f,      // G[4][2]
+        -0x1.3e51p-7f,    // G[4][3]
+        0x1.277dcp-5f,    // G[4][4]
+        0x1.a86fp-4f,     // G[5][0]
+        0x1.1e5p-6f,      // G[5][1]
+        0x1.de36p-7f,     // G[5][2]
+        0x1.323ap-7f,     // G[5][3]
+        -0x1.c8dbp-6f,    // G[5][4]
+        0x1.3535p-7f,     // G[5][5]
+        -0x1.dfdbp-6f,    // G[6][0]
+        -0x1.979cp-7f,    // G[6][1]
+        -0x1.787bp-7f,    // G[6][2]
+        -0x1.fc14p-8f,    // G[6][3]
+        0x1.ae5p-9f,      // G[6][4]
+        -0x1.28bp-9f,     // G[6][5]
+        0x1.9ep-12f,      // G[6][6]
+    };
+    return k[t];
+}
+__host__ __device__ constexpr int tap_a(int t) { int a = 0; while ((a + 1) * (a + 2) / 2 <= t) ++a; return a; }
+__host__ __device__ constexpr int tap_b(int t) { return t - tap_a(t) * (tap_a(t) + 1) / 2; }
+
+// the sum of the values at the mirrored offsets (di, dj) of class (A, B), in the specification's order; s points at the
+// centre of a row-major array of row stride kHalo
+template <int A, int B>
+__device__ __forceinline__ float orbit(const float* s) {
+    constexpr int W = kHalo;
+    if constexpr (A == 0) {
+        return s[0];
+    } else if constexpr (B == 0) {
+        return __fadd_rn(__fadd_rn(__fadd_rn(s[A], s[-A]), s[A * W]), s[-A * W]);
+    } else if constexpr (A == B) {
+        return __fadd_rn(__fadd_rn(__fadd_rn(s[A + A * W], s[A - A * W]), s[-A + A * W]), s[-A - A * W]);
+    } else {
+        float v = __fadd_rn(s[A + B * W], s[A - B * W]);
+        v = __fadd_rn(v, s[-A + B * W]);
+        v = __fadd_rn(v, s[-A - B * W]);
+        v = __fadd_rn(v, s[B + A * W]);
+        v = __fadd_rn(v, s[B - A * W]);
+        v = __fadd_rn(v, s[-B + A * W]);
+        return __fadd_rn(v, s[-B - A * W]);
+    }
+}
+
+template <int T>
+__device__ __forceinline__ float convolve_from(const float* s, float c) {
+    if constexpr (T == 28) {
+        return c;
+    } else {
+        return convolve_from<T + 1>(s, __fadd_rn(c, __fmul_rn(wake_tap(T), orbit<tap_a(T), tap_b(T)>(s))));
+    }
+}
+
+__device__ __forceinline__ float convolve(const float* s) { return convolve_from<1>(s, __fmul_rn(wake_tap(0), s[0])); }
+
+// h at window cell (i, j) of the field f ([n][n]), 0 outside
+__device__ __forceinline__ float cell(const float* __restrict__ f, int n, int i, int j) {
+    return (unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n ? f[(size_t)j * n + i] : 0.0f;
+}
+
+__global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
+    __shared__ float s[kHaloCells];
+    __shared__ float4 list[kThreads];               // culled sources: cx, cz, r2, head
+    __shared__ int warp_count[kThreads / 32];
+    const int t = threadIdx.x;
+    const int n = a.n;
+    const int ti0 = blockIdx.x * kTile - kR, tj0 = blockIdx.y * kTile - kR;   // window cell of halo cell (0, 0)
+    const float dx = a.cell;
+
+    float phi[kCellsPerThread];
+#pragma unroll
+    for (int m = 0; m < kCellsPerThread; ++m) phi[m] = 0.0f;
+
+    if (a.num_sources > 0) {
+        // the halo's cell centres span [lo, hi] per axis; one cell of margin keeps the cull conservative under rounding
+        const float xlo = __fadd_rn(a.x0, __fmul_rn(__fadd_rn((float)(ti0 - 1), 0.5f), dx));
+        const float xhi = __fadd_rn(a.x0, __fmul_rn(__fadd_rn((float)(ti0 + kHalo), 0.5f), dx));
+        const float zlo = __fadd_rn(a.z0, __fmul_rn(__fadd_rn((float)(tj0 - 1), 0.5f), dx));
+        const float zhi = __fadd_rn(a.z0, __fmul_rn(__fadd_rn((float)(tj0 + kHalo), 0.5f), dx));
+        for (int base = 0; base < a.num_sources; base += kThreads) {
+            const int k = base + t;
+            bool keep = false;
+            float4 e = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+            if (k < a.num_sources) {
+                const ocean_wake_source src = static_cast<const ocean_wake_source*>(a.sources)[k];
+                float cx = __fadd_rn(src.x, __fmul_rn(src.vx, a.tau));
+                float cz = __fadd_rn(src.z, __fmul_rn(src.vz, a.tau));
+                bool ok = src.body < a.num_states;
+                if (ok && src.body >= 0) {
+                    const ocean_body_state& b = static_cast<const ocean_body_state*>(a.states)[src.body];
+                    cx = __fadd_rn(cx, __fadd_rn(b.position[0], __fmul_rn(b.linear_velocity[0], a.tau)));
+                    cz = __fadd_rn(cz, __fadd_rn(b.position[2], __fmul_rn(b.linear_velocity[2], a.tau)));
+                }
+                const float r = src.radius;
+                const float r2 = __fmul_rn(r, r);
+                ok = ok && isfinite(cx) && isfinite(cz) && isfinite(src.head) && isfinite(r) && r > 0.0f && isfinite(r2);
+                keep = ok && __fadd_rn(cx, r) >= xlo && __fsub_rn(cx, r) <= xhi && __fadd_rn(cz, r) >= zlo && __fsub_rn(cz, r) <= zhi;
+                e = make_float4(cx, cz, r2, src.head);
+            }
+            const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+            const int lane = t & 31, warp = t >> 5;
+            if (lane == 0) warp_count[warp] = __popc(ballot);
+            __syncthreads();
+            int offset = 0, total = 0;
+#pragma unroll
+            for (int w = 0; w < kThreads / 32; ++w) {
+                offset += w < warp ? warp_count[w] : 0;
+                total += warp_count[w];
+            }
+            if (keep) list[offset + __popc(ballot & ((1u << lane) - 1u))] = e;
+            __syncthreads();
+#pragma unroll
+            for (int m = 0; m < kCellsPerThread; ++m) {
+                const int c = t + m * kThreads;
+                const int i = ti0 + c % kHalo, j = tj0 + c / kHalo;
+                if (c < kHaloCells && (unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n) {
+                    const float px = __fadd_rn(a.x0, __fmul_rn(__fadd_rn((float)i, 0.5f), dx));
+                    const float pz = __fadd_rn(a.z0, __fmul_rn(__fadd_rn((float)j, 0.5f), dx));
+                    float p = phi[m];
+                    for (int q = 0; q < total; ++q) {
+                        const float4 e2 = list[q];
+                        const float ex = __fsub_rn(px, e2.x), ez = __fsub_rn(pz, e2.y);
+                        const float d2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ez, ez));
+                        if (d2 < e2.z) {
+                            const float w = __fsub_rn(1.0f, __fdiv_rn(d2, e2.z));
+                            p = __fadd_rn(p, __fmul_rn(e2.w, __fmul_rn(w, w)));
+                        }
+                    }
+                    phi[m] = p;
+                }
+            }
+            __syncthreads();                        // the list and the counts are rewritten by the next chunk
+        }
+    }
+
+    // s = h + phi over the halo, 0 outside the window
+#pragma unroll
+    for (int m = 0; m < kCellsPerThread; ++m) {
+        const int c = t + m * kThreads;
+        if (c < kHaloCells) {
+            const int i = ti0 + c % kHalo, j = tj0 + c / kHalo;
+            float v = 0.0f;
+            if ((unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n) v = __fadd_rn(cell(a.h, n, i + a.di, j + a.dj), phi[m]);
+            s[c] = v;
+        }
+    }
+    __syncthreads();
+
+    const int li = t & 31;
+#pragma unroll
+    for (int r = 0; r < kTile / 8; ++r) {
+        const int lj = (t >> 5) + 8 * r;
+        const int i = blockIdx.x * kTile + li, j = blockIdx.y * kTile + lj;
+        const float c = convolve(&s[(lj + kR) * kHalo + li + kR]);
+        const float h = cell(a.h, n, i + a.di, j + a.dj);
+        const float hp = cell(a.h_prev, n, i + a.di, j + a.dj);
+        const int edge = min(min(i, j), min(n - 1 - i, n - 1 - j));
+        const int ring = min(edge, a.sponge_cells);
+        const float hn = __fsub_rn(__fsub_rn(__fmul_rn(a.a1[ring], h), __fmul_rn(a.a2[ring], hp)), __fmul_rn(a.a3[ring], c));
+        const size_t o = (size_t)j * n + i;
+        a.out_h[o] = hn;
+        if (a.out_h_prev) a.out_h_prev[o] = h;
+    }
+}
+
+__device__ __forceinline__ float grad_x(const float* __restrict__ h, int n, int i, int j, float two_dx) {
+    return __fdiv_rn(__fsub_rn(cell(h, n, i + 1, j), cell(h, n, i - 1, j)), two_dx);
+}
+__device__ __forceinline__ float grad_z(const float* __restrict__ h, int n, int i, int j, float two_dx) {
+    return __fdiv_rn(__fsub_rn(cell(h, n, i, j + 1), cell(h, n, i, j - 1)), two_dx);
+}
+
+__global__ void __launch_bounds__(256) k_wake_map(const float* __restrict__ h, int n, float two_dx, __half2* __restrict__ out) {
+    const int o = blockIdx.x * blockDim.x + threadIdx.x;
+    if (o >= n * n) return;
+    const int i = o % n, j = o / n;
+    out[2 * (size_t)o] = __halves2half2(__float2half_rn(h[o]), __float2half_rn(grad_x(h, n, i, j, two_dx)));
+    out[2 * (size_t)o + 1] = __halves2half2(__float2half_rn(grad_z(h, n, i, j, two_dx)), __float2half_rn(0.0f));
+}
+
+__device__ __forceinline__ float bilerp(float f00, float f10, float f01, float f11, float fu, float fv) {
+    const float top = __fadd_rn(f00, __fmul_rn(fu, __fsub_rn(f10, f00)));
+    const float bot = __fadd_rn(f01, __fmul_rn(fu, __fsub_rn(f11, f01)));
+    return __fadd_rn(top, __fmul_rn(fv, __fsub_rn(bot, top)));
+}
+
+__global__ void __launch_bounds__(256) k_wake_sample(const float* __restrict__ h, int n, float dx, float x0, float z0,
+                                                     const float2* __restrict__ xz, int count, float* __restrict__ out) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= count) return;
+    const float2 p = xz[k];
+    const float ext = __fmul_rn((float)n, dx);
+    float r[3] = {0.0f, 0.0f, 0.0f};
+    if (p.x >= x0 && p.x < __fadd_rn(x0, ext) && p.y >= z0 && p.y < __fadd_rn(z0, ext)) {
+        const float u = __fsub_rn(__fdiv_rn(__fsub_rn(p.x, x0), dx), 0.5f);
+        const float v = __fsub_rn(__fdiv_rn(__fsub_rn(p.y, z0), dx), 0.5f);
+        const float fi = floorf(u), fj = floorf(v);
+        const float fu = __fsub_rn(u, fi), fv = __fsub_rn(v, fj);
+        const int i = (int)fi, j = (int)fj;
+        const float two_dx = __fmul_rn(2.0f, dx);
+        r[0] = bilerp(cell(h, n, i, j), cell(h, n, i + 1, j), cell(h, n, i, j + 1), cell(h, n, i + 1, j + 1), fu, fv);
+        // central differences of cells outside the window are 0, like their heights
+        auto gx = [&](int ii, int jj) { return (unsigned)ii < (unsigned)n && (unsigned)jj < (unsigned)n ? grad_x(h, n, ii, jj, two_dx) : 0.0f; };
+        auto gz = [&](int ii, int jj) { return (unsigned)ii < (unsigned)n && (unsigned)jj < (unsigned)n ? grad_z(h, n, ii, jj, two_dx) : 0.0f; };
+        r[1] = bilerp(gx(i, j), gx(i + 1, j), gx(i, j + 1), gx(i + 1, j + 1), fu, fv);
+        r[2] = bilerp(gz(i, j), gz(i + 1, j), gz(i, j + 1), gz(i + 1, j + 1), fu, fv);
+    }
+    for (int m = 0; m < 3; ++m) out[3 * (size_t)k + m] = r[m];
+}
+
+}  // namespace
+
+void wake_kernel_taps(float* out) {
+    for (int t = 0; t < 28; ++t) out[t] = wake_tap(t);
+}
+
+cudaError_t launch_wake_step(const WakeStepArgs& args, cudaStream_t stream) {
+    const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
+    k_wake_step<<<grid, kThreads, 0, stream>>>(args);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wake_map(const float* h_dev, int n, float cell, void* map_dev, cudaStream_t stream) {
+    const unsigned blocks = (unsigned)(((size_t)n * n + 255) / 256);
+    k_wake_map<<<blocks, 256, 0, stream>>>(h_dev, n, 2.0f * cell, static_cast<__half2*>(map_dev));    // exact
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wake_sample(const float* h_dev, int n, float cell, float x0, float z0, const float2* xz_dev, int count, float* out_dev,
+                               cudaStream_t stream) {
+    if (count <= 0) return cudaSuccess;
+    k_wake_sample<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(h_dev, n, cell, x0, z0, xz_dev, count, out_dev);
+    return cudaGetLastError();
+}
+
+}  // namespace ocean

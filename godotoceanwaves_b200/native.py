@@ -97,6 +97,20 @@ class SprayParticleC(C.Structure):
                 ("userdata3", C.c_float * 4), ("number", C.c_uint32), ("flags", C.c_uint32)]
 
 
+class WakeParamsC(C.Structure):
+    """struct ocean_wake_params (include/ocean.h), 20 B"""
+    _fields_ = [("size", C.c_int32), ("sponge_cells", C.c_int32), ("cell_size", C.c_float), ("damping", C.c_float),
+                ("sponge_damping", C.c_float)]
+
+
+class WakeSourceC(C.Structure):
+    """struct ocean_wake_source (include/ocean.h), 28 B"""
+    _fields_ = [("x", C.c_float), ("z", C.c_float), ("vx", C.c_float), ("vz", C.c_float), ("radius", C.c_float),
+                ("head", C.c_float), ("body", C.c_int32)]
+
+
+assert C.sizeof(WakeParamsC) == 20 and WakeParamsC.sponge_damping.offset == 16
+assert C.sizeof(WakeSourceC) == 28 and WakeSourceC.body.offset == 24
 assert C.sizeof(SprayEmitterC) == 88 and SprayEmitterC.emitter_lifetime.offset == 80
 assert C.sizeof(SprayParticleC) == 120 and SprayParticleC.flags.offset == 116
 
@@ -166,6 +180,15 @@ SIGNATURES = {
                                         C.c_void_p, _P(C.c_int)]),
     "ocean_spray_particles_device": (C.c_int, [_H, _P(SprayEmitterC), C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                                C.c_void_p, C.c_void_p]),
+    "ocean_wake_kernel_taps": (C.c_int, [C.c_void_p]),
+    "ocean_wake_init": (C.c_int, [_H, _P(WakeParamsC)]),
+    "ocean_wake_step": (C.c_int, [_H, C.c_double, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    "ocean_wake_step_device": (C.c_int, [_H, C.c_double, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    "ocean_wake_render_map": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
+    "ocean_sample_wake": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p]),
+    "ocean_sample_wake_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p]),
+    "ocean_wake_get_state": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ocean_wake_set_state": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64]),
     "ocean_get_foam_state": (C.c_int, [_H, C.c_int, C.c_void_p]),
     "ocean_set_foam_state": (C.c_int, [_H, C.c_int, C.c_void_p]),
     "ocean_jonswap_alpha": (C.c_double, [C.c_double, C.c_double]),

@@ -41,6 +41,7 @@ class WaveGenerator:
         self._num_cascades = 0
         self._carr = None
         self._seen = None
+        self._wake_size = 0
 
     # ---- wave_generator.gd:17-54
     def init_gpu(self, num_cascades: int) -> None:
@@ -454,6 +455,74 @@ class WaveGenerator:
         check(load_library().ocean_spray_particles(self.context, C.byref(ec), float(t0), float(t1), sc.shape[0], sc.ctypes.data,
                                                    s.ctypes.data, cap, inst.ctypes.data, C.byref(count)))
         return s, inst[:min(count.value, cap)], count.value
+
+    # -- wake layer: a local height field driven by moving sources and floating bodies --------------------------------
+    WAKE_PARAMS = np.dtype([("size", np.int32), ("sponge_cells", np.int32), ("cell_size", np.float32), ("damping", np.float32),
+                            ("sponge_damping", np.float32)])                                     # struct ocean_wake_params
+    WAKE_SOURCE = np.dtype([("x", np.float32), ("z", np.float32), ("vx", np.float32), ("vz", np.float32), ("radius", np.float32),
+                            ("head", np.float32), ("body", np.int32)])                           # struct ocean_wake_source
+
+    @staticmethod
+    def wake_kernel_taps() -> np.ndarray:
+        """The 28 float32 taps G[a][b] of the wake step's stencil, (0,0), (1,0), (1,1), ... (6,6) (no device needed)."""
+        out = np.zeros(28, np.float32)
+        check(load_library().ocean_wake_kernel_taps(out.ctypes.data))
+        return out
+
+    def wake_init(self, size: int, cell_size: float = 0.5, damping: float = 0.0, sponge_cells: int = 48,
+                  sponge_damping: float = 1.0) -> None:
+        """(Re)create the wake layer, zeroed at origin (0, 0): size x size cells of cell_size metres (include/ocean.h,
+        ocean_wake_init).  size = 0 releases it."""
+        self._require()
+        p = native.WakeParamsC(int(size), int(sponge_cells), float(cell_size), float(damping), float(sponge_damping))
+        check(load_library().ocean_wake_init(self.context, C.byref(p)))
+        self._wake_size = int(size)
+
+    def wake_step(self, dt: float, substeps: int = 1, origin=(0, 0), sources=None, states=None) -> None:
+        """Advance the wake layer by `substeps` sub-steps of dt / substeps with the window at `origin` (whole cells), forced
+        by the WAKE_SOURCE rows of `sources`; `states` are the BODY_STATE rows body-attached sources follow."""
+        self._require()
+        src = np.zeros(0, self.WAKE_SOURCE) if sources is None else np.ascontiguousarray(sources, self.WAKE_SOURCE).reshape(-1)
+        st = np.zeros(0, self.BODY_STATE) if states is None else np.ascontiguousarray(states, self.BODY_STATE).reshape(-1)
+        check(load_library().ocean_wake_step(self.context, float(dt), int(substeps), int(origin[0]), int(origin[1]), len(src),
+                                             src.ctypes.data if len(src) else None, len(st), st.ctypes.data if len(st) else None))
+
+    def wake_map(self):
+        """(map [N][N][4] float16 (h, dh/dx, dh/dz, 0), world rect (x0, z0, width, depth)) of the wake layer."""
+        import torch
+        self._require()
+        n = self._wake_size
+        dev = torch.empty(n * n * 4, dtype=torch.float16, device=torch.device("cuda", self.device))
+        rect = np.zeros(4, np.float32)
+        torch.cuda.synchronize(dev.device)
+        check(load_library().ocean_wake_render_map(self.context, dev.data_ptr(), rect.ctypes.data))
+        self.synchronize()
+        return dev.cpu().numpy().reshape(n, n, 4), rect
+
+    def sample_wake(self, points_xz) -> np.ndarray:
+        """[n][3] float32 (h, dh/dx, dh/dz) of the wake layer at world points (x, z), bilinear; 0 outside the window."""
+        self._require()
+        pts = np.ascontiguousarray(points_xz, np.float32).reshape(-1, 2)
+        out = np.zeros((len(pts), 3), np.float32)
+        check(load_library().ocean_sample_wake(self.context, len(pts), pts.ctypes.data, out.ctypes.data))
+        return out
+
+    def wake_state(self):
+        """(h, h_prev, origin): host copies of the wake layer's fields ([N][N] float32) and its origin in cells."""
+        self._require()
+        n = self._wake_size
+        h, hp, o = np.zeros((n, n), np.float32), np.zeros((n, n), np.float32), np.zeros(2, np.int64)
+        check(load_library().ocean_wake_get_state(self.context, h.ctypes.data, hp.ctypes.data, o.ctypes.data))
+        return h, hp, (int(o[0]), int(o[1]))
+
+    def set_wake_state(self, h, h_prev, origin=(0, 0)) -> None:
+        self._require()
+        n = self._wake_size
+        h = np.ascontiguousarray(h, np.float32)
+        hp = np.ascontiguousarray(h_prev, np.float32)
+        if h.shape != (n, n) or hp.shape != (n, n):
+            raise ValueError(f"wake fields must be [{n}][{n}]")
+        check(load_library().ocean_wake_set_state(self.context, h.ctypes.data, hp.ctypes.data, int(origin[0]), int(origin[1])))
 
     def twiddles_to_host(self) -> np.ndarray:
         self._require()

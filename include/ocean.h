@@ -350,7 +350,7 @@ int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoy
  * it uses the SURFACE water velocity at every submerged point, while the orbital velocity of a wave decays as e^(-k z) with
  * depth z (at 1 m of draft this overstates the longest wave of a 16 m tile about 1.5 times, shorter waves more); there is no
  * added mass, radiation or wave-making damping, skin friction, or separate normal and tangential coefficients; nothing is
- * written back into the maps (no wake or foam).  Quadratic drag is stiff for light bodies under explicit integration: the op
+ * written back into the maps (no foam; wakes are the separate wake layer below, which these ops do not read).  Quadratic drag is stiff for light bodies under explicit integration: the op
  * does not integrate, and max_relative_speed lets a host choose sub-steps (ocean_simulate_bodies below integrates on the
  * device with a step that stays stable under it).
  * The call first brings stale velocity layers up to date (as ocean_sample_velocity does; the velocity buffers are allocated
@@ -558,6 +558,93 @@ int ocean_spray_particles(ocean_generator* gen, const ocean_spray_emitter* emitt
 int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter* emitter, double t0, double t1, int num_cascades,
                                  const float* map_scales_host, ocean_spray_particle* states_dev, int max_instances, float* instances_dev,
                                  int* num_live_dev);
+
+/* Wake layer -- interactive wakes: a local, dynamic height field that moving sources (boats, swimmers, splashes) and
+ * floating bodies drive, to be added to the spectral ocean.  The FFT cascades are periodic tiles rebuilt from h0 every
+ * update and cannot carry a propagating disturbance; this layer has its own state.  oracle/wake.py is the specification,
+ * bit for bit.
+ *   window    N x N cells of size dx (N a power of two in [128, 2048]) whose corner cell sits at the integer cell origin
+ *             (ox, oz): cell (i, j) covers world x in [(ox + i) dx, (ox + i + 1) dx), z likewise; fields are [N][N]
+ *             binary32, row j along z.  The world corner is x0 = (float)((double)ox * dx), z0 likewise.
+ *   state     h (the current height) and h_prev (the height one sub-step earlier), in metres.
+ *   model     iWave (Tessendorf, "Interactive Water Surfaces", 2004) with deep-water dispersion w^2 = g |k|:
+ *             one sub-step of h = (float)(dt / S), per cell:
+ *               s = h + phi;  c = sum over 28 classes (a, b), 0 <= b <= a <= 6, of G[a][b] * (the sum of the up-to-8 mirrored
+ *               neighbours of s), cells outside the window reading 0;  h_new = (a1 h - a2 h_prev) - a3 c
+ *             with a1 = (2 - alpha h) / (1 + alpha h), a2 = 1 / (1 + alpha h), a3 = g h^2 / (dx (1 + alpha h)), evaluated in
+ *             binary64 and rounded once per ring; alpha is `damping` in the interior and damping + (sponge_damping -
+ *             damping) t^2, t = (sponge_cells - r) / sponge_cells, on the ring r < sponge_cells cells from the edge (the
+ *             sponge absorbs outgoing waves).
+ *   stencil   G (ocean_wake_kernel_taps, fitted by tools/fit_wake_kernel.py) is a radius-6 radial stencil whose symbol
+ *             Ghat(k) approximates |k| dx: sum G = 0 exactly, 0 <= Ghat <= 4 over the Brillouin zone, and |Ghat / (|k| dx)
+ *             - 1| <= 3.9 % for |k| dx in [0.4, 2.0].  Waves propagate correctly for wavelengths from 3.1 dx to 15.7 dx;
+ *             longer ones are too slow (no finite stencil is accurate near k = 0), shorter ones are dispersive.  A source
+ *             moving at U leaves a Kelvin wake of wavelength 2 pi U^2 / g: choose dx near 2 pi U^2 / (8 g) = 0.08 U^2
+ *             (U = 5 m/s: dx = 2 m, 8 cells per wavelength).  The band holds the Kelvin wavelength while |k| dx = g dx / U^2
+ *             lies in [0.4, 2.0], i.e. dx between 0.4 U^2 / g = 0.041 U^2 and 2 U^2 / g = 0.204 U^2.  The source radius
+ *             should span a few cells.
+ *   stability with alpha = 0 a mode is stable iff 0 <= a3 Ghat(k) <= 4.  A call with g h^2 / dx * 4 > 4 (binary64) is
+ *             rejected, so the largest sub-step is h = sqrt(dx / g) (dx = 1 m: 0.319 s; dx = 0.25 m: 0.160 s).
+ *   sources   at sub-step k of a call a source sits at c = (x, z) + (vx, vz) tau, tau = (float)k * h, plus, when body >= 0,
+ *             states[body].position.xz + states[body].linear_velocity.xz * tau (the device states of
+ *             ocean_simulate_bodies_device: a boat's wake follows it with nothing crossing PCIe).  At each cell centre p,
+ *             in source index order, phi += head * (1 - q2)^2 with q2 = |p - c|^2 / radius^2 < 1.  A source whose centre,
+ *             head or radius is not finite, whose radius is <= 0 or radius^2 not finite, or (device sources) whose body
+ *             index is not below num_states contributes nothing.  head is the pressure head p / (rho g); a stationary
+ *             source with damping 0 is at rest at h = -phi.  The iWave damping term also pulls h itself towards 0, so with
+ *             damping > 0 the rest state is a shallower depression (G(h + phi) = -(2 alpha dx / (g h)) h).
+ *   scroll    each step call takes the origin; moving it by (di, dj) is exactly a shift of h and h_prev by those cells with
+ *             zero fill (a move of N cells or more clears the layer), folded into the first sub-step's reads.
+ * The sponge is sized for waves in the band: with iWave's damping it reflects about 4 % of a pulse in the band through a
+ * 48-cell ramp to 1 / s, but much more of waves longer than the band, and a strong sponge_damping (which also acts as a
+ * spring of stiffness 2 alpha / h) reflects more than a moderate one.
+ * Limits: wakes do not enter the surface query, buoyancy, drag, ray cast or spray (they read the FFT maps only); bodies do
+ * not block waves (no obstruction mask); wakes make no foam; linear deep water only (no breaking, shallow water or
+ * nonlinearity); the layer and the cascades interact by superposition only.
+ * Entry points (an invalid call returns OCEAN_ERR_INVALID_ARGUMENT, launches nothing and leaves the layer untouched; a call
+ * on a generator without a layer returns OCEAN_ERR_STATE):
+ *   ocean_wake_kernel_taps   the 28 taps G[a][b] in the order (0,0), (1,0), (1,1), (2,0), ... (6,6); host only, no device.
+ *   ocean_wake_init          params->size = 0 releases the layer; otherwise (re)creates it zeroed at origin (0, 0).  A
+ *                            valid call that fails in CUDA (OCEAN_ERR_CUDA) leaves the generator without a layer.
+ *                            size a power of two in [128, 2048], cell_size finite > 0, damping and sponge_damping finite
+ *                            >= 0, sponge_cells in [0, 64] and <= size / 2.
+ *   ocean_wake_step          dt finite > 0, substeps in [1, 256], the stability rule above, num_sources and num_states
+ *                            >= 0 with non-NULL arrays when > 0, and (host form) every source's body < num_states.
+ *                            Launches `substeps` kernels.  The host form takes host sources and states and returns when
+ *                            the work is enqueued; the device form takes device pointers; both are asynchronous on the
+ *                            generator's stream.
+ *   ocean_wake_render_map    writes [N][N][4] half (h, dh/dx, dh/dz, 0) in window order into map_dev (device memory),
+ *                            central differences (h[i+1] - h[i-1]) / (2 dx), cells outside reading 0; world_rect (host,
+ *                            may be NULL) receives (x0, z0, N dx, N dx).  One kernel, asynchronous.
+ *   ocean_sample_wake        bilinear h, dh/dx and dh/dz ([n][3] float) from the binary32 state at world (x, z); 0 outside
+ *                            the window.  One kernel; the host form is synchronous, the device form asynchronous.
+ *   ocean_wake_get_state / ocean_wake_set_state   host copies of h, h_prev ([N][N] float) and the origin, for tests and
+ *                            checkpoints (synchronous). */
+typedef struct ocean_wake_params {
+    int32_t size;               /* N: 0 (release) or a power of two in [128, 2048] */
+    int32_t sponge_cells;       /* width of the absorbing ring, [0, 64] and <= size / 2 */
+    float cell_size;            /* dx, metres */
+    float damping;              /* alpha in the interior, 1/s */
+    float sponge_damping;       /* alpha at the window edge, 1/s */
+} ocean_wake_params;            /* 20 B */
+typedef struct ocean_wake_source {
+    float x, z;                 /* world position at the start of the call (offset from the body when body >= 0) */
+    float vx, vz;               /* velocity, m/s */
+    float radius;               /* m, > 0 */
+    float head;                 /* pressure head p / (rho g), m (positive pushes the surface down) */
+    int32_t body;               /* index into the body states, or -1 */
+} ocean_wake_source;            /* 28 B */
+int ocean_wake_kernel_taps(float* taps_host);
+int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params);
+int ocean_wake_step(ocean_generator* gen, double dt, int substeps, int64_t origin_x, int64_t origin_z, int num_sources,
+                    const ocean_wake_source* sources_host, int num_states, const ocean_body_state* states_host);
+int ocean_wake_step_device(ocean_generator* gen, double dt, int substeps, int64_t origin_x, int64_t origin_z, int num_sources,
+                           const ocean_wake_source* sources_dev, int num_states, const ocean_body_state* states_dev);
+int ocean_wake_render_map(ocean_generator* gen, void* map_dev, float* world_rect);
+int ocean_sample_wake(ocean_generator* gen, int num_points, const float* points_xz_host, float* out_host);
+int ocean_sample_wake_device(ocean_generator* gen, int num_points, const float* points_xz_dev, float* out_dev);
+int ocean_wake_get_state(ocean_generator* gen, float* h_host, float* h_prev_host, int64_t* origin_xz);
+int ocean_wake_set_state(ocean_generator* gen, const float* h_host, const float* h_prev_host, int64_t origin_x, int64_t origin_z);
 
 /* Parity/debug taps (not timed): binary32 maps before the half conversion, the row-pass output
  * ([4][N][N][2] float, == fft_buffer half 1 after the first fft_compute, wave_generator.gd:79) and

@@ -2,6 +2,7 @@
 config.
 
     python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast] [--spray-particles]
+                                [--wake]
 
 Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
 --query.  An unknown argument exits before anything touches the GPU."""
@@ -207,6 +208,31 @@ def run_spray_particles(N, C, amount, reps, label):
     per = alternate(lambda: timed(g, call, reps, 180 if clock[0] == 0.0 else 3))[0]
     out = {"config": label, **card(), "map_size": N, "cascades": C, "particles": amount, "live": int(count.item()),
            "us_per_call": [1e3 * v for v in per], "best_us": 1e3 * min(per), "mparticles_per_s": amount / (min(per) * 1e-3) / 1e6}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
+def run_wake(N, sources, reps, label, substeps=8, dx=0.5):
+    """Wake layer: ocean_wake_step_device with `sources` device-resident sources of radius 2 m spread over the window, moving
+    at 3 m/s; `substeps` sub-steps of 1/60 s per call, the window fixed.  Per cell and sub-step the specification's step
+    reads 169 values of s (13 x 13) and does 141 + 27 adds, 28 multiplies and 5 operations of the update."""
+    g, _, _ = warmed_generator(128, 2, 1)
+    g.wake_init(N, dx, 0.05, 32, 3.0)
+    rng = np.random.default_rng(N + sources)
+    s = np.zeros(sources, gow.WaveGenerator.WAKE_SOURCE)
+    s["x"], s["z"] = rng.uniform(0, N * dx, sources), rng.uniform(0, N * dx, sources)
+    s["vx"], s["vz"] = 3.0, 0.0
+    s["radius"], s["head"], s["body"] = 2.0, 0.1, -1
+    src = upload(s)
+    lib = load_library()
+    call = lambda: check(lib.ocean_wake_step_device(g.context, substeps / 60.0, substeps, 0, 0, sources, src.data_ptr(), 0, None))
+    per = alternate(lambda: timed(g, call, reps, 3))[0]
+    sub_us = [1e3 * v / substeps for v in per]
+    best = min(sub_us)
+    cells = N * N
+    out = {"config": label, **card(), "size": N, "cell_size": dx, "sources": sources, "substeps_per_call": substeps,
+           "us_per_substep": sub_us, "best_us_per_substep": best, "gcells_per_s": cells / (best * 1e-6) / 1e9,
+           "smem_GBps_spec": 169 * 4 * cells / (best * 1e-6) / 1e9, "fp32_Gops_spec": 201 * cells / (best * 1e-6) / 1e9}
     g.free()
     print(json.dumps(out), flush=True)
 
@@ -569,6 +595,10 @@ GROUPS = {          # flag: its configs, in the order they run
     "--spray-particles": [
         partial(run_spray_particles, 256, 4, 32768, 100, "spray particles: the reference emitter (32768 particles) over 4 cascades of 256x256"),
         partial(run_spray_particles, 256, 4, 1 << 20, 50, "spray particles: 2^20 particles over 4 cascades of 256x256"),
+    ],
+    "--wake": [
+        partial(run_wake, N, k, 200 if N < 1024 else 50, f"wake layer: {N}x{N} cells, {k} source(s)")
+        for N in (256, 512, 1024) for k in (1, 64, 1024)
     ],
 }
 DEFAULT = ("--updates", "--query")
