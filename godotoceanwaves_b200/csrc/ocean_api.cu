@@ -1214,7 +1214,7 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
     const int blocks = ocean::spray_blocks(emitter->amount);
     OCEAN_CUDA(gen->spray_counts.grow(gen, (size_t)blocks + 1));
-    OCEAN_CUDA(ocean::launch_spray_particles(gen->buf, num_cascades, gen->q_scales.ptr, emitter, t0, t1, states_dev, gen->spray_counts.ptr,
+    OCEAN_CUDA(ocean::launch_spray_particles(gen->buf, num_cascades, gen->q_scales.ptr, *emitter, t0, t1, states_dev, gen->spray_counts.ptr,
                                              instances_dev, max_instances, gen->stream));
     gen->kernel_launches += 3;
     OCEAN_CUDA(cudaMemcpyAsync(num_live_dev, gen->spray_counts.ptr + blocks, sizeof(int), cudaMemcpyDeviceToDevice, gen->stream));
@@ -1912,8 +1912,8 @@ int check_wake_layer(ocean_generator* g) {
 }
 
 // The call's sub-step and per-ring coefficients, or an error for an invalid step.
-int wake_step_args(ocean_generator* g, double dt, int substeps, int num_sources, const void* sources, int num_states, const void* states,
-                   ocean::WakeStepArgs* a, float* h_sub) {
+int wake_step_args(ocean_generator* g, double dt, int substeps, int num_sources, const ocean_wake_source* sources, int num_states,
+                   const ocean_body_state* states, ocean::WakeStepArgs* a, float* h_sub) {
     if (!(dt > 0.0) || !std::isfinite(dt)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "dt %g is not finite and > 0", dt);
     if (substeps < 1 || substeps > 256) return fail(OCEAN_ERR_INVALID_ARGUMENT, "substeps %d outside [1, 256]", substeps);
     if (num_sources < 0 || num_states < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "negative source or state count");

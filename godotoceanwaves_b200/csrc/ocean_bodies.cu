@@ -131,24 +131,23 @@ __global__ void __launch_bounds__(256) k_bodies_integrate(const ocean_floating_b
 
 }  // namespace
 
-cudaError_t launch_bodies_prepare(const void* bodies_dev, const void* states_dev, int num_bodies, const void* points_dev, float* r2_dev,
-                                  void* pose_dev, void* velocities_dev, cudaStream_t stream) {
+cudaError_t launch_bodies_prepare(const ocean_floating_body* bodies_dev, const ocean_body_state* states_dev, int num_bodies,
+                                  const ocean_buoyancy_point* points_dev, float* r2_dev, ocean_buoyancy_body* pose_dev,
+                                  ocean_body_velocity* velocities_dev, cudaStream_t stream) {
     if (num_bodies <= 0) return cudaSuccess;
     const unsigned blocks = (unsigned)(((size_t)num_bodies * 32 + 255) / 256);      // 8 bodies per block
-    k_bodies_prepare<<<blocks, 256, 0, stream>>>(static_cast<const ocean_floating_body*>(bodies_dev), static_cast<const ocean_body_state*>(states_dev),
-                                                 num_bodies, static_cast<const ocean_buoyancy_point*>(points_dev), r2_dev,
-                                                 static_cast<ocean_buoyancy_body*>(pose_dev), static_cast<ocean_body_velocity*>(velocities_dev));
+    k_bodies_prepare<<<blocks, 256, 0, stream>>>(bodies_dev, states_dev, num_bodies, points_dev, r2_dev, pose_dev, velocities_dev);
     return cudaGetLastError();
 }
 
-cudaError_t launch_bodies_integrate(const void* bodies_dev, const float* r2_dev, int num_bodies, const void* hydrostatic_dev, const void* drag_dev,
-                                    float density, float h, void* states_dev, void* pose_dev, void* velocities_dev, float* transforms_dev,
-                                    cudaStream_t stream) {
+cudaError_t launch_bodies_integrate(const ocean_floating_body* bodies_dev, const float* r2_dev, int num_bodies,
+                                    const ocean_buoyancy_result* hydrostatic_dev, const ocean_drag_result* drag_dev, float density, float h,
+                                    ocean_body_state* states_dev, ocean_buoyancy_body* pose_dev, ocean_body_velocity* velocities_dev,
+                                    float* transforms_dev, cudaStream_t stream) {
     if (num_bodies <= 0) return cudaSuccess;
-    k_bodies_integrate<<<(unsigned)((num_bodies + 255) / 256), 256, 0, stream>>>(
-        static_cast<const ocean_floating_body*>(bodies_dev), r2_dev, num_bodies, static_cast<const ocean_buoyancy_result*>(hydrostatic_dev),
-        static_cast<const ocean_drag_result*>(drag_dev), density, h, static_cast<ocean_body_state*>(states_dev),
-        static_cast<ocean_buoyancy_body*>(pose_dev), static_cast<ocean_body_velocity*>(velocities_dev), transforms_dev);
+    k_bodies_integrate<<<(unsigned)((num_bodies + 255) / 256), 256, 0, stream>>>(bodies_dev, r2_dev, num_bodies, hydrostatic_dev, drag_dev,
+                                                                                 density, h, states_dev, pose_dev, velocities_dev,
+                                                                                 transforms_dev);
     return cudaGetLastError();
 }
 

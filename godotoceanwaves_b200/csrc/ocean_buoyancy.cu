@@ -190,35 +190,30 @@ __global__ void __launch_bounds__(256) k_drag_reduce(const ocean_buoyancy_body* 
 
 }  // namespace
 
-cudaError_t launch_buoyancy_transform(const void* bodies_dev, const int* offsets_dev, int num_bodies, const void* points_dev, int n,
-                                      float2* q_dev, cudaStream_t stream) {
+cudaError_t launch_buoyancy_transform(const ocean_buoyancy_body* bodies_dev, const int* offsets_dev, int num_bodies,
+                                      const ocean_buoyancy_point* points_dev, int n, float2* q_dev, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
-    k_buoyancy_transform<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(static_cast<const ocean_buoyancy_body*>(bodies_dev), offsets_dev,
-                                                                         num_bodies, static_cast<const ocean_buoyancy_point*>(points_dev), n, q_dev);
+    k_buoyancy_transform<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(bodies_dev, offsets_dev, num_bodies, points_dev, n, q_dev);
     return cudaGetLastError();
 }
 
-cudaError_t launch_buoyancy_reduce(const void* bodies_dev, const int* offsets_dev, int num_bodies, const void* points_dev,
-                                   const void* samples_dev, float rho_g, float tolerance, void* results_dev, cudaStream_t stream) {
+cudaError_t launch_buoyancy_reduce(const ocean_buoyancy_body* bodies_dev, const int* offsets_dev, int num_bodies,
+                                   const ocean_buoyancy_point* points_dev, const ocean_surface_sample* samples_dev, float rho_g,
+                                   float tolerance, ocean_buoyancy_result* results_dev, cudaStream_t stream) {
     if (num_bodies <= 0) return cudaSuccess;
     const unsigned blocks = (unsigned)(((size_t)num_bodies * 32 + 255) / 256);      // 8 bodies per block
-    k_buoyancy_reduce<<<blocks, 256, 0, stream>>>(static_cast<const ocean_buoyancy_body*>(bodies_dev), offsets_dev, num_bodies,
-                                                  static_cast<const ocean_buoyancy_point*>(points_dev),
-                                                  static_cast<const ocean_surface_sample*>(samples_dev), rho_g, tolerance,
-                                                  static_cast<ocean_buoyancy_result*>(results_dev));
+    k_buoyancy_reduce<<<blocks, 256, 0, stream>>>(bodies_dev, offsets_dev, num_bodies, points_dev, samples_dev, rho_g, tolerance, results_dev);
     return cudaGetLastError();
 }
 
-cudaError_t launch_drag_reduce(const void* bodies_dev, const void* velocities_dev, const int* offsets_dev, int num_bodies,
-                               const void* points_dev, const float* drag_areas_dev, const void* samples_dev, const uint2* velocity_dev,
-                               int map_size, int num_cascades, const float4* scales_dev, float half_rho, void* results_dev, cudaStream_t stream) {
+cudaError_t launch_drag_reduce(const ocean_buoyancy_body* bodies_dev, const ocean_body_velocity* velocities_dev, const int* offsets_dev,
+                               int num_bodies, const ocean_buoyancy_point* points_dev, const float* drag_areas_dev,
+                               const ocean_surface_sample* samples_dev, const uint2* velocity_dev, int map_size, int num_cascades,
+                               const float4* scales_dev, float half_rho, ocean_drag_result* results_dev, cudaStream_t stream) {
     if (num_bodies <= 0) return cudaSuccess;
     const unsigned blocks = (unsigned)(((size_t)num_bodies * 32 + 255) / 256);      // 8 bodies per block
-    k_drag_reduce<<<blocks, 256, 0, stream>>>(static_cast<const ocean_buoyancy_body*>(bodies_dev),
-                                              static_cast<const ocean_body_velocity*>(velocities_dev), offsets_dev, num_bodies,
-                                              static_cast<const ocean_buoyancy_point*>(points_dev), drag_areas_dev,
-                                              static_cast<const ocean_surface_sample*>(samples_dev), velocity_dev, map_size, num_cascades,
-                                              scales_dev, half_rho, static_cast<ocean_drag_result*>(results_dev));
+    k_drag_reduce<<<blocks, 256, 0, stream>>>(bodies_dev, velocities_dev, offsets_dev, num_bodies, points_dev, drag_areas_dev, samples_dev,
+                                              velocity_dev, map_size, num_cascades, scales_dev, half_rho, results_dev);
     return cudaGetLastError();
 }
 

@@ -5,6 +5,8 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include "../../include/ocean.h"
+
 namespace ocean {
 
 constexpr int kMaxMapSize = 1024;
@@ -120,40 +122,43 @@ cudaError_t launch_rowpass_export(const DeviceBuffers& b, int scratch_layer, flo
 // ocean_sample.cu: batched map queries (water.gdshader:27-39,42-84); scales_dev = map_scales[num_cascades] as float4
 cudaError_t launch_sample_maps(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
                                float* disp_out_dev, float* grad_out_dev, cudaStream_t stream);
-// ocean_sample.cu: surface query (P + D_xz(P) = Q solved for P, then sampled; oracle/surface.py); out_dev = ocean_surface_sample[n],
+// ocean_sample.cu: surface query (P + D_xz(P) = Q solved for P, then sampled; oracle/surface.py); out_dev = [n] records,
 // scratch_dev = [surface_scratch_ints(num_cascades, n)] ints
 size_t surface_scratch_ints(int num_cascades, int n);
 cudaError_t launch_query_surface(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
-                                 float tolerance, int max_iterations, void* out_dev, int* scratch_dev, cudaStream_t stream);
-// ocean_sample.cu: ray cast against the displaced surface (oracle/raycast.py); rays_dev = ocean_ray[n], out_dev = ocean_ray_hit[n],
+                                 float tolerance, int max_iterations, ocean_surface_sample* out_dev, int* scratch_dev, cudaStream_t stream);
+// ocean_sample.cu: ray cast against the displaced surface (oracle/raycast.py); rays_dev / out_dev = [n] rays / hits,
 // bounds_dev = [3 * num_cascades] unsigned of scratch (the per-layer height and displacement bounds)
-cudaError_t launch_raycast(const DeviceBuffers& b, int num_cascades, const void* rays_dev, int n, const float4* scales_dev, float step,
-                           int max_samples, float tolerance, int max_iterations, unsigned* bounds_dev, void* out_dev, cudaStream_t stream);
+cudaError_t launch_raycast(const DeviceBuffers& b, int num_cascades, const ocean_ray* rays_dev, int n, const float4* scales_dev, float step,
+                           int max_samples, float tolerance, int max_iterations, unsigned* bounds_dev, ocean_ray_hit* out_dev,
+                           cudaStream_t stream);
 
-// ocean_buoyancy.cu: buoyancy (oracle/buoyancy.py).  bodies_dev = ocean_buoyancy_body[num_bodies], offsets_dev = the exclusive
-// prefix of their num_points (body-major world points), points_dev = ocean_buoyancy_point[], q_dev / samples_dev = [n] world
-// points' (x, z) / surface records, results_dev = ocean_buoyancy_result[num_bodies]
-cudaError_t launch_buoyancy_transform(const void* bodies_dev, const int* offsets_dev, int num_bodies, const void* points_dev, int n,
-                                      float2* q_dev, cudaStream_t stream);
-cudaError_t launch_buoyancy_reduce(const void* bodies_dev, const int* offsets_dev, int num_bodies, const void* points_dev,
-                                   const void* samples_dev, float rho_g, float tolerance, void* results_dev, cudaStream_t stream);
+// ocean_buoyancy.cu: buoyancy (oracle/buoyancy.py).  bodies_dev = [num_bodies], offsets_dev = the exclusive prefix of their
+// num_points (body-major world points), q_dev / samples_dev = [n] world points' (x, z) / surface records, results_dev = [num_bodies]
+cudaError_t launch_buoyancy_transform(const ocean_buoyancy_body* bodies_dev, const int* offsets_dev, int num_bodies,
+                                      const ocean_buoyancy_point* points_dev, int n, float2* q_dev, cudaStream_t stream);
+cudaError_t launch_buoyancy_reduce(const ocean_buoyancy_body* bodies_dev, const int* offsets_dev, int num_bodies,
+                                   const ocean_buoyancy_point* points_dev, const ocean_surface_sample* samples_dev, float rho_g,
+                                   float tolerance, ocean_buoyancy_result* results_dev, cudaStream_t stream);
 // The drag half of the body-forces op (oracle/drag.py), on the same bodies, offsets, points and surface records:
-// velocities_dev = ocean_body_velocity[num_bodies], drag_areas_dev = [num_points] C_d A parallel to points_dev, velocity_dev =
-// the velocity maps ([num_cascades used][map_size^2] 4 x half), results_dev = ocean_drag_result[num_bodies]
-cudaError_t launch_drag_reduce(const void* bodies_dev, const void* velocities_dev, const int* offsets_dev, int num_bodies,
-                               const void* points_dev, const float* drag_areas_dev, const void* samples_dev, const uint2* velocity_dev,
-                               int map_size, int num_cascades, const float4* scales_dev, float half_rho, void* results_dev, cudaStream_t stream);
+// velocities_dev = [num_bodies], drag_areas_dev = [num_points] C_d A parallel to points_dev, velocity_dev = the velocity maps
+// ([num_cascades used][map_size^2] 4 x half), results_dev = [num_bodies]
+cudaError_t launch_drag_reduce(const ocean_buoyancy_body* bodies_dev, const ocean_body_velocity* velocities_dev, const int* offsets_dev,
+                               int num_bodies, const ocean_buoyancy_point* points_dev, const float* drag_areas_dev,
+                               const ocean_surface_sample* samples_dev, const uint2* velocity_dev, int map_size, int num_cascades,
+                               const float4* scales_dev, float half_rho, ocean_drag_result* results_dev, cudaStream_t stream);
 
-// ocean_bodies.cu: the floating-body integrator (oracle/bodies.py).  bodies_dev = ocean_floating_body[num_bodies], states_dev =
-// ocean_body_state[num_bodies], r2_dev = [num_bodies] max |p|^2 over each hull, pose_dev / velocities_dev = the
-// ocean_buoyancy_body / ocean_body_velocity tables the body-forces kernels read.  prepare fills r2 and the first sub-step's
-// tables; integrate takes one sub-step of h from the records of the tables' pose and writes the next sub-step's tables, and
-// the 3 x 4 transforms ([num_bodies][12]) when transforms_dev is not null.
-cudaError_t launch_bodies_prepare(const void* bodies_dev, const void* states_dev, int num_bodies, const void* points_dev, float* r2_dev,
-                                  void* pose_dev, void* velocities_dev, cudaStream_t stream);
-cudaError_t launch_bodies_integrate(const void* bodies_dev, const float* r2_dev, int num_bodies, const void* hydrostatic_dev, const void* drag_dev,
-                                    float density, float h, void* states_dev, void* pose_dev, void* velocities_dev, float* transforms_dev,
-                                    cudaStream_t stream);
+// ocean_bodies.cu: the floating-body integrator (oracle/bodies.py).  bodies_dev / states_dev = [num_bodies], r2_dev =
+// [num_bodies] max |p|^2 over each hull, pose_dev / velocities_dev = the tables the body-forces kernels read.  prepare fills r2
+// and the first sub-step's tables; integrate takes one sub-step of h from the records of the tables' pose and writes the next
+// sub-step's tables, and the 3 x 4 transforms ([num_bodies][12]) when transforms_dev is not null.
+cudaError_t launch_bodies_prepare(const ocean_floating_body* bodies_dev, const ocean_body_state* states_dev, int num_bodies,
+                                  const ocean_buoyancy_point* points_dev, float* r2_dev, ocean_buoyancy_body* pose_dev,
+                                  ocean_body_velocity* velocities_dev, cudaStream_t stream);
+cudaError_t launch_bodies_integrate(const ocean_floating_body* bodies_dev, const float* r2_dev, int num_bodies,
+                                    const ocean_buoyancy_result* hydrostatic_dev, const ocean_drag_result* drag_dev, float density, float h,
+                                    ocean_body_state* states_dev, ocean_buoyancy_body* pose_dev, ocean_body_velocity* velocities_dev,
+                                    float* transforms_dev, cudaStream_t stream);
 
 // ocean_velocity.cu: velocity maps (oracle_velocity_update).  One record per cascade to recompute: the table slot and time of
 // the update that built the cascade's current maps.
@@ -177,13 +182,13 @@ cudaError_t launch_sample_velocity(const uint2* velocity_dev, int map_size, int 
 // [spray_blocks(n) + 1] ints of scratch whose last element receives the number of active candidates
 int spray_blocks(int n);
 cudaError_t launch_extract_spray(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
-                                 float3 particle_scale, int* counts_dev, void* records_dev, int max_records, cudaStream_t stream);
+                                 float3 particle_scale, int* counts_dev, ocean_spray_record* records_dev, int max_records, cudaStream_t stream);
 // ocean_spray.cu: one particle-process frame [t0, t1) of a spray emitter (oracle/spray_particles.py), three launches when
-// amount > 0.  emitter_host = ocean_spray_emitter, states_dev = ocean_spray_particle[amount] (updated in place), counts_dev =
-// [spray_blocks(amount) + 1] ints of scratch whose last element receives the number of live particles, instances_dev =
-// [max_instances][16] floats
-cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const void* emitter_host, double t0,
-                                   double t1, void* states_dev, int* counts_dev, float* instances_dev, int max_instances, cudaStream_t stream);
+// amount > 0.  states_dev = [amount] (updated in place), counts_dev = [spray_blocks(amount) + 1] ints of scratch whose last
+// element receives the number of live particles, instances_dev = [max_instances][16] floats
+cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const ocean_spray_emitter& emitter,
+                                   double t0, double t1, ocean_spray_particle* states_dev, int* counts_dev, float* instances_dev,
+                                   int max_instances, cudaStream_t stream);
 
 // ocean_wake.cu: the wake layer (oracle/wake.py).  One sub-step of the layer: h / h_prev ([n][n], read at (i + di, j + dj),
 // 0 outside: the scroll folded into the reads) to out_h, and, when out_h_prev is not null, the scrolled h to out_h_prev.
@@ -194,8 +199,8 @@ struct WakeStepArgs {
     const float* h_prev;
     float* out_h;
     float* out_h_prev;
-    const void* sources;                            // ocean_wake_source[num_sources]
-    const void* states;                             // ocean_body_state[num_states]
+    const ocean_wake_source* sources;               // [num_sources]
+    const ocean_body_state* states;                 // [num_states]
     int num_sources, num_states;
     int n, di, dj, sponge_cells;
     float cell, x0, z0, tau;

@@ -18,6 +18,7 @@
 // trial give D and its exact bilinear Jacobian), then samples the maps at P with the same per-point body as k_sample_maps.
 // The ray cast (ocean_raycast; oracle/raycast.py is the specification) marches each ray through the height slab of the maps
 // with the same inversion, warm-started from sample to sample, and refines the first crossing.
+#include "../../include/ocean.h"
 #include "ocean_kernels.cuh"
 #include "ocean_texture.cuh"
 
@@ -108,14 +109,6 @@ __global__ void __launch_bounds__(256) k_sample_velocity(const uint2* __restrict
 // The shader reads the maps at the undisplaced point P and moves the vertex to P + D_xz(P) (:28,37), so the query solves
 // P + D_xz(P) = Q by damped Newton steps on the displacement layers, then samples the maps at P.
 
-struct SurfaceSample {       // == ocean_surface_sample (include/ocean.h), 40 bytes
-    float source_x, source_z;
-    float displacement[3];
-    float gradient_foam[3];
-    float residual;
-    uint32_t iterations;
-};
-
 struct SurfaceEval {         // D_xz(P) and J = dD_xz/dP
     float dx, dz, jxx, jxz, jzx, jzz;
 };
@@ -176,10 +169,10 @@ __device__ float surface_solve(const uint2* __restrict__ displacement, int N, in
 
 __device__ __forceinline__ void surface_write(const uint2* __restrict__ displacement, const uint2* __restrict__ normal, int N, int C,
                                               const float4* __restrict__ scales, float px, float pz, float r, uint32_t iterations,
-                                              SurfaceSample* __restrict__ out) {
+                                              ocean_surface_sample* __restrict__ out) {
     float3 d, g;
     sample_point(displacement, normal, N, C, make_float2(px, pz), scales, d, g);
-    SurfaceSample s;
+    ocean_surface_sample s;
     s.source_x = px;
     s.source_z = pz;
     s.displacement[0] = d.x; s.displacement[1] = d.y; s.displacement[2] = d.z;
@@ -193,7 +186,7 @@ __device__ __forceinline__ void surface_write(const uint2* __restrict__ displace
 // its end point, residual and steps into its own record and appends its index to `pending` for k_surface_restart.
 __global__ void __launch_bounds__(256) k_surface_first(const uint2* __restrict__ displacement, const uint2* __restrict__ normal, int N, int C,
                                                        const float2* __restrict__ points, int n, const float4* __restrict__ scales, float tol,
-                                                       int max_iterations, SurfaceSample* __restrict__ out, int* __restrict__ pending_count,
+                                                       int max_iterations, ocean_surface_sample* __restrict__ out, int* __restrict__ pending_count,
                                                        int* __restrict__ pending) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -231,7 +224,7 @@ __global__ void __launch_bounds__(256) k_surface_bound(const uint2* __restrict__
 constexpr int kRestartBlock = 64;
 __global__ void __launch_bounds__(kRestartBlock, 8) k_surface_restart(const uint2* __restrict__ displacement, const uint2* __restrict__ normal, int N, int C,
                                                          const float2* __restrict__ points, const float4* __restrict__ scales, float tol,
-                                                         int max_iterations, SurfaceSample* __restrict__ out, const int* __restrict__ pending_count,
+                                                         int max_iterations, ocean_surface_sample* __restrict__ out, const int* __restrict__ pending_count,
                                                          const int* __restrict__ pending, const unsigned* __restrict__ layer_max) {
     const int count = *pending_count;
     float rho = 0.0f;
@@ -264,21 +257,6 @@ __global__ void __launch_bounds__(kRestartBlock, 8) k_surface_restart(const uint
 
 // ---- ray cast: the first crossing of each ray with the displaced surface (oracle/raycast.py is the specification) ----
 
-struct Ray {                 // == ocean_ray (include/ocean.h), 28 bytes
-    float ox, oy, oz, dx, dy, dz, t_max;
-};
-
-struct RayHit {              // == ocean_ray_hit (include/ocean.h), 72 bytes
-    float t;
-    float position[3];
-    float source_x, source_z;
-    float displacement[3];
-    float gradient_foam[3];
-    float gap;
-    float residual;
-    uint32_t status, evaluations, iterations, unconverged;
-};
-constexpr uint32_t kRayMiss = 0, kRayFromAbove = 1, kRayFromBelow = 2, kRayTruncated = 3, kRayInvalid = 4;
 constexpr int kRayRefineSteps = 32;
 
 // Signed floats as unsigned keys in the same order (atomicMax over signed values).
@@ -320,13 +298,13 @@ struct RayPoint {
 // One gap evaluation at parameter t, started at Q or (warm) from the evaluated point `base` shifted by the ray's horizontal
 // advance since it, with the surface query's restarts when that start does not converge.
 __device__ __forceinline__ RayPoint ray_gap(const uint2* __restrict__ displacement, int N, int C, const float4* __restrict__ scales,
-                                            const Ray& ray, float t, bool warm, float base_x, float base_z, float base_px, float base_pz,
+                                            const ocean_ray& ray, float t, bool warm, float base_x, float base_z, float base_px, float base_pz,
                                             float tol, int max_iterations, float rho, uint32_t& iterations, uint32_t& unconverged) {
     RayPoint e;
     e.t = t;
-    e.x = ray.ox + t * ray.dx;
-    e.y = ray.oy + t * ray.dy;
-    e.z = ray.oz + t * ray.dz;
+    e.x = ray.origin[0] + t * ray.direction[0];
+    e.y = ray.origin[1] + t * ray.direction[1];
+    e.z = ray.origin[2] + t * ray.direction[2];
     const float2 q = make_float2(e.x, e.z);
     float px = q.x, pz = q.y;
     if (warm && max_iterations > 0) {
@@ -380,16 +358,17 @@ __device__ __forceinline__ RayPoint ray_gap(const uint2* __restrict__ displaceme
 // One thread per ray: slab clip, march, Illinois refinement, and the map sample at the reported point.  bounds = the
 // per-layer maxima of k_raycast_bound.  (128, 4) lets ptxas keep the ray's state in registers (no spill).
 __global__ void __launch_bounds__(128, 4) k_raycast(const uint2* __restrict__ displacement, const uint2* __restrict__ normal, int N, int C,
-                                                 const Ray* __restrict__ rays, int n, const float4* __restrict__ scales, float step,
+                                                 const ocean_ray* __restrict__ rays, int n, const float4* __restrict__ scales, float step,
                                                  int max_samples, float tol, int max_iterations, const unsigned* __restrict__ bounds,
-                                                 RayHit* __restrict__ out) {
+                                                 ocean_ray_hit* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const Ray ray = rays[i];
-    RayHit hit = {};
-    const bool finite = isfinite(ray.ox) && isfinite(ray.oy) && isfinite(ray.oz) && isfinite(ray.dx) && isfinite(ray.dy) && isfinite(ray.dz);
-    if (!finite || (ray.dx == 0.0f && ray.dy == 0.0f && ray.dz == 0.0f) || !(ray.t_max >= 0.0f)) {
-        hit.status = kRayInvalid;
+    const ocean_ray ray = rays[i];
+    ocean_ray_hit hit = {};
+    const bool finite = isfinite(ray.origin[0]) && isfinite(ray.origin[1]) && isfinite(ray.origin[2]) && isfinite(ray.direction[0]) &&
+                        isfinite(ray.direction[1]) && isfinite(ray.direction[2]);
+    if (!finite || (ray.direction[0] == 0.0f && ray.direction[1] == 0.0f && ray.direction[2] == 0.0f) || !(ray.t_max >= 0.0f)) {
+        hit.status = OCEAN_RAY_INVALID;
         out[i] = hit;
         return;
     }
@@ -409,25 +388,25 @@ __global__ void __launch_bounds__(128, 4) k_raycast(const uint2* __restrict__ di
     const float lo = y_lo - pad, hi = y_hi + pad;
     float t_in, t_out;
     bool enters;
-    if (ray.dy == 0.0f) {
+    if (ray.direction[1] == 0.0f) {
         t_in = 0.0f;
         t_out = ray.t_max;
-        enters = lo <= ray.oy && ray.oy <= hi;
+        enters = lo <= ray.origin[1] && ray.origin[1] <= hi;
     } else {
-        const float ta = __fdiv_rn(lo - ray.oy, ray.dy), tb = __fdiv_rn(hi - ray.oy, ray.dy);
+        const float ta = __fdiv_rn(lo - ray.origin[1], ray.direction[1]), tb = __fdiv_rn(hi - ray.origin[1], ray.direction[1]);
         const float tn = ta < tb ? ta : tb, tf = ta < tb ? tb : ta;
         t_in = tn > 0.0f ? tn : 0.0f;
         t_out = tf < ray.t_max ? tf : ray.t_max;
         enters = t_in <= t_out && isfinite(t_in);
     }
     if (!enters) {
-        hit.status = kRayMiss;
-        hit.position[0] = ray.ox; hit.position[1] = ray.oy; hit.position[2] = ray.oz;
+        hit.status = OCEAN_RAY_MISS;
+        hit.position[0] = ray.origin[0]; hit.position[1] = ray.origin[1]; hit.position[2] = ray.origin[2];
         out[i] = hit;
         return;
     }
-    const float h = __fdiv_rn(step, __fsqrt_rn(ray.dx * ray.dx + ray.dz * ray.dz));
-    uint32_t evaluations = 0, iterations = 0, unconverged = 0, status = kRayMiss;
+    const float h = __fdiv_rn(step, __fsqrt_rn(ray.direction[0] * ray.direction[0] + ray.direction[2] * ray.direction[2]));
+    uint32_t evaluations = 0, iterations = 0, unconverged = 0, status = OCEAN_RAY_MISS;
     // One evaluation per trip, so that ray_gap is inlined once.  March: a = the previous sample.  Refinement: [a, b] is the
     // bracket, wa / wb its Illinois weights, last = 1 (2) when the previous step replaced a (b).
     RayPoint a = {}, b = {}, rep = {};
@@ -438,14 +417,14 @@ __global__ void __launch_bounds__(128, 4) k_raycast(const uint2* __restrict__ di
         const RayPoint e = ray_gap(displacement, N, C, scales, ray, t, evaluations > 0, base_x, base_z, base_px, base_pz, tol, max_iterations,
                                    rho, iterations, unconverged);
         ++evaluations;
-        if (isnan(e.g)) { status = kRayInvalid; rep = e; break; }
+        if (isnan(e.g)) { status = OCEAN_RAY_INVALID; rep = e; break; }
         if (!refining) {
             const bool side = e.g > 0.0f;
             if (k == 0) above = side;
             if (k == 0 || side == above) {
                 rep = e;
                 if (t == t_out) break;                                      // MISS
-                if (evaluations == (uint32_t)max_samples) { status = kRayTruncated; break; }
+                if (evaluations == (uint32_t)max_samples) { status = OCEAN_RAY_TRUNCATED; break; }
                 ++k;
                 float tn = t_in + (float)k * h;
                 if (!(tn < t_out)) tn = t_out;
@@ -459,7 +438,7 @@ __global__ void __launch_bounds__(128, 4) k_raycast(const uint2* __restrict__ di
             b = e;
             wa = a.g;
             wb = b.g;
-            status = above ? kRayFromAbove : kRayFromBelow;
+            status = above ? OCEAN_RAY_HIT_FROM_ABOVE : OCEAN_RAY_HIT_FROM_BELOW;
         } else {
             ++steps;
             if ((e.g > 0.0f) == above) {
@@ -519,30 +498,30 @@ size_t surface_scratch_ints(int num_cascades, int n) { return 1 + (size_t)num_ca
 // Kernels: k_surface_first over all queries; with max_iterations > 0 also k_surface_bound (rho) and k_surface_restart over
 // the pending list, whose length only the device knows: a grid-stride loop on a grid sized for up to one query per thread.
 cudaError_t launch_query_surface(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
-                                 float tolerance, int max_iterations, void* out_dev, int* scratch_dev, cudaStream_t stream) {
+                                 float tolerance, int max_iterations, ocean_surface_sample* out_dev, int* scratch_dev, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     const int N = b.map_size;
-    SurfaceSample* out = static_cast<SurfaceSample*>(out_dev);
     int* count = scratch_dev;
     unsigned* layer_max = reinterpret_cast<unsigned*>(scratch_dev + 1);
     int* pending = scratch_dev + 1 + num_cascades;
     cudaError_t e = cudaMemsetAsync(scratch_dev, 0, sizeof(int) * (size_t)(1 + num_cascades), stream);
     if (e != cudaSuccess) return e;
     k_surface_first<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(b.displacement, b.normal, N, num_cascades, points_dev, n, scales_dev,
-                                                                    tolerance, max_iterations, out, count, pending);
+                                                                    tolerance, max_iterations, out_dev, count, pending);
     if ((e = cudaGetLastError()) != cudaSuccess || max_iterations == 0) return e;
     const unsigned bound_blocks = (unsigned)(((size_t)N * N + 4095) / 4096);     // 16 texels per thread
     k_surface_bound<<<dim3(bound_blocks, (unsigned)num_cascades), 256, 0, stream>>>(b.displacement, N, layer_max);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     const int restart_blocks = (n + kRestartBlock - 1) / kRestartBlock < 2048 ? (n + kRestartBlock - 1) / kRestartBlock : 2048;
     k_surface_restart<<<restart_blocks, kRestartBlock, 0, stream>>>(b.displacement, b.normal, N, num_cascades, points_dev, scales_dev, tolerance,
-                                                                   max_iterations, out, count, pending, layer_max);
+                                                                   max_iterations, out_dev, count, pending, layer_max);
     return cudaGetLastError();
 }
 
 // bounds_dev: [3 * num_cascades] unsigned, cleared here, then filled by k_raycast_bound; k_raycast reads them.
-cudaError_t launch_raycast(const DeviceBuffers& b, int num_cascades, const void* rays_dev, int n, const float4* scales_dev, float step,
-                           int max_samples, float tolerance, int max_iterations, unsigned* bounds_dev, void* out_dev, cudaStream_t stream) {
+cudaError_t launch_raycast(const DeviceBuffers& b, int num_cascades, const ocean_ray* rays_dev, int n, const float4* scales_dev, float step,
+                           int max_samples, float tolerance, int max_iterations, unsigned* bounds_dev, ocean_ray_hit* out_dev,
+                           cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     const int N = b.map_size;
     cudaError_t e = cudaMemsetAsync(bounds_dev, 0, sizeof(unsigned) * 3 * (size_t)num_cascades, stream);
@@ -550,9 +529,8 @@ cudaError_t launch_raycast(const DeviceBuffers& b, int num_cascades, const void*
     const unsigned bound_blocks = (unsigned)(((size_t)N * N + 4095) / 4096);     // 16 texels per thread
     k_raycast_bound<<<dim3(bound_blocks, (unsigned)num_cascades), 256, 0, stream>>>(b.displacement, N, bounds_dev);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    k_raycast<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(b.displacement, b.normal, N, num_cascades, static_cast<const Ray*>(rays_dev), n,
-                                                              scales_dev, step, max_samples, tolerance, max_iterations, bounds_dev,
-                                                              static_cast<RayHit*>(out_dev));
+    k_raycast<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(b.displacement, b.normal, N, num_cascades, rays_dev, n, scales_dev, step,
+                                                              max_samples, tolerance, max_iterations, bounds_dev, out_dev);
     return cudaGetLastError();
 }
 

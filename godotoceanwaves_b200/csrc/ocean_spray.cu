@@ -19,11 +19,10 @@
 //           particles are counted per block of 256
 //   scan    k_spray_scan on the block counts
 //   write   the instances of the live particles at block offset + rank (warp ballots): a stable compaction in INDEX order
+#include "../../include/ocean.h"
 #include "ocean_kernels.cuh"
 #include "ocean_texture.cuh"
 #include "detmath.cuh"
-
-#include <cstring>
 
 namespace ocean {
 
@@ -121,16 +120,10 @@ __global__ void __launch_bounds__(1024) k_spray_scan(int* __restrict__ counts, i
     if (threadIdx.x == 0) counts[blocks] = s_carry;
 }
 
-struct SprayRecord {        // == ocean_spray_record (include/ocean.h), 32 bytes
-    uint32_t index;
-    float start_x, start_z, scale_factor;
-    float particle_scale[3];
-    float foam;
-};
-
 __global__ void __launch_bounds__(kSprayBlock) k_spray_write(const uint2* __restrict__ normal, int N, int C, const float2* __restrict__ points, int n,
                                                              const float4* __restrict__ scales, float3 particle_scale,
-                                                             const int* __restrict__ block_offsets, SprayRecord* __restrict__ out, int max_records) {
+                                                             const int* __restrict__ block_offsets, ocean_spray_record* __restrict__ out,
+                                                             int max_records) {
     __shared__ int s_warp[kSprayBlock / 32];
     const int i = blockIdx.x * kSprayBlock + threadIdx.x;
     SprayEval e;
@@ -148,7 +141,7 @@ __global__ void __launch_bounds__(kSprayBlock) k_spray_write(const uint2* __rest
     for (int w = 0; w < warp; ++w) off += s_warp[w];
     off += __popc(ballot & ((1u << lane) - 1u));
     if (e.active && off < max_records) {
-        SprayRecord r;
+        ocean_spray_record r;
         r.index = (uint32_t)i;
         r.start_x = p.x;
         r.start_z = p.y;
@@ -162,24 +155,6 @@ __global__ void __launch_bounds__(kSprayBlock) k_spray_write(const uint2* __rest
 }
 
 // ---- the particle op ----
-struct SprayEmitter {       // == ocean_spray_emitter (include/ocean.h), 88 bytes
-    int32_t amount, num_particles;
-    float emission_transform[12];
-    float particle_scale[3];
-    float lifetime, lifetime_randomness;
-    uint32_t random_seed;
-    double emitter_lifetime;
-};
-
-struct SprayParticle {      // == ocean_spray_particle (include/ocean.h), 120 bytes
-    float transform[12];    // 3 x 4 row-major: basis x, basis y, basis z, origin
-    float custom[4];
-    float userdata1[4];     // START_POS, START_TIME
-    float userdata2[4];     // PARTICLE_SCALE, PARTICLE_LIFETIME
-    float userdata3[4];     // .z SCALE_FACTOR, .w HAS_STARTED
-    uint32_t number, flags;
-};
-constexpr uint32_t kParticleActive = 1u, kParticleEmitted = 2u;
 
 // :32-38
 __device__ __forceinline__ float3 spray_hash32(uint32_t px, uint32_t py) {
@@ -224,7 +199,7 @@ __device__ __forceinline__ long long restart_cycle(double L, double f, double t0
 }
 
 // start() :45-66, after the restart's reset of TRANSFORM and CUSTOM
-__device__ __forceinline__ void spray_start(SprayParticle& p, const SprayEmitter& e, uint32_t index, float time) {
+__device__ __forceinline__ void spray_start(ocean_spray_particle& p, const ocean_spray_emitter& e, uint32_t index, float time) {
     const uint32_t u = __float2uint_rz(time);
     const float3 rand = spray_hash32(p.number + u + e.random_seed, 1u + u + e.random_seed);
     const uint32_t t = __float2uint_rz(__fsqrt_rn(__uint2float_rn((uint32_t)e.num_particles)));
@@ -256,11 +231,12 @@ __device__ __forceinline__ void spray_start(SprayParticle& p, const SprayEmitter
 }
 
 // process() :74-126 of an ACTIVE particle
-__device__ __forceinline__ void spray_process(SprayParticle& p, const SprayEmitter& e, float time, const uint2* __restrict__ disp,
-                                              const uint2* __restrict__ normal, int N, int C, const float4* __restrict__ scales) {
+__device__ __forceinline__ void spray_process(ocean_spray_particle& p, const ocean_spray_emitter& e, float time,
+                                              const uint2* __restrict__ disp, const uint2* __restrict__ normal, int N, int C,
+                                              const float4* __restrict__ scales) {
     const float st = p.userdata1[3], pl = p.userdata2[3];
     if (time > st + pl) {
-        p.flags &= ~kParticleActive;
+        p.flags &= ~OCEAN_SPRAY_ACTIVE;
         return;
     }
     if (!(time >= st)) return;
@@ -269,7 +245,7 @@ __device__ __forceinline__ void spray_process(SprayParticle& p, const SprayEmitt
         const SprayFactors f = spray_factors(normal, N, C, sp, scales);
         const float nf = f.normal_factor, ff = f.foam_factor;
         const bool active = nf >= 0.0f && nf <= 1.0f && f.foam > 0.9f;
-        p.flags = active ? (p.flags | kParticleActive) : (p.flags & ~kParticleActive);
+        p.flags = active ? (p.flags | OCEAN_SPRAY_ACTIVE) : (p.flags & ~OCEAN_SPRAY_ACTIVE);
         p.userdata3[2] = nf * ff;
         const float s0 = ff * ((active ? 1.0f : 0.0f) + 1e-3f);
         p.userdata2[0] = (s0 * 1.0f) * e.particle_scale[0];
@@ -277,7 +253,7 @@ __device__ __forceinline__ void spray_process(SprayParticle& p, const SprayEmitt
         p.userdata2[2] = (s0 * 1.0f) * e.particle_scale[2];
         p.userdata3[3] = 1.0f;
     }
-    if (!(p.flags & kParticleActive)) return;
+    if (!(p.flags & OCEAN_SPRAY_ACTIVE)) return;
     const float t = __fdiv_rn(time - st, pl);                                                      // :99
     p.custom[3] = exp_impulse(t, 10.0f);
     float dx = 0.0f, dy = 0.0f, dz = 0.0f;
@@ -303,16 +279,19 @@ __device__ __forceinline__ void spray_process(SprayParticle& p, const SprayEmitt
     spray_set_scale(p.transform, p.userdata2[0] * mx, p.userdata2[1] * my, p.userdata2[2] * mz);
 }
 
-__device__ __forceinline__ bool spray_live(const SprayParticle& p) { return (p.flags & kParticleActive) && p.userdata3[3] != 0.0f; }
+__device__ __forceinline__ bool spray_live(const ocean_spray_particle& p) {
+    return (p.flags & OCEAN_SPRAY_ACTIVE) && p.userdata3[3] != 0.0f;
+}
 
-__global__ void __launch_bounds__(kSprayBlock) k_spray_particles_update(const SprayEmitter e, double t0, double t1, float time,
+__global__ void __launch_bounds__(kSprayBlock) k_spray_particles_update(const ocean_spray_emitter e, double t0, double t1, float time,
                                                                         const uint2* __restrict__ disp, const uint2* __restrict__ normal,
                                                                         int N, int C, const float4* __restrict__ scales,
-                                                                        SprayParticle* __restrict__ states, int* __restrict__ block_counts) {
+                                                                        ocean_spray_particle* __restrict__ states,
+                                                                        int* __restrict__ block_counts) {
     const int i = blockIdx.x * kSprayBlock + threadIdx.x;
     bool live = false;
     if (i < e.amount) {
-        SprayParticle p = states[i];
+        ocean_spray_particle p = states[i];
         const double f = __ddiv_rn((double)i, (double)e.amount);
         const long long k = restart_cycle(e.emitter_lifetime, f, t0, t1);
         if (k >= 0) {
@@ -321,10 +300,10 @@ __global__ void __launch_bounds__(kSprayBlock) k_spray_particles_update(const Sp
             for (int j = 0; j < 12; ++j) p.transform[j] = (j % 5 == 0) ? 1.0f : 0.0f;
 #pragma unroll
             for (int j = 0; j < 4; ++j) p.custom[j] = 0.0f;
-            p.flags |= kParticleActive | kParticleEmitted;
+            p.flags |= OCEAN_SPRAY_ACTIVE | OCEAN_SPRAY_EMITTED;
             spray_start(p, e, (uint32_t)i, time);
         }
-        if (p.flags & kParticleActive) spray_process(p, e, time, disp, normal, N, C, scales);
+        if (p.flags & OCEAN_SPRAY_ACTIVE) spray_process(p, e, time, disp, normal, N, C, scales);
         states[i] = p;
         live = spray_live(p);
     }
@@ -332,7 +311,7 @@ __global__ void __launch_bounds__(kSprayBlock) k_spray_particles_update(const Sp
     if (threadIdx.x == 0) block_counts[blockIdx.x] = total;
 }
 
-__global__ void __launch_bounds__(kSprayBlock) k_spray_particles_write(const SprayParticle* __restrict__ states, int n,
+__global__ void __launch_bounds__(kSprayBlock) k_spray_particles_write(const ocean_spray_particle* __restrict__ states, int n,
                                                                        const int* __restrict__ block_offsets, float* __restrict__ instances,
                                                                        int max_instances) {
     __shared__ int s_warp[kSprayBlock / 32];
@@ -346,7 +325,7 @@ __global__ void __launch_bounds__(kSprayBlock) k_spray_particles_write(const Spr
     for (int w = 0; w < warp; ++w) off += s_warp[w];
     off += __popc(ballot & ((1u << lane) - 1u));
     if (live && off < max_instances) {
-        const SprayParticle& p = states[i];
+        const ocean_spray_particle& p = states[i];
         float* o = instances + (size_t)off * 16;
 #pragma unroll
         for (int j = 0; j < 12; ++j) o[j] = p.transform[j];
@@ -362,7 +341,7 @@ int spray_blocks(int n) { return (n + kSprayBlock - 1) / kSprayBlock; }
 // counts_dev: [spray_blocks(n) + 1] ints of scratch; on completion counts_dev[spray_blocks(n)] = number of active
 // candidates (which may exceed max_records: the records beyond it are dropped, the count is not clamped).
 cudaError_t launch_extract_spray(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
-                                 float3 particle_scale, int* counts_dev, void* records_dev, int max_records, cudaStream_t stream) {
+                                 float3 particle_scale, int* counts_dev, ocean_spray_record* records_dev, int max_records, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     const int blocks = spray_blocks(n);
     k_spray_count<<<blocks, kSprayBlock, 0, stream>>>(b.normal, b.map_size, num_cascades, points_dev, n, scales_dev, particle_scale, counts_dev);
@@ -372,28 +351,25 @@ cudaError_t launch_extract_spray(const DeviceBuffers& b, int num_cascades, const
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     k_spray_write<<<blocks, kSprayBlock, 0, stream>>>(b.normal, b.map_size, num_cascades, points_dev, n, scales_dev, particle_scale, counts_dev,
-                                                      static_cast<SprayRecord*>(records_dev), max_records);
+                                                      records_dev, max_records);
     return cudaGetLastError();
 }
 
 // counts_dev: [spray_blocks(amount) + 1] ints of scratch; on completion counts_dev[spray_blocks(amount)] = number of live
 // particles (which may exceed max_instances: the instances beyond it are dropped, the count is not clamped).
-cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const void* emitter_host, double t0,
-                                   double t1, void* states_dev, int* counts_dev, float* instances_dev, int max_instances, cudaStream_t stream) {
-    static_assert(sizeof(SprayEmitter) == 88 && sizeof(SprayParticle) == 120, "spray particle op layouts");
-    SprayEmitter e;
-    memcpy(&e, emitter_host, sizeof e);
-    if (e.amount <= 0) return cudaSuccess;
-    const int blocks = spray_blocks(e.amount);
-    SprayParticle* states = static_cast<SprayParticle*>(states_dev);
-    k_spray_particles_update<<<blocks, kSprayBlock, 0, stream>>>(e, t0, t1, (float)t1, b.displacement, b.normal, b.map_size, num_cascades,
-                                                                 scales_dev, states, counts_dev);
+cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const ocean_spray_emitter& emitter,
+                                   double t0, double t1, ocean_spray_particle* states_dev, int* counts_dev, float* instances_dev,
+                                   int max_instances, cudaStream_t stream) {
+    if (emitter.amount <= 0) return cudaSuccess;
+    const int blocks = spray_blocks(emitter.amount);
+    k_spray_particles_update<<<blocks, kSprayBlock, 0, stream>>>(emitter, t0, t1, (float)t1, b.displacement, b.normal, b.map_size, num_cascades,
+                                                                 scales_dev, states_dev, counts_dev);
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) return err;
     k_spray_scan<<<1, 1024, 0, stream>>>(counts_dev, blocks);
     err = cudaGetLastError();
     if (err != cudaSuccess) return err;
-    k_spray_particles_write<<<blocks, kSprayBlock, 0, stream>>>(states, e.amount, counts_dev, instances_dev, max_instances);
+    k_spray_particles_write<<<blocks, kSprayBlock, 0, stream>>>(states_dev, emitter.amount, counts_dev, instances_dev, max_instances);
     return cudaGetLastError();
 }
 

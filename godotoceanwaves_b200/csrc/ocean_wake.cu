@@ -127,12 +127,12 @@ __global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
             bool keep = false;
             float4 e = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
             if (k < a.num_sources) {
-                const ocean_wake_source src = static_cast<const ocean_wake_source*>(a.sources)[k];
+                const ocean_wake_source src = a.sources[k];
                 float cx = __fadd_rn(src.x, __fmul_rn(src.vx, a.tau));
                 float cz = __fadd_rn(src.z, __fmul_rn(src.vz, a.tau));
                 bool ok = src.body < a.num_states;
                 if (ok && src.body >= 0) {
-                    const ocean_body_state& b = static_cast<const ocean_body_state*>(a.states)[src.body];
+                    const ocean_body_state& b = a.states[src.body];
                     cx = __fadd_rn(cx, __fadd_rn(b.position[0], __fmul_rn(b.linear_velocity[0], a.tau)));
                     cz = __fadd_rn(cz, __fadd_rn(b.position[2], __fmul_rn(b.linear_velocity[2], a.tau)));
                 }

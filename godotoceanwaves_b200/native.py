@@ -35,85 +35,6 @@ class InfoC(C.Structure):
                 ("cascade_updates", C.c_uint64), ("device_bytes", C.c_uint64)]
 
 
-class RayC(C.Structure):
-    """struct ocean_ray (include/ocean.h), 28 B: origin, direction (need not be unit), t_max (+inf allowed)"""
-    _fields_ = [("origin", C.c_float * 3), ("direction", C.c_float * 3), ("t_max", C.c_float)]
-
-
-class RayHitC(C.Structure):
-    """struct ocean_ray_hit (include/ocean.h), 72 B"""
-    _fields_ = [("t", C.c_float), ("position", C.c_float * 3), ("source_x", C.c_float), ("source_z", C.c_float),
-                ("displacement", C.c_float * 3), ("gradient_foam", C.c_float * 3), ("gap", C.c_float), ("residual", C.c_float),
-                ("status", C.c_uint32), ("evaluations", C.c_uint32), ("iterations", C.c_uint32), ("unconverged", C.c_uint32)]
-
-
-class BuoyancyPointC(C.Structure):
-    """struct ocean_buoyancy_point (include/ocean.h), 20 B: body-local position, volume (m^3), half height (m)"""
-    _fields_ = [("position", C.c_float * 3), ("volume", C.c_float), ("half_height", C.c_float)]
-
-
-class BuoyancyBodyC(C.Structure):
-    """struct ocean_buoyancy_body (include/ocean.h), 56 B: 3 x 4 row-major body-to-world [R | t], hull-point range"""
-    _fields_ = [("transform", C.c_float * 12), ("first_point", C.c_int32), ("num_points", C.c_int32)]
-
-
-class BuoyancyResultC(C.Structure):
-    """struct ocean_buoyancy_result (include/ocean.h), 48 B"""
-    _fields_ = [("force", C.c_float * 3), ("torque", C.c_float * 3), ("submerged_volume", C.c_float),
-                ("center_offset", C.c_float * 3), ("max_residual", C.c_float), ("unconverged", C.c_uint32)]
-
-
-class BodyVelocityC(C.Structure):
-    """struct ocean_body_velocity (include/ocean.h), 24 B: world-frame velocity of the body origin (m/s), angular velocity (rad/s)"""
-    _fields_ = [("linear", C.c_float * 3), ("angular", C.c_float * 3)]
-
-
-class DragResultC(C.Structure):
-    """struct ocean_drag_result (include/ocean.h), 32 B"""
-    _fields_ = [("force", C.c_float * 3), ("torque", C.c_float * 3), ("wetted_drag_area", C.c_float), ("max_relative_speed", C.c_float)]
-
-
-class FloatingBodyC(C.Structure):
-    """struct ocean_floating_body (include/ocean.h), 24 B: mass (kg), principal inertia (kg m^2), range into the hull points"""
-    _fields_ = [("mass", C.c_float), ("inertia", C.c_float * 3), ("first_point", C.c_int32), ("num_points", C.c_int32)]
-
-
-class BodyStateC(C.Structure):
-    """struct ocean_body_state (include/ocean.h), 52 B: centre of mass, unit quaternion (x, y, z, w), world-frame velocities"""
-    _fields_ = [("position", C.c_float * 3), ("orientation", C.c_float * 4), ("linear_velocity", C.c_float * 3),
-                ("angular_velocity", C.c_float * 3)]
-
-
-class SprayEmitterC(C.Structure):
-    """struct ocean_spray_emitter (include/ocean.h), 88 B"""
-    _fields_ = [("amount", C.c_int32), ("num_particles", C.c_int32), ("emission_transform", C.c_float * 12),
-                ("particle_scale", C.c_float * 3), ("lifetime", C.c_float), ("lifetime_randomness", C.c_float),
-                ("random_seed", C.c_uint32), ("emitter_lifetime", C.c_double)]
-
-
-class SprayParticleC(C.Structure):
-    """struct ocean_spray_particle (include/ocean.h), 120 B: TRANSFORM (3 x 4 row-major), CUSTOM, USERDATA1..3, NUMBER, flags"""
-    _fields_ = [("transform", C.c_float * 12), ("custom", C.c_float * 4), ("userdata1", C.c_float * 4), ("userdata2", C.c_float * 4),
-                ("userdata3", C.c_float * 4), ("number", C.c_uint32), ("flags", C.c_uint32)]
-
-
-class WakeParamsC(C.Structure):
-    """struct ocean_wake_params (include/ocean.h), 20 B"""
-    _fields_ = [("size", C.c_int32), ("sponge_cells", C.c_int32), ("cell_size", C.c_float), ("damping", C.c_float),
-                ("sponge_damping", C.c_float)]
-
-
-class WakeSourceC(C.Structure):
-    """struct ocean_wake_source (include/ocean.h), 28 B"""
-    _fields_ = [("x", C.c_float), ("z", C.c_float), ("vx", C.c_float), ("vz", C.c_float), ("radius", C.c_float),
-                ("head", C.c_float), ("body", C.c_int32)]
-
-
-assert C.sizeof(WakeParamsC) == 20 and WakeParamsC.sponge_damping.offset == 16
-assert C.sizeof(WakeSourceC) == 28 and WakeSourceC.body.offset == 24
-assert C.sizeof(SprayEmitterC) == 88 and SprayEmitterC.emitter_lifetime.offset == 80
-assert C.sizeof(SprayParticleC) == 120 and SprayParticleC.flags.offset == 116
-
 # every symbol include/ocean.h declares: name -> (restype, argtypes)
 _H = C.c_void_p
 _P = C.POINTER
@@ -175,13 +96,13 @@ SIGNATURES = {
     "ocean_spray_grid":(C.c_int, [C.c_int, C.c_void_p, C.c_void_p]),
     "ocean_extract_spray": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, _P(C.c_int)]),
     "ocean_extract_spray_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "ocean_default_spray_emitter": (C.c_int, [_P(SprayEmitterC)]),
-    "ocean_spray_particles": (C.c_int, [_H, _P(SprayEmitterC), C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+    "ocean_default_spray_emitter": (C.c_int, [C.c_void_p]),
+    "ocean_spray_particles": (C.c_int, [_H, C.c_void_p, C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                         C.c_void_p, _P(C.c_int)]),
-    "ocean_spray_particles_device": (C.c_int, [_H, _P(SprayEmitterC), C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+    "ocean_spray_particles_device": (C.c_int, [_H, C.c_void_p, C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                                C.c_void_p, C.c_void_p]),
     "ocean_wake_kernel_taps": (C.c_int, [C.c_void_p]),
-    "ocean_wake_init": (C.c_int, [_H, _P(WakeParamsC)]),
+    "ocean_wake_init": (C.c_int, [_H, C.c_void_p]),
     "ocean_wake_step": (C.c_int, [_H, C.c_double, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
     "ocean_wake_step_device": (C.c_int, [_H, C.c_double, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
     "ocean_wake_render_map": (C.c_int, [_H, C.c_void_p, C.c_void_p]),

@@ -10,7 +10,6 @@ import ctypes as C
 
 import numpy as np
 
-from . import native
 from .native import CascadeParamsC, InfoC, OceanError, check, load_library
 
 G = 9.81        # wave_generator.gd:5
@@ -432,9 +431,9 @@ class WaveGenerator:
     @staticmethod
     def default_spray_emitter() -> np.ndarray:
         """The reference scene's emitter (ocean_default_spray_emitter) as a 0-d SPRAY_EMITTER array."""
-        e = native.SprayEmitterC()
-        check(load_library().ocean_default_spray_emitter(C.byref(e)))
-        return np.frombuffer(C.string_at(C.addressof(e), C.sizeof(e)), WaveGenerator.SPRAY_EMITTER).reshape(()).copy()
+        e = np.zeros((), WaveGenerator.SPRAY_EMITTER)
+        check(load_library().ocean_default_spray_emitter(e.ctypes.data))
+        return e
 
     def spray_particles(self, emitter, states, t0: float, t1: float, map_scales, max_instances: int | None = None):
         """One particle-process frame [t0, t1) of the emitter (include/ocean.h, ocean_spray_particles): the restarts, start()
@@ -443,7 +442,6 @@ class WaveGenerator:
         particles), where n = min(count, max_instances)."""
         self._require()
         e = np.array(emitter, self.SPRAY_EMITTER).reshape(())
-        ec = native.SprayEmitterC.from_buffer_copy(e.tobytes())
         amount = max(int(e["amount"]), 0)
         s = np.zeros(amount, self.SPRAY_PARTICLE) if states is None else np.array(states, self.SPRAY_PARTICLE, copy=True).reshape(-1)
         if len(s) != amount:
@@ -452,7 +450,7 @@ class WaveGenerator:
         cap = amount if max_instances is None else int(max_instances)
         inst = np.zeros((max(cap, 0), 16), np.float32)
         count = C.c_int(0)
-        check(load_library().ocean_spray_particles(self.context, C.byref(ec), float(t0), float(t1), sc.shape[0], sc.ctypes.data,
+        check(load_library().ocean_spray_particles(self.context, e.ctypes.data, float(t0), float(t1), sc.shape[0], sc.ctypes.data,
                                                    s.ctypes.data, cap, inst.ctypes.data, C.byref(count)))
         return s, inst[:min(count.value, cap)], count.value
 
@@ -474,8 +472,8 @@ class WaveGenerator:
         """(Re)create the wake layer, zeroed at origin (0, 0): size x size cells of cell_size metres (include/ocean.h,
         ocean_wake_init).  size = 0 releases it."""
         self._require()
-        p = native.WakeParamsC(int(size), int(sponge_cells), float(cell_size), float(damping), float(sponge_damping))
-        check(load_library().ocean_wake_init(self.context, C.byref(p)))
+        p = np.array((int(size), int(sponge_cells), float(cell_size), float(damping), float(sponge_damping)), self.WAKE_PARAMS)
+        check(load_library().ocean_wake_init(self.context, p.ctypes.data))
         self._wake_size = int(size)
 
     def wake_step(self, dt: float, substeps: int = 1, origin=(0, 0), sources=None, states=None) -> None:

@@ -2,8 +2,6 @@
 the generator's own maps and velocity maps: byte-identical 52-byte states, buoyancy and drag records and transforms after
 several calls of several sub-steps; the records against ocean_body_forces; composition, isolation of bad bodies, rest on
 flat water, launch counts, side effects and arguments."""
-import ctypes
-
 import numpy as np
 import pytest
 
@@ -176,10 +174,9 @@ def test_box_at_equilibrium_on_flat_water_stays_exactly_at_rest():
 
 def test_launch_counts_and_host_equals_device():
     import torch
-    from godotoceanwaves_b200 import native
     from godotoceanwaves_b200.native import check, load_library
-    assert ctypes.sizeof(native.FloatingBodyC) == 24 and ctypes.sizeof(native.BodyStateC) == 52
     gow, g, params = _gen(256, 4)
+    assert gow.WaveGenerator.FLOATING_BODY.itemsize == 24 and gow.WaveGenerator.BODY_STATE.itemsize == 52
     scales = _scales(gow, params, 4)
     bodies, s0, hull, cda = _bodies(431, np.random.default_rng(430).integers(0, 80, 600))
     g.update_velocity()

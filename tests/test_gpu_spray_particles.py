@@ -140,7 +140,7 @@ def _warm(g, e, scales, until=5.0):
 
 def test_device_entry_point_equals_host_and_truncation():
     import torch
-    from godotoceanwaves_b200.native import SprayEmitterC, check, load_library
+    from godotoceanwaves_b200.native import check, load_library
     gow, g, p, scales = _foamy()
     e = _rotated_emitter(gow)
     st, t = _warm(g, e, scales)
@@ -150,9 +150,9 @@ def test_device_entry_point_equals_host_and_truncation():
     st_d = torch.from_numpy(st.view(np.uint8).copy()).to(dev)
     inst_d = torch.full((len(st) * 16,), -1.0, dtype=torch.float32, device=dev)
     count_d = torch.full((1,), -1, dtype=torch.int32, device=dev)
-    ec = SprayEmitterC.from_buffer_copy(np.array(e, g.SPRAY_EMITTER).tobytes())
+    ec = np.array(e, g.SPRAY_EMITTER)
     torch.cuda.synchronize()
-    check(load_library().ocean_spray_particles_device(g.context, C.byref(ec), t, t + 0.04, 4, scales.ctypes.data, st_d.data_ptr(), len(st),
+    check(load_library().ocean_spray_particles_device(g.context, ec.ctypes.data, t, t + 0.04, 4, scales.ctypes.data, st_d.data_ptr(), len(st),
                                                       inst_d.data_ptr(), count_d.data_ptr()))
     g.synchronize()
     assert int(count_d.cpu()[0]) == count
@@ -173,7 +173,6 @@ def _lib():
 
 def test_launch_counts_and_arguments():
     import torch
-    from godotoceanwaves_b200.native import SprayEmitterC
     gow, g, p, scales = _foamy(128, 2)
     e = gow.WaveGenerator.default_spray_emitter()
     e["amount"] = 5000
@@ -207,20 +206,20 @@ def test_launch_counts_and_arguments():
     bad.append((tiny, 0.0, 10.0, 2, scales, 5000))                  # t1 / emitter_lifetime >= 2^32
     for host in (True, False):
         for b, t0, t1, nc, sc, cap in bad:
-            ec = SprayEmitterC.from_buffer_copy(np.array(b, g.SPRAY_EMITTER).tobytes())
+            ec = np.array(b, g.SPRAY_EMITTER)
             s_host = st.copy()
             before = g.info().kernel_launches
             if host:
-                rc = lib.ocean_spray_particles(g.context, C.byref(ec), t0, t1, nc, None if sc is None else sc.ctypes.data, s_host.ctypes.data,
+                rc = lib.ocean_spray_particles(g.context, ec.ctypes.data, t0, t1, nc, None if sc is None else sc.ctypes.data, s_host.ctypes.data,
                                                cap, inst.ctypes.data, C.byref(count))
             else:
-                rc = lib.ocean_spray_particles_device(g.context, C.byref(ec), t0, t1, nc, None if sc is None else sc.ctypes.data,
+                rc = lib.ocean_spray_particles_device(g.context, ec.ctypes.data, t0, t1, nc, None if sc is None else sc.ctypes.data,
                                                       st_d.data_ptr(), cap, inst_d.data_ptr(), count_d.data_ptr())
             assert rc == INVALID, (host, b, t0, t1, nc, cap)
             assert g.info().kernel_launches == before
             assert s_host.tobytes() == st.tobytes()
         # NULL where a count needs the buffer
-        ec = SprayEmitterC.from_buffer_copy(np.array(e, g.SPRAY_EMITTER).tobytes())
+        ec = np.array(e, g.SPRAY_EMITTER)
         fn = lib.ocean_spray_particles if host else lib.ocean_spray_particles_device
         st_host = st.copy()
         sp_ = st_host.ctypes.data if host else st_d.data_ptr()
@@ -228,14 +227,14 @@ def test_launch_counts_and_arguments():
         cp = C.byref(count) if host else count_d.data_ptr()
         before = g.info().kernel_launches
         assert fn(g.context, None, t, t + 0.03, 2, scales.ctypes.data, sp_, 5000, ip, cp) == INVALID
-        assert fn(g.context, C.byref(ec), t, t + 0.03, 2, scales.ctypes.data, None, 5000, ip, cp) == INVALID
-        assert fn(g.context, C.byref(ec), t, t + 0.03, 2, scales.ctypes.data, sp_, 5000, None, cp) == INVALID
-        assert fn(g.context, C.byref(ec), t, t + 0.03, 2, scales.ctypes.data, sp_, 5000, ip, None) == INVALID
+        assert fn(g.context, ec.ctypes.data, t, t + 0.03, 2, scales.ctypes.data, None, 5000, ip, cp) == INVALID
+        assert fn(g.context, ec.ctypes.data, t, t + 0.03, 2, scales.ctypes.data, sp_, 5000, None, cp) == INVALID
+        assert fn(g.context, ec.ctypes.data, t, t + 0.03, 2, scales.ctypes.data, sp_, 5000, ip, None) == INVALID
         assert g.info().kernel_launches == before
         # ... and NULL is fine where no count needs it
-        assert fn(g.context, C.byref(ec), t, t + 0.03, 2, scales.ctypes.data, sp_, 0, None, cp) == 0
-        z = SprayEmitterC.from_buffer_copy(np.array(zero, g.SPRAY_EMITTER).tobytes())
-        assert fn(g.context, C.byref(z), t, t + 0.03, 2, scales.ctypes.data, None, 0, None, cp) == 0
+        assert fn(g.context, ec.ctypes.data, t, t + 0.03, 2, scales.ctypes.data, sp_, 0, None, cp) == 0
+        z = np.array(zero, g.SPRAY_EMITTER)
+        assert fn(g.context, z.ctypes.data, t, t + 0.03, 2, scales.ctypes.data, None, 0, None, cp) == 0
         assert g.info().kernel_launches == before + 3
     g.synchronize()
     assert int(count_d.cpu()[0]) == 0 and count.value == 0

@@ -256,11 +256,11 @@ def test_launch_counts_and_invalid_arguments():
     assert lib.ocean_wake_render_map(g.context, None, None) == INVALID
     assert lib.ocean_sample_wake(g.context, -1, None, None) == INVALID
     assert lib.ocean_sample_wake(g.context, 3, None, None) == INVALID
-    from godotoceanwaves_b200.native import WakeParamsC
     for bad in [(100, 16, 0.5, 0.0, 1.0), (4096, 16, 0.5, 0.0, 1.0), (256, 65, 0.5, 0.0, 1.0), (128, 65, 0.5, 0.0, 1.0),
                 (256, 16, 0.0, 0.0, 1.0), (256, 16, np.nan, 0.0, 1.0), (256, 16, 0.5, -1.0, 1.0), (256, 16, 0.5, 0.0, np.inf),
                 (256, -1, 0.5, 0.0, 1.0)]:
-        assert lib.ocean_wake_init(g.context, ctypes.byref(WakeParamsC(*bad))) == INVALID, bad
+        p = np.array(bad, g.WAKE_PARAMS)
+        assert lib.ocean_wake_init(g.context, p.ctypes.data) == INVALID, bad
     assert g.info().kernel_launches == before
     h2, hp2, o2 = g.wake_state()
     assert h2.tobytes() == h.tobytes() and hp2.tobytes() == hp.tobytes() and o2 == o

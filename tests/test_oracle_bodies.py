@@ -44,12 +44,13 @@ def _run(maps, bodies, states, hull, cda, dt, substeps, calls, density=RHO):
     return states, out
 
 
-def test_layouts_match_the_ctypes_structures_and_the_header():
-    from godotoceanwaves_b200 import native
+def test_layouts_match_the_bindings():
     from godotoceanwaves_b200.wave_generator import WaveGenerator
-    import ctypes
-    assert ob.BODY.itemsize == ctypes.sizeof(native.FloatingBodyC) == 24
-    assert ob.STATE.itemsize == ctypes.sizeof(native.BodyStateC) == 52
+    for dt, wg, size in [(ob.BODY, WaveGenerator.FLOATING_BODY, 24), (ob.STATE, WaveGenerator.BODY_STATE, 52)]:
+        assert dt.itemsize == wg.itemsize == size
+        assert dt.names == wg.names
+        for name in dt.names:
+            assert dt.fields[name][1] == wg.fields[name][1], name
     assert WaveGenerator.FLOATING_BODY == ob.BODY and WaveGenerator.BODY_STATE == ob.STATE
 
 

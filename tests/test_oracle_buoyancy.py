@@ -1,6 +1,5 @@
 """CPU checks of the buoyancy specification (oracle/buoyancy.py): hydrostatic force and torque per body from hull points
 on the displaced water surface, with a fixed per-body reduction order."""
-import ctypes as C
 import math
 
 import numpy as np
@@ -93,15 +92,14 @@ def _trochoid_height(A, kn, khat, x, z):
     return A * np.cos(kn * s)
 
 
-def test_record_layouts_match_the_ctypes_structures():
-    from godotoceanwaves_b200 import native
+def test_record_layouts_match_the_bindings():
     from godotoceanwaves_b200.wave_generator import WaveGenerator
-    for dt, st, size in [(bu.POINT, native.BuoyancyPointC, 20), (bu.BODY, native.BuoyancyBodyC, 56),
-                         (bu.RESULT, native.BuoyancyResultC, 48)]:
-        assert dt.itemsize == C.sizeof(st) == size
-        assert list(dt.names) == [f[0] for f in st._fields_]
+    for dt, wg, size in [(bu.POINT, WaveGenerator.BUOYANCY_POINT, 20), (bu.BODY, WaveGenerator.BUOYANCY_BODY, 56),
+                         (bu.RESULT, WaveGenerator.BUOYANCY_RESULT, 48)]:
+        assert dt.itemsize == wg.itemsize == size
+        assert dt.names == wg.names
         for name in dt.names:
-            assert dt.fields[name][1] == getattr(st, name).offset, name
+            assert dt.fields[name][1] == wg.fields[name][1], name
     assert WaveGenerator.BUOYANCY_POINT == bu.POINT and WaveGenerator.BUOYANCY_BODY == bu.BODY
     assert WaveGenerator.BUOYANCY_RESULT == bu.RESULT
 

@@ -1,6 +1,5 @@
 """CPU checks of the body-forces specification (oracle/drag.py): quadratic drag against the water velocity per body, next to
 the unchanged buoyancy record, with the buoyancy op's fixed per-body reduction order."""
-import ctypes as C
 import math
 import os
 import re
@@ -39,16 +38,15 @@ def _velocities(linear, angular=None):
     return v
 
 
-def test_record_layouts_match_the_ctypes_structures_and_the_header():
-    from godotoceanwaves_b200 import native
+def test_record_layouts_match_the_bindings_and_the_header():
     from godotoceanwaves_b200.wave_generator import WaveGenerator
     header = open(os.path.join(ROOT, "include", "ocean.h")).read()
-    for dt, st, size, name in [(dr.VELOCITY, native.BodyVelocityC, 24, "ocean_body_velocity"),
-                               (dr.RESULT, native.DragResultC, 32, "ocean_drag_result")]:
-        assert dt.itemsize == C.sizeof(st) == size
-        assert list(dt.names) == [f[0] for f in st._fields_]
+    for dt, wg, size, name in [(dr.VELOCITY, WaveGenerator.BODY_VELOCITY, 24, "ocean_body_velocity"),
+                               (dr.RESULT, WaveGenerator.DRAG_RESULT, 32, "ocean_drag_result")]:
+        assert dt.itemsize == wg.itemsize == size
+        assert dt.names == wg.names
         for field in dt.names:
-            assert dt.fields[field][1] == getattr(st, field).offset, field
+            assert dt.fields[field][1] == wg.fields[field][1], field
         body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (name, name), header, re.S).group(1)
         fields = re.findall(r"float (\w+)(?:\[(\d)\])?;", body)
         assert [f for f, _ in fields] == list(dt.names)

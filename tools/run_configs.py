@@ -6,7 +6,6 @@ config.
 
 Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
 --query.  An unknown argument exits before anything touches the GPU."""
-import ctypes
 import json
 import os
 import subprocess
@@ -21,7 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import godotoceanwaves_b200 as gow
 from bench import synth_params
-from godotoceanwaves_b200.native import SprayEmitterC, check, load_library
+from godotoceanwaves_b200.native import check, load_library
 from oracle import bodies as ob
 from oracle import buoyancy as bu
 from oracle import drag as dr
@@ -192,7 +191,6 @@ def run_spray_particles(N, C, amount, reps, label):
     g, _, scales = warmed_generator(N, C, 25, configure)
     e = gow.WaveGenerator.default_spray_emitter()
     e["amount"] = e["num_particles"] = amount
-    ec = SprayEmitterC.from_buffer_copy(e.tobytes())
     states = torch.zeros(amount * gow.WaveGenerator.SPRAY_PARTICLE.itemsize, dtype=torch.uint8, device=DEV)
     inst = torch.empty(amount * 16, dtype=torch.float32, device=DEV)
     count = torch.zeros(1, dtype=torch.int32, device=DEV)
@@ -202,7 +200,7 @@ def run_spray_particles(N, C, amount, reps, label):
     def call():
         t0 = clock[0]
         clock[0] = t0 + 1.0 / 30.0
-        check(lib.ocean_spray_particles_device(g.context, ctypes.byref(ec), t0, clock[0], C, scales.ctypes.data, states.data_ptr(), amount, inst.data_ptr(),
+        check(lib.ocean_spray_particles_device(g.context, e.ctypes.data, t0, clock[0], C, scales.ctypes.data, states.data_ptr(), amount, inst.data_ptr(),
                                                count.data_ptr()))
 
     per = alternate(lambda: timed(g, call, reps, 180 if clock[0] == 0.0 else 3))[0]
