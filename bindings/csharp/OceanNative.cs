@@ -275,6 +275,11 @@ namespace OceanB200
         internal static partial int ocean_wake_get_state(IntPtr handle, float* h, float* h_prev, long* origin_xz);
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_wake_set_state(IntPtr handle, float* h, float* h_prev, long origin_x, long origin_z);
+        // wake coupling: the surface query, buoyancy, body forces and the body integrator read the wake free surface (enable 0 or 1)
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_set_coupling(IntPtr handle, int enable);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_get_coupling(IntPtr handle, float* e, float* e_old, long* origins, float* interval);
         // surface query: the surface at world positions points [n][2] (P + D_xz(P) = Q solved for P, then the map query at P)
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,

@@ -6,6 +6,7 @@
 #include "../../include/ocean.h"
 #include "ocean_kernels.cuh"
 
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -159,6 +160,14 @@ struct ocean_generator {
     ocean_wake_params wake{};                           // size 0: no layer
     int wake_h = 0, wake_hp = 1;                        // which fields hold h and h_prev
     int64_t wake_origin[2] = {0, 0};
+    // wake coupling (ocean_wake_set_coupling): two [size][size] snapshots of the free surface e = h + phi, each with its window
+    // origin, the interval between them, and the drag pass's per-world-point vertical velocity
+    DeviceArray<float> wake_snapshots;
+    DeviceArray<float> wake_wv;
+    bool wake_coupled = false, wake_primed = false;
+    int wake_e = 0;                                     // which snapshot holds e (the other holds e_old)
+    int64_t wake_snapshot_origin[2][2] = {};            // [snapshot][x, z]
+    float wake_interval = 0.0f;                         // T
 };
 
 namespace {
@@ -1260,14 +1269,37 @@ int check_surface_args(int num_points, float tolerance, int max_iterations) {
     return OCEAN_OK;
 }
 
+float wake_corner(int64_t origin, float cell);
+
+// The surface query reads the wake layer while its coupling is on and primed (ocean_wake_set_coupling).
+bool wake_coupling_live(const ocean_generator* g) { return g->wake.size > 0 && g->wake_coupled && g->wake_primed; }
+
 // The surface query on validated arguments, with the map scales already in gen->q_scales (ocean_query_surface_device and
-// ocean_buoyancy_device).
+// ocean_buoyancy_device).  With the wake coupling live, one more kernel adds the wake free surface to the records and, when
+// wv_dev is not null (a drag pass follows), writes the wake's vertical velocity of each point there.
 int run_query_surface(ocean_generator* gen, int num_points, const float2* points_xz_dev, int num_cascades, float tolerance,
-                      int max_iterations, ocean_surface_sample* out_dev) {
+                      int max_iterations, ocean_surface_sample* out_dev, float* wv_dev = nullptr) {
     OCEAN_CUDA(gen->surf_scratch.grow(gen, ocean::surface_scratch_ints(gen->num_cascades, num_points)));
     OCEAN_CUDA(ocean::launch_query_surface(gen->buf, num_cascades, points_xz_dev, num_points, gen->q_scales.ptr, tolerance, max_iterations,
                                            out_dev, gen->surf_scratch.ptr, gen->stream));
     gen->kernel_launches += max_iterations > 0 ? 3 : 1;
+    if (wake_coupling_live(gen)) {
+        const size_t cells = (size_t)gen->wake.size * gen->wake.size;
+        const int e = gen->wake_e, o = e ^ 1;
+        const float dx = gen->wake.cell_size;
+        ocean::WakeCoupleArgs a{};
+        a.e = gen->wake_snapshots.ptr + e * cells;
+        a.e_old = gen->wake_snapshots.ptr + o * cells;
+        a.n = gen->wake.size;
+        a.cell = dx;
+        a.x0 = wake_corner(gen->wake_snapshot_origin[e][0], dx);
+        a.z0 = wake_corner(gen->wake_snapshot_origin[e][1], dx);
+        a.x0_old = wake_corner(gen->wake_snapshot_origin[o][0], dx);
+        a.z0_old = wake_corner(gen->wake_snapshot_origin[o][1], dx);
+        a.interval = gen->wake_interval;
+        OCEAN_CUDA(ocean::launch_wake_couple(a, points_xz_dev, num_points, out_dev, wv_dev, gen->stream));
+        gen->kernel_launches += 1;
+    }
     return OCEAN_OK;
 }
 }  // namespace
@@ -1395,15 +1427,16 @@ int upload_offsets(ocean_generator* gen, int num_bodies, const Body* bodies_host
 }
 
 // The buoyancy launches on a body table and offsets already in device memory (bodies_dev may be written by earlier kernels on
-// the stream), with the map scales in gen->q_scales and gen->buoy_q grown to `world`: samples receives the surface records.
+// the stream), with the map scales in gen->q_scales and gen->buoy_q grown to `world`: samples receives the surface records, and
+// wv_dev (may be null) the wake's vertical velocity of each world point while the wake coupling is live.
 int launch_buoyancy_sequence(ocean_generator* gen, const ocean_buoyancy_body* bodies_dev, const int* offsets_dev, int num_bodies, int world,
                              const ocean_buoyancy_point* points_dev, int num_cascades, float density, float tolerance, int max_iterations,
-                             ocean_buoyancy_result* results_dev, ocean_surface_sample* samples) {
+                             ocean_buoyancy_result* results_dev, ocean_surface_sample* samples, float* wv_dev = nullptr) {
     int rc;
     if (world > 0) {
         OCEAN_CUDA(ocean::launch_buoyancy_transform(bodies_dev, offsets_dev, num_bodies, points_dev, world, gen->buoy_q.ptr, gen->stream));
         gen->kernel_launches += 1;
-        if ((rc = run_query_surface(gen, world, gen->buoy_q.ptr, num_cascades, tolerance, max_iterations, samples))) return rc;
+        if ((rc = run_query_surface(gen, world, gen->buoy_q.ptr, num_cascades, tolerance, max_iterations, samples, wv_dev))) return rc;
     }
     const float rho_g = density * 9.81f;                                 // G, wave_generator.gd:5, in binary32
     OCEAN_CUDA(ocean::launch_buoyancy_reduce(bodies_dev, offsets_dev, num_bodies, points_dev, samples, rho_g, tolerance, results_dev,
@@ -1417,7 +1450,7 @@ int launch_buoyancy_sequence(ocean_generator* gen, const ocean_buoyancy_body* bo
 // (samples_dev, or the generator's staging when samples_dev is NULL) for a drag pass on the same points.
 int run_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int world, const ocean_buoyancy_point* points_dev,
                  int num_cascades, float density, float tolerance, int max_iterations, ocean_buoyancy_result* results_dev,
-                 ocean_surface_sample* samples_dev, ocean_surface_sample** samples_used) {
+                 ocean_surface_sample* samples_dev, ocean_surface_sample** samples_used, float* wv_dev = nullptr) {
     int rc;
     OCEAN_CUDA(gen->buoy_q.grow(gen, (size_t)world));
     if (!samples_dev) OCEAN_CUDA(gen->buoy_samples.grow(gen, (size_t)world));
@@ -1425,7 +1458,7 @@ int run_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body
     OCEAN_CUDA(gen->buoy_bodies.upload(gen, bodies_host, (size_t)num_bodies));
     if ((rc = upload_offsets(gen, num_bodies, bodies_host))) return rc;
     if ((rc = launch_buoyancy_sequence(gen, gen->buoy_bodies.ptr, gen->buoy_offsets.ptr, num_bodies, world, points_dev, num_cascades, density,
-                                       tolerance, max_iterations, results_dev, samples)))
+                                       tolerance, max_iterations, results_dev, samples, wv_dev)))
         return rc;
     if (samples_used) *samples_used = samples;
     return OCEAN_OK;
@@ -1618,14 +1651,19 @@ int ocean_body_forces_device(ocean_generator* gen, int num_bodies, const ocean_b
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
     OCEAN_CUDA(gen->drag_velocities.upload(gen, velocities_host, (size_t)num_bodies));
+    float* wv = nullptr;
+    if (world > 0 && wake_coupling_live(gen)) {
+        OCEAN_CUDA(gen->wake_wv.grow(gen, (size_t)world));
+        wv = gen->wake_wv.ptr;
+    }
     ocean_surface_sample* samples = nullptr;
     if ((rc = run_buoyancy(gen, num_bodies, bodies_host, world, points_dev, num_cascades, density, tolerance, max_iterations, hydrostatic_dev,
-                           samples_dev, &samples)))
+                           samples_dev, &samples, wv)))
         return rc;
     const float half_rho = 0.5f * density;
     OCEAN_CUDA(ocean::launch_drag_reduce(gen->buoy_bodies.ptr, gen->drag_velocities.ptr, gen->buoy_offsets.ptr, num_bodies, points_dev,
                                          drag_areas_dev, samples, gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, half_rho,
-                                         drag_dev, gen->stream));
+                                         drag_dev, wv, gen->stream));
     gen->kernel_launches += 1;
     return OCEAN_OK;
 }
@@ -1715,6 +1753,11 @@ int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const oce
     OCEAN_CUDA(gen->drag_velocities.grow(gen, B));
     OCEAN_CUDA(gen->buoy_q.grow(gen, (size_t)world));
     OCEAN_CUDA(gen->buoy_samples.grow(gen, (size_t)world));
+    float* wv = nullptr;                                // every sub-step reads the same snapshots
+    if (world > 0 && wake_coupling_live(gen)) {
+        OCEAN_CUDA(gen->wake_wv.grow(gen, (size_t)world));
+        wv = gen->wake_wv.ptr;
+    }
     if (!hydrostatic_dev) {
         OCEAN_CUDA(gen->buoy_results.grow(gen, B));
         hydrostatic_dev = gen->buoy_results.ptr;
@@ -1734,11 +1777,11 @@ int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const oce
     const float half_rho = 0.5f * density;
     for (int s = 0; s < substeps; ++s) {
         if ((rc = launch_buoyancy_sequence(gen, poses, gen->buoy_offsets.ptr, num_bodies, world, points_dev, num_cascades, density, tolerance,
-                                           max_iterations, hydrostatic_dev, gen->buoy_samples.ptr)))
+                                           max_iterations, hydrostatic_dev, gen->buoy_samples.ptr, wv)))
             return rc;
         OCEAN_CUDA(ocean::launch_drag_reduce(poses, velocities, gen->buoy_offsets.ptr, num_bodies, points_dev, drag_areas_dev,
                                              gen->buoy_samples.ptr, gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, half_rho,
-                                             drag_dev, gen->stream));
+                                             drag_dev, wv, gen->stream));
         OCEAN_CUDA(ocean::launch_bodies_integrate(bodies, gen->sim_r2.ptr, num_bodies, hydrostatic_dev, drag_dev, density, h, states_dev, poses,
                                                   velocities, s == substeps - 1 ? transforms_dev : nullptr, gen->stream));
         gen->kernel_launches += 2;
@@ -1949,6 +1992,18 @@ int wake_step_args(ocean_generator* g, double dt, int substeps, int num_sources,
 // (float)((double)origin * dx), the window's world corner
 float wake_corner(int64_t origin, float cell) { return (float)((double)origin * (double)cell); }
 
+// Turns the coupling off and releases its buffers (the caller has entered the generator).
+int wake_uncouple(ocean_generator* g) {
+    if (g->wake_snapshots.ptr || g->wake_wv.ptr) OCEAN_CUDA(cudaStreamSynchronize(g->stream));    // kernels may still read them
+    g->wake_snapshots.release();
+    g->wake_wv.release();
+    g->wake_coupled = g->wake_primed = false;
+    g->wake_e = 0;
+    g->wake_interval = 0.0f;
+    for (auto& o : g->wake_snapshot_origin) o[0] = o[1] = 0;
+    return OCEAN_OK;
+}
+
 int check_wake_points(int num_points, const void* points, const void* out) {
     if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
     if (num_points > 0 && (!points || !out)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "points or out is NULL");
@@ -1962,6 +2017,7 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
     if (!params) return fail(OCEAN_ERR_INVALID_ARGUMENT, "params is NULL");
     const ocean_wake_params p = *params;
     if (p.size == 0) {
+        if ((rc = wake_uncouple(gen))) return rc;
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
         gen->wake_fields.release();
         gen->wake_sources.release();
@@ -1978,6 +2034,7 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
     if (p.sponge_cells < 0 || p.sponge_cells > ocean::kWakeMaxSponge || 2 * p.sponge_cells > p.size)
         return fail(OCEAN_ERR_INVALID_ARGUMENT, "sponge_cells %d outside [0, min(64, size / 2)]", p.sponge_cells);
     const size_t cells = 4 * (size_t)p.size * p.size;  // h, h_prev and two fields a scrolled sub-step writes
+    if ((rc = wake_uncouple(gen))) return rc;
     gen->wake = ocean_wake_params{};                    // no layer until the fields below are allocated and cleared
     if (gen->wake_fields.capacity != cells) {
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
@@ -2028,6 +2085,34 @@ int ocean_wake_step_device(ocean_generator* gen, double dt, int substeps, int64_
         gen->wake_origin[0] = origin_x;
         gen->wake_origin[1] = origin_z;
         a.di = a.dj = 0;
+    }
+    if (gen->wake_coupled) {
+        // e = h + phi at the end of the call into the snapshot that held e_old (on a priming call into both)
+        const size_t cells = (size_t)n * n;
+        const int e = gen->wake_primed ? gen->wake_e ^ 1 : gen->wake_e;
+        ocean::WakeFreeSurfaceArgs f{};
+        f.h = wake_field(gen, gen->wake_h);
+        f.e = gen->wake_snapshots.ptr + e * cells;
+        f.e_old = gen->wake_primed ? nullptr : gen->wake_snapshots.ptr + (e ^ 1) * cells;
+        f.sources = a.sources;
+        f.states = a.states;
+        f.num_sources = a.num_sources;
+        f.num_states = a.num_states;
+        f.n = n;
+        f.cell = a.cell;
+        f.x0 = a.x0;
+        f.z0 = a.z0;
+        f.tau = (float)substeps * h;
+        OCEAN_CUDA(ocean::launch_wake_free_surface(f, gen->stream));
+        gen->kernel_launches += 1;
+        for (int k = 0; k < 2; ++k) {
+            if (k != e && gen->wake_primed) continue;
+            gen->wake_snapshot_origin[k][0] = origin_x;
+            gen->wake_snapshot_origin[k][1] = origin_z;
+        }
+        gen->wake_e = e;
+        gen->wake_interval = f.tau;
+        gen->wake_primed = true;
     }
     return OCEAN_OK;
 }
@@ -2117,6 +2202,46 @@ int ocean_wake_set_state(ocean_generator* gen, const float* h_host, const float*
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     gen->wake_origin[0] = origin_x;
     gen->wake_origin[1] = origin_z;
+    gen->wake_primed = false;                           // the snapshots no longer describe the layer
+    return OCEAN_OK;
+}
+
+int ocean_wake_set_coupling(ocean_generator* gen, int enable) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (enable != 0 && enable != 1) return fail(OCEAN_ERR_INVALID_ARGUMENT, "enable %d is not 0 or 1", enable);
+    if (!enable) return wake_uncouple(gen);
+    if (gen->wake_coupled) return OCEAN_OK;
+    OCEAN_CUDA(gen->wake_snapshots.grow(gen, 2 * (size_t)gen->wake.size * gen->wake.size));
+    gen->wake_coupled = true;
+    gen->wake_primed = false;
+    return OCEAN_OK;
+}
+
+int ocean_wake_get_coupling(ocean_generator* gen, float* e_host, float* e_old_host, int64_t* origins, float* interval) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (!gen->wake_coupled) return fail(OCEAN_ERR_STATE, "the wake layer's coupling is off (ocean_wake_set_coupling)");
+    if (!e_host || !e_old_host || !origins || !interval) return fail(OCEAN_ERR_INVALID_ARGUMENT, "NULL argument");
+    const size_t cells = (size_t)gen->wake.size * gen->wake.size;
+    if (!gen->wake_primed) {
+        std::fill(e_host, e_host + cells, 0.0f);
+        std::fill(e_old_host, e_old_host + cells, 0.0f);
+        std::fill(origins, origins + 4, (int64_t)0);
+        *interval = 0.0f;
+        return OCEAN_OK;
+    }
+    const int e = gen->wake_e, o = e ^ 1;
+    OCEAN_CUDA(cudaMemcpyAsync(e_host, gen->wake_snapshots.ptr + e * cells, sizeof(float) * cells, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(e_old_host, gen->wake_snapshots.ptr + o * cells, sizeof(float) * cells, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    origins[0] = gen->wake_snapshot_origin[e][0];
+    origins[1] = gen->wake_snapshot_origin[e][1];
+    origins[2] = gen->wake_snapshot_origin[o][0];
+    origins[3] = gen->wake_snapshot_origin[o][1];
+    *interval = gen->wake_interval;
     return OCEAN_OK;
 }
 

@@ -15,6 +15,8 @@
 //   k_drag_reduce         one warp per body in the same lane order: recomputes r and f as k_buoyancy_reduce does; for a
 //                         submerged point (f > 0) gathers the velocity maps at the record's source point (4 texels per
 //                         cascade), and sums the quadratic drag force, its torque about the body origin and f * C_d A.
+//   k_drag_reduce_wake    the same with the wake layer's vertical velocity per world point added to the water velocity
+//                         (ocean_wake_set_coupling); both kernels are one inlined template, k_drag_reduce its uncoupled form.
 // Numeric policy: binary32, the specification's operation order, no contraction (-fmad=false).
 #include "../../include/ocean.h"
 #include "ocean_kernels.cuh"
@@ -116,12 +118,14 @@ __global__ void __launch_bounds__(256) k_buoyancy_reduce(const ocean_buoyancy_bo
 }
 
 // d = u - (v + w x r) per submerged point, F = ((f * cda) * |d|) d, T = r x F; per body half_rho * sum F, half_rho * sum T,
-// sum f * cda and the NaN-dropping max of |d| (from 0), each summed in k_buoyancy_reduce's order.
-__global__ void __launch_bounds__(256) k_drag_reduce(const ocean_buoyancy_body* __restrict__ bodies, const ocean_body_velocity* __restrict__ velocities,
-                                                     const int* __restrict__ offsets, int num_bodies, const ocean_buoyancy_point* __restrict__ points,
-                                                     const float* __restrict__ drag_areas, const ocean_surface_sample* __restrict__ samples,
-                                                     const uint2* __restrict__ velocity, int N, int C, const float4* __restrict__ scales,
-                                                     float half_rho, ocean_drag_result* __restrict__ out) {
+// sum f * cda and the NaN-dropping max of |d| (from 0), each summed in k_buoyancy_reduce's order.  With kWake, u.y also gets
+// the wake layer's vertical velocity wv of the world point.
+template <bool kWake>
+__device__ __forceinline__ void drag_reduce(const ocean_buoyancy_body* __restrict__ bodies, const ocean_body_velocity* __restrict__ velocities,
+                                            const int* __restrict__ offsets, int num_bodies, const ocean_buoyancy_point* __restrict__ points,
+                                            const float* __restrict__ drag_areas, const ocean_surface_sample* __restrict__ samples,
+                                            const uint2* __restrict__ velocity, int N, int C, const float4* __restrict__ scales,
+                                            float half_rho, ocean_drag_result* __restrict__ out, const float* __restrict__ wv) {
     const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (warp >= (size_t)num_bodies) return;        // whole warps: the shuffles below see all 32 lanes
     const int body = (int)warp;
@@ -135,6 +139,7 @@ __global__ void __launch_bounds__(256) k_drag_reduce(const ocean_buoyancy_body* 
     const ocean_buoyancy_point* hull = points + b.first_point;
     const float* cda = drag_areas + b.first_point;
     const ocean_surface_sample* rec = samples + offsets[body];
+    const float* wake = kWake ? wv + offsets[body] : nullptr;
     const ocean_body_velocity bv = velocities[body];
     const float ty = b.transform[7];
     float sfx = 0.0f, sfy = 0.0f, sfz = 0.0f, stx = 0.0f, sty = 0.0f, stz = 0.0f, sa = 0.0f, max_s = 0.0f;
@@ -148,6 +153,7 @@ __global__ void __launch_bounds__(256) k_drag_reduce(const ocean_buoyancy_body* 
             const float4 s = __ldg(&scales[c]);
             add_displacement(velocity + (size_t)c * N * N, N, px * s.x, pz * s.y, s.z, ux, uy, uz);
         }
+        if constexpr (kWake) uy = uy + __ldg(&wake[j]);
         const float dx = ux - (bv.linear[0] + (bv.angular[1] * r.z - bv.angular[2] * r.y));
         const float dy = uy - (bv.linear[1] + (bv.angular[2] * r.x - bv.angular[0] * r.z));
         const float dz = uz - (bv.linear[2] + (bv.angular[0] * r.y - bv.angular[1] * r.x));
@@ -188,6 +194,25 @@ __global__ void __launch_bounds__(256) k_drag_reduce(const ocean_buoyancy_body* 
     out[body] = o;
 }
 
+
+__global__ void __launch_bounds__(256) k_drag_reduce(const ocean_buoyancy_body* __restrict__ bodies, const ocean_body_velocity* __restrict__ velocities,
+                                                     const int* __restrict__ offsets, int num_bodies, const ocean_buoyancy_point* __restrict__ points,
+                                                     const float* __restrict__ drag_areas, const ocean_surface_sample* __restrict__ samples,
+                                                     const uint2* __restrict__ velocity, int N, int C, const float4* __restrict__ scales,
+                                                     float half_rho, ocean_drag_result* __restrict__ out) {
+    drag_reduce<false>(bodies, velocities, offsets, num_bodies, points, drag_areas, samples, velocity, N, C, scales, half_rho, out, nullptr);
+}
+
+// k_drag_reduce with the wake layer's vertical velocity per world point (ocean_wake_set_coupling)
+__global__ void __launch_bounds__(256) k_drag_reduce_wake(const ocean_buoyancy_body* __restrict__ bodies,
+                                                          const ocean_body_velocity* __restrict__ velocities, const int* __restrict__ offsets,
+                                                          int num_bodies, const ocean_buoyancy_point* __restrict__ points,
+                                                          const float* __restrict__ drag_areas, const ocean_surface_sample* __restrict__ samples,
+                                                          const uint2* __restrict__ velocity, int N, int C, const float4* __restrict__ scales,
+                                                          float half_rho, ocean_drag_result* __restrict__ out, const float* __restrict__ wv) {
+    drag_reduce<true>(bodies, velocities, offsets, num_bodies, points, drag_areas, samples, velocity, N, C, scales, half_rho, out, wv);
+}
+
 }  // namespace
 
 cudaError_t launch_buoyancy_transform(const ocean_buoyancy_body* bodies_dev, const int* offsets_dev, int num_bodies,
@@ -209,11 +234,17 @@ cudaError_t launch_buoyancy_reduce(const ocean_buoyancy_body* bodies_dev, const 
 cudaError_t launch_drag_reduce(const ocean_buoyancy_body* bodies_dev, const ocean_body_velocity* velocities_dev, const int* offsets_dev,
                                int num_bodies, const ocean_buoyancy_point* points_dev, const float* drag_areas_dev,
                                const ocean_surface_sample* samples_dev, const uint2* velocity_dev, int map_size, int num_cascades,
-                               const float4* scales_dev, float half_rho, ocean_drag_result* results_dev, cudaStream_t stream) {
+                               const float4* scales_dev, float half_rho, ocean_drag_result* results_dev, const float* wake_wv_dev,
+                               cudaStream_t stream) {
     if (num_bodies <= 0) return cudaSuccess;
     const unsigned blocks = (unsigned)(((size_t)num_bodies * 32 + 255) / 256);      // 8 bodies per block
-    k_drag_reduce<<<blocks, 256, 0, stream>>>(bodies_dev, velocities_dev, offsets_dev, num_bodies, points_dev, drag_areas_dev, samples_dev,
-                                              velocity_dev, map_size, num_cascades, scales_dev, half_rho, results_dev);
+    if (wake_wv_dev)
+        k_drag_reduce_wake<<<blocks, 256, 0, stream>>>(bodies_dev, velocities_dev, offsets_dev, num_bodies, points_dev, drag_areas_dev,
+                                                       samples_dev, velocity_dev, map_size, num_cascades, scales_dev, half_rho, results_dev,
+                                                       wake_wv_dev);
+    else
+        k_drag_reduce<<<blocks, 256, 0, stream>>>(bodies_dev, velocities_dev, offsets_dev, num_bodies, points_dev, drag_areas_dev, samples_dev,
+                                                  velocity_dev, map_size, num_cascades, scales_dev, half_rho, results_dev);
     return cudaGetLastError();
 }
 

@@ -142,11 +142,13 @@ cudaError_t launch_buoyancy_reduce(const ocean_buoyancy_body* bodies_dev, const 
                                    float tolerance, ocean_buoyancy_result* results_dev, cudaStream_t stream);
 // The drag half of the body-forces op (oracle/drag.py), on the same bodies, offsets, points and surface records:
 // velocities_dev = [num_bodies], drag_areas_dev = [num_points] C_d A parallel to points_dev, velocity_dev = the velocity maps
-// ([num_cascades used][map_size^2] 4 x half), results_dev = [num_bodies]
+// ([num_cascades used][map_size^2] 4 x half), results_dev = [num_bodies]; wake_wv_dev (may be null) = [n] vertical water
+// velocities of the wake layer per world point, added to the water velocity's y (ocean_wake_set_coupling)
 cudaError_t launch_drag_reduce(const ocean_buoyancy_body* bodies_dev, const ocean_body_velocity* velocities_dev, const int* offsets_dev,
                                int num_bodies, const ocean_buoyancy_point* points_dev, const float* drag_areas_dev,
                                const ocean_surface_sample* samples_dev, const uint2* velocity_dev, int map_size, int num_cascades,
-                               const float4* scales_dev, float half_rho, ocean_drag_result* results_dev, cudaStream_t stream);
+                               const float4* scales_dev, float half_rho, ocean_drag_result* results_dev, const float* wake_wv_dev,
+                               cudaStream_t stream);
 
 // ocean_bodies.cu: the floating-body integrator (oracle/bodies.py).  bodies_dev / states_dev = [num_bodies], r2_dev =
 // [num_bodies] max |p|^2 over each hull, pose_dev / velocities_dev = the tables the body-forces kernels read.  prepare fills r2
@@ -211,6 +213,30 @@ cudaError_t launch_wake_step(const WakeStepArgs& args, cudaStream_t stream);
 // map_dev = [n][n][4] half (h, dh/dx, dh/dz, 0); out_dev = [count][3] floats
 cudaError_t launch_wake_map(const float* h_dev, int n, float cell, void* map_dev, cudaStream_t stream);
 cudaError_t launch_wake_sample(const float* h_dev, int n, float cell, float x0, float z0, const float2* xz_dev, int count, float* out_dev,
+                               cudaStream_t stream);
+// The coupling (ocean_wake_set_coupling; oracle/wake_coupling.py).  free_surface: e = h + phi of the sources at tau (the end
+// of the step call) in the window at corner (x0, z0), into e, and into e_old when it is not null (a priming call).
+struct WakeFreeSurfaceArgs {
+    const float* h;                                 // [n][n], the layer after the call's sub-steps
+    float* e;                                       // [n][n]
+    float* e_old;                                   // [n][n] or null
+    const ocean_wake_source* sources;               // [num_sources]
+    const ocean_body_state* states;                 // [num_states]
+    int num_sources, num_states;
+    int n;
+    float cell, x0, z0, tau;
+};
+cudaError_t launch_wake_free_surface(const WakeFreeSurfaceArgs& args, cudaStream_t stream);
+// The snapshots e and e_old ([n][n]) with their window corners, and the interval T between them.
+struct WakeCoupleArgs {
+    const float* e;
+    const float* e_old;
+    int n;
+    float cell, x0, z0, x0_old, z0_old, interval;
+};
+// couple: records_dev[k] += sample(e, q_dev[k]) (height into displacement[1], slopes into gradient_foam[0..1]); wv_dev (may be
+// null) = [count] vertical velocities (sample(e) - sample(e_old)) / T
+cudaError_t launch_wake_couple(const WakeCoupleArgs& args, const float2* q_dev, int count, ocean_surface_sample* records_dev, float* wv_dev,
                                cudaStream_t stream);
 
 }  // namespace ocean

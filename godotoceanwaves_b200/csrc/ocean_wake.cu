@@ -10,6 +10,12 @@
 //                   (i + di, j + dj), 0 outside, and on a scrolled sub-step the scrolled h is written as the new h_prev.
 //   k_wake_map      one thread per cell: (h, dh/dx, dh/dz, 0) as half, central differences.
 //   k_wake_sample   one thread per point: bilinear h and central differences.
+// The coupling of the layer to the surface query (ocean_wake_set_coupling; oracle/wake_coupling.py):
+//   k_wake_free_surface  after a coupled step call: e = h + phi of the sources at the end of the call, one CTA per 32 x 32
+//                        tile; the source cull and the rasterisation are k_wake_step's (one __device__ template, over the
+//                        tile instead of the halo), without the convolution.
+//   k_wake_couple        one thread per query point: k_wake_sample's bilinear sample of e added to the surface record, and
+//                        on request the wake's vertical velocity (e - e_old) / T at the point for the drag pass.
 // No atomics.  Numeric policy: binary32 in the specification's order with explicit _rn operations, no contraction
 // (-fmad=false), IEEE division.
 #include "../../include/ocean.h"
@@ -103,25 +109,25 @@ __device__ __forceinline__ float cell(const float* __restrict__ f, int n, int i,
     return (unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n ? f[(size_t)j * n + i] : 0.0f;
 }
 
-__global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
-    __shared__ float s[kHaloCells];
-    __shared__ float4 list[kThreads];               // culled sources: cx, cz, r2, head
-    __shared__ int warp_count[kThreads / 32];
+// phi at the cells of the kSpan x kSpan square whose first cell is window cell (ti0, tj0): thread t holds square cells
+// c = t + m * kThreads (row-major) in phi[m], and adds, in source index order, the sources of `a` at a.tau.  The CTA culls
+// the sources against the square, 256 at a time, with a warp ballot and a prefix over the warps (index order is kept);
+// list and warp_count are its shared scratch.  Cells outside the window are left as they are.  Args is WakeStepArgs or
+// WakeFreeSurfaceArgs: the source, window and time fields of both have the same names.
+template <int kSpan, typename Args>
+__device__ __forceinline__ void rasterise(const Args& a, int ti0, int tj0, float4* list, int* warp_count,
+                                          float (&phi)[(kSpan * kSpan + kThreads - 1) / kThreads]) {
+    constexpr int kCells = kSpan * kSpan;
+    constexpr int kPer = (kCells + kThreads - 1) / kThreads;
     const int t = threadIdx.x;
     const int n = a.n;
-    const int ti0 = blockIdx.x * kTile - kR, tj0 = blockIdx.y * kTile - kR;   // window cell of halo cell (0, 0)
     const float dx = a.cell;
-
-    float phi[kCellsPerThread];
-#pragma unroll
-    for (int m = 0; m < kCellsPerThread; ++m) phi[m] = 0.0f;
-
     if (a.num_sources > 0) {
-        // the halo's cell centres span [lo, hi] per axis; one cell of margin keeps the cull conservative under rounding
+        // the square's cell centres span [lo, hi] per axis; one cell of margin keeps the cull conservative under rounding
         const float xlo = __fadd_rn(a.x0, __fmul_rn(__fadd_rn((float)(ti0 - 1), 0.5f), dx));
-        const float xhi = __fadd_rn(a.x0, __fmul_rn(__fadd_rn((float)(ti0 + kHalo), 0.5f), dx));
+        const float xhi = __fadd_rn(a.x0, __fmul_rn(__fadd_rn((float)(ti0 + kSpan), 0.5f), dx));
         const float zlo = __fadd_rn(a.z0, __fmul_rn(__fadd_rn((float)(tj0 - 1), 0.5f), dx));
-        const float zhi = __fadd_rn(a.z0, __fmul_rn(__fadd_rn((float)(tj0 + kHalo), 0.5f), dx));
+        const float zhi = __fadd_rn(a.z0, __fmul_rn(__fadd_rn((float)(tj0 + kSpan), 0.5f), dx));
         for (int base = 0; base < a.num_sources; base += kThreads) {
             const int k = base + t;
             bool keep = false;
@@ -155,10 +161,10 @@ __global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
             if (keep) list[offset + __popc(ballot & ((1u << lane) - 1u))] = e;
             __syncthreads();
 #pragma unroll
-            for (int m = 0; m < kCellsPerThread; ++m) {
+            for (int m = 0; m < kPer; ++m) {
                 const int c = t + m * kThreads;
-                const int i = ti0 + c % kHalo, j = tj0 + c / kHalo;
-                if (c < kHaloCells && (unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n) {
+                const int i = ti0 + c % kSpan, j = tj0 + c / kSpan;
+                if (c < kCells && (unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n) {
                     const float px = __fadd_rn(a.x0, __fmul_rn(__fadd_rn((float)i, 0.5f), dx));
                     const float pz = __fadd_rn(a.z0, __fmul_rn(__fadd_rn((float)j, 0.5f), dx));
                     float p = phi[m];
@@ -177,6 +183,20 @@ __global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
             __syncthreads();                        // the list and the counts are rewritten by the next chunk
         }
     }
+}
+
+__global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
+    __shared__ float s[kHaloCells];
+    __shared__ float4 list[kThreads];               // culled sources: cx, cz, r2, head
+    __shared__ int warp_count[kThreads / 32];
+    const int t = threadIdx.x;
+    const int n = a.n;
+    const int ti0 = blockIdx.x * kTile - kR, tj0 = blockIdx.y * kTile - kR;   // window cell of halo cell (0, 0)
+
+    float phi[kCellsPerThread];
+#pragma unroll
+    for (int m = 0; m < kCellsPerThread; ++m) phi[m] = 0.0f;
+    rasterise<kHalo>(a, ti0, tj0, list, warp_count, phi);
 
     // s = h + phi over the halo, 0 outside the window
 #pragma unroll
@@ -208,6 +228,29 @@ __global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
     }
 }
 
+// e = h + phi of the sources at a.tau over one 32 x 32 tile (256 threads, 4 cells each), into a.e, and into a.e_old when it
+// is not null (the priming call writes both snapshots)
+__global__ void __launch_bounds__(kThreads) k_wake_free_surface(const WakeFreeSurfaceArgs a) {
+    __shared__ float4 list[kThreads];
+    __shared__ int warp_count[kThreads / 32];
+    constexpr int kPer = kTile * kTile / kThreads;
+    const int t = threadIdx.x;
+    const int n = a.n;
+    const int ti0 = blockIdx.x * kTile, tj0 = blockIdx.y * kTile;
+    float phi[kPer];
+#pragma unroll
+    for (int m = 0; m < kPer; ++m) phi[m] = 0.0f;
+    rasterise<kTile>(a, ti0, tj0, list, warp_count, phi);
+#pragma unroll
+    for (int m = 0; m < kPer; ++m) {
+        const int c = t + m * kThreads;
+        const size_t o = (size_t)(tj0 + c / kTile) * n + (ti0 + c % kTile);
+        const float e = __fadd_rn(a.h[o], phi[m]);
+        a.e[o] = e;
+        if (a.e_old) a.e_old[o] = e;
+    }
+}
+
 __device__ __forceinline__ float grad_x(const float* __restrict__ h, int n, int i, int j, float two_dx) {
     return __fdiv_rn(__fsub_rn(cell(h, n, i + 1, j), cell(h, n, i - 1, j)), two_dx);
 }
@@ -229,13 +272,11 @@ __device__ __forceinline__ float bilerp(float f00, float f10, float f01, float f
     return __fadd_rn(top, __fmul_rn(fv, __fsub_rn(bot, top)));
 }
 
-__global__ void __launch_bounds__(256) k_wake_sample(const float* __restrict__ h, int n, float dx, float x0, float z0,
-                                                     const float2* __restrict__ xz, int count, float* __restrict__ out) {
-    const int k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= count) return;
-    const float2 p = xz[k];
+// oracle/wake.py sample() of the field h at world point p: r[0] = bilinear h and, with kGradients, r[1], r[2] = bilinear
+// central differences; r is left as it is (the caller's zeros) outside the window
+template <bool kGradients>
+__device__ __forceinline__ void sample_field(const float* __restrict__ h, int n, float dx, float x0, float z0, float2 p, float* r) {
     const float ext = __fmul_rn((float)n, dx);
-    float r[3] = {0.0f, 0.0f, 0.0f};
     if (p.x >= x0 && p.x < __fadd_rn(x0, ext) && p.y >= z0 && p.y < __fadd_rn(z0, ext)) {
         const float u = __fsub_rn(__fdiv_rn(__fsub_rn(p.x, x0), dx), 0.5f);
         const float v = __fsub_rn(__fdiv_rn(__fsub_rn(p.y, z0), dx), 0.5f);
@@ -244,13 +285,43 @@ __global__ void __launch_bounds__(256) k_wake_sample(const float* __restrict__ h
         const int i = (int)fi, j = (int)fj;
         const float two_dx = __fmul_rn(2.0f, dx);
         r[0] = bilerp(cell(h, n, i, j), cell(h, n, i + 1, j), cell(h, n, i, j + 1), cell(h, n, i + 1, j + 1), fu, fv);
-        // central differences of cells outside the window are 0, like their heights
-        auto gx = [&](int ii, int jj) { return (unsigned)ii < (unsigned)n && (unsigned)jj < (unsigned)n ? grad_x(h, n, ii, jj, two_dx) : 0.0f; };
-        auto gz = [&](int ii, int jj) { return (unsigned)ii < (unsigned)n && (unsigned)jj < (unsigned)n ? grad_z(h, n, ii, jj, two_dx) : 0.0f; };
-        r[1] = bilerp(gx(i, j), gx(i + 1, j), gx(i, j + 1), gx(i + 1, j + 1), fu, fv);
-        r[2] = bilerp(gz(i, j), gz(i + 1, j), gz(i, j + 1), gz(i + 1, j + 1), fu, fv);
+        if constexpr (kGradients) {
+            // central differences of cells outside the window are 0, like their heights
+            auto gx = [&](int ii, int jj) { return (unsigned)ii < (unsigned)n && (unsigned)jj < (unsigned)n ? grad_x(h, n, ii, jj, two_dx) : 0.0f; };
+            auto gz = [&](int ii, int jj) { return (unsigned)ii < (unsigned)n && (unsigned)jj < (unsigned)n ? grad_z(h, n, ii, jj, two_dx) : 0.0f; };
+            r[1] = bilerp(gx(i, j), gx(i + 1, j), gx(i, j + 1), gx(i + 1, j + 1), fu, fv);
+            r[2] = bilerp(gz(i, j), gz(i + 1, j), gz(i, j + 1), gz(i + 1, j + 1), fu, fv);
+        }
     }
+}
+
+__global__ void __launch_bounds__(256) k_wake_sample(const float* __restrict__ h, int n, float dx, float x0, float z0,
+                                                     const float2* __restrict__ xz, int count, float* __restrict__ out) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= count) return;
+    float r[3] = {0.0f, 0.0f, 0.0f};
+    sample_field<true>(h, n, dx, x0, z0, xz[k], r);
     for (int m = 0; m < 3; ++m) out[3 * (size_t)k + m] = r[m];
+}
+
+// The coupling of the surface records to the wake free surface e: one thread per query point Q, (we, gx, gz) = sample(e, Q)
+// added to (displacement[1], gradient_foam[0], gradient_foam[1]); with wv not null also wv = (we - sample(e_old, Q)[0]) / T.
+__global__ void __launch_bounds__(256) k_wake_couple(const WakeCoupleArgs a, const float2* __restrict__ q, int count,
+                                                     ocean_surface_sample* __restrict__ rec, float* __restrict__ wv) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= count) return;
+    const float2 p = q[k];
+    float r[3] = {0.0f, 0.0f, 0.0f};
+    sample_field<true>(a.e, a.n, a.cell, a.x0, a.z0, p, r);
+    ocean_surface_sample& s = rec[k];
+    s.displacement[1] = __fadd_rn(s.displacement[1], r[0]);
+    s.gradient_foam[0] = __fadd_rn(s.gradient_foam[0], r[1]);
+    s.gradient_foam[1] = __fadd_rn(s.gradient_foam[1], r[2]);
+    if (wv) {
+        float o = 0.0f;
+        sample_field<false>(a.e_old, a.n, a.cell, a.x0_old, a.z0_old, p, &o);
+        wv[k] = __fdiv_rn(__fsub_rn(r[0], o), a.interval);
+    }
 }
 
 }  // namespace
@@ -265,6 +336,12 @@ cudaError_t launch_wake_step(const WakeStepArgs& args, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
+cudaError_t launch_wake_free_surface(const WakeFreeSurfaceArgs& args, cudaStream_t stream) {
+    const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
+    k_wake_free_surface<<<grid, kThreads, 0, stream>>>(args);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_wake_map(const float* h_dev, int n, float cell, void* map_dev, cudaStream_t stream) {
     const unsigned blocks = (unsigned)(((size_t)n * n + 255) / 256);
     k_wake_map<<<blocks, 256, 0, stream>>>(h_dev, n, 2.0f * cell, static_cast<__half2*>(map_dev));    // exact
@@ -275,6 +352,13 @@ cudaError_t launch_wake_sample(const float* h_dev, int n, float cell, float x0, 
                                cudaStream_t stream) {
     if (count <= 0) return cudaSuccess;
     k_wake_sample<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(h_dev, n, cell, x0, z0, xz_dev, count, out_dev);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wake_couple(const WakeCoupleArgs& args, const float2* q_dev, int count, ocean_surface_sample* records_dev, float* wv_dev,
+                               cudaStream_t stream) {
+    if (count <= 0) return cudaSuccess;
+    k_wake_couple<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(args, q_dev, count, records_dev, wv_dev);
     return cudaGetLastError();
 }
 

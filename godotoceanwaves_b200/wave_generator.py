@@ -522,6 +522,21 @@ class WaveGenerator:
             raise ValueError(f"wake fields must be [{n}][{n}]")
         check(load_library().ocean_wake_set_state(self.context, h.ctypes.data, hp.ctypes.data, int(origin[0]), int(origin[1])))
 
+    def wake_set_coupling(self, enable: bool) -> None:
+        """Couple the wake layer into the surface query, buoyancy, body forces and the body integrator (include/ocean.h,
+        ocean_wake_set_coupling): they read the wake free surface h + phi of the last step call.  Off releases the snapshots."""
+        self._require()
+        check(load_library().ocean_wake_set_coupling(self.context, int(enable)))
+
+    def wake_coupling(self):
+        """(e, e_old, origins, T): the coupling's snapshots ([N][N] float32), their origins ((e.x, e.z), (e_old.x, e_old.z))
+        in cells and the interval between them; zeros and T = 0 until the first coupled step call."""
+        self._require()
+        n = self._wake_size
+        e, eo, o, t = np.zeros((n, n), np.float32), np.zeros((n, n), np.float32), np.zeros(4, np.int64), np.zeros(1, np.float32)
+        check(load_library().ocean_wake_get_coupling(self.context, e.ctypes.data, eo.ctypes.data, o.ctypes.data, t.ctypes.data))
+        return e, eo, ((int(o[0]), int(o[1])), (int(o[2]), int(o[3]))), np.float32(t[0])
+
     def twiddles_to_host(self) -> np.ndarray:
         self._require()
         out = np.empty((self.map_size - 1, 2), np.float32)

@@ -201,7 +201,9 @@ int ocean_sample_maps_device(ocean_generator* gen, int num_points, const float* 
  * folds, several points P may map to Q, and any converged one may be returned.  tolerance (metres) must exceed a few
  * binary32 ulps of |Q|, or points far from the origin cannot converge.  tolerance must be finite and > 0, max_iterations in
  * [0, 64].  ocean_query_surface takes host buffers and is synchronous; ocean_query_surface_device takes device pointers for
- * the points and the records (map_scales stays a host array) and is asynchronous on the generator's stream. */
+ * the points and the records (map_scales stays a host array) and is asynchronous on the generator's stream.  A call with
+ * points launches 3 kernels (1 with max_iterations = 0), one more that adds the wake free surface to the records while the
+ * wake coupling is live (ocean_wake_set_coupling, "Wake layer"). */
 typedef struct ocean_surface_sample {
     float source_x, source_z;
     float displacement[3];
@@ -304,7 +306,7 @@ int ocean_raycast_device(ocean_generator* gen, int num_rays, const ocean_ray* ra
  * ([sum of num_points], body-major, j increasing).  The bodies and map_scales are host arrays in both entry points (the poses
  * come from the host's physics engine every tick); ocean_buoyancy takes host points, results and samples and is synchronous;
  * ocean_buoyancy_device takes device pointers for them and is asynchronous on the generator's stream.  A call with world
- * points launches 5 kernels (3 with max_iterations = 0). */
+ * points launches 5 kernels (3 with max_iterations = 0), one more while the wake coupling is live (ocean_wake_set_coupling). */
 typedef struct ocean_buoyancy_point {
     float position[3];
     float volume;
@@ -350,7 +352,7 @@ int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoy
  * it uses the SURFACE water velocity at every submerged point, while the orbital velocity of a wave decays as e^(-k z) with
  * depth z (at 1 m of draft this overstates the longest wave of a 16 m tile about 1.5 times, shorter waves more); there is no
  * added mass, radiation or wave-making damping, skin friction, or separate normal and tangential coefficients; nothing is
- * written back into the maps (no foam; wakes are the separate wake layer below, which these ops do not read).  Quadratic drag is stiff for light bodies under explicit integration: the op
+ * written back into the maps (no foam; wakes are the separate wake layer below, which these ops read only while its coupling is on).  Quadratic drag is stiff for light bodies under explicit integration: the op
  * does not integrate, and max_relative_speed lets a host choose sub-steps (ocean_simulate_bodies below integrates on the
  * device with a step that stays stable under it).
  * The call first brings stale velocity layers up to date (as ocean_sample_velocity does; the velocity buffers are allocated
@@ -358,7 +360,8 @@ int ocean_buoyancy_device(ocean_generator* gen, int num_bodies, const ocean_buoy
  * outputs non-NULL; an invalid call launches nothing.  samples may be NULL, as for ocean_buoyancy.  The bodies, velocities
  * and map_scales are host arrays in both entry points; ocean_body_forces takes host points, areas and outputs and is
  * synchronous; ocean_body_forces_device takes device pointers for them and is asynchronous on the generator's stream.  With
- * no stale velocity layer, a call with world points launches 6 kernels (4 with max_iterations = 0). */
+ * no stale velocity layer, a call with world points launches 6 kernels (4 with max_iterations = 0), one more while the wake
+ * coupling is live (ocean_wake_set_coupling). */
 typedef struct ocean_body_velocity {
     float linear[3];       /* velocity of the body origin t (m/s) */
     float angular[3];      /* rad/s */
@@ -411,7 +414,8 @@ int ocean_body_forces_device(ocean_generator* gen, int num_bodies, const ocean_b
  * offsets and uploads both once.  Validation is ocean_body_forces' (without its velocities and outputs), plus mass and every
  * inertia finite and > 0, dt finite and > 0, substeps in [1, 64] and states non-NULL when num_bodies > 0; an invalid call
  * launches nothing and refreshes nothing.  The call brings stale velocity layers up to date once, then launches 1 + 7 S
- * kernels (1 + 5 S with max_iterations = 0, 1 + 3 S when no body has hull points).  ocean_simulate_bodies takes host
+ * kernels (1 + 5 S with max_iterations = 0, 1 + 3 S when no body has hull points), and S more with world points while the
+ * wake coupling is live (ocean_wake_set_coupling; every sub-step reads the same wake snapshots).  ocean_simulate_bodies takes host
  * states, points, areas and outputs and is synchronous; ocean_simulate_bodies_device takes device pointers for them and is
  * asynchronous on the generator's stream. */
 typedef struct ocean_floating_body {
@@ -598,9 +602,35 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  * The sponge is sized for waves in the band: with iWave's damping it reflects about 4 % of a pulse in the band through a
  * 48-cell ramp to 1 / s, but much more of waves longer than the band, and a strong sponge_damping (which also acts as a
  * spring of stiffness 2 alpha / h) reflects more than a moderate one.
- * Limits: wakes do not enter the surface query, buoyancy, drag, ray cast or spray (they read the FFT maps only); bodies do
- * not block waves (no obstruction mask); wakes make no foam; linear deep water only (no breaking, shallow water or
- * nonlinearity); the layer and the cascades interact by superposition only.
+ * Coupling (ocean_wake_set_coupling, opt-in per generator; off, every op is bit-identical to a generator without a layer):
+ * the surface query, buoyancy, body forces and the body integrator then read the wake on top of the maps, so bodies ride
+ * each other's wakes.  oracle/wake_coupling.py is the specification, bit for bit.
+ *   free surface  what they read is e = h + phi_end, not h: phi_end is the sources rasterised at the end of the step call,
+ *             tau_end = (float)S * h (body-attached sources at position.xz + linear_velocity.xz * tau_end of the states the
+ *             call was given).  The stencil acts on h + phi, which is 0 at rest under a stationary source, so a body that
+ *             carries a source does not feel the depression its own head presses into the layer (that depression is the
+ *             hull; reading h would sink it by about the head), while waves from other sources and the body's own radiated
+ *             waves pass through e unchanged.  The render map and ocean_sample_wake keep showing h.
+ *   snapshots enabling allocates two [N][N] binary32 snapshots e and e_old (counted in device_bytes), each with its own
+ *             window origin, and marks them unprimed.  A step call on a coupled layer launches one more kernel after its
+ *             sub-steps: the previous e (with its origin) becomes e_old and e = h + phi_end is written in the call's window;
+ *             the first call after enabling or after ocean_wake_set_state writes e into both (primed from then on).  The
+ *             interval T becomes tau_end of the call.  Disabling releases the snapshots; ocean_wake_init turns the coupling
+ *             off.  While the coupling is on but unprimed the ops read nothing of the wake and launch nothing extra.
+ *   ops       for each query point Q, after the inversion: (we, gx, gz) = the bilinear sample of e and of its central
+ *             differences at Q in e's window (ocean_sample_wake's, 0 outside); displacement[1] += we, gradient_foam[0] += gx,
+ *             gradient_foam[1] += gz; source_xz, displacement[0] and [2], foam, residual and iterations are unchanged (the
+ *             wake has no horizontal displacement).  ocean_query_surface[_device], and ocean_buoyancy[_device],
+ *             ocean_body_forces[_device] and ocean_simulate_bodies[_device] on their world hull points Q = (w.x, w.z), whose
+ *             samples outputs carry the coupled records.  Drag adds the wake's vertical water velocity
+ *             wv = (sample(e, Q) - sample(e_old, Q)) / T, each snapshot in its own window, to u.y before d = u - vb.
+ *             Every sub-step of a simulate call reads the same e and e_old, as it reads the same maps.
+ *   launches  while primed, one more kernel per step call, per surface query, per buoyancy or body-forces call with world
+ *             points and per simulate sub-step with world points.
+ * Limits: the ray cast, spray, ocean_sample_maps and ocean_sample_velocity read the FFT maps only (the ray cast's slab
+ * would also need a bound on e); the wake has no horizontal water velocity (iWave is vertical only); bodies do not block
+ * waves (no obstruction mask); wakes make no foam; linear deep water only (no breaking, shallow water or nonlinearity); the
+ * layer and the cascades interact by superposition only.
  * Entry points (an invalid call returns OCEAN_ERR_INVALID_ARGUMENT, launches nothing and leaves the layer untouched; a call
  * on a generator without a layer returns OCEAN_ERR_STATE):
  *   ocean_wake_kernel_taps   the 28 taps G[a][b] in the order (0,0), (1,0), (1,1), (2,0), ... (6,6); host only, no device.
@@ -610,7 +640,7 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *                            >= 0, sponge_cells in [0, 64] and <= size / 2.
  *   ocean_wake_step          dt finite > 0, substeps in [1, 256], the stability rule above, num_sources and num_states
  *                            >= 0 with non-NULL arrays when > 0, and (host form) every source's body < num_states.
- *                            Launches `substeps` kernels.  The host form takes host sources and states and returns when
+ *                            Launches `substeps` kernels, one more while the coupling is on.  The host form takes host sources and states and returns when
  *                            the work is enqueued; the device form takes device pointers; both are asynchronous on the
  *                            generator's stream.
  *   ocean_wake_render_map    writes [N][N][4] half (h, dh/dx, dh/dz, 0) in window order into map_dev (device memory),
@@ -619,7 +649,12 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *   ocean_sample_wake        bilinear h, dh/dx and dh/dz ([n][3] float) from the binary32 state at world (x, z); 0 outside
  *                            the window.  One kernel; the host form is synchronous, the device form asynchronous.
  *   ocean_wake_get_state / ocean_wake_set_state   host copies of h, h_prev ([N][N] float) and the origin, for tests and
- *                            checkpoints (synchronous). */
+ *                            checkpoints (synchronous).  set_state makes the coupling's snapshots unprimed.
+ *   ocean_wake_set_coupling  enable 0 or 1 (anything else: OCEAN_ERR_INVALID_ARGUMENT, nothing changes); enabling a
+ *                            coupled layer again changes nothing.  Synchronous on disable.
+ *   ocean_wake_get_coupling  host copies of e and e_old ([N][N] float), origins[4] = (e.x, e.z, e_old.x, e_old.z) in cells
+ *                            and the interval T; zeros, origins 0 and T = 0 while unprimed.  OCEAN_ERR_STATE while the
+ *                            coupling is off; every pointer non-NULL.  Synchronous. */
 typedef struct ocean_wake_params {
     int32_t size;               /* N: 0 (release) or a power of two in [128, 2048] */
     int32_t sponge_cells;       /* width of the absorbing ring, [0, 64] and <= size / 2 */
@@ -645,6 +680,8 @@ int ocean_sample_wake(ocean_generator* gen, int num_points, const float* points_
 int ocean_sample_wake_device(ocean_generator* gen, int num_points, const float* points_xz_dev, float* out_dev);
 int ocean_wake_get_state(ocean_generator* gen, float* h_host, float* h_prev_host, int64_t* origin_xz);
 int ocean_wake_set_state(ocean_generator* gen, const float* h_host, const float* h_prev_host, int64_t origin_x, int64_t origin_z);
+int ocean_wake_set_coupling(ocean_generator* gen, int enable);
+int ocean_wake_get_coupling(ocean_generator* gen, float* e_host, float* e_old_host, int64_t* origins, float* interval);
 
 /* Parity/debug taps (not timed): binary32 maps before the half conversion, the row-pass output
  * ([4][N][N][2] float, == fft_buffer half 1 after the first fft_compute, wave_generator.gd:79) and

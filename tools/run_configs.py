@@ -2,7 +2,7 @@
 config.
 
     python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast] [--spray-particles]
-                                [--wake]
+                                [--wake] [--wake-coupling]
 
 Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
 --query.  An unknown argument exits before anything touches the GPU."""
@@ -417,14 +417,9 @@ def run_velocity(N, C, reps, label, sample_points=0):
     print(json.dumps(out), flush=True)
 
 
-def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, tolerance=1e-3, max_iterations=8):
-    """Floating-body integrator (ocean_simulate_bodies_device, S sub-steps per call, states in device memory) against
-    S x ocean_body_forces_device on the same bodies and device-resident hulls (the integrator's own overhead), and against
-    a host loop of S rounds of ocean_body_forces_device, read-back of the records and the numpy step of oracle/bodies.py
-    (what the op saves a host).  Device times from CUDA events, the host loop from the wall clock after a synchronise; the
-    states are restored before each window; alternating windows.  The card's name, power limit and max SM clock are read
-    in the same run."""
-    g, _, scales = warmed_generator(N, C, 2)
+def _floating_scene(n_bodies, per_body):
+    """_buoyancy_scene's hulls as floating bodies of 200 to 900 kg/m^3 of their hull volume, with random orientations and
+    velocities: (bodies, states, hull, drag areas) in the layouts of oracle/bodies.py."""
     table, hull = _buoyancy_scene(n_bodies, per_body)
     rng = np.random.default_rng(3)
     bodies = np.zeros(n_bodies, ob.BODY)
@@ -438,6 +433,18 @@ def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, t
     states["linear_velocity"] = rng.uniform(-2.0, 2.0, (n_bodies, 3))
     states["angular_velocity"] = rng.uniform(-1.0, 1.0, (n_bodies, 3))
     cda = rng.uniform(0.01, 0.2, len(hull)).astype(np.float32)
+    return bodies, states, hull, cda
+
+
+def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, tolerance=1e-3, max_iterations=8):
+    """Floating-body integrator (ocean_simulate_bodies_device, S sub-steps per call, states in device memory) against
+    S x ocean_body_forces_device on the same bodies and device-resident hulls (the integrator's own overhead), and against
+    a host loop of S rounds of ocean_body_forces_device, read-back of the records and the numpy step of oracle/bodies.py
+    (what the op saves a host).  Device times from CUDA events, the host loop from the wall clock after a synchronise; the
+    states are restored before each window; alternating windows.  The card's name, power limit and max SM clock are read
+    in the same run."""
+    g, _, scales = warmed_generator(N, C, 2)
+    bodies, states, hull, cda = _floating_scene(n_bodies, per_body)
     pose, vel = ob.pose(bodies, states)
     hull_d = upload(hull)
     cda_d = torch.from_numpy(cda).to(DEV)
@@ -481,6 +488,64 @@ def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, t
            "simulate_us_per_call": [1e3 * v for v in t_s], "S_x_body_forces_us": [1e3 * v for v in t_f],
            "host_loop_us_per_call": [1e3 * v for v in t_h], "overhead_over_S_x_body_forces": min(t_s) / min(t_f) - 1.0,
            "host_loop_over_simulate": min(t_h) / min(t_s)}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
+def run_simulate_coupling(N, C, n_bodies, per_body, substeps, reps, label, wake=512, dx=1.0, dt=1.0 / 60.0):
+    """Wake coupling's cost in the body integrator: ocean_simulate_bodies_device on two generators with the same maps and a
+    wake layer of wake x wake cells of dx centred on the world origin (it covers [-256, 256]^2 m of the scene's
+    [-300, 300]^2 m), coupled (primed by one step with 64 sources) and uncoupled.  Device times from CUDA events, the states
+    restored before each window, alternating windows; the card's name, power limit and max SM clock read in the same run."""
+    bodies, states, hull, cda = _floating_scene(n_bodies, per_body)
+    rng = np.random.default_rng(4)
+    s = np.zeros(64, gow.WaveGenerator.WAKE_SOURCE)
+    s["x"], s["z"] = rng.uniform(-200, 200, 64), rng.uniform(-200, 200, 64)
+    s["vx"], s["radius"], s["head"], s["body"] = 3.0, 3.0, 0.2, -1
+    lib = load_library()
+    hull_d = upload(hull)
+    cda_d = torch.from_numpy(cda).to(DEV)
+    st0_d = upload(states)
+    runs = []
+    for coupled in (False, True):
+        g, _, scales = warmed_generator(N, C, 2)
+        g.wake_init(wake, dx, 0.05, 32, 3.0)
+        g.wake_set_coupling(coupled)
+        g.wake_step(0.1, 2, (-wake // 2, -wake // 2), s)
+        st_d = st0_d.clone()
+        torch.cuda.synchronize()
+        sim = partial(lambda g, st_d, sc: check(lib.ocean_simulate_bodies_device(
+            g.context, n_bodies, bodies.ctypes.data, st_d.data_ptr(), len(hull), hull_d.data_ptr(), cda_d.data_ptr(), C, sc.ctypes.data,
+            1025.0, dt, substeps, 1e-3, 8, None, None, None)), g, st_d, scales)
+        runs.append((g, sim, partial(lambda st_d: st_d.copy_(st0_d), st_d)))
+    t_off, t_on = alternate(*[partial(lambda g, sim, restore: timed(g, sim, reps, 3, restore), *r) for r in runs])
+    out = {"config": label, **card(), "map_size": N, "cascades": C, "bodies": n_bodies, "points_per_body": per_body,
+           "substeps": substeps, "wake_size": wake, "wake_cell_size": dx,
+           "uncoupled_us_per_call": [1e3 * v for v in t_off], "coupled_us_per_call": [1e3 * v for v in t_on],
+           "coupled_over_uncoupled": min(t_on) / min(t_off) - 1.0}
+    for g, _, _ in runs:
+        g.free()
+    print(json.dumps(out), flush=True)
+
+
+def run_wake_step_coupling(N, sources, reps, label, substeps=8, dx=0.5):
+    """Wake coupling's cost in the step call: run_wake's ocean_wake_step_device with the coupling off and on (one more
+    kernel per call, the free surface e = h + phi at the end of the call); alternating windows on one generator."""
+    g, _, _ = warmed_generator(128, 2, 1)
+    g.wake_init(N, dx, 0.05, 32, 3.0)
+    rng = np.random.default_rng(N + sources)
+    s = np.zeros(sources, gow.WaveGenerator.WAKE_SOURCE)
+    s["x"], s["z"] = rng.uniform(0, N * dx, sources), rng.uniform(0, N * dx, sources)
+    s["vx"], s["vz"] = 3.0, 0.0
+    s["radius"], s["head"], s["body"] = 2.0, 0.1, -1
+    src = upload(s)
+    lib = load_library()
+    call = lambda: check(lib.ocean_wake_step_device(g.context, substeps / 60.0, substeps, 0, 0, sources, src.data_ptr(), 0, None))
+    t_off, t_on = alternate(lambda: timed(g, call, reps, 3, lambda: g.wake_set_coupling(False)),
+                            lambda: timed(g, call, reps, 3, lambda: g.wake_set_coupling(True)))
+    out = {"config": label, **card(), "size": N, "cell_size": dx, "sources": sources, "substeps_per_call": substeps,
+           "uncoupled_us_per_call": [1e3 * v for v in t_off], "coupled_us_per_call": [1e3 * v for v in t_on],
+           "free_surface_us_per_call": 1e3 * (min(t_on) - min(t_off))}
     g.free()
     print(json.dumps(out), flush=True)
 
@@ -597,6 +662,13 @@ GROUPS = {          # flag: its configs, in the order they run
     "--wake": [
         partial(run_wake, N, k, 200 if N < 1024 else 50, f"wake layer: {N}x{N} cells, {k} source(s)")
         for N in (256, 512, 1024) for k in (1, 64, 1024)
+    ],
+    "--wake-coupling": [
+        *[partial(run_simulate_coupling, N, C, 1 << 14, 64, S, reps,
+                  f"wake coupling, simulate: 2^14 bodies x 64 points, {S} sub-step(s), {C} cascades of {N}x{N}, 512x512 wake")
+          for S in (1, 4) for N, C, reps in ((256, 4, 50), (1024, 8, 20))],
+        *[partial(run_wake_step_coupling, N, k, 200 if N < 1024 else 50, f"wake coupling, step: {N}x{N} cells, {k} source(s), 8 sub-steps")
+          for N in (256, 512, 1024) for k in (1, 64, 1024)],
     ],
 }
 DEFAULT = ("--updates", "--query")
