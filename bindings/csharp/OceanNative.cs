@@ -82,6 +82,13 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public struct OceanWakeFoamParams                               // struct ocean_wake_foam_params (16 B)
+    {
+        public float whitecap;                                      // beta = c / dx above which the wake breaks
+        public float grow_rate, stir_rate, decay_rate;              // >= 0; 1/s, 1/s per (m/s)^2, 1/s
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public unsafe struct OceanSurfaceSample                         // struct ocean_surface_sample (40 B) <- water.gdshader:28,37 inverted
     {
         public float source_x, source_z;
@@ -280,6 +287,13 @@ namespace OceanB200
         internal static partial int ocean_wake_set_coupling(IntPtr handle, int enable);
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_wake_get_coupling(IntPtr handle, float* e, float* e_old, long* origins, float* interval);
+        // wake foam: the foam field F, advanced with the layer, in the render map's fourth channel (null parameters: off)
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_set_foam(IntPtr handle, OceanWakeFoamParams* parameters);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_get_foam_state(IntPtr handle, float* foam);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_set_foam_state(IntPtr handle, float* foam);
         // surface query: the surface at world positions points [n][2] (P + D_xz(P) = Q solved for P, then the map query at P)
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,

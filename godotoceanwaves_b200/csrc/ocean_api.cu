@@ -168,6 +168,11 @@ struct ocean_generator {
     int wake_e = 0;                                     // which snapshot holds e (the other holds e_old)
     int64_t wake_snapshot_origin[2][2] = {};            // [snapshot][x, z]
     float wake_interval = 0.0f;                         // T
+    // wake foam (ocean_wake_set_foam): two [size][size] foam fields, F and the one a sub-step writes, and the parameters
+    DeviceArray<float> wake_foam;
+    ocean_wake_foam_params wake_foam_params{};
+    bool wake_foam_on = false;
+    int wake_f = 0;                                     // which foam field holds F
 };
 
 namespace {
@@ -1937,6 +1942,7 @@ int ocean_debug_device_math(ocean_generator* gen, int fn, int n, const float* a_
 // ---- wake layer: a local height field driven by moving sources (oracle/wake.py) ----
 static_assert(sizeof(ocean_wake_params) == 20, "ocean_wake_params layout");
 static_assert(sizeof(ocean_wake_source) == 28, "ocean_wake_source layout");
+static_assert(sizeof(ocean_wake_foam_params) == 16, "ocean_wake_foam_params layout");
 
 int ocean_wake_kernel_taps(float* taps_host) {
     if (!taps_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "taps_host is NULL");
@@ -2004,6 +2010,18 @@ int wake_uncouple(ocean_generator* g) {
     return OCEAN_OK;
 }
 
+// Turns foam off and releases its fields (the caller has entered the generator).
+int wake_foam_off(ocean_generator* g) {
+    if (g->wake_foam.ptr) OCEAN_CUDA(cudaStreamSynchronize(g->stream));     // kernels may still read them
+    g->wake_foam.release();
+    g->wake_foam_on = false;
+    g->wake_foam_params = ocean_wake_foam_params{};
+    g->wake_f = 0;
+    return OCEAN_OK;
+}
+
+float* wake_foam_field(ocean_generator* g, int k) { return g->wake_foam.ptr + (size_t)k * g->wake.size * g->wake.size; }
+
 int check_wake_points(int num_points, const void* points, const void* out) {
     if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
     if (num_points > 0 && (!points || !out)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "points or out is NULL");
@@ -2018,6 +2036,7 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
     const ocean_wake_params p = *params;
     if (p.size == 0) {
         if ((rc = wake_uncouple(gen))) return rc;
+        if ((rc = wake_foam_off(gen))) return rc;
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
         gen->wake_fields.release();
         gen->wake_sources.release();
@@ -2035,6 +2054,7 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
         return fail(OCEAN_ERR_INVALID_ARGUMENT, "sponge_cells %d outside [0, min(64, size / 2)]", p.sponge_cells);
     const size_t cells = 4 * (size_t)p.size * p.size;  // h, h_prev and two fields a scrolled sub-step writes
     if ((rc = wake_uncouple(gen))) return rc;
+    if ((rc = wake_foam_off(gen))) return rc;
     gen->wake = ocean_wake_params{};                    // no layer until the fields below are allocated and cleared
     if (gen->wake_fields.capacity != cells) {
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
@@ -2067,6 +2087,14 @@ int ocean_wake_step_device(ocean_generator* gen, double dt, int substeps, int64_
     a.dj = shift(origin_z, gen->wake_origin[1]);
     a.x0 = wake_corner(origin_x, gen->wake.cell_size);
     a.z0 = wake_corner(origin_z, gen->wake.cell_size);
+    ocean::WakeFoamStepArgs f{};
+    if (gen->wake_foam_on) {
+        const ocean_wake_foam_params& fp = gen->wake_foam_params;
+        f.whitecap = fp.whitecap;
+        f.decay = exp_det_host(-(fp.decay_rate * h));  // binary32 products, the cascades' DETMATH exp
+        f.grow = fp.grow_rate * h;
+        f.stir = fp.stir_rate * h;
+    }
     for (int k = 0; k < substeps; ++k) {
         int spare[2], m = 0;
         for (int b = 0; b < 4 && m < 2; ++b)
@@ -2077,7 +2105,15 @@ int ocean_wake_step_device(ocean_generator* gen, double dt, int substeps, int64_
         a.out_h = wake_field(gen, spare[0]);
         a.out_h_prev = scrolled ? wake_field(gen, spare[1]) : nullptr;
         a.tau = (float)k * h;
-        OCEAN_CUDA(ocean::launch_wake_step(a, gen->stream));
+        if (gen->wake_foam_on) {
+            f.step = a;
+            f.foam = wake_foam_field(gen, gen->wake_f);
+            f.out_foam = wake_foam_field(gen, gen->wake_f ^ 1);
+            OCEAN_CUDA(ocean::launch_wake_step_foam(f, gen->stream));
+            gen->wake_f ^= 1;
+        } else {
+            OCEAN_CUDA(ocean::launch_wake_step(a, gen->stream));
+        }
         gen->kernel_launches += 1;
         gen->wake_hp = scrolled ? spare[1] : gen->wake_h;
         gen->wake_h = spare[0];
@@ -2139,7 +2175,8 @@ int ocean_wake_render_map(ocean_generator* gen, void* map_dev, float* world_rect
     if ((rc = check_wake_layer(gen))) return rc;
     if (!map_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "map_dev is NULL");
     const ocean_wake_params& p = gen->wake;
-    OCEAN_CUDA(ocean::launch_wake_map(wake_field(gen, gen->wake_h), p.size, p.cell_size, map_dev, gen->stream));
+    const float* foam = gen->wake_foam_on ? wake_foam_field(gen, gen->wake_f) : nullptr;
+    OCEAN_CUDA(ocean::launch_wake_map(wake_field(gen, gen->wake_h), foam, p.size, p.cell_size, map_dev, gen->stream));
     gen->kernel_launches += 1;
     if (world_rect) {
         world_rect[0] = wake_corner(gen->wake_origin[0], p.cell_size);
@@ -2242,6 +2279,52 @@ int ocean_wake_get_coupling(ocean_generator* gen, float* e_host, float* e_old_ho
     origins[2] = gen->wake_snapshot_origin[o][0];
     origins[3] = gen->wake_snapshot_origin[o][1];
     *interval = gen->wake_interval;
+    return OCEAN_OK;
+}
+
+int ocean_wake_set_foam(ocean_generator* gen, const ocean_wake_foam_params* params) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (!params) return wake_foam_off(gen);
+    const ocean_wake_foam_params p = *params;
+    if (!std::isfinite(p.whitecap) || !std::isfinite(p.grow_rate) || !std::isfinite(p.stir_rate) || !std::isfinite(p.decay_rate))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "foam parameters not finite");
+    if (!(p.grow_rate >= 0.0f) || !(p.stir_rate >= 0.0f) || !(p.decay_rate >= 0.0f))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "grow_rate %g, stir_rate %g or decay_rate %g is negative", p.grow_rate, p.stir_rate,
+                    p.decay_rate);
+    if (!gen->wake_foam_on) {
+        const size_t cells = (size_t)gen->wake.size * gen->wake.size;
+        OCEAN_CUDA(gen->wake_foam.grow(gen, 2 * cells));
+        OCEAN_CUDA(cudaMemsetAsync(gen->wake_foam.ptr, 0, 2 * cells * sizeof(float), gen->stream));
+        gen->wake_f = 0;
+        gen->wake_foam_on = true;
+    }
+    gen->wake_foam_params = p;
+    return OCEAN_OK;
+}
+
+int ocean_wake_get_foam_state(ocean_generator* gen, float* foam_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (!gen->wake_foam_on) return fail(OCEAN_ERR_STATE, "the wake layer's foam is off (ocean_wake_set_foam)");
+    if (!foam_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "foam_host is NULL");
+    const size_t bytes = sizeof(float) * gen->wake.size * gen->wake.size;
+    OCEAN_CUDA(cudaMemcpyAsync(foam_host, wake_foam_field(gen, gen->wake_f), bytes, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    return OCEAN_OK;
+}
+
+int ocean_wake_set_foam_state(ocean_generator* gen, const float* foam_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (!gen->wake_foam_on) return fail(OCEAN_ERR_STATE, "the wake layer's foam is off (ocean_wake_set_foam)");
+    if (!foam_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "foam_host is NULL");
+    const size_t bytes = sizeof(float) * gen->wake.size * gen->wake.size;
+    OCEAN_CUDA(cudaMemcpyAsync(wake_foam_field(gen, gen->wake_f), foam_host, bytes, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
 

@@ -210,8 +210,19 @@ struct WakeStepArgs {
 };
 void wake_kernel_taps(float* out);                  // host: the 28 taps in the specification's order
 cudaError_t launch_wake_step(const WakeStepArgs& args, cudaStream_t stream);
-// map_dev = [n][n][4] half (h, dh/dx, dh/dz, 0); out_dev = [count][3] floats
-cudaError_t launch_wake_map(const float* h_dev, int n, float cell, void* map_dev, cudaStream_t stream);
+// The foam sub-step (ocean_wake_set_foam; oracle/wake_foam.py): the sub-step of `step`, and F ([n][n], read at (i + di, j + dj),
+// 0 outside) advanced to out_foam (another [n][n] field) with the call's constants.
+struct WakeFoamStepArgs {
+    WakeStepArgs step;
+    const float* foam;
+    float* out_foam;
+    float whitecap;
+    float decay;                                    // d = exp(-decay_rate h)
+    float grow, stir;                               // grow_rate h, stir_rate h
+};
+cudaError_t launch_wake_step_foam(const WakeFoamStepArgs& args, cudaStream_t stream);
+// map_dev = [n][n][4] half (h, dh/dx, dh/dz, F), F = foam_dev or 0 when foam_dev is null; out_dev = [count][3] floats
+cudaError_t launch_wake_map(const float* h_dev, const float* foam_dev, int n, float cell, void* map_dev, cudaStream_t stream);
 cudaError_t launch_wake_sample(const float* h_dev, int n, float cell, float x0, float z0, const float2* xz_dev, int count, float* out_dev,
                                cudaStream_t stream);
 // The coupling (ocean_wake_set_coupling; oracle/wake_coupling.py).  free_surface: e = h + phi of the sources at tau (the end

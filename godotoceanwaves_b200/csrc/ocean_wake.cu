@@ -8,7 +8,13 @@
 //                   s = h + phi (0 outside the window) in shared memory and each thread takes the 28-class symmetric
 //                   convolution of its four cells from there.  The scroll is folded into the reads: h and h_prev are read at
 //                   (i + di, j + dj), 0 outside, and on a scrolled sub-step the scrolled h is written as the new h_prev.
-//   k_wake_map      one thread per cell: (h, dh/dx, dh/dz, 0) as half, central differences.
+//   k_wake_step_foam  k_wake_step (one inlined template) that also advances the foam field F (ocean_wake_set_foam;
+//                   oracle/wake_foam.py) in the same pass: the cull carries each kept source's |v|^2, the halo pass adds
+//                   w^2 |v|^2 next to phi (kept per halo cell in shared memory), and each output cell
+//                   updates F from its convolution c and that sum.  F is read at (i + di, j + dj) and written to a second
+//                   field, as h is.
+//   k_wake_map      one thread per cell: (h, dh/dx, dh/dz, 0) as half, central differences; k_wake_map_foam writes F as
+//                   the fourth channel.
 //   k_wake_sample   one thread per point: bilinear h and central differences.
 // The coupling of the layer to the surface query (ocean_wake_set_coupling; oracle/wake_coupling.py):
 //   k_wake_free_surface  after a coupled step call: e = h + phi of the sources at the end of the call, one CTA per 32 x 32
@@ -113,10 +119,14 @@ __device__ __forceinline__ float cell(const float* __restrict__ f, int n, int i,
 // c = t + m * kThreads (row-major) in phi[m], and adds, in source index order, the sources of `a` at a.tau.  The CTA culls
 // the sources against the square, 256 at a time, with a warp ballot and a prefix over the warps (index order is kept);
 // list and warp_count are its shared scratch.  Cells outside the window are left as they are.  Args is WakeStepArgs or
-// WakeFreeSurfaceArgs: the source, window and time fields of both have the same names.
-template <int kSpan, typename Args>
+// WakeFreeSurfaceArgs: the source, window and time fields of both have the same names.  With kStir the same pass adds
+// (w w) |v|^2 of each source to the shared sigma[c] of the square's cell c (v its centre velocity, |v|^2 = vx vx + vz vz),
+// the cull keeping |v|^2 of the kept sources in the shared speed2; the caller zeroes sigma, and each cell is only touched by
+// the thread that holds it, so it needs no barrier.
+template <int kSpan, bool kStir = false, typename Args>
 __device__ __forceinline__ void rasterise(const Args& a, int ti0, int tj0, float4* list, int* warp_count,
-                                          float (&phi)[(kSpan * kSpan + kThreads - 1) / kThreads]) {
+                                          float (&phi)[(kSpan * kSpan + kThreads - 1) / kThreads], float* speed2 = nullptr,
+                                          float* sigma = nullptr) {
     constexpr int kCells = kSpan * kSpan;
     constexpr int kPer = (kCells + kThreads - 1) / kThreads;
     const int t = threadIdx.x;
@@ -132,16 +142,23 @@ __device__ __forceinline__ void rasterise(const Args& a, int ti0, int tj0, float
             const int k = base + t;
             bool keep = false;
             float4 e = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+            float v2 = 0.0f;
             if (k < a.num_sources) {
                 const ocean_wake_source src = a.sources[k];
                 float cx = __fadd_rn(src.x, __fmul_rn(src.vx, a.tau));
                 float cz = __fadd_rn(src.z, __fmul_rn(src.vz, a.tau));
+                float vx = src.vx, vz = src.vz;
                 bool ok = src.body < a.num_states;
                 if (ok && src.body >= 0) {
                     const ocean_body_state& b = a.states[src.body];
                     cx = __fadd_rn(cx, __fadd_rn(b.position[0], __fmul_rn(b.linear_velocity[0], a.tau)));
                     cz = __fadd_rn(cz, __fadd_rn(b.position[2], __fmul_rn(b.linear_velocity[2], a.tau)));
+                    if constexpr (kStir) {
+                        vx = __fadd_rn(vx, b.linear_velocity[0]);
+                        vz = __fadd_rn(vz, b.linear_velocity[2]);
+                    }
                 }
+                if constexpr (kStir) v2 = __fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vz, vz));
                 const float r = src.radius;
                 const float r2 = __fmul_rn(r, r);
                 ok = ok && isfinite(cx) && isfinite(cz) && isfinite(src.head) && isfinite(r) && r > 0.0f && isfinite(r2);
@@ -158,7 +175,11 @@ __device__ __forceinline__ void rasterise(const Args& a, int ti0, int tj0, float
                 offset += w < warp ? warp_count[w] : 0;
                 total += warp_count[w];
             }
-            if (keep) list[offset + __popc(ballot & ((1u << lane) - 1u))] = e;
+            if (keep) {
+                const int slot = offset + __popc(ballot & ((1u << lane) - 1u));
+                list[slot] = e;
+                if constexpr (kStir) speed2[slot] = v2;
+            }
             __syncthreads();
 #pragma unroll
             for (int m = 0; m < kPer; ++m) {
@@ -168,16 +189,21 @@ __device__ __forceinline__ void rasterise(const Args& a, int ti0, int tj0, float
                     const float px = __fadd_rn(a.x0, __fmul_rn(__fadd_rn((float)i, 0.5f), dx));
                     const float pz = __fadd_rn(a.z0, __fmul_rn(__fadd_rn((float)j, 0.5f), dx));
                     float p = phi[m];
+                    float sg = 0.0f;
+                    if constexpr (kStir) sg = sigma[c];
                     for (int q = 0; q < total; ++q) {
                         const float4 e2 = list[q];
                         const float ex = __fsub_rn(px, e2.x), ez = __fsub_rn(pz, e2.y);
                         const float d2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ez, ez));
                         if (d2 < e2.z) {
                             const float w = __fsub_rn(1.0f, __fdiv_rn(d2, e2.z));
-                            p = __fadd_rn(p, __fmul_rn(e2.w, __fmul_rn(w, w)));
+                            const float ww = __fmul_rn(w, w);
+                            p = __fadd_rn(p, __fmul_rn(e2.w, ww));
+                            if constexpr (kStir) sg = __fadd_rn(sg, __fmul_rn(ww, speed2[q]));
                         }
                     }
                     phi[m] = p;
+                    if constexpr (kStir) sigma[c] = sg;
                 }
             }
             __syncthreads();                        // the list and the counts are rewritten by the next chunk
@@ -185,10 +211,12 @@ __device__ __forceinline__ void rasterise(const Args& a, int ti0, int tj0, float
     }
 }
 
-__global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
-    __shared__ float s[kHaloCells];
-    __shared__ float4 list[kThreads];               // culled sources: cx, cz, r2, head
-    __shared__ int warp_count[kThreads / 32];
+// One sub-step over one 32 x 32 output tile: k_wake_step, and with kFoam k_wake_step_foam (f is its foam arguments, the
+// foam-only shared arrays speed2 [kThreads] and sig [kHaloCells] are not null).  sigma lives in shared memory rather than
+// in registers next to phi: eight more live registers per thread made the foam form spill.
+template <bool kFoam>
+__device__ __forceinline__ void wake_step(const WakeStepArgs& a, const WakeFoamStepArgs* f, float* s, float4* list, int* warp_count,
+                                          float* speed2, float* sig) {
     const int t = threadIdx.x;
     const int n = a.n;
     const int ti0 = blockIdx.x * kTile - kR, tj0 = blockIdx.y * kTile - kR;   // window cell of halo cell (0, 0)
@@ -196,7 +224,14 @@ __global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
     float phi[kCellsPerThread];
 #pragma unroll
     for (int m = 0; m < kCellsPerThread; ++m) phi[m] = 0.0f;
-    rasterise<kHalo>(a, ti0, tj0, list, warp_count, phi);
+    if constexpr (kFoam) {
+#pragma unroll
+        for (int m = 0; m < kCellsPerThread; ++m)
+            if (t + m * kThreads < kHaloCells) sig[t + m * kThreads] = 0.0f;
+        rasterise<kHalo, true>(a, ti0, tj0, list, warp_count, phi, speed2, sig);
+    } else {
+        rasterise<kHalo>(a, ti0, tj0, list, warp_count, phi);
+    }
 
     // s = h + phi over the halo, 0 outside the window
 #pragma unroll
@@ -225,7 +260,33 @@ __global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
         const size_t o = (size_t)j * n + i;
         a.out_h[o] = hn;
         if (a.out_h_prev) a.out_h_prev[o] = h;
+        if constexpr (kFoam) {
+            // F' = clamp(F d + (gh max(c / dx - whitecap, 0) + sh sigma), 0, 1); "x > 0 ? x : 0" is fmaxf(x, 0) (NaN -> 0)
+            // with -0 -> +0, so the result has one encoding
+            const float beta = __fdiv_rn(c, a.cell);
+            float b = __fsub_rn(beta, f->whitecap);
+            b = b > 0.0f ? b : 0.0f;
+            const float grow = __fadd_rn(__fmul_rn(f->grow, b), __fmul_rn(f->stir, sig[(lj + kR) * kHalo + li + kR]));
+            const float v = __fadd_rn(__fmul_rn(cell(f->foam, n, i + a.di, j + a.dj), f->decay), grow);
+            f->out_foam[o] = v > 0.0f ? fminf(v, 1.0f) : 0.0f;
+        }
     }
+}
+
+__global__ void __launch_bounds__(kThreads) k_wake_step(const WakeStepArgs a) {
+    __shared__ float s[kHaloCells];
+    __shared__ float4 list[kThreads];               // culled sources: cx, cz, r2, head
+    __shared__ int warp_count[kThreads / 32];
+    wake_step<false>(a, nullptr, s, list, warp_count, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(kThreads) k_wake_step_foam(const WakeFoamStepArgs f) {
+    __shared__ float s[kHaloCells];
+    __shared__ float4 list[kThreads];               // culled sources: cx, cz, r2, head
+    __shared__ int warp_count[kThreads / 32];
+    __shared__ float speed2[kThreads];              // |v|^2 of the culled sources
+    __shared__ float sig[kHaloCells];               // sigma of the halo cells
+    wake_step<true>(f.step, &f, s, list, warp_count, speed2, sig);
 }
 
 // e = h + phi of the sources at a.tau over one 32 x 32 tile (256 threads, 4 cells each), into a.e, and into a.e_old when it
@@ -258,12 +319,24 @@ __device__ __forceinline__ float grad_z(const float* __restrict__ h, int n, int 
     return __fdiv_rn(__fsub_rn(cell(h, n, i, j + 1), cell(h, n, i, j - 1)), two_dx);
 }
 
-__global__ void __launch_bounds__(256) k_wake_map(const float* __restrict__ h, int n, float two_dx, __half2* __restrict__ out) {
+// (h, dh/dx, dh/dz, F) of one cell as half; F is 0 without kFoam
+template <bool kFoam>
+__device__ __forceinline__ void wake_map(const float* __restrict__ h, const float* __restrict__ foam, int n, float two_dx,
+                                         __half2* __restrict__ out) {
     const int o = blockIdx.x * blockDim.x + threadIdx.x;
     if (o >= n * n) return;
     const int i = o % n, j = o / n;
     out[2 * (size_t)o] = __halves2half2(__float2half_rn(h[o]), __float2half_rn(grad_x(h, n, i, j, two_dx)));
-    out[2 * (size_t)o + 1] = __halves2half2(__float2half_rn(grad_z(h, n, i, j, two_dx)), __float2half_rn(0.0f));
+    out[2 * (size_t)o + 1] = __halves2half2(__float2half_rn(grad_z(h, n, i, j, two_dx)), __float2half_rn(kFoam ? foam[o] : 0.0f));
+}
+
+__global__ void __launch_bounds__(256) k_wake_map(const float* __restrict__ h, int n, float two_dx, __half2* __restrict__ out) {
+    wake_map<false>(h, nullptr, n, two_dx, out);
+}
+
+__global__ void __launch_bounds__(256) k_wake_map_foam(const float* __restrict__ h, const float* __restrict__ foam, int n, float two_dx,
+                                                       __half2* __restrict__ out) {
+    wake_map<true>(h, foam, n, two_dx, out);
 }
 
 __device__ __forceinline__ float bilerp(float f00, float f10, float f01, float f11, float fu, float fv) {
@@ -336,15 +409,24 @@ cudaError_t launch_wake_step(const WakeStepArgs& args, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
+cudaError_t launch_wake_step_foam(const WakeFoamStepArgs& args, cudaStream_t stream) {
+    const dim3 grid((unsigned)(args.step.n / kTile), (unsigned)(args.step.n / kTile));
+    k_wake_step_foam<<<grid, kThreads, 0, stream>>>(args);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_wake_free_surface(const WakeFreeSurfaceArgs& args, cudaStream_t stream) {
     const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
     k_wake_free_surface<<<grid, kThreads, 0, stream>>>(args);
     return cudaGetLastError();
 }
 
-cudaError_t launch_wake_map(const float* h_dev, int n, float cell, void* map_dev, cudaStream_t stream) {
+cudaError_t launch_wake_map(const float* h_dev, const float* foam_dev, int n, float cell, void* map_dev, cudaStream_t stream) {
     const unsigned blocks = (unsigned)(((size_t)n * n + 255) / 256);
-    k_wake_map<<<blocks, 256, 0, stream>>>(h_dev, n, 2.0f * cell, static_cast<__half2*>(map_dev));    // exact
+    if (foam_dev)
+        k_wake_map_foam<<<blocks, 256, 0, stream>>>(h_dev, foam_dev, n, 2.0f * cell, static_cast<__half2*>(map_dev));
+    else
+        k_wake_map<<<blocks, 256, 0, stream>>>(h_dev, n, 2.0f * cell, static_cast<__half2*>(map_dev));    // exact
     return cudaGetLastError();
 }
 

@@ -112,6 +112,9 @@ SIGNATURES = {
     "ocean_wake_set_state": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64]),
     "ocean_wake_set_coupling": (C.c_int, [_H, C.c_int]),
     "ocean_wake_get_coupling": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ocean_wake_set_foam": (C.c_int, [_H, C.c_void_p]),
+    "ocean_wake_get_foam_state": (C.c_int, [_H, C.c_void_p]),
+    "ocean_wake_set_foam_state": (C.c_int, [_H, C.c_void_p]),
     "ocean_get_foam_state": (C.c_int, [_H, C.c_int, C.c_void_p]),
     "ocean_set_foam_state": (C.c_int, [_H, C.c_int, C.c_void_p]),
     "ocean_jonswap_alpha": (C.c_double, [C.c_double, C.c_double]),

@@ -537,6 +537,37 @@ class WaveGenerator:
         check(load_library().ocean_wake_get_coupling(self.context, e.ctypes.data, eo.ctypes.data, o.ctypes.data, t.ctypes.data))
         return e, eo, ((int(o[0]), int(o[1])), (int(o[2]), int(o[3]))), np.float32(t[0])
 
+    WAKE_FOAM_PARAMS = np.dtype([("whitecap", np.float32), ("grow_rate", np.float32), ("stir_rate", np.float32),
+                                 ("decay_rate", np.float32)])                                   # struct ocean_wake_foam_params
+
+    def wake_set_foam(self, whitecap: float | None = 0.3, grow_rate: float = 1.0, stir_rate: float = 0.0,
+                      decay_rate: float = 0.5) -> None:
+        """Advance a foam field with the wake layer (include/ocean.h, ocean_wake_set_foam): white water where beta = c / dx
+        exceeds `whitecap` and where sources stir the water, decaying at `decay_rate`; it becomes the render map's fourth
+        channel.  whitecap=None turns foam off and releases the field; enabling zeroes it, changing parameters keeps it."""
+        self._require()
+        if whitecap is None:
+            check(load_library().ocean_wake_set_foam(self.context, None))
+            return
+        p = np.array((float(whitecap), float(grow_rate), float(stir_rate), float(decay_rate)), self.WAKE_FOAM_PARAMS)
+        check(load_library().ocean_wake_set_foam(self.context, p.ctypes.data))
+
+    def wake_foam(self) -> np.ndarray:
+        """A host copy of the wake layer's foam field F ([N][N] float32, window order)."""
+        self._require()
+        n = self._wake_size
+        out = np.zeros((n, n), np.float32)
+        check(load_library().ocean_wake_get_foam_state(self.context, out.ctypes.data))
+        return out
+
+    def set_wake_foam(self, foam) -> None:
+        self._require()
+        n = self._wake_size
+        f = np.ascontiguousarray(foam, np.float32)
+        if f.shape != (n, n):
+            raise ValueError(f"the wake foam field must be [{n}][{n}]")
+        check(load_library().ocean_wake_set_foam_state(self.context, f.ctypes.data))
+
     def twiddles_to_host(self) -> np.ndarray:
         self._require()
         out = np.empty((self.map_size - 1, 2), np.float32)

@@ -627,9 +627,32 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *             Every sub-step of a simulate call reads the same e and e_old, as it reads the same maps.
  *   launches  while primed, one more kernel per step call, per surface query, per buoyancy or body-forces call with world
  *             points and per simulate sub-step with world points.
+ * Foam (ocean_wake_set_foam, opt-in per generator): a foam field F ([N][N] binary32 in window order, values in [0, 1]) of
+ * white water where the wake breaks and where sources stir it, advanced by each sub-step in the same kernel as h, for the
+ * render map's fourth channel.  oracle/wake_foam.py is the specification, bit for bit.  F feeds nothing back: h, h_prev,
+ * the coupling's snapshots and every op are byte-identical with foam on or off.
+ *   model     per call the binary32 constants d = ocean_detmath_expf(-(decay_rate * h)) (the cascades' foam decay exp),
+ *             gh = grow_rate * h and sh = stir_rate * h; per sub-step at tau_k, per cell, with c the cell's convolution of
+ *             s = h + phi above:
+ *               beta = c / dx   (at alpha = 0, h_new - 2 h + h_prev = -(g h^2 / dx) c: beta is the cell's downward vertical
+ *                               acceleration in units of g, about the steepness kA on a crest of a wave in the stencil's
+ *                               band; 0 at rest under a stationary source, so a boat at rest makes no foam)
+ *               sigma = sum, in source index order over the sources that add to phi at the cell, of (w w) * |v|^2, with
+ *                       w = 1 - q2 the weight above and v the centre velocity (vx, vz), plus linear_velocity.xz of its body
+ *                       state when body >= 0; |v|^2 = vx vx + vz vz.  A source of radius r moving straight at U deposits
+ *                       stir_rate (16 / 15) r U (1 - y^2 / r^2)^(5/2) at lateral offset y (with no decay)
+ *               b = beta - whitecap, 0 unless b > 0;  x = F d + (gh b + sh sigma);  F' = min(x, 1) if x > 0, else 0
+ *             (so NaN gives 0).  F scrolls with the window exactly as h does (shift with zero fill).
+ *   memory    enabling allocates two [N][N] binary32 fields (counted in device_bytes), F zeroed; disabling releases them.
+ *             ocean_wake_init turns foam off; ocean_wake_set_state leaves F as it is.
+ *   launches  none extra: while foam is on each sub-step runs the foam form of the same kernel, and the render map the
+ *             foam form of its kernel.
+ *   limits    foam is not advected (the wake has no horizontal velocity; it stays where it forms, as the cascades' foam
+ *             does); wake foam emits no spray; the ray cast and the sampling ops do not read it; there is no per-source
+ *             foam rate; the cascades' foam is unchanged.
  * Limits: the ray cast, spray, ocean_sample_maps and ocean_sample_velocity read the FFT maps only (the ray cast's slab
  * would also need a bound on e); the wake has no horizontal water velocity (iWave is vertical only); bodies do not block
- * waves (no obstruction mask); wakes make no foam; linear deep water only (no breaking, shallow water or nonlinearity); the
+ * waves (no obstruction mask); linear deep water only (no breaking, shallow water or nonlinearity); the
  * layer and the cascades interact by superposition only.
  * Entry points (an invalid call returns OCEAN_ERR_INVALID_ARGUMENT, launches nothing and leaves the layer untouched; a call
  * on a generator without a layer returns OCEAN_ERR_STATE):
@@ -643,8 +666,9 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *                            Launches `substeps` kernels, one more while the coupling is on.  The host form takes host sources and states and returns when
  *                            the work is enqueued; the device form takes device pointers; both are asynchronous on the
  *                            generator's stream.
- *   ocean_wake_render_map    writes [N][N][4] half (h, dh/dx, dh/dz, 0) in window order into map_dev (device memory),
- *                            central differences (h[i+1] - h[i-1]) / (2 dx), cells outside reading 0; world_rect (host,
+ *   ocean_wake_render_map    writes [N][N][4] half (h, dh/dx, dh/dz, F) in window order into map_dev (device memory), F
+ *                            while foam is on and 0 while it is off, each rounded to nearest even from binary32, central
+ *                            differences (h[i+1] - h[i-1]) / (2 dx), cells outside reading 0; world_rect (host,
  *                            may be NULL) receives (x0, z0, N dx, N dx).  One kernel, asynchronous.
  *   ocean_sample_wake        bilinear h, dh/dx and dh/dz ([n][3] float) from the binary32 state at world (x, z); 0 outside
  *                            the window.  One kernel; the host form is synchronous, the device form asynchronous.
@@ -654,7 +678,12 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *                            coupled layer again changes nothing.  Synchronous on disable.
  *   ocean_wake_get_coupling  host copies of e and e_old ([N][N] float), origins[4] = (e.x, e.z, e_old.x, e_old.z) in cells
  *                            and the interval T; zeros, origins 0 and T = 0 while unprimed.  OCEAN_ERR_STATE while the
- *                            coupling is off; every pointer non-NULL.  Synchronous. */
+ *                            coupling is off; every pointer non-NULL.  Synchronous.
+ *   ocean_wake_set_foam      a non-NULL params enables foam (F zeroed) or, when it is on, changes its parameters and keeps
+ *                            F; NULL disables it and releases F (synchronous).  Every field finite, grow_rate, stir_rate and
+ *                            decay_rate >= 0.
+ *   ocean_wake_get_foam_state / ocean_wake_set_foam_state   host copies of F ([N][N] float) in the current window, for
+ *                            tests and checkpoints (synchronous).  OCEAN_ERR_STATE while foam is off; non-NULL array. */
 typedef struct ocean_wake_params {
     int32_t size;               /* N: 0 (release) or a power of two in [128, 2048] */
     int32_t sponge_cells;       /* width of the absorbing ring, [0, 64] and <= size / 2 */
@@ -669,6 +698,12 @@ typedef struct ocean_wake_source {
     float head;                 /* pressure head p / (rho g), m (positive pushes the surface down) */
     int32_t body;               /* index into the body states, or -1 */
 } ocean_wake_source;            /* 28 B */
+typedef struct ocean_wake_foam_params {
+    float whitecap;             /* beta = c / dx above which the wake breaks (units of g) */
+    float grow_rate;            /* foam per second per unit of beta above whitecap, >= 0 */
+    float stir_rate;            /* foam per second per (m/s)^2 of the sources' weighted squared speed, >= 0 */
+    float decay_rate;           /* 1/s, >= 0: F decays as exp(-decay_rate t) */
+} ocean_wake_foam_params;       /* 16 B */
 int ocean_wake_kernel_taps(float* taps_host);
 int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params);
 int ocean_wake_step(ocean_generator* gen, double dt, int substeps, int64_t origin_x, int64_t origin_z, int num_sources,
@@ -682,6 +717,9 @@ int ocean_wake_get_state(ocean_generator* gen, float* h_host, float* h_prev_host
 int ocean_wake_set_state(ocean_generator* gen, const float* h_host, const float* h_prev_host, int64_t origin_x, int64_t origin_z);
 int ocean_wake_set_coupling(ocean_generator* gen, int enable);
 int ocean_wake_get_coupling(ocean_generator* gen, float* e_host, float* e_old_host, int64_t* origins, float* interval);
+int ocean_wake_set_foam(ocean_generator* gen, const ocean_wake_foam_params* params);
+int ocean_wake_get_foam_state(ocean_generator* gen, float* foam_host);
+int ocean_wake_set_foam_state(ocean_generator* gen, const float* foam_host);
 
 /* Parity/debug taps (not timed): binary32 maps before the half conversion, the row-pass output
  * ([4][N][N][2] float, == fft_buffer half 1 after the first fft_compute, wave_generator.gd:79) and
