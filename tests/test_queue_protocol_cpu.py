@@ -139,8 +139,37 @@ class Truth:
         self.fin[k] = self.fin.get(k, 0) + 1
 
 
+def default_queue(map_size):
+    """(group, lag) of persistent_group / persistent_lag without overrides: two thirds of an L2-sized chunk of the two-kernel
+    pipeline per group (chunk_cascades: 24 MiB of scratch at 32 B per texel), lag 2 at 1024^2."""
+    chunk = max(1, (24 << 20) // (map_size * map_size * 32))
+    return max(1, chunk * 2 // 3), (2 if map_size >= 1024 else 1)
+
+
+def batch_queue_shapes():
+    """The queue shapes tests/test_gpu_batch_shapes.py forces on the GPU through OCEAN_QUEUE_GROUP / OCEAN_QUEUE_LAG, as
+    (map_size, count, name, group, lag) with None for "no override": per size the default, the most waits (group 1, lag 1),
+    a group that does not divide the count (a short last group), one group, a lag beyond the number of groups (every row
+    pass before any column pass) and lag 3.  At 256^2 x 24 the default makes 3 groups, at 128^2 x 70 groups of 32, 32
+    and 6, at 512^2 x 7 groups of 2, 2, 2 and 1, and 1024^2 x 8 is cfg4-strong's shape on one GPU (group 1, lag 2)."""
+    out = []
+    for N, C in ((256, 24), (128, 70), (512, 7), (1024, 8)):
+        short = next(g for g in range(3, C) if C % g)
+        out += [(N, C, "default", None, None), (N, C, "group1_lag1", 1, 1), (N, C, "short_last_group", short, None),
+                (N, C, "single_group", C + 1, None), (N, C, "every_row_pass_first", None, 64), (N, C, "lag3", None, 3)]
+    return out
+
+
+def _resolved(shape):
+    N, C, _, group, lag = shape
+    dg, dl = default_queue(N)
+    return N, C, group or dg, lag or dl
+
+
 @pytest.mark.parametrize("map_size,count,group,lag,teams,seed", [
-    (256, 9, 2, 1, 7, 1), (256, 9, 2, 3, 5, 2), (128, 6, 1, 1, 3, 3), (128, 7, 3, 4, 11, 4), (256, 20, 16, 1, 23, 5), (512, 5, 0, 0, 6, 6)])
+    (256, 9, 2, 1, 7, 1), (256, 9, 2, 3, 5, 2), (128, 6, 1, 1, 3, 3), (128, 7, 3, 4, 11, 4), (256, 20, 16, 1, 23, 5), (512, 5, 0, 0, 6, 6),
+    (256, 128, 8, 1, 33, 100)]                                  # the bench workload: 16 groups of 8 cascades, lag 1
+    + [(*_resolved(s), 4 + (13 * k) % 41, 101 + k) for k, s in enumerate(batch_queue_shapes())])
 def test_single_update_protocol_under_random_schedules(map_size, count, group, lag, teams, seed):
     lib = native.load_library()
     items = _queue(lib, map_size, count, group, lag, 0)
@@ -158,7 +187,9 @@ def test_single_update_protocol_under_random_schedules(map_size, count, group, l
 
 
 @pytest.mark.parametrize("map_size,num_cascades,count,launches,teams,seed", [
-    (256, 4, 4, [3, 2], 7, 1), (256, 4, 4, [5], 13, 2), (512, 4, 4, [4, 4, 1], 9, 3), (128, 3, 2, [1, 2, 6], 4, 4), (1024, 8, 8, [2, 3], 10, 5)])
+    (256, 4, 4, [3, 2], 7, 1), (256, 4, 4, [5], 13, 2), (512, 4, 4, [4, 4, 1], 9, 3), (128, 3, 2, [1, 2, 6], 4, 4), (1024, 8, 8, [2, 3], 10, 5),
+    # full dispatch tables of 256 records: 4 frames of 64 cascades and 2 frames of the bench workload's 128 per launch
+    (256, 64, 64, [4, 4, 1], 29, 6), (256, 128, 128, [2, 2], 37, 7)])
 def test_fused_frames_protocol_under_random_schedules(map_size, num_cascades, count, launches, teams, seed):
     lib = native.load_library()
     rng = random.Random(seed)
