@@ -294,6 +294,9 @@ namespace OceanB200
         internal static partial int ocean_wake_get_foam_state(IntPtr handle, float* foam);
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_wake_set_foam_state(IntPtr handle, float* foam);
+        // wake obstacles: a world-fixed mask [depth][width] of blocked cells (nonzero) at world cell origin (x, z); null, 0, 0: none
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_set_obstacles(IntPtr handle, byte* mask, int width, int depth, long origin_x, long origin_z);
         // surface query: the surface at world positions points [n][2] (P + D_xz(P) = Q solved for P, then the map query at P)
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,

@@ -173,6 +173,10 @@ struct ocean_generator {
     ocean_wake_foam_params wake_foam_params{};
     bool wake_foam_on = false;
     int wake_f = 0;                                     // which foam field holds F
+    // wake obstacles (ocean_wake_set_obstacles): the mask's bytes ([depth][width], nonzero = blocked) and its world cell origin
+    DeviceArray<uint8_t> wake_mask;
+    int32_t wake_mask_size[2] = {0, 0};                 // width, depth; 0: no mask
+    int64_t wake_mask_origin[2] = {0, 0};
 };
 
 namespace {
@@ -2022,6 +2026,33 @@ int wake_foam_off(ocean_generator* g) {
 
 float* wake_foam_field(ocean_generator* g, int k) { return g->wake_foam.ptr + (size_t)k * g->wake.size * g->wake.size; }
 
+// Removes the obstacle mask and releases it (the caller has entered the generator).
+int wake_obstacles_off(ocean_generator* g) {
+    if (g->wake_mask.ptr) OCEAN_CUDA(cudaStreamSynchronize(g->stream));     // kernels may still read it
+    g->wake_mask.release();
+    g->wake_mask_size[0] = g->wake_mask_size[1] = 0;
+    g->wake_mask_origin[0] = g->wake_mask_origin[1] = 0;
+    return OCEAN_OK;
+}
+
+// The mask in the window at (origin_x, origin_z): the mask cell of window cell (0, 0), exact in __int128 and clamped to
+// [-2^30, 2^30] per axis.  The halo spans window cells [-6, size + 6) and the mask at most 2^28 cells, so a clamped offset
+// leaves the whole halo outside the mask exactly when the exact one does.
+ocean::WakeObstacles wake_obstacles(const ocean_generator* g, int64_t origin_x, int64_t origin_z) {
+    auto offset = [](int64_t window, int64_t mask) -> int {
+        constexpr __int128 kClamp = (__int128)1 << 30;
+        const __int128 d = (__int128)window - (__int128)mask;
+        return (int)(d > kClamp ? kClamp : d < -kClamp ? -kClamp : d);
+    };
+    ocean::WakeObstacles o{};
+    o.mask = g->wake_mask.ptr;
+    o.width = g->wake_mask_size[0];
+    o.depth = g->wake_mask_size[1];
+    o.qx = offset(origin_x, g->wake_mask_origin[0]);
+    o.qz = offset(origin_z, g->wake_mask_origin[1]);
+    return o;
+}
+
 int check_wake_points(int num_points, const void* points, const void* out) {
     if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
     if (num_points > 0 && (!points || !out)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "points or out is NULL");
@@ -2037,6 +2068,7 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
     if (p.size == 0) {
         if ((rc = wake_uncouple(gen))) return rc;
         if ((rc = wake_foam_off(gen))) return rc;
+        if ((rc = wake_obstacles_off(gen))) return rc;
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
         gen->wake_fields.release();
         gen->wake_sources.release();
@@ -2055,6 +2087,7 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
     const size_t cells = 4 * (size_t)p.size * p.size;  // h, h_prev and two fields a scrolled sub-step writes
     if ((rc = wake_uncouple(gen))) return rc;
     if ((rc = wake_foam_off(gen))) return rc;
+    if ((rc = wake_obstacles_off(gen))) return rc;      // the mask's cells are cells of the old cell size
     gen->wake = ocean_wake_params{};                    // no layer until the fields below are allocated and cleared
     if (gen->wake_fields.capacity != cells) {
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
@@ -2095,6 +2128,9 @@ int ocean_wake_step_device(ocean_generator* gen, double dt, int substeps, int64_
         f.grow = fp.grow_rate * h;
         f.stir = fp.stir_rate * h;
     }
+    // while a mask is set every kernel of the call runs its obstacle form, the mask read in the call's window
+    const bool masked = gen->wake_mask.ptr != nullptr;
+    const ocean::WakeObstacles ob = wake_obstacles(gen, origin_x, origin_z);
     for (int k = 0; k < substeps; ++k) {
         int spare[2], m = 0;
         for (int b = 0; b < 4 && m < 2; ++b)
@@ -2109,8 +2145,13 @@ int ocean_wake_step_device(ocean_generator* gen, double dt, int substeps, int64_
             f.step = a;
             f.foam = wake_foam_field(gen, gen->wake_f);
             f.out_foam = wake_foam_field(gen, gen->wake_f ^ 1);
-            OCEAN_CUDA(ocean::launch_wake_step_foam(f, gen->stream));
+            if (masked)
+                OCEAN_CUDA(ocean::launch_wake_step_foam_obstacles(f, ob, gen->stream));
+            else
+                OCEAN_CUDA(ocean::launch_wake_step_foam(f, gen->stream));
             gen->wake_f ^= 1;
+        } else if (masked) {
+            OCEAN_CUDA(ocean::launch_wake_step_obstacles(a, ob, gen->stream));
         } else {
             OCEAN_CUDA(ocean::launch_wake_step(a, gen->stream));
         }
@@ -2139,7 +2180,10 @@ int ocean_wake_step_device(ocean_generator* gen, double dt, int substeps, int64_
         f.x0 = a.x0;
         f.z0 = a.z0;
         f.tau = (float)substeps * h;
-        OCEAN_CUDA(ocean::launch_wake_free_surface(f, gen->stream));
+        if (masked)
+            OCEAN_CUDA(ocean::launch_wake_free_surface_obstacles(f, ob, gen->stream));
+        else
+            OCEAN_CUDA(ocean::launch_wake_free_surface(f, gen->stream));
         gen->kernel_launches += 1;
         for (int k = 0; k < 2; ++k) {
             if (k != e && gen->wake_primed) continue;
@@ -2301,6 +2345,33 @@ int ocean_wake_set_foam(ocean_generator* gen, const ocean_wake_foam_params* para
         gen->wake_foam_on = true;
     }
     gen->wake_foam_params = p;
+    return OCEAN_OK;
+}
+
+int ocean_wake_set_obstacles(ocean_generator* gen, const uint8_t* mask_host, int32_t width, int32_t depth, int64_t origin_x,
+                             int64_t origin_z) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (!mask_host && width == 0 && depth == 0) return wake_obstacles_off(gen);
+    if (!mask_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "mask_host is NULL with width %d, depth %d", width, depth);
+    if (width < 1 || depth < 1) return fail(OCEAN_ERR_INVALID_ARGUMENT, "mask size %d x %d is not at least 1 x 1", width, depth);
+    if ((int64_t)width * depth > ((int64_t)1 << 28))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "mask size %d x %d above 2^28 cells", width, depth);
+    if (origin_x > INT64_MAX - width || origin_z > INT64_MAX - depth)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "mask origin + size not representable in int64");
+    const size_t cells = (size_t)width * depth;
+    if (gen->wake_mask.capacity != cells) {
+        if ((rc = wake_obstacles_off(gen))) return rc;
+        OCEAN_CUDA(gen->wake_mask.grow(gen, cells));
+    }
+    // stream order puts the copy after the steps that read the old mask; the call returns once the copy is done
+    OCEAN_CUDA(cudaMemcpyAsync(gen->wake_mask.ptr, mask_host, cells, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    gen->wake_mask_size[0] = width;
+    gen->wake_mask_size[1] = depth;
+    gen->wake_mask_origin[0] = origin_x;
+    gen->wake_mask_origin[1] = origin_z;
     return OCEAN_OK;
 }
 

@@ -209,7 +209,19 @@ struct WakeStepArgs {
     float a1[kWakeMaxSponge + 1], a2[kWakeMaxSponge + 1], a3[kWakeMaxSponge + 1];
 };
 void wake_kernel_taps(float* out);                  // host: the 28 taps in the specification's order
+// The obstacle mask (ocean_wake_set_obstacles; oracle/wake_obstacles.py) in the call's window: window cell (i, j) is blocked
+// iff q = qx + i and r = qz + j lie in [0, width) x [0, depth) and mask[r][q] != 0.  qx = origin_x - mask origin x,
+// computed exactly and clamped to [-2^30, 2^30] (a clamped offset leaves every cell of the halo outside the mask, as the
+// exact one does), so q and r are exact in int.
+struct WakeObstacles {
+    const uint8_t* mask;                            // [depth][width] bytes, nonzero = blocked
+    int width, depth;
+    int qx, qz;
+};
 cudaError_t launch_wake_step(const WakeStepArgs& args, cudaStream_t stream);
+// The obstacle forms of the sub-step, the foam sub-step and the free surface: blocked cells read s = 0 and are written 0
+// (h, F and e); h_prev is written unmasked.
+cudaError_t launch_wake_step_obstacles(const WakeStepArgs& args, const WakeObstacles& obstacles, cudaStream_t stream);
 // The foam sub-step (ocean_wake_set_foam; oracle/wake_foam.py): the sub-step of `step`, and F ([n][n], read at (i + di, j + dj),
 // 0 outside) advanced to out_foam (another [n][n] field) with the call's constants.
 struct WakeFoamStepArgs {
@@ -221,6 +233,7 @@ struct WakeFoamStepArgs {
     float grow, stir;                               // grow_rate h, stir_rate h
 };
 cudaError_t launch_wake_step_foam(const WakeFoamStepArgs& args, cudaStream_t stream);
+cudaError_t launch_wake_step_foam_obstacles(const WakeFoamStepArgs& args, const WakeObstacles& obstacles, cudaStream_t stream);
 // map_dev = [n][n][4] half (h, dh/dx, dh/dz, F), F = foam_dev or 0 when foam_dev is null; out_dev = [count][3] floats
 cudaError_t launch_wake_map(const float* h_dev, const float* foam_dev, int n, float cell, void* map_dev, cudaStream_t stream);
 cudaError_t launch_wake_sample(const float* h_dev, int n, float cell, float x0, float z0, const float2* xz_dev, int count, float* out_dev,
@@ -238,6 +251,7 @@ struct WakeFreeSurfaceArgs {
     float cell, x0, z0, tau;
 };
 cudaError_t launch_wake_free_surface(const WakeFreeSurfaceArgs& args, cudaStream_t stream);
+cudaError_t launch_wake_free_surface_obstacles(const WakeFreeSurfaceArgs& args, const WakeObstacles& obstacles, cudaStream_t stream);
 // The snapshots e and e_old ([n][n]) with their window corners, and the interval T between them.
 struct WakeCoupleArgs {
     const float* e;

@@ -13,13 +13,18 @@
 //                   w^2 |v|^2 next to phi (kept per halo cell in shared memory), and each output cell
 //                   updates F from its convolution c and that sum.  F is read at (i + di, j + dj) and written to a second
 //                   field, as h is.
+//   k_wake_step_obstacles, k_wake_step_foam_obstacles  the two sub-steps (the same template) while an obstacle mask is set
+//                   (ocean_wake_set_obstacles; oracle/wake_obstacles.py): the halo pass reads the mask byte of each halo
+//                   cell once, stores s = 0 on blocked cells and marks the blocked output cells in shared memory; those
+//                   are written h = 0 (and F = 0).  h_prev is written unmasked.
 //   k_wake_map      one thread per cell: (h, dh/dx, dh/dz, 0) as half, central differences; k_wake_map_foam writes F as
 //                   the fourth channel.
 //   k_wake_sample   one thread per point: bilinear h and central differences.
 // The coupling of the layer to the surface query (ocean_wake_set_coupling; oracle/wake_coupling.py):
 //   k_wake_free_surface  after a coupled step call: e = h + phi of the sources at the end of the call, one CTA per 32 x 32
 //                        tile; the source cull and the rasterisation are k_wake_step's (one __device__ template, over the
-//                        tile instead of the halo), without the convolution.
+//                        tile instead of the halo), without the convolution.  k_wake_free_surface_obstacles also writes
+//                        e = 0 on blocked cells.
 //   k_wake_couple        one thread per query point: k_wake_sample's bilinear sample of e added to the surface record, and
 //                        on request the wake's vertical velocity (e - e_old) / T at the point for the drag pass.
 // No atomics.  Numeric policy: binary32 in the specification's order with explicit _rn operations, no contraction
@@ -211,12 +216,21 @@ __device__ __forceinline__ void rasterise(const Args& a, int ti0, int tj0, float
     }
 }
 
+// whether window cell (i, j) of the call's window is blocked by the obstacle mask
+__device__ __forceinline__ bool blocked(const WakeObstacles& o, int i, int j) {
+    const int q = o.qx + i, r = o.qz + j;
+    return (unsigned)q < (unsigned)o.width && (unsigned)r < (unsigned)o.depth && o.mask[(size_t)r * o.width + q] != 0;
+}
+
 // One sub-step over one 32 x 32 output tile: k_wake_step, and with kFoam k_wake_step_foam (f is its foam arguments, the
 // foam-only shared arrays speed2 [kThreads] and sig [kHaloCells] are not null).  sigma lives in shared memory rather than
-// in registers next to phi: eight more live registers per thread made the foam form spill.
-template <bool kFoam>
+// in registers next to phi: eight more live registers per thread made the foam form spill.  With kObstacles (ob and the
+// shared [kTile * kTile] out_blocked are not null) the halo pass reads the mask once per halo cell, stores s = 0 on blocked
+// cells and marks the blocked output cells, which are then written 0 (h and F; h_prev is the scrolled h, unmasked).
+template <bool kFoam, bool kObstacles = false>
 __device__ __forceinline__ void wake_step(const WakeStepArgs& a, const WakeFoamStepArgs* f, float* s, float4* list, int* warp_count,
-                                          float* speed2, float* sig) {
+                                          float* speed2, float* sig, const WakeObstacles* ob = nullptr,
+                                          unsigned char* out_blocked = nullptr) {
     const int t = threadIdx.x;
     const int n = a.n;
     const int ti0 = blockIdx.x * kTile - kR, tj0 = blockIdx.y * kTile - kR;   // window cell of halo cell (0, 0)
@@ -240,7 +254,14 @@ __device__ __forceinline__ void wake_step(const WakeStepArgs& a, const WakeFoamS
         if (c < kHaloCells) {
             const int i = ti0 + c % kHalo, j = tj0 + c / kHalo;
             float v = 0.0f;
-            if ((unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n) v = __fadd_rn(cell(a.h, n, i + a.di, j + a.dj), phi[m]);
+            if constexpr (kObstacles) {
+                const bool b = (unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n && blocked(*ob, i, j);
+                if (!b && (unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n) v = __fadd_rn(cell(a.h, n, i + a.di, j + a.dj), phi[m]);
+                const int oi = c % kHalo - kR, oj = c / kHalo - kR;
+                if ((unsigned)oi < (unsigned)kTile && (unsigned)oj < (unsigned)kTile) out_blocked[oj * kTile + oi] = b;
+            } else {
+                if ((unsigned)i < (unsigned)n && (unsigned)j < (unsigned)n) v = __fadd_rn(cell(a.h, n, i + a.di, j + a.dj), phi[m]);
+            }
             s[c] = v;
         }
     }
@@ -256,7 +277,12 @@ __device__ __forceinline__ void wake_step(const WakeStepArgs& a, const WakeFoamS
         const float hp = cell(a.h_prev, n, i + a.di, j + a.dj);
         const int edge = min(min(i, j), min(n - 1 - i, n - 1 - j));
         const int ring = min(edge, a.sponge_cells);
-        const float hn = __fsub_rn(__fsub_rn(__fmul_rn(a.a1[ring], h), __fmul_rn(a.a2[ring], hp)), __fmul_rn(a.a3[ring], c));
+        float hn = __fsub_rn(__fsub_rn(__fmul_rn(a.a1[ring], h), __fmul_rn(a.a2[ring], hp)), __fmul_rn(a.a3[ring], c));
+        bool shut = false;
+        if constexpr (kObstacles) {
+            shut = out_blocked[lj * kTile + li] != 0;
+            if (shut) hn = 0.0f;
+        }
         const size_t o = (size_t)j * n + i;
         a.out_h[o] = hn;
         if (a.out_h_prev) a.out_h_prev[o] = h;
@@ -268,7 +294,7 @@ __device__ __forceinline__ void wake_step(const WakeStepArgs& a, const WakeFoamS
             b = b > 0.0f ? b : 0.0f;
             const float grow = __fadd_rn(__fmul_rn(f->grow, b), __fmul_rn(f->stir, sig[(lj + kR) * kHalo + li + kR]));
             const float v = __fadd_rn(__fmul_rn(cell(f->foam, n, i + a.di, j + a.dj), f->decay), grow);
-            f->out_foam[o] = v > 0.0f ? fminf(v, 1.0f) : 0.0f;
+            f->out_foam[o] = v > 0.0f && !shut ? fminf(v, 1.0f) : 0.0f;
         }
     }
 }
@@ -289,9 +315,28 @@ __global__ void __launch_bounds__(kThreads) k_wake_step_foam(const WakeFoamStepA
     wake_step<true>(f.step, &f, s, list, warp_count, speed2, sig);
 }
 
+__global__ void __launch_bounds__(kThreads) k_wake_step_obstacles(const WakeStepArgs a, const WakeObstacles ob) {
+    __shared__ float s[kHaloCells];
+    __shared__ float4 list[kThreads];               // culled sources: cx, cz, r2, head
+    __shared__ int warp_count[kThreads / 32];
+    __shared__ unsigned char out_blocked[kTile * kTile];
+    wake_step<false, true>(a, nullptr, s, list, warp_count, nullptr, nullptr, &ob, out_blocked);
+}
+
+__global__ void __launch_bounds__(kThreads) k_wake_step_foam_obstacles(const WakeFoamStepArgs f, const WakeObstacles ob) {
+    __shared__ float s[kHaloCells];
+    __shared__ float4 list[kThreads];               // culled sources: cx, cz, r2, head
+    __shared__ int warp_count[kThreads / 32];
+    __shared__ float speed2[kThreads];              // |v|^2 of the culled sources
+    __shared__ float sig[kHaloCells];               // sigma of the halo cells
+    __shared__ unsigned char out_blocked[kTile * kTile];
+    wake_step<true, true>(f.step, &f, s, list, warp_count, speed2, sig, &ob, out_blocked);
+}
+
 // e = h + phi of the sources at a.tau over one 32 x 32 tile (256 threads, 4 cells each), into a.e, and into a.e_old when it
-// is not null (the priming call writes both snapshots)
-__global__ void __launch_bounds__(kThreads) k_wake_free_surface(const WakeFreeSurfaceArgs a) {
+// is not null (the priming call writes both snapshots); with kObstacles e = 0 on blocked cells
+template <bool kObstacles>
+__device__ __forceinline__ void free_surface(const WakeFreeSurfaceArgs& a, const WakeObstacles* ob) {
     __shared__ float4 list[kThreads];
     __shared__ int warp_count[kThreads / 32];
     constexpr int kPer = kTile * kTile / kThreads;
@@ -306,10 +351,19 @@ __global__ void __launch_bounds__(kThreads) k_wake_free_surface(const WakeFreeSu
     for (int m = 0; m < kPer; ++m) {
         const int c = t + m * kThreads;
         const size_t o = (size_t)(tj0 + c / kTile) * n + (ti0 + c % kTile);
-        const float e = __fadd_rn(a.h[o], phi[m]);
+        float e = __fadd_rn(a.h[o], phi[m]);
+        if constexpr (kObstacles) {
+            if (blocked(*ob, ti0 + c % kTile, tj0 + c / kTile)) e = 0.0f;
+        }
         a.e[o] = e;
         if (a.e_old) a.e_old[o] = e;
     }
+}
+
+__global__ void __launch_bounds__(kThreads) k_wake_free_surface(const WakeFreeSurfaceArgs a) { free_surface<false>(a, nullptr); }
+
+__global__ void __launch_bounds__(kThreads) k_wake_free_surface_obstacles(const WakeFreeSurfaceArgs a, const WakeObstacles ob) {
+    free_surface<true>(a, &ob);
 }
 
 __device__ __forceinline__ float grad_x(const float* __restrict__ h, int n, int i, int j, float two_dx) {
@@ -418,6 +472,24 @@ cudaError_t launch_wake_step_foam(const WakeFoamStepArgs& args, cudaStream_t str
 cudaError_t launch_wake_free_surface(const WakeFreeSurfaceArgs& args, cudaStream_t stream) {
     const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
     k_wake_free_surface<<<grid, kThreads, 0, stream>>>(args);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wake_step_obstacles(const WakeStepArgs& args, const WakeObstacles& obstacles, cudaStream_t stream) {
+    const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
+    k_wake_step_obstacles<<<grid, kThreads, 0, stream>>>(args, obstacles);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wake_step_foam_obstacles(const WakeFoamStepArgs& args, const WakeObstacles& obstacles, cudaStream_t stream) {
+    const dim3 grid((unsigned)(args.step.n / kTile), (unsigned)(args.step.n / kTile));
+    k_wake_step_foam_obstacles<<<grid, kThreads, 0, stream>>>(args, obstacles);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wake_free_surface_obstacles(const WakeFreeSurfaceArgs& args, const WakeObstacles& obstacles, cudaStream_t stream) {
+    const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
+    k_wake_free_surface_obstacles<<<grid, kThreads, 0, stream>>>(args, obstacles);
     return cudaGetLastError();
 }
 

@@ -568,6 +568,20 @@ class WaveGenerator:
             raise ValueError(f"the wake foam field must be [{n}][{n}]")
         check(load_library().ocean_wake_set_foam_state(self.context, f.ctypes.data))
 
+    def wake_set_obstacles(self, mask, origin=(0, 0)) -> None:
+        """Block wake waves with a world-fixed mask (include/ocean.h, ocean_wake_set_obstacles): mask [depth][width], nonzero
+        where the cell is land, a quay or a breakwater; row r is world cell row origin[1] + r along z, column q world cell
+        column origin[0] + q along x (cells of the layer's cell size).  mask=None removes it."""
+        self._require()
+        if mask is None:
+            check(load_library().ocean_wake_set_obstacles(self.context, None, 0, 0, 0, 0))
+            return
+        m = np.ascontiguousarray(np.asarray(mask) != 0, np.uint8)
+        if m.ndim != 2:
+            raise ValueError("the obstacle mask must be [depth][width]")
+        check(load_library().ocean_wake_set_obstacles(self.context, m.ctypes.data, m.shape[1], m.shape[0], int(origin[0]),
+                                                      int(origin[1])))
+
     def twiddles_to_host(self) -> np.ndarray:
         self._require()
         out = np.empty((self.map_size - 1, 2), np.float32)

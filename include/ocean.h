@@ -650,10 +650,43 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *   limits    foam is not advected (the wake has no horizontal velocity; it stays where it forms, as the cascades' foam
  *             does); wake foam emits no spray; the ray cast and the sampling ops do not read it; there is no per-source
  *             foam rate; the cascades' foam is unchanged.
+ * Obstacles (ocean_wake_set_obstacles, opt-in per generator; without a mask every kernel and record is as above): a
+ * world-fixed binary mask of blocked cells (quays, breakwaters, islands, the shore) that wake waves reflect from and cannot
+ * cross.  oracle/wake_obstacles.py is the specification, bit for bit.
+ *   grid      the mask lies on the layer's world cell grid: window cell (i, j) at origin (ox, oz) is world cell
+ *             (I, J) = (ox + i, oz + j).  Mask bytes [depth][width]: row r is world cell row J = mz + r along z, column q
+ *             world cell column I = mx + q along x; nonzero = blocked; every cell outside the rectangle is open.  No
+ *             resampling: the window scrolls over the mask in whole cells.
+ *   model     B(i, j): whether window cell (i, j) of the step call's window (the origin it is given; on a scrolled first
+ *             sub-step the new window, the same world cell h is read at through the scroll) is blocked.  Per sub-step
+ *             s = B ? +0 : h + phi;  h_new = B ? +0 : (a1 h - a2 h_prev) - a3 c;  with foam F' = B ? +0 : the update above;
+ *             with the coupling e = B ? +0 : h + phi_end.  h_prev is the previous h, unmasked (on a scrolled sub-step the
+ *             scrolled h); no open cell reads h_prev at a blocked cell.  The render map, ocean_sample_wake and the coupling's
+ *             sampling and wv read h and e unchanged; h is +0 on blocked cells after every sub-step.  Three properties:
+ *             1. A blocked cell is exactly a cell outside the window, which the step reads as s = +0: the open cells evolve
+ *                bit for bit as in a window whose edge ran along the obstacle, so obstacles reflect as the window's edge
+ *                always has (a vertical wall: a shoreline reflects more than a real beach would).
+ *             2. Stability is unchanged: on the open cells the operator is P G P, a principal submatrix of the symmetric
+ *                stencil G, which is positive semi-definite with 0 <= Ghat <= 4, so every eigenvalue of P G P lies in
+ *                [0, 4] and the rule g h^2 / dx * 4 <= 4 above still holds.  The argument needs a 0/1 mask (a fractional
+ *                mask multiplying h has none), which is why the mask is binary.
+ *             3. Barriers and leaks: two open cells interact only if |di| <= 6 and |dj| <= 6, the stencil's radius.  A
+ *                blocked band at least 6 cells thick in that sense (any two open cells on opposite sides more than 6
+ *                cells apart along x or along z) is an exact barrier: water that starts at rest on its far side stays
+ *                exactly +0, unless a source's own footprint reaches across the band (phi is rasterised at every cell
+ *                within a source's radius).  A thinner band transmits part of a wave (a 1-cell wall passes about 6 % of
+ *                an in-band pulse, a 5-cell one about 1 %).  In metres the barrier is 6 dx: at dx = 0.5 m a pier must be
+ *                at least 3 m of blocked cells to stop waves entirely.
+ *   memory    the mask is copied to the device as one byte per cell (width * depth bytes, counted in device_bytes).
+ *   lifetime  a mask takes effect at the next step call.  Setting one touches none of h, h_prev, F or the snapshots (a
+ *             blocked cell keeps its value until the next sub-step writes +0).  ocean_wake_init (re-create or release)
+ *             removes the mask, since the cell size may change; ocean_wake_set_state, ocean_wake_set_foam and
+ *             ocean_wake_set_coupling leave it as it is.
+ *   launches  none extra: while a mask is set each sub-step and the free surface run the obstacle forms of their kernels.
  * Limits: the ray cast, spray, ocean_sample_maps and ocean_sample_velocity read the FFT maps only (the ray cast's slab
- * would also need a bound on e); the wake has no horizontal water velocity (iWave is vertical only); bodies do not block
- * waves (no obstruction mask); linear deep water only (no breaking, shallow water or nonlinearity); the
- * layer and the cascades interact by superposition only.
+ * would also need a bound on e); the wake has no horizontal water velocity (iWave is vertical only); static obstacles block
+ * waves (ocean_wake_set_obstacles) but hulls do not (they are pressure sources); linear deep water only (no breaking,
+ * shallow water or nonlinearity); the layer and the cascades interact by superposition only.
  * Entry points (an invalid call returns OCEAN_ERR_INVALID_ARGUMENT, launches nothing and leaves the layer untouched; a call
  * on a generator without a layer returns OCEAN_ERR_STATE):
  *   ocean_wake_kernel_taps   the 28 taps G[a][b] in the order (0,0), (1,0), (1,1), (2,0), ... (6,6); host only, no device.
@@ -683,7 +716,11 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *                            F; NULL disables it and releases F (synchronous).  Every field finite, grow_rate, stir_rate and
  *                            decay_rate >= 0.
  *   ocean_wake_get_foam_state / ocean_wake_set_foam_state   host copies of F ([N][N] float) in the current window, for
- *                            tests and checkpoints (synchronous).  OCEAN_ERR_STATE while foam is off; non-NULL array. */
+ *                            tests and checkpoints (synchronous).  OCEAN_ERR_STATE while foam is off; non-NULL array.
+ *   ocean_wake_set_obstacles mask_host = NULL with width = depth = 0 removes the mask and releases it; otherwise width and
+ *                            depth >= 1, width * depth <= 2^28 (a 16384^2 mask: 8 km on a side at dx = 0.5 m), and
+ *                            origin + width and origin + depth representable in int64.  An invalid call keeps the previous
+ *                            mask.  Synchronous: returns once the mask is on the device. */
 typedef struct ocean_wake_params {
     int32_t size;               /* N: 0 (release) or a power of two in [128, 2048] */
     int32_t sponge_cells;       /* width of the absorbing ring, [0, 64] and <= size / 2 */
@@ -720,6 +757,8 @@ int ocean_wake_get_coupling(ocean_generator* gen, float* e_host, float* e_old_ho
 int ocean_wake_set_foam(ocean_generator* gen, const ocean_wake_foam_params* params);
 int ocean_wake_get_foam_state(ocean_generator* gen, float* foam_host);
 int ocean_wake_set_foam_state(ocean_generator* gen, const float* foam_host);
+int ocean_wake_set_obstacles(ocean_generator* gen, const uint8_t* mask_host, int32_t width, int32_t depth, int64_t origin_x,
+                             int64_t origin_z);
 
 /* Parity/debug taps (not timed): binary32 maps before the half conversion, the row-pass output
  * ([4][N][N][2] float, == fft_buffer half 1 after the first fft_compute, wave_generator.gd:79) and

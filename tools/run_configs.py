@@ -2,7 +2,7 @@
 config.
 
     python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast] [--spray-particles]
-                                [--wake] [--wake-coupling] [--wake-foam]
+                                [--wake] [--wake-coupling] [--wake-foam] [--wake-obstacles]
 
 Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
 --query.  An unknown argument exits before anything touches the GPU."""
@@ -573,6 +573,35 @@ def run_wake_step_foam(N, sources, reps, label, substeps=8, dx=0.5):
     print(json.dumps(out), flush=True)
 
 
+def run_wake_step_obstacles(N, sources, reps, label, substeps=8, dx=0.5):
+    """Wake obstacles' cost in the step call: run_wake's ocean_wake_step_device with no mask, with a coastline mask over the
+    window (the rows z >= 0.6 N plus a wavy shore: about 40 % of the cells blocked) and with the same mask moved entirely
+    outside the window (the obstacle form still runs, reading nothing but open cells); alternating windows on one generator."""
+    g, _, _ = warmed_generator(128, 2, 1)
+    g.wake_init(N, dx, 0.05, 32, 3.0)
+    rng = np.random.default_rng(N + sources)
+    s = np.zeros(sources, gow.WaveGenerator.WAKE_SOURCE)
+    s["x"], s["z"] = rng.uniform(0, N * dx, sources), rng.uniform(0, 0.55 * N * dx, sources)
+    s["vx"], s["vz"] = 3.0, 0.0
+    s["radius"], s["head"], s["body"] = 2.0, 0.1, -1
+    src = upload(s)
+    q = np.arange(N)
+    shore = (0.6 * N + 0.05 * N * np.sin(q * 4 * np.pi / N)).astype(int)
+    mask = (np.arange(N)[:, None] >= shore[None, :]).astype(np.uint8)
+    lib = load_library()
+    call = lambda: check(lib.ocean_wake_step_device(g.context, substeps / 60.0, substeps, 0, 0, sources, src.data_ptr(), 0, None))
+    t_off, t_on, t_out = alternate(lambda: timed(g, call, reps, 3, lambda: g.wake_set_obstacles(None)),
+                                   lambda: timed(g, call, reps, 3, lambda: g.wake_set_obstacles(mask, (0, 0))),
+                                   lambda: timed(g, call, reps, 3, lambda: g.wake_set_obstacles(mask, (10 * N, 0))))
+    out = {"config": label, **card(), "size": N, "cell_size": dx, "sources": sources, "substeps_per_call": substeps,
+           "blocked_share": float(mask.mean()),
+           "mask_off_us_per_call": [1e3 * v for v in t_off], "coastline_us_per_call": [1e3 * v for v in t_on],
+           "outside_us_per_call": [1e3 * v for v in t_out],
+           "coastline_over_off": min(t_on) / min(t_off) - 1.0, "outside_over_off": min(t_out) / min(t_off) - 1.0}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
 def _picking_rays(side, y=12.0, fov_deg=90.0, pitch_deg=-20.0):
     """side x side camera rays from (0, y, 0) through a square image plane of fov_deg pitched pitch_deg: (RAY array)."""
     f = np.tan(np.radians(fov_deg) / 2.0)
@@ -695,6 +724,10 @@ GROUPS = {          # flag: its configs, in the order they run
     ],
     "--wake-foam": [
         partial(run_wake_step_foam, N, k, 200 if N < 1024 else 50, f"wake foam, step: {N}x{N} cells, {k} source(s), 8 sub-steps")
+        for N in (256, 512, 1024) for k in (1, 64, 1024)
+    ],
+    "--wake-obstacles": [
+        partial(run_wake_step_obstacles, N, k, 200 if N < 1024 else 50, f"wake obstacles, step: {N}x{N} cells, {k} source(s), 8 sub-steps")
         for N in (256, 512, 1024) for k in (1, 64, 1024)
     ],
 }
