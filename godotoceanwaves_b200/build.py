@@ -35,22 +35,20 @@ def is_stale() -> bool:
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build_native(force: bool = False, verbose: bool = False, out: str | None = None, defines=()) -> str:
-    """Compile csrc/*.cu into godotoceanwaves_b200/libocean.so. No-op when up to date.
-    `out`/`defines` build a tuning variant next to it (loaded with OCEAN_LIB=...)."""
-    if out is None and not force and not is_stale():
+def build_native(force: bool = False, verbose: bool = False) -> str:
+    """Compile csrc/*.cu into godotoceanwaves_b200/libocean.so. No-op when up to date."""
+    if not force and not is_stale():
         return LIB_PATH
-    target = out or LIB_PATH
     # several ranks of one job may get here together: one builds (into a temporary file, renamed into place), the others
     # wait on the lock and then find the library up to date
     import fcntl
-    with open(target + ".lock", "w") as lock:
+    with open(LIB_PATH + ".lock", "w") as lock:
         fcntl.flock(lock, fcntl.LOCK_EX)
         try:
-            if out is None and not force and not is_stale():
+            if not force and not is_stale():
                 return LIB_PATH
-            tmp = f"{target}.tmp{os.getpid()}"
-            cmd = [_nvcc(), *NVCC_FLAGS, *[f"-D{d}" for d in defines], "-o", tmp] + [os.path.join(CSRC, s) for s in SOURCES]
+            tmp = f"{LIB_PATH}.tmp{os.getpid()}"
+            cmd = [_nvcc(), *NVCC_FLAGS, "-o", tmp] + [os.path.join(CSRC, s) for s in SOURCES]
             if os.path.exists("/usr/bin/g++"):
                 cmd[1:1] = ["-ccbin", "/usr/bin/g++"]
             if verbose:
@@ -60,12 +58,12 @@ def build_native(force: bool = False, verbose: bool = False, out: str | None = N
                 if os.path.exists(tmp):
                     os.remove(tmp)
                 raise RuntimeError("nvcc failed:\n" + res.stdout)
-            os.replace(tmp, target)
+            os.replace(tmp, LIB_PATH)
             if verbose:
                 print(res.stdout)
         finally:
             fcntl.flock(lock, fcntl.LOCK_UN)
-    return target
+    return LIB_PATH
 
 
 if __name__ == "__main__":

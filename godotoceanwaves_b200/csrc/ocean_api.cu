@@ -10,7 +10,6 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <new>
 #include <string>
@@ -143,7 +142,6 @@ struct ocean_generator {
     int resident_ctas = 0;
     std::map<int, DeviceArray<int>> item_tables;        // cascades per launch -> item table (capacity = item count)
     std::map<std::pair<int, int>, DeviceArray<int>> frame_tables;   // (cascades, frames per launch) -> same, multi-frame order
-    bool persistent = true;                             // OCEAN_PIPELINE=split selects the two-kernel path
     std::vector<ocean_cascade_params> pass_parameters;  // wave_generator.gd:14
     int pass_num_cascades_remaining = 0;                // wave_generator.gd:15
     uint64_t kernel_launches = 0;
@@ -440,7 +438,7 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
         RUN_CUDA(cudaMemcpyAsync(g->d_tables.ptr, ht, sizeof(ocean::TableDispatch) * n_tables, cudaMemcpyHostToDevice, g->stream));
         RUN_CUDA(ocean::launch_dispersion_tables(g->buf, g->d_tables.ptr, n_tables, g->stream));
     }
-    const bool two_kernel = !(g->persistent && !g->profiling);
+    const bool two_kernel = g->profiling;              // profiled updates time the row and the column pass apart
     if (two_kernel)   // the persistent launch takes its dispatch records by value
         RUN_CUDA(cudaMemcpyAsync(g->d_cascade.ptr, hc, sizeof(ocean::CascadeDispatch) * n, cudaMemcpyHostToDevice, g->stream));
     RUN_CUDA(cudaEventRecord(g->ring_done[slot], g->stream));
@@ -461,8 +459,7 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
             launched += 1;
         }
     } else {
-        RUN_CUDA(ocean::launch_cascade_update(g->buf, g->d_cascade.ptr, n, g->stream, &launched, g->profiling ? g->prof[2] : nullptr,
-                                              g->profiling ? g->prof[4] : nullptr));
+        RUN_CUDA(ocean::launch_cascade_update(g->buf, g->d_cascade.ptr, n, g->stream, &launched, g->prof[2], g->prof[4]));
         // (the device-side completion counters are brought in step with the host mirror at the commit below)
     }
     if (g->profiling) {
@@ -604,10 +601,6 @@ int ocean_create(int device, int map_size, int num_cascades, ocean_generator** o
     g->vel_has_source.assign(C, 0);
     g->vel_stale.assign(C, 0);
     for (int i = 0; i < C; ++i) g->scratch_layer_of[i] = 2 * i;
-    {
-        const char* mode = std::getenv("OCEAN_PIPELINE");
-        g->persistent = !(mode && std::strcmp(mode, "split") == 0);
-    }
     CREATE_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&g->h_cascade), sizeof(ocean::CascadeDispatch) * kRing * C, cudaHostAllocDefault));
     CREATE_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&g->h_spectrum), sizeof(ocean::SpectrumDispatch) * kRing * C, cudaHostAllocDefault));
     CREATE_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&g->h_tables), sizeof(ocean::TableDispatch) * kRing * C, cudaHostAllocDefault));
@@ -746,7 +739,7 @@ int ocean_update_frames(ocean_generator* gen, double delta, ocean_cascade_params
     if (frames < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "frames %d is negative", frames);
     if (frames == 0) return OCEAN_OK;
     const int per_launch = count > 0 ? ocean::kMaxPersistentCascades / count : 0;
-    if (!gen->persistent || gen->profiling || per_launch < 2) {        // two-kernel path / huge sets: frame by frame
+    if (gen->profiling || per_launch < 2) {                            // two-kernel path / huge sets: frame by frame
         for (int f = 0; f < frames; ++f)
             if ((rc = ocean_update_all(gen, delta, parameters, count))) return rc;
         return OCEAN_OK;

@@ -82,10 +82,10 @@ cudaError_t launch_dispersion_tables(const DeviceBuffers& b, const TableDispatch
 
 // spectrum_modulate + row IFFT (kernel A) and column IFFT + fft_unpack (kernel B) for `count`
 // cascades, issued as L2-sized chunks (chunk_cascades) of one launch pair each.
-// Returns the number of kernels launched through *launched.  `mid` / `mid2` (optional) are recorded
-// after kernel A / kernel B of the FIRST chunk (per-kernel timing for bench.py).
+// Returns the number of kernels launched through *launched.  `mid` / `mid2` are recorded after kernel A / kernel B
+// of the FIRST chunk: this path serves profiled updates (per-kernel timing for bench.py).
 cudaError_t launch_cascade_update(const DeviceBuffers& b, const CascadeDispatch* dispatch_dev, int count,
-                                  cudaStream_t stream, int* launched, cudaEvent_t mid = nullptr, cudaEvent_t mid2 = nullptr);
+                                  cudaStream_t stream, int* launched, cudaEvent_t mid, cudaEvent_t mid2);
 int chunk_cascades(int map_size);
 
 // Same work as launch_cascade_update in ONE persistent launch (work queue over A and B items, B items

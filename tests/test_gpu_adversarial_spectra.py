@@ -18,7 +18,7 @@ on exactly those bits (should_generate_spectrum = False).  Families, one cascade
     is 0 or 1 (u0 = 0), beside a normal cascade, then a clean seed.
 
 Paths: the production persistent kernel without taps (k_update_persistent<N, false>), the taps kernel (binary32 maps and the
-row pass compared too), and the two-kernel pipeline (OCEAN_PIPELINE=split); fused frames (ocean_update_frames) carry the
+row pass compared too), and the two-kernel pipeline (profiling on); fused frames (ocean_update_frames) carry the
 foam plane through the ladder and the mixed spectrum.
 
 Comparison rule: equal bits wherever the oracle's value is not NaN, signed zeros included, NaN exactly where the oracle's
@@ -178,14 +178,14 @@ def oracle_run(family, N, cases, deltas, frames):
     return snaps
 
 
-def gpu_run(N, cases, deltas, frames, path, monkeypatch):
+def gpu_run(N, cases, deltas, frames, path):
     import godotoceanwaves_b200 as gow
-    if path == "split":
-        monkeypatch.setenv("OCEAN_PIPELINE", "split")
     C = len(cases)
     g = gow.WaveGenerator()
     g.map_size = N
     g.init_gpu(max(2, C))
+    if path == "split":
+        g.set_profiling(True)
     if path == "taps":
         g.enable_f32_taps(True)
     pg = [_params(gow.WaveCascadeParameters, over) for _, _, over in cases]
@@ -232,9 +232,9 @@ def _allowed(name, N, shape):
     return m
 
 
-def compare(family, N, cases, deltas, frames, path, monkeypatch):
+def compare(family, N, cases, deltas, frames, path):
     ref = oracle_run(family, N, cases, deltas, frames)
-    got = gpu_run(N, cases, deltas, frames if path == "persistent" else 0, path, monkeypatch)
+    got = gpu_run(N, cases, deltas, frames if path == "persistent" else 0, path)
     for k, s in enumerate(got):
         r = ref[k]
         for c, (name, _, _) in enumerate(cases):
@@ -308,17 +308,17 @@ def assert_ladder_regimes(N, snap):
 
 @pytest.mark.parametrize("path", PATHS)
 @pytest.mark.parametrize("N", SIZES)
-def test_magnitude_ladder(N, path, monkeypatch):
+def test_magnitude_ladder(N, path):
     cases = ladder_cases(N)
-    ref = compare("ladder", N, cases, (0.02,), 3, path, monkeypatch)
+    ref = compare("ladder", N, cases, (0.02,), 3, path)
     assert_ladder_regimes(N, ref[0])
 
 
 @pytest.mark.parametrize("path", PATHS)
 @pytest.mark.parametrize("N", SIZES)
-def test_mixed_magnitudes(N, path, monkeypatch):
+def test_mixed_magnitudes(N, path):
     cases = mixed_cases(N)
-    ref = compare("mixed", N, cases, (0.02, 0.02), 3, path, monkeypatch)
+    ref = compare("mixed", N, cases, (0.02, 0.02), 3, path)
     h1 = ref[0]["h1"][0]
     out = (_denominator_terms(h1) > 2.0 ** 20).any(0) | (_numerators(h1) < 2.0 ** -100).any(0)
     g = _thread_groups(out, N)
@@ -329,9 +329,9 @@ def test_mixed_magnitudes(N, path, monkeypatch):
 
 @pytest.mark.parametrize("path", PATHS)
 @pytest.mark.parametrize("N", SIZES)
-def test_structured_sparse_spectra(N, path, monkeypatch):
+def test_structured_sparse_spectra(N, path):
     cases = sparse_cases(N)
-    ref = compare("sparse", N, cases, (0.02,), 0, path, monkeypatch)
+    ref = compare("sparse", N, cases, (0.02,), 0, path)
     assert_sparse_regimes(N, cases, ref[0])
 
 

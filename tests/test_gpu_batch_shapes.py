@@ -43,7 +43,6 @@ def _default_queue_shape(monkeypatch):
     """Without overrides from the environment unless a test sets them."""
     monkeypatch.delenv("OCEAN_QUEUE_GROUP", raising=False)
     monkeypatch.delenv("OCEAN_QUEUE_LAG", raising=False)
-    monkeypatch.delenv("OCEAN_PIPELINE", raising=False)
 
 
 def _generator(N, C, taps=False):

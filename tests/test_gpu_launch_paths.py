@@ -4,7 +4,7 @@ CPU oracle, bit for bit:
   * the production persistent kernel without taps (k_update_persistent<N, false>) at 512^2 and 1024^2, default queue;
   * fused frames (ocean_update_frames) at 1024^2;
   * the two-kernel pipeline (k_modulate_rowfft<N> + k_colfft_unpack<N, TAPS>) at every N, chunked by chunk_cascades(N),
-    which OCEAN_PIPELINE=split selects and which every update takes while profiling is on;
+    which every update takes while profiling is on;
   * switching between the two pipelines in the middle of a run (profiling on and off, pending cascades, fused frames);
   * the parameter corners and the generic-math kernels of test_gpu_parity.py (run there at 128^2) at 256^2 to 1024^2;
   * the cold exact-division fix-up of the column pass next to cascades that take the fast path.
@@ -110,18 +110,18 @@ def test_fused_frames_full_size():
 
 @pytest.mark.parametrize("taps", [False, True], ids=["untapped", "taps"])
 @pytest.mark.parametrize("N", [128, 256, 512, 1024])
-def test_two_kernel_pipeline(N, taps, monkeypatch):
-    """OCEAN_PIPELINE=split: chunk_cascades(N) + 1 cascades, so every update is two chunks of one launch pair each.
+def test_profiled_two_kernel_pipeline(N, taps):
+    """Profiling on: chunk_cascades(N) + 1 cascades, so every update is two chunks of one launch pair each.
     Cascades of both chunks are compared with the oracle; with taps (k_colfft_unpack<N, true>) also their binary32 maps
     and row pass."""
     gow = _gow()
-    monkeypatch.setenv("OCEAN_PIPELINE", "split")              # read in ocean_create
     ch = _chunk(N)
     C = ch + 1
     pick = sorted({0, ch - 1, ch})                             # first and last of chunk 1, the only cascade of chunk 2
     pg = [demo_params(gow.WaveCascadeParameters, c) for c in range(C)]
     pcpu = [demo_params(po.CascadeParams, c) for c in pick]
     g = _generator(N, C)
+    g.set_profiling(True)
     if taps:
         g.enable_f32_taps(True)
     o = _oracle(N, keep_f32=taps)

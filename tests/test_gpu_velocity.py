@@ -100,12 +100,12 @@ def test_velocity_after_fused_frames():
 
 
 @pytest.mark.parametrize("taps", [False, True], ids=["untapped", "taps"])
-def test_velocity_two_kernel_pipeline(taps, monkeypatch):
+def test_velocity_two_kernel_pipeline(taps):
     gow = _gow()
-    monkeypatch.setenv("OCEAN_PIPELINE", "split")
     N, C = 512, 4
     pg, pc = _pair(gow.WaveCascadeParameters, C)
     g, o = _generator(N, C, taps=taps), _oracle(N)
+    g.set_profiling(True)
     for delta in (0.02, 0.025):
         g.update_all(delta, pg)
         o.update_all(delta, pc)
