@@ -506,6 +506,13 @@ int check_cascade(ocean_generator* g, int cascade) {
     return OCEAN_OK;
 }
 
+// Layers [first, first + count) inside [0, num_cascades); compared without forming first + count, which can overflow an int.
+int check_layer_range(ocean_generator* g, int first, int count) {
+    if (first < 0 || count < 0 || count > g->num_cascades - first)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "layer range [%d,%lld) outside [0,%d)", first, (long long)first + count, g->num_cascades);
+    return OCEAN_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -859,8 +866,7 @@ int ocean_get_maps(ocean_generator* gen, void** displacement_dev, void** normal_
 int ocean_copy_maps_to_host_async(ocean_generator* gen, int first, int count, void* displacement_host, void* normal_host) {
     OCEAN_ENTER(gen);
     if (rc) return rc;
-    if (first < 0 || count < 0 || first + count > gen->num_cascades)
-        return fail(OCEAN_ERR_INVALID_ARGUMENT, "layer range [%d,%d) outside [0,%d)", first, first + count, gen->num_cascades);
+    if ((rc = check_layer_range(gen, first, count))) return rc;
     const size_t layer = (size_t)gen->map_size * gen->map_size;
     if (displacement_host)
         OCEAN_CUDA(cudaMemcpyAsync(displacement_host, gen->buf.displacement + first * layer, sizeof(uint2) * layer * count, cudaMemcpyDeviceToHost, gen->stream));
@@ -872,8 +878,7 @@ int ocean_copy_maps_to_host_async(ocean_generator* gen, int first, int count, vo
 int ocean_snapshot_maps_to_host_async(ocean_generator* gen, int first, int count, void* displacement_host, void* normal_host) {
     OCEAN_ENTER(gen);
     if (rc) return rc;
-    if (first < 0 || count < 0 || first + count > gen->num_cascades)
-        return fail(OCEAN_ERR_INVALID_ARGUMENT, "layer range [%d,%d) outside [0,%d)", first, first + count, gen->num_cascades);
+    if ((rc = check_layer_range(gen, first, count))) return rc;
     if (count == 0) return OCEAN_OK;
     const size_t layer = (size_t)gen->map_size * gen->map_size;
     if (!gen->copy_stream) {
@@ -1564,8 +1569,7 @@ int ocean_get_velocity_map(ocean_generator* gen, void** velocity_dev, size_t* la
 int ocean_copy_velocity_to_host(ocean_generator* gen, int first, int count, void* velocity_host) {
     OCEAN_ENTER(gen);
     if (rc) return rc;
-    if (first < 0 || count < 0 || first + count > gen->num_cascades)
-        return fail(OCEAN_ERR_INVALID_ARGUMENT, "layer range [%d,%d) outside [0,%d)", first, first + count, gen->num_cascades);
+    if ((rc = check_layer_range(gen, first, count))) return rc;
     if (count == 0) return OCEAN_OK;
     if (!velocity_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "velocity_host is NULL");
     if ((rc = refresh_velocity(gen, nullptr))) return rc;

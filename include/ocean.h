@@ -144,7 +144,8 @@ int ocean_copy_maps_to_host_async(ocean_generator* gen, int first, int count, vo
 /* Overlapped hand-off: snapshots the layers on the device (one device-to-device copy on the generator's stream) and moves the
  * snapshot to (pinned) host memory on a second stream, so the NEXT update runs while the maps of this one cross PCIe.
  * ocean_wait_snapshot() returns when the most recent snapshot has arrived; a new snapshot waits for the previous one to have left
- * the device.  Use two host buffers alternately. */
+ * the device.  Use two host buffers alternately.  ocean_destroy() waits for a snapshot still in flight, so its host buffers
+ * are complete when it returns. */
 int ocean_snapshot_maps_to_host_async(ocean_generator* gen, int first, int count, void* displacement_host, void* normal_host);
 int ocean_wait_snapshot(ocean_generator* gen);
 int ocean_synchronize(ocean_generator* gen);
