@@ -76,6 +76,7 @@ struct ocean_generator {
     // the maps, scratch and tables of ocean_create; `buf` is the view of them (and of the taps) that the kernels take
     DeviceArray<float4> spectrum, rowpass, disp_table;
     DeviceArray<uint2> displacement, normal;
+    DeviceArray<uint16_t> foam;                         // the foam state; normal.a holds a copy of it
     DeviceArray<float4> displacement_f32, normal_f32;   // binary32 taps, while they are on
     DeviceArray<float> disp_kvy;
     DeviceArray<float2> twiddles;
@@ -583,6 +584,7 @@ int ocean_create(int device, int map_size, int num_cascades, ocean_generator** o
     CREATE_CUDA(g->rowpass.grow(g, ocean::kScratchHalves * C * 2 * NN));  // replaces fft_buffer, :33
     CREATE_CUDA(g->displacement.grow(g, C * NN));                         // :34
     CREATE_CUDA(g->normal.grow(g, C * NN));                               // :35
+    CREATE_CUDA(g->foam.grow(g, C * NN));
     CREATE_CUDA(g->twiddles.grow(g, (size_t)ocean::kTwiddleCount + 1));   // :32
     CREATE_CUDA(g->disp_table.grow(g, C * (size_t)(map_size / 2 + 1) * map_size));   // one slot per cascade at most
     CREATE_CUDA(g->disp_kvy.grow(g, C * (size_t)map_size));
@@ -594,6 +596,7 @@ int ocean_create(int device, int map_size, int num_cascades, ocean_generator** o
     g->buf.rowpass = g->rowpass.ptr;
     g->buf.displacement = g->displacement.ptr;
     g->buf.normal = g->normal.ptr;
+    g->buf.foam = g->foam.ptr;
     g->buf.twiddles = g->twiddles.ptr;
     g->buf.disp_table = g->disp_table.ptr;
     g->buf.disp_kvy = g->disp_kvy.ptr;
@@ -620,6 +623,7 @@ int ocean_create(int device, int map_size, int num_cascades, ocean_generator** o
     CREATE_CUDA(cudaMemsetAsync(g->buf.rowpass, 0, sizeof(float4) * ocean::kScratchHalves * C * 2 * NN, g->stream));
     CREATE_CUDA(cudaMemsetAsync(g->buf.displacement, 0, sizeof(uint2) * C * NN, g->stream));
     CREATE_CUDA(cudaMemsetAsync(g->buf.normal, 0, sizeof(uint2) * C * NN, g->stream));
+    CREATE_CUDA(cudaMemsetAsync(g->buf.foam, 0, sizeof(uint16_t) * C * NN, g->stream));
     g->buf.map_size = map_size;
     g->buf.num_cascades = num_cascades;
     CREATE_CUDA(ocean::make_rowpass_tensor_map(g->buf.rowpass, map_size, num_cascades, &g->buf.rowpass_tmap));
@@ -1848,8 +1852,7 @@ int ocean_get_foam_state(ocean_generator* gen, int cascade, uint16_t* host) {
     if ((rc = check_cascade(gen, cascade))) return rc;
     if (!host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "host is NULL");
     const size_t layer = (size_t)gen->map_size * gen->map_size;
-    const uint16_t* src = reinterpret_cast<const uint16_t*>(gen->buf.normal + cascade * layer) + 3;
-    OCEAN_CUDA(cudaMemcpy2DAsync(host, sizeof(uint16_t), src, sizeof(uint2), sizeof(uint16_t), layer, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(host, gen->buf.foam + cascade * layer, sizeof(uint16_t) * layer, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -1860,7 +1863,9 @@ int ocean_set_foam_state(ocean_generator* gen, int cascade, const uint16_t* host
     if ((rc = check_cascade(gen, cascade))) return rc;
     if (!host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "host is NULL");
     const size_t layer = (size_t)gen->map_size * gen->map_size;
+    // the plane is the state the next update reads; normal.a is its copy in the map
     uint16_t* dst = reinterpret_cast<uint16_t*>(gen->buf.normal + cascade * layer) + 3;
+    OCEAN_CUDA(cudaMemcpyAsync(gen->buf.foam + cascade * layer, host, sizeof(uint16_t) * layer, cudaMemcpyHostToDevice, gen->stream));
     OCEAN_CUDA(cudaMemcpy2DAsync(dst, sizeof(uint2), host, sizeof(uint16_t), sizeof(uint16_t), layer, cudaMemcpyHostToDevice, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;

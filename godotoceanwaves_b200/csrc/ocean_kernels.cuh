@@ -53,7 +53,8 @@ struct DeviceBuffers {
     float4* spectrum;      // [C][N][N] (Re h0(k), Im h0(k), Re h0(-k), -Im h0(-k))      RGBA32F
     float4* rowpass;       // [kScratchHalves][C][2][N][N] (re_a, re_b, im_a, im_b), pair p = layers (2p, 2p+1)
     uint2* displacement;   // [C][N][N] 4 x half                                          RGBA16F
-    uint2* normal;         // [C][N][N] 4 x half, .a = foam state                         RGBA16F
+    uint2* normal;         // [C][N][N] 4 x half, .a = copy of the foam state               RGBA16F
+    uint16_t* foam;        // [C][N][N] half, the foam state (fft_unpack.glsl:61-64): read and written by the column pass
     float4* displacement_f32;  // optional taps (nullptr when disabled)
     float4* normal_f32;
     const float2* twiddles;    // [kTwiddleCount] global copy of the universal twiddle table

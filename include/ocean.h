@@ -771,8 +771,9 @@ int ocean_copy_f32_maps_to_host(ocean_generator* gen, int cascade, float* displa
 int ocean_copy_rowpass_to_host(ocean_generator* gen, int cascade, float* host);
 int ocean_copy_twiddles_to_host(ocean_generator* gen, float* host);
 
-/* Checkpoint/resume of the only frame-to-frame state, normal_map.a (fft_unpack.glsl:61-64):
- * [map_size][map_size] IEEE half for one cascade. */
+/* Checkpoint/resume of the only frame-to-frame state, the foam of fft_unpack.glsl:61-64: [map_size][map_size] IEEE half
+ * for one cascade.  The state lives in a plane of its own; every update copies it into normal_map.a, and ocean_set_foam_state
+ * writes both.  Writing normal_map.a through ocean_get_maps does not seed the next update's foam. */
 int ocean_get_foam_state(ocean_generator* gen, int cascade, uint16_t* host);
 int ocean_set_foam_state(ocean_generator* gen, int cascade, const uint16_t* host);
 
