@@ -687,7 +687,12 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  * Limits: the ray cast, spray, ocean_sample_maps and ocean_sample_velocity read the FFT maps only (the ray cast's slab
  * would also need a bound on e); the wake has no horizontal water velocity (iWave is vertical only); static obstacles block
  * waves (ocean_wake_set_obstacles) but hulls do not (they are pressure sources); linear deep water only (no breaking,
- * shallow water or nonlinearity); the layer and the cascades interact by superposition only.
+ * shallow water or nonlinearity); the layer and the cascades interact by superposition only.  Far from the world origin
+ * positions are binary32: phi, the cull and the samples use the cell centres x0 + (float)(i + 1/2) * dx, which lie within
+ * about ulp(|x0|) of the exact (ox + i + 1/2) dx, i.e. up to 2^-23 |ox| cells (measured: 1.5 cells at |ox| = 2^24, 130 at
+ * 2^31).  Keep |ox| and |oz| below about 2^21 cells (at most a quarter of a cell) for sources and samples to land
+ * where the integer window says; beyond, the layer stays bit-identical to the specification, and the integer window, the
+ * scroll and the mask remain exact.
  * Entry points (an invalid call returns OCEAN_ERR_INVALID_ARGUMENT, launches nothing and leaves the layer untouched; a call
  * on a generator without a layer returns OCEAN_ERR_STATE):
  *   ocean_wake_kernel_taps   the 28 taps G[a][b] in the order (0,0), (1,0), (1,1), (2,0), ... (6,6); host only, no device.
