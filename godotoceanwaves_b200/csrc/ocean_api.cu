@@ -61,6 +61,13 @@ struct DeviceArray {
     cudaError_t upload(ocean_generator* g, const void* host, size_t n);
     void release();
 };
+
+// The host entry points that stage the caller's arrays, one staging block each (ocean_generator::staging, see Staging).
+enum StagedOp {
+    kStageSampleMaps, kStageExtractSpray, kStageSprayParticles, kStageQuerySurface, kStageRaycast, kStageBuoyancy,
+    kStageSampleVelocity, kStageBodyForces, kStageSimulateBodies, kStageDeviceMath, kStageWakeStep, kStageSampleWake,
+    kNumStagedOps
+};
 }  // namespace
 
 struct ocean_generator {
@@ -82,35 +89,25 @@ struct ocean_generator {
     DeviceArray<float2> twiddles;
     ocean::DeviceBuffers buf{};
     DeviceArray<float2> export_buf;                     // rowpass export scratch (lazy)
-    // query staging, grown on demand: points and map-query outputs for the host entry points, map scales
-    DeviceArray<float2> q_points;
-    DeviceArray<float> q_disp, q_grad;
-    DeviceArray<float4> q_scales;
+    DeviceArray<unsigned char> staging[kNumStagedOps];  // each host entry point's copies of the caller's arrays (Staging)
+    DeviceArray<float4> q_scales;                       // map scales of the query ops
     DeviceArray<int> spray_counts;                      // spray op scratch: block counts / offsets (+ total)
-    DeviceArray<ocean_spray_record> spray_records;      // spray op staging for the host entry point (+ one slot for the count)
-    DeviceArray<ocean_spray_particle> spray_states;     // spray particle staging for the host entry point: states
-    DeviceArray<float> spray_instances;                 // and instances (+ one slot for the count); block counts in spray_counts
     DeviceArray<int> surf_scratch;                      // surface query scratch: pending count, layer maxima, pending list
-    DeviceArray<ocean_surface_sample> surf_records;     // surface query staging for the host entry point
-    // buoyancy staging: body table and world-point offsets, query positions, surface records (when the caller wants none),
-    // and the host entry point's hull points and results
+    // buoyancy scratch: body table and world-point offsets, query positions, surface records (when the caller wants none)
     DeviceArray<ocean_buoyancy_body> buoy_bodies;
     DeviceArray<int> buoy_offsets;
     std::vector<int> buoy_offsets_host;
     DeviceArray<float2> buoy_q;
     DeviceArray<ocean_surface_sample> buoy_samples;
-    DeviceArray<ocean_buoyancy_point> buoy_points;
-    DeviceArray<ocean_buoyancy_result> buoy_results;
-    // body-forces staging: body velocities, and the host entry point's drag areas and drag results
+    // the body velocities of the drag pass
     DeviceArray<ocean_body_velocity> drag_velocities;
-    DeviceArray<float> drag_areas;
+    // ocean_simulate_bodies_device's hydrostatic and drag results when its caller passes NULL for them
+    DeviceArray<ocean_buoyancy_result> buoy_results;
     DeviceArray<ocean_drag_result> drag_results;
-    // floating-body staging: the body table, max |p|^2 per hull, and the host entry point's states and transforms (the pose
-    // and velocity tables are buoy_bodies and drag_velocities)
+    // floating-body scratch: the body table and max |p|^2 per hull (the pose and velocity tables are buoy_bodies and
+    // drag_velocities)
     DeviceArray<ocean_floating_body> sim_bodies;
     DeviceArray<float> sim_r2;
-    DeviceArray<ocean_body_state> sim_states;
-    DeviceArray<float> sim_transforms;
     // velocity maps, allocated by the first velocity call: row-pass scratch, the map, its binary32 tap while the taps are on
     DeviceArray<float4> vel_scratch;                    // [num_cascades][N][N]
     DeviceArray<uint2> velocity;                        // [num_cascades][N][N] 4 x half
@@ -148,14 +145,8 @@ struct ocean_generator {
     uint64_t kernel_launches = 0;
     uint64_t cascade_updates = 0;
     DeviceArray<unsigned> ray_bounds;                   // ray cast scratch: [3 * num_cascades] per-layer bounds (first use)
-    DeviceArray<ocean_ray> ray_in;                      // ray cast staging for the host entry point
-    DeviceArray<ocean_ray_hit> ray_out;
-    // wake layer (ocean_wake_init): four [size][size] fields -- h, h_prev and the two a sub-step writes -- and the host
-    // entry points' staging
+    // wake layer (ocean_wake_init): four [size][size] fields -- h, h_prev and the two a sub-step writes
     DeviceArray<float> wake_fields;
-    DeviceArray<ocean_wake_source> wake_sources;
-    DeviceArray<ocean_body_state> wake_states;
-    DeviceArray<float> wake_samples;
     ocean_wake_params wake{};                           // size 0: no layer
     int wake_h = 0, wake_hp = 1;                        // which fields hold h and h_prev
     int64_t wake_origin[2] = {0, 0};
@@ -241,6 +232,44 @@ void DeviceArray<T>::release() {
     ptr = nullptr;
     capacity = 0;
 }
+
+// A host entry point's device copies of the caller's arrays: one slice per array in the entry point's own block
+// gen->staging[op], each at a 256-byte boundary (the kernels load float4 and record types).  upload() grows the block once and
+// copies the `in` and `inout` arrays to it; st[slice] is then the slice's device pointer, NULL when the slice is empty (a count
+// of 0 or a NULL host array).  finish() copies the `out` and `inout` arrays back and synchronises; `scratch` is not copied.
+struct Staging {
+    template <typename T> struct Slice { size_t offset, bytes; };
+    struct Copy { size_t offset, bytes; const void* up; void* down; };
+    std::vector<Copy> copies;
+    size_t total = 0;
+    unsigned char* base = nullptr;
+
+    template <typename T> Slice<T> add(const void* up, void* down, size_t bytes) {
+        copies.push_back({(total + 255) & ~(size_t)255, bytes, up, down});
+        total = copies.back().offset + bytes;
+        return {copies.back().offset, bytes};
+    }
+    template <typename T> Slice<const T> in(const T* host, size_t n) { return add<const T>(host, nullptr, host ? n * sizeof(T) : 0); }
+    template <typename T> Slice<T> out(T* host, size_t n) { return add<T>(nullptr, host, host ? n * sizeof(T) : 0); }
+    template <typename T> Slice<T> inout(T* host, size_t n) { return add<T>(host, host, host ? n * sizeof(T) : 0); }
+    template <typename T> Slice<T> scratch(size_t n) { return add<T>(nullptr, nullptr, n * sizeof(T)); }
+    template <typename T> T* operator[](Slice<T> s) const { return s.bytes ? reinterpret_cast<T*>(base + s.offset) : nullptr; }
+
+    int upload(ocean_generator* g, StagedOp op) {
+        OCEAN_CUDA(g->staging[op].grow(g, total));
+        base = g->staging[op].ptr;
+        for (const Copy& c : copies)
+            if (c.up && c.bytes) OCEAN_CUDA(cudaMemcpyAsync(base + c.offset, c.up, c.bytes, cudaMemcpyHostToDevice, g->stream));
+        return OCEAN_OK;
+    }
+    int finish(ocean_generator* g, int rc) {            // rc: the status of the device work; nothing is copied after a failure
+        if (rc) return rc;
+        for (const Copy& c : copies)
+            if (c.down && c.bytes) OCEAN_CUDA(cudaMemcpyAsync(c.down, base + c.offset, c.bytes, cudaMemcpyDeviceToHost, g->stream));
+        OCEAN_CUDA(cudaStreamSynchronize(g->stream));
+        return OCEAN_OK;
+    }
+};
 
 // Device memory is released by the generator's DeviceArrays; the rest is released here.
 void release(ocean_generator* g) {
@@ -1081,17 +1110,11 @@ int ocean_sample_maps(ocean_generator* gen, int num_points, const float* points_
     if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
     if (num_points == 0) return OCEAN_OK;
     if (!points_xz_host || !displacement_host || !gradient_foam_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    const size_t n = (size_t)num_points;
-    OCEAN_CUDA(gen->q_disp.grow(gen, 3 * n));
-    OCEAN_CUDA(gen->q_grad.grow(gen, 3 * n));
-    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, n));
-    if ((rc = ocean_sample_maps_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points.ptr), num_cascades, map_scales_host,
-                                       gen->q_disp.ptr, gen->q_grad.ptr)))
-        return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(displacement_host, gen->q_disp.ptr, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(gradient_foam_host, gen->q_grad.ptr, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    return OCEAN_OK;
+    Staging st;
+    const auto points = st.in(points_xz_host, 2 * (size_t)num_points);
+    const auto disp = st.out(displacement_host, 3 * (size_t)num_points), grad = st.out(gradient_foam_host, 3 * (size_t)num_points);
+    if ((rc = st.upload(gen, kStageSampleMaps))) return rc;
+    return st.finish(gen, ocean_sample_maps_device(gen, num_points, st[points], num_cascades, map_scales_host, st[disp], st[grad]));
 }
 
 // ---- spray candidates (SURVEY 8f row f3) ----
@@ -1156,18 +1179,17 @@ int ocean_extract_spray(ocean_generator* gen, int num_candidates, const float* p
     *num_active = 0;
     if (num_candidates == 0) return OCEAN_OK;
     if (!points_xz_host || (max_records > 0 && !records_host)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    OCEAN_CUDA(gen->spray_records.grow(gen, (size_t)max_records + 1));                 // + one slot for the count
-    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, (size_t)num_candidates));
-    ocean_spray_record* recs = gen->spray_records.ptr;
-    int* count_dev = reinterpret_cast<int*>(recs + max_records);
-    if ((rc = ocean_extract_spray_device(gen, num_candidates, reinterpret_cast<const float*>(gen->q_points.ptr), num_cascades, map_scales_host,
-                                         particle_scale, max_records, recs, count_dev)))
-        return rc;
     int count = 0;
-    OCEAN_CUDA(cudaMemcpyAsync(&count, count_dev, sizeof(int), cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    const int kept = count < max_records ? count : max_records;
-    if (kept > 0) OCEAN_CUDA(cudaMemcpy(records_host, recs, sizeof(ocean_spray_record) * (size_t)kept, cudaMemcpyDeviceToHost));
+    Staging st;
+    const auto points = st.in(points_xz_host, 2 * (size_t)num_candidates);
+    const auto records = st.scratch<ocean_spray_record>((size_t)max_records);         // copied back below: only those kept
+    const auto count_dev = st.out(&count, 1);
+    if ((rc = st.upload(gen, kStageExtractSpray))) return rc;
+    if ((rc = st.finish(gen, ocean_extract_spray_device(gen, num_candidates, st[points], num_cascades, map_scales_host, particle_scale,
+                                                        max_records, st[records], st[count_dev]))))
+        return rc;
+    const int kept = std::min(count, max_records);
+    if (kept > 0) OCEAN_CUDA(cudaMemcpy(records_host, st[records], sizeof(ocean_spray_record) * (size_t)kept, cudaMemcpyDeviceToHost));
     *num_active = count;
     return OCEAN_OK;
 }
@@ -1251,20 +1273,17 @@ int ocean_spray_particles(ocean_generator* gen, const ocean_spray_emitter* emitt
         return rc;
     *num_live = 0;
     if (emitter->amount == 0) return OCEAN_OK;
-    const size_t n = (size_t)emitter->amount;
-    OCEAN_CUDA(gen->spray_instances.grow(gen, 16 * (size_t)max_instances + 1));          // + one slot for the count
-    OCEAN_CUDA(gen->spray_states.upload(gen, states_host, n));
-    float* inst = gen->spray_instances.ptr;
-    int* count_dev = reinterpret_cast<int*>(inst + 16 * (size_t)max_instances);
-    if ((rc = ocean_spray_particles_device(gen, emitter, t0, t1, num_cascades, map_scales_host, gen->spray_states.ptr, max_instances, inst,
-                                           count_dev)))
-        return rc;
     int count = 0;
-    OCEAN_CUDA(cudaMemcpyAsync(states_host, gen->spray_states.ptr, sizeof(ocean_spray_particle) * n, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(&count, count_dev, sizeof(int), cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    const int kept = count < max_instances ? count : max_instances;
-    if (kept > 0) OCEAN_CUDA(cudaMemcpy(instances_host, inst, sizeof(float) * 16 * (size_t)kept, cudaMemcpyDeviceToHost));
+    Staging st;
+    const auto states = st.inout(states_host, (size_t)emitter->amount);
+    const auto instances = st.scratch<float>(16 * (size_t)max_instances);             // copied back below: only those kept
+    const auto count_dev = st.out(&count, 1);
+    if ((rc = st.upload(gen, kStageSprayParticles))) return rc;
+    if ((rc = st.finish(gen, ocean_spray_particles_device(gen, emitter, t0, t1, num_cascades, map_scales_host, st[states], max_instances,
+                                                          st[instances], st[count_dev]))))
+        return rc;
+    const int kept = std::min(count, max_instances);
+    if (kept > 0) OCEAN_CUDA(cudaMemcpy(instances_host, st[instances], sizeof(float) * 16 * (size_t)kept, cudaMemcpyDeviceToHost));
     *num_live = count;
     return OCEAN_OK;
 }
@@ -1333,15 +1352,12 @@ int ocean_query_surface(ocean_generator* gen, int num_points, const float* point
     if ((rc = check_surface_args(num_points, tolerance, max_iterations))) return rc;
     if (num_points == 0) return OCEAN_OK;
     if (!points_xz_host || !out_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    const size_t n = (size_t)num_points;
-    OCEAN_CUDA(gen->surf_records.grow(gen, n));
-    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, n));
-    if ((rc = ocean_query_surface_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points.ptr), num_cascades, map_scales_host,
-                                         tolerance, max_iterations, gen->surf_records.ptr)))
-        return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->surf_records.ptr, sizeof(ocean_surface_sample) * n, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    return OCEAN_OK;
+    Staging st;
+    const auto points = st.in(points_xz_host, 2 * (size_t)num_points);
+    const auto out = st.out(out_host, (size_t)num_points);
+    if ((rc = st.upload(gen, kStageQuerySurface))) return rc;
+    return st.finish(gen, ocean_query_surface_device(gen, num_points, st[points], num_cascades, map_scales_host, tolerance, max_iterations,
+                                                     st[out]));
 }
 
 // ---- ray cast: the first crossing of each ray with the displaced surface (slab bounds, then one thread per ray) ----
@@ -1380,15 +1396,12 @@ int ocean_raycast(ocean_generator* gen, int num_rays, const ocean_ray* rays_host
     if ((rc = check_raycast_args(num_rays, step, max_samples, tolerance, max_iterations))) return rc;
     if (num_rays == 0) return OCEAN_OK;
     if (!rays_host || !out_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    const size_t n = (size_t)num_rays;
-    OCEAN_CUDA(gen->ray_out.grow(gen, n));
-    OCEAN_CUDA(gen->ray_in.upload(gen, rays_host, n));
-    if ((rc = ocean_raycast_device(gen, num_rays, gen->ray_in.ptr, num_cascades, map_scales_host, step, max_samples, tolerance, max_iterations,
-                                   gen->ray_out.ptr)))
-        return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->ray_out.ptr, sizeof(ocean_ray_hit) * n, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    return OCEAN_OK;
+    Staging st;
+    const auto rays = st.in(rays_host, (size_t)num_rays);
+    const auto out = st.out(out_host, (size_t)num_rays);
+    if ((rc = st.upload(gen, kStageRaycast))) return rc;
+    return st.finish(gen, ocean_raycast_device(gen, num_rays, st[rays], num_cascades, map_scales_host, step, max_samples, tolerance,
+                                               max_iterations, st[out]));
 }
 
 // ---- buoyancy: per-body force and torque from hull points on the surface (the surface query between two buoyancy kernels) ----
@@ -1458,7 +1471,7 @@ int launch_buoyancy_sequence(ocean_generator* gen, const ocean_buoyancy_body* bo
 
 // The buoyancy launch sequence on validated arguments (num_bodies > 0), with the map scales already in gen->q_scales: the body
 // table and offsets are uploaded to gen->buoy_bodies / gen->buoy_offsets, and *samples_used receives the surface records
-// (samples_dev, or the generator's staging when samples_dev is NULL) for a drag pass on the same points.
+// (samples_dev, or gen->buoy_samples when samples_dev is NULL) for a drag pass on the same points.
 int run_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int world, const ocean_buoyancy_point* points_dev,
                  int num_cascades, float density, float tolerance, int max_iterations, ocean_buoyancy_result* results_dev,
                  ocean_surface_sample* samples_dev, ocean_surface_sample** samples_used, float* wv_dev = nullptr) {
@@ -1499,18 +1512,13 @@ int ocean_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_bo
     if ((rc = check_buoyancy_args(num_bodies, bodies_host, num_points, density, tolerance, max_iterations, &world))) return rc;
     if (num_bodies == 0) return OCEAN_OK;
     if (!results_host || (world > 0 && !points_host)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    OCEAN_CUDA(gen->buoy_results.grow(gen, (size_t)num_bodies));
-    if (world > 0) OCEAN_CUDA(gen->buoy_points.upload(gen, points_host, (size_t)num_points));
-    if ((rc = ocean_buoyancy_device(gen, num_bodies, bodies_host, num_points, world > 0 ? gen->buoy_points.ptr : nullptr, num_cascades,
-                                    map_scales_host, density, tolerance, max_iterations, gen->buoy_results.ptr, nullptr)))
-        return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(results_host, gen->buoy_results.ptr, sizeof(ocean_buoyancy_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost,
-                               gen->stream));
-    if (samples_host && world > 0)
-        OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples.ptr, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
-                                   gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    return OCEAN_OK;
+    Staging st;
+    const auto points = st.in(points_host, world > 0 ? (size_t)num_points : 0);
+    const auto results = st.out(results_host, (size_t)num_bodies);
+    const auto samples = st.out(samples_host, (size_t)world);
+    if ((rc = st.upload(gen, kStageBuoyancy))) return rc;
+    return st.finish(gen, ocean_buoyancy_device(gen, num_bodies, bodies_host, num_points, st[points], num_cascades, map_scales_host, density,
+                                                tolerance, max_iterations, st[results], st[samples]));
 }
 
 // ---- velocity maps: the time derivative of the displacement map (ocean_velocity.cu; oracle_velocity_update) ----
@@ -1618,15 +1626,11 @@ int ocean_sample_velocity(ocean_generator* gen, int num_points, const float* poi
     if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
     if (num_points == 0) return OCEAN_OK;
     if (!points_xz_host || !velocity_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    const size_t n = (size_t)num_points;
-    OCEAN_CUDA(gen->q_disp.grow(gen, 3 * n));
-    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, n));
-    if ((rc = ocean_sample_velocity_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points.ptr), num_cascades, map_scales_host,
-                                           gen->q_disp.ptr)))
-        return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(velocity_host, gen->q_disp.ptr, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    return OCEAN_OK;
+    Staging st;
+    const auto points = st.in(points_xz_host, 2 * (size_t)num_points);
+    const auto velocity = st.out(velocity_host, 3 * (size_t)num_points);
+    if ((rc = st.upload(gen, kStageSampleVelocity))) return rc;
+    return st.finish(gen, ocean_sample_velocity_device(gen, num_points, st[points], num_cascades, map_scales_host, st[velocity]));
 }
 
 // ---- body forces: buoyancy plus quadratic drag against the water velocity, from one surface query (oracle/drag.py) ----
@@ -1690,25 +1694,17 @@ int ocean_body_forces(ocean_generator* gen, int num_bodies, const ocean_buoyancy
         return rc;
     if (num_bodies == 0) return OCEAN_OK;
     if (!hydrostatic_host || !drag_host || (world > 0 && !points_host)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    OCEAN_CUDA(gen->buoy_results.grow(gen, (size_t)num_bodies));
-    OCEAN_CUDA(gen->drag_results.grow(gen, (size_t)num_bodies));
-    if (world > 0) {
-        OCEAN_CUDA(gen->buoy_points.upload(gen, points_host, (size_t)num_points));
-        OCEAN_CUDA(gen->drag_areas.upload(gen, drag_areas_host, (size_t)num_points));
-    }
-    if ((rc = ocean_body_forces_device(gen, num_bodies, bodies_host, velocities_host, num_points, world > 0 ? gen->buoy_points.ptr : nullptr,
-                                       world > 0 ? gen->drag_areas.ptr : nullptr, num_cascades, map_scales_host, density, tolerance,
-                                       max_iterations, gen->buoy_results.ptr, gen->drag_results.ptr, nullptr)))
-        return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(hydrostatic_host, gen->buoy_results.ptr, sizeof(ocean_buoyancy_result) * (size_t)num_bodies,
-                               cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(drag_host, gen->drag_results.ptr, sizeof(ocean_drag_result) * (size_t)num_bodies, cudaMemcpyDeviceToHost,
-                               gen->stream));
-    if (samples_host && world > 0)
-        OCEAN_CUDA(cudaMemcpyAsync(samples_host, gen->buoy_samples.ptr, sizeof(ocean_surface_sample) * (size_t)world, cudaMemcpyDeviceToHost,
-                                   gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    return OCEAN_OK;
+    const size_t P = world > 0 ? (size_t)num_points : 0, B = (size_t)num_bodies;
+    Staging st;
+    const auto points = st.in(points_host, P);
+    const auto areas = st.in(drag_areas_host, P);
+    const auto hydrostatic = st.out(hydrostatic_host, B);
+    const auto drag = st.out(drag_host, B);
+    const auto samples = st.out(samples_host, (size_t)world);
+    if ((rc = st.upload(gen, kStageBodyForces))) return rc;
+    return st.finish(gen, ocean_body_forces_device(gen, num_bodies, bodies_host, velocities_host, num_points, st[points], st[areas],
+                                                   num_cascades, map_scales_host, density, tolerance, max_iterations, st[hydrostatic],
+                                                   st[drag], st[samples]));
 }
 
 // ---- floating bodies: sub-stepped buoyancy and drag with the body state on the device (ocean_bodies.cu; oracle/bodies.py) ----
@@ -1811,30 +1807,18 @@ int ocean_simulate_bodies(ocean_generator* gen, int num_bodies, const ocean_floa
         return rc;
     if (num_bodies == 0) return OCEAN_OK;
     if (world > 0 && !points_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
-    const size_t B = (size_t)num_bodies;
-    OCEAN_CUDA(gen->buoy_results.grow(gen, B));
-    OCEAN_CUDA(gen->drag_results.grow(gen, B));
-    if (transforms_host) OCEAN_CUDA(gen->sim_transforms.grow(gen, 12 * B));
-    if (world > 0) {
-        OCEAN_CUDA(gen->buoy_points.upload(gen, points_host, (size_t)num_points));
-        OCEAN_CUDA(gen->drag_areas.upload(gen, drag_areas_host, (size_t)num_points));
-    }
-    OCEAN_CUDA(gen->sim_states.upload(gen, states_host, B));
-    if ((rc = ocean_simulate_bodies_device(gen, num_bodies, bodies_host, gen->sim_states.ptr, num_points, world > 0 ? gen->buoy_points.ptr : nullptr,
-                                           world > 0 ? gen->drag_areas.ptr : nullptr, num_cascades, map_scales_host, density, dt, substeps,
-                                           tolerance, max_iterations, gen->buoy_results.ptr, gen->drag_results.ptr,
-                                           transforms_host ? gen->sim_transforms.ptr : nullptr)))
-        return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(states_host, gen->sim_states.ptr, sizeof(ocean_body_state) * B, cudaMemcpyDeviceToHost, gen->stream));
-    if (hydrostatic_host)
-        OCEAN_CUDA(cudaMemcpyAsync(hydrostatic_host, gen->buoy_results.ptr, sizeof(ocean_buoyancy_result) * B, cudaMemcpyDeviceToHost,
-                                   gen->stream));
-    if (drag_host)
-        OCEAN_CUDA(cudaMemcpyAsync(drag_host, gen->drag_results.ptr, sizeof(ocean_drag_result) * B, cudaMemcpyDeviceToHost, gen->stream));
-    if (transforms_host)
-        OCEAN_CUDA(cudaMemcpyAsync(transforms_host, gen->sim_transforms.ptr, sizeof(float) * 12 * B, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    return OCEAN_OK;
+    const size_t P = world > 0 ? (size_t)num_points : 0, B = (size_t)num_bodies;
+    Staging st;                                         // an output not asked for stays NULL: the twin uses its own
+    const auto points = st.in(points_host, P);
+    const auto areas = st.in(drag_areas_host, P);
+    const auto states = st.inout(states_host, B);
+    const auto hydrostatic = st.out(hydrostatic_host, B);
+    const auto drag = st.out(drag_host, B);
+    const auto transforms = st.out(transforms_host, 12 * B);
+    if ((rc = st.upload(gen, kStageSimulateBodies))) return rc;
+    return st.finish(gen, ocean_simulate_bodies_device(gen, num_bodies, bodies_host, st[states], num_points, st[points], st[areas],
+                                                       num_cascades, map_scales_host, density, dt, substeps, tolerance, max_iterations,
+                                                       st[hydrostatic], st[drag], st[transforms]));
 }
 
 int ocean_copy_twiddles_to_host(ocean_generator* gen, float* host) {
@@ -1933,16 +1917,13 @@ int ocean_debug_device_math(ocean_generator* gen, int fn, int n, const float* a_
     if (n < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "n = %d is negative", n);
     if (n == 0) return OCEAN_OK;
     if (!a_host || !b_host || !out_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "NULL argument");
-    // the query staging buffers: a and b in the first 2n floats of q_disp, the results in q_points
-    OCEAN_CUDA(gen->q_points.grow(gen, (size_t)n));
-    OCEAN_CUDA(gen->q_disp.grow(gen, 2 * (size_t)n));
-    OCEAN_CUDA(cudaMemcpyAsync(gen->q_disp.ptr, a_host, sizeof(float) * n, cudaMemcpyHostToDevice, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(gen->q_disp.ptr + n, b_host, sizeof(float) * n, cudaMemcpyHostToDevice, gen->stream));
-    OCEAN_CUDA(ocean::launch_debug_device_math(fn, n, gen->q_disp.ptr, gen->q_disp.ptr + n, gen->q_points.ptr, gen->stream));
+    Staging st;
+    const auto a = st.in(a_host, (size_t)n), b = st.in(b_host, (size_t)n);
+    const auto out = st.out(reinterpret_cast<float2*>(out_host), (size_t)n);
+    if ((rc = st.upload(gen, kStageDeviceMath))) return rc;
+    OCEAN_CUDA(ocean::launch_debug_device_math(fn, n, st[a], st[b], st[out], gen->stream));
     gen->kernel_launches += 1;
-    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->q_points.ptr, sizeof(float2) * n, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    return OCEAN_OK;
+    return st.finish(gen, OCEAN_OK);
 }
 
 // ---- wake layer: a local height field driven by moving sources (oracle/wake.py) ----
@@ -2073,9 +2054,8 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
         if ((rc = wake_obstacles_off(gen))) return rc;
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
         gen->wake_fields.release();
-        gen->wake_sources.release();
-        gen->wake_states.release();
-        gen->wake_samples.release();
+        gen->staging[kStageWakeStep].release();
+        gen->staging[kStageSampleWake].release();
         gen->wake = ocean_wake_params{};
         return OCEAN_OK;
     }
@@ -2210,9 +2190,11 @@ int ocean_wake_step(ocean_generator* gen, double dt, int substeps, int64_t origi
     for (int k = 0; k < num_sources; ++k)
         if (sources_host[k].body >= num_states)
             return fail(OCEAN_ERR_INVALID_ARGUMENT, "source %d: body %d is not below num_states %d", k, sources_host[k].body, num_states);
-    if (num_sources > 0) OCEAN_CUDA(gen->wake_sources.upload(gen, sources_host, (size_t)num_sources));
-    if (num_states > 0) OCEAN_CUDA(gen->wake_states.upload(gen, states_host, (size_t)num_states));
-    return ocean_wake_step_device(gen, dt, substeps, origin_x, origin_z, num_sources, gen->wake_sources.ptr, num_states, gen->wake_states.ptr);
+    Staging st;
+    const auto sources = st.in(sources_host, (size_t)num_sources);
+    const auto states = st.in(states_host, (size_t)num_states);
+    if ((rc = st.upload(gen, kStageWakeStep))) return rc;  // and no finish(): the call returns once the step is enqueued
+    return ocean_wake_step_device(gen, dt, substeps, origin_x, origin_z, num_sources, st[sources], num_states, st[states]);
 }
 
 int ocean_wake_render_map(ocean_generator* gen, void* map_dev, float* world_rect) {
@@ -2252,12 +2234,11 @@ int ocean_sample_wake(ocean_generator* gen, int num_points, const float* points_
     if ((rc = check_wake_layer(gen))) return rc;
     if ((rc = check_wake_points(num_points, points_xz_host, out_host))) return rc;
     if (num_points == 0) return OCEAN_OK;
-    OCEAN_CUDA(gen->q_points.upload(gen, points_xz_host, (size_t)num_points));
-    OCEAN_CUDA(gen->wake_samples.grow(gen, 3 * (size_t)num_points));
-    if ((rc = ocean_sample_wake_device(gen, num_points, reinterpret_cast<const float*>(gen->q_points.ptr), gen->wake_samples.ptr))) return rc;
-    OCEAN_CUDA(cudaMemcpyAsync(out_host, gen->wake_samples.ptr, sizeof(float) * 3 * (size_t)num_points, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    return OCEAN_OK;
+    Staging st;
+    const auto points = st.in(points_xz_host, 2 * (size_t)num_points);
+    const auto out = st.out(out_host, 3 * (size_t)num_points);
+    if ((rc = st.upload(gen, kStageSampleWake))) return rc;
+    return st.finish(gen, ocean_sample_wake_device(gen, num_points, st[points], st[out]));
 }
 
 int ocean_wake_get_state(ocean_generator* gen, float* h_host, float* h_prev_host, int64_t* origin_xz) {

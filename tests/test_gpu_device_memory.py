@@ -14,6 +14,8 @@ pytestmark = pytest.mark.gpu
 N, C = 128, 2
 SMALL, LARGE = 64, 5000
 POINTS_PER_BODY = 4
+WAKE = 128                                                      # cells per side of the wake layer the wake ops run on
+INVALID = 1                                                     # OCEAN_ERR_INVALID_ARGUMENT
 
 
 def _gen():
@@ -92,8 +94,8 @@ def _body_forces(g, scales, n):
     g.body_forces(_poses(g, n), np.zeros(n, g.BODY_VELOCITY), pts, cda, scales, return_samples=True)
 
 
-def _simulate_bodies(g, scales, n):
-    pts, cda = _hull(g, n)
+def _floating(g, n):
+    """n floating bodies over _hull(g, n), and their states."""
     b = np.zeros(n, g.FLOATING_BODY)
     b["mass"] = 200.0
     b["inertia"] = 50.0
@@ -102,6 +104,12 @@ def _simulate_bodies(g, scales, n):
     s = np.zeros(n, g.BODY_STATE)
     s["position"][:, [0, 2]] = _points(n)
     s["orientation"][:, 3] = 1.0
+    return b, s
+
+
+def _simulate_bodies(g, scales, n):
+    pts, cda = _hull(g, n)
+    b, s = _floating(g, n)
     g.simulate_bodies(b, s, pts, cda, scales, 1.0 / 60.0, 2, return_records=True, return_transforms=True)
 
 
@@ -112,8 +120,29 @@ def _debug_device_math(g, scales, n):
     check(load_library().ocean_debug_device_math(g.context, 0, n, a.ctypes.data, a.ctypes.data, out.ctypes.data))   # OCEAN_MATH_SINCOS
 
 
+def _wake_layer(g):
+    g.wake_init(WAKE, 0.5)                                      # the same size again keeps the fields and the staging
+
+
+def _wake_step(g, scales, n):
+    """n sources, every other one attached to one of n body states, so that both arrays are staged."""
+    _wake_layer(g)
+    src = np.zeros(n, g.WAKE_SOURCE)
+    src["x"], src["z"] = np.random.default_rng(n).uniform(0, 0.5 * WAKE, (2, n))
+    src["vx"], src["radius"], src["head"] = 2.0, 1.5, 0.2
+    src["body"] = np.where(np.arange(n) % 2 == 0, np.arange(n), -1)
+    states = np.zeros(n, g.BODY_STATE)
+    states["orientation"][:, 3] = 1.0
+    g.wake_step(0.05, 1, (0, 0), src, states)
+
+
+def _sample_wake(g, scales, n):
+    _wake_layer(g)
+    g.sample_wake(_points(n))
+
+
 OPS = [_sample_maps, _sample_velocity, _query_surface, _raycast, _extract_spray, _buoyancy, _body_forces, _simulate_bodies,
-       _debug_device_math]
+       _debug_device_math, _wake_step, _sample_wake]
 
 
 @pytest.mark.parametrize("op", OPS, ids=[op.__name__[1:] for op in OPS])
@@ -132,6 +161,52 @@ def test_growth_counts_only_the_live_block(op):
     assert _bytes(a) == _bytes(b)
     a.free()
     b.free()
+
+
+def _invalid_call(op, g, scales):
+    """One call of host entry point `op` with a NULL host buffer where a positive count needs one; returns its status."""
+    from godotoceanwaves_b200.native import load_library
+    lib, h, n = load_library(), g.context, 8
+    pts, out = _points(n), np.zeros(16 * n, np.float32)        # inputs, and room for any output
+    P, O, S = pts.ctypes.data, out.ctypes.data, scales.ctypes.data
+    rays, ps, emitter = _rays(g, n), np.ones(3, np.float32), g.default_spray_emitter()
+    poses, velocities, (hull, cda) = _poses(g, 2), np.zeros(2, g.BODY_VELOCITY), _hull(g, 2)
+    bodies, states = _floating(g, 2)
+    count = ctypes.c_int()
+    calls = {
+        "sample_maps": lambda: lib.ocean_sample_maps(h, n, P, C, S, None, O),
+        "sample_velocity": lambda: lib.ocean_sample_velocity(h, n, P, C, S, None),
+        "query_surface": lambda: lib.ocean_query_surface(h, n, P, C, S, 1e-3, 8, None),
+        "raycast": lambda: lib.ocean_raycast(h, n, rays.ctypes.data, C, S, 0.5, 64, 1e-3, 8, None),
+        "extract_spray": lambda: lib.ocean_extract_spray(h, n, P, C, S, ps.ctypes.data, n, None, ctypes.byref(count)),
+        "spray_particles": lambda: lib.ocean_spray_particles(h, emitter.ctypes.data, 0.0, 0.02, C, S, None, n, O, ctypes.byref(count)),
+        "buoyancy": lambda: lib.ocean_buoyancy(h, 2, poses.ctypes.data, len(hull), hull.ctypes.data, C, S, 1025.0, 1e-3, 8, None, None),
+        "body_forces": lambda: lib.ocean_body_forces(h, 2, poses.ctypes.data, velocities.ctypes.data, len(hull), hull.ctypes.data,
+                                                     cda.ctypes.data, C, S, 1025.0, 1e-3, 8, None, O, None),
+        "simulate_bodies": lambda: lib.ocean_simulate_bodies(h, 2, bodies.ctypes.data, states.ctypes.data, len(hull), None, cda.ctypes.data,
+                                                             C, S, 1025.0, 1.0 / 60.0, 1, 1e-3, 8, None, None, None),
+        "debug_device_math": lambda: lib.ocean_debug_device_math(h, 0, n, P, P, None),
+        "wake_step": lambda: lib.ocean_wake_step(h, 0.05, 1, 0, 0, n, None, 0, None),
+        "sample_wake": lambda: lib.ocean_sample_wake(h, n, P, None),
+    }
+    return calls[op]()
+
+
+HOST_OPS = ["sample_maps", "sample_velocity", "query_surface", "raycast", "extract_spray", "spray_particles", "buoyancy", "body_forces",
+            "simulate_bodies", "debug_device_math", "wake_step", "sample_wake"]
+
+
+@pytest.mark.parametrize("op", HOST_OPS)
+def test_invalid_host_call_stages_nothing(op):
+    """A host entry point validates its arguments before it stages anything: an invalid call on a generator whose staging is
+    still empty allocates nothing and launches nothing."""
+    g, _, scales = _gen()
+    if op in ("wake_step", "sample_wake"):
+        _wake_layer(g)
+    before = _bytes(g), g.info().kernel_launches
+    assert _invalid_call(op, g, scales) == INVALID
+    assert (_bytes(g), g.info().kernel_launches) == before
+    g.free()
 
 
 def test_taps_return_their_bytes():

@@ -298,6 +298,7 @@ def test_device_memory_is_exact():
     staged = g.info().device_bytes
     _init(g, _params(1024, 0.5))
     assert g.info().device_bytes == staged + 4 * 4 * (1024 * 1024 - 256 * 256)
+    g.sample_wake(np.random.default_rng(2).uniform(0, 512, (100, 2)))    # its staging goes with the layer too
     _init(g, _params(0, 0.5))
     assert g.info().device_bytes == base
     g.free()
