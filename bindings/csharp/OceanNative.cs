@@ -297,6 +297,9 @@ namespace OceanB200
         // wake obstacles: a world-fixed mask [depth][width] of blocked cells (nonzero) at world cell origin (x, z); null, 0, 0: none
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_wake_set_obstacles(IntPtr handle, byte* mask, int width, int depth, long origin_x, long origin_z);
+        // wake readers: OCEAN_WAKE_READ_RAYCAST (1) makes the ray cast hit the coupled surface, OCEAN_WAKE_READ_SPRAY (2) lets spray read h and F
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_wake_set_readers(IntPtr handle, uint readers);
         // surface query: the surface at world positions points [n][2] (P + D_xz(P) = Q solved for P, then the map query at P)
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,

@@ -10,7 +10,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libocean.so")
 SOURCES = ["ocean_kernels.cu", "ocean_sample.cu", "ocean_spray.cu", "ocean_buoyancy.cu", "ocean_bodies.cu", "ocean_velocity.cu",
            "ocean_wake.cu", "ocean_api.cu"]
-HEADERS = ["ocean_kernels.cuh", "ocean_texture.cuh", "detmath.cuh", "fft_core.cuh", os.path.join("..", "..", "include", "ocean.h")]
+HEADERS = ["ocean_kernels.cuh", "ocean_texture.cuh", "detmath.cuh", "fft_core.cuh", "wake_sample.cuh", os.path.join("..", "..", "include", "ocean.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -167,6 +167,8 @@ struct ocean_generator {
     DeviceArray<uint8_t> wake_mask;
     int32_t wake_mask_size[2] = {0, 0};                 // width, depth; 0: no mask
     int64_t wake_mask_origin[2] = {0, 0};
+    // wake readers (ocean_wake_set_readers): OCEAN_WAKE_READ_* bits of the ops that read the layer besides the coupling's
+    uint32_t wake_readers = 0;
 };
 
 namespace {
@@ -1146,6 +1148,11 @@ int ocean_spray_grid(int num_particles, const float* emission_transform, float* 
     return OCEAN_OK;
 }
 
+namespace {
+// The layer's h and F in its current window, when the spray reader is set (ocean_wake_set_readers); false otherwise.
+bool wake_spray_read(ocean_generator* g, ocean::WakeRead* out);
+}  // namespace
+
 int ocean_extract_spray_device(ocean_generator* gen, int num_candidates, const float* points_xz_dev, int num_cascades,
                                const float* map_scales_host, const float* particle_scale, int max_records,
                                ocean_spray_record* records_dev, int* num_active_dev) {
@@ -1161,9 +1168,11 @@ int ocean_extract_spray_device(ocean_generator* gen, int num_candidates, const f
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
     const int blocks = ocean::spray_blocks(num_candidates);
     OCEAN_CUDA(gen->spray_counts.grow(gen, (size_t)blocks + 1));
+    ocean::WakeRead wake;
+    const bool wk = wake_spray_read(gen, &wake);
     OCEAN_CUDA(ocean::launch_extract_spray(gen->buf, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_candidates,
                                            gen->q_scales.ptr, make_float3(particle_scale[0], particle_scale[1], particle_scale[2]),
-                                           gen->spray_counts.ptr, records_dev, max_records, gen->stream));
+                                           gen->spray_counts.ptr, records_dev, max_records, wk ? &wake : nullptr, gen->stream));
     gen->kernel_launches += 3;
     OCEAN_CUDA(cudaMemcpyAsync(num_active_dev, gen->spray_counts.ptr + blocks, sizeof(int), cudaMemcpyDeviceToDevice, gen->stream));
     return OCEAN_OK;
@@ -1256,8 +1265,10 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
     const int blocks = ocean::spray_blocks(emitter->amount);
     OCEAN_CUDA(gen->spray_counts.grow(gen, (size_t)blocks + 1));
+    ocean::WakeRead wake;
+    const bool wk = wake_spray_read(gen, &wake);
     OCEAN_CUDA(ocean::launch_spray_particles(gen->buf, num_cascades, gen->q_scales.ptr, *emitter, t0, t1, states_dev, gen->spray_counts.ptr,
-                                             instances_dev, max_instances, gen->stream));
+                                             instances_dev, max_instances, wk ? &wake : nullptr, gen->stream));
     gen->kernel_launches += 3;
     OCEAN_CUDA(cudaMemcpyAsync(num_live_dev, gen->spray_counts.ptr + blocks, sizeof(int), cudaMemcpyDeviceToDevice, gen->stream));
     return OCEAN_OK;
@@ -1382,10 +1393,21 @@ int ocean_raycast_device(ocean_generator* gen, int num_rays, const ocean_ray* ra
     if (num_rays == 0) return OCEAN_OK;
     if (!rays_dev || !out_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
-    OCEAN_CUDA(gen->ray_bounds.grow(gen, 3 * (size_t)gen->num_cascades));
+    // with the ray cast reader set and the coupling live, the coupled surface: e in its own window, and one more kernel (its bounds)
+    const bool wk = (gen->wake_readers & OCEAN_WAKE_READ_RAYCAST) && wake_coupling_live(gen);
+    ocean::WakeRead wake{};
+    if (wk) {
+        const int e = gen->wake_e;
+        wake.field = gen->wake_snapshots.ptr + e * (size_t)gen->wake.size * gen->wake.size;
+        wake.n = gen->wake.size;
+        wake.cell = gen->wake.cell_size;
+        wake.x0 = wake_corner(gen->wake_snapshot_origin[e][0], wake.cell);
+        wake.z0 = wake_corner(gen->wake_snapshot_origin[e][1], wake.cell);
+    }
+    OCEAN_CUDA(gen->ray_bounds.grow(gen, 3 * (size_t)gen->num_cascades + (wk ? 2 : 0)));
     OCEAN_CUDA(ocean::launch_raycast(gen->buf, num_cascades, rays_dev, num_rays, gen->q_scales.ptr, step, max_samples, tolerance, max_iterations,
-                                     gen->ray_bounds.ptr, out_dev, gen->stream));
-    gen->kernel_launches += 2;
+                                     gen->ray_bounds.ptr, out_dev, wk ? &wake : nullptr, gen->stream));
+    gen->kernel_launches += wk ? 3 : 2;
     return OCEAN_OK;
 }
 
@@ -2009,6 +2031,17 @@ int wake_foam_off(ocean_generator* g) {
 
 float* wake_foam_field(ocean_generator* g, int k) { return g->wake_foam.ptr + (size_t)k * g->wake.size * g->wake.size; }
 
+bool wake_spray_read(ocean_generator* g, ocean::WakeRead* out) {
+    if (!(g->wake_readers & OCEAN_WAKE_READ_SPRAY) || g->wake.size == 0) return false;
+    out->field = wake_field(g, g->wake_h);
+    out->foam = g->wake_foam_on ? wake_foam_field(g, g->wake_f) : nullptr;
+    out->n = g->wake.size;
+    out->cell = g->wake.cell_size;
+    out->x0 = wake_corner(g->wake_origin[0], out->cell);
+    out->z0 = wake_corner(g->wake_origin[1], out->cell);
+    return true;
+}
+
 // Removes the obstacle mask and releases it (the caller has entered the generator).
 int wake_obstacles_off(ocean_generator* g) {
     if (g->wake_mask.ptr) OCEAN_CUDA(cudaStreamSynchronize(g->stream));     // kernels may still read it
@@ -2052,6 +2085,7 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
         if ((rc = wake_uncouple(gen))) return rc;
         if ((rc = wake_foam_off(gen))) return rc;
         if ((rc = wake_obstacles_off(gen))) return rc;
+        gen->wake_readers = 0;
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
         gen->wake_fields.release();
         gen->staging[kStageWakeStep].release();
@@ -2070,6 +2104,7 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
     if ((rc = wake_uncouple(gen))) return rc;
     if ((rc = wake_foam_off(gen))) return rc;
     if ((rc = wake_obstacles_off(gen))) return rc;      // the mask's cells are cells of the old cell size
+    gen->wake_readers = 0;
     gen->wake = ocean_wake_params{};                    // no layer until the fields below are allocated and cleared
     if (gen->wake_fields.capacity != cells) {
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
@@ -2355,6 +2390,15 @@ int ocean_wake_set_obstacles(ocean_generator* gen, const uint8_t* mask_host, int
     gen->wake_mask_size[1] = depth;
     gen->wake_mask_origin[0] = origin_x;
     gen->wake_mask_origin[1] = origin_z;
+    return OCEAN_OK;
+}
+
+int ocean_wake_set_readers(ocean_generator* gen, uint32_t readers) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_wake_layer(gen))) return rc;
+    if (readers & ~(OCEAN_WAKE_READ_RAYCAST | OCEAN_WAKE_READ_SPRAY)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "readers 0x%x: unknown bits", readers);
+    gen->wake_readers = readers;
     return OCEAN_OK;
 }
 

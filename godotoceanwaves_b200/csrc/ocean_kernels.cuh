@@ -128,11 +128,21 @@ cudaError_t launch_sample_maps(const DeviceBuffers& b, int num_cascades, const f
 size_t surface_scratch_ints(int num_cascades, int n);
 cudaError_t launch_query_surface(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
                                  float tolerance, int max_iterations, ocean_surface_sample* out_dev, int* scratch_dev, cudaStream_t stream);
+// A wake field the ray cast or spray reads (ocean_wake_set_readers; oracle/wake_readers.py): field and foam are [n][n]
+// binary32 in the window at world corner (x0, z0), sampled as ocean_sample_wake (0 outside).  The ray cast reads the
+// coupling's free surface e in `field`; spray reads h in `field` and F in `foam` (null while wake foam is off: F reads +0).
+struct WakeRead {
+    const float* field;
+    const float* foam;
+    int n;
+    float cell, x0, z0;
+};
 // ocean_sample.cu: ray cast against the displaced surface (oracle/raycast.py); rays_dev / out_dev = [n] rays / hits,
-// bounds_dev = [3 * num_cascades] unsigned of scratch (the per-layer height and displacement bounds)
+// bounds_dev = [3 * num_cascades] unsigned of scratch (the per-layer height and displacement bounds), [3 * num_cascades + 2]
+// with a wake (wake not null: the coupled surface, its e bounds after the layers')
 cudaError_t launch_raycast(const DeviceBuffers& b, int num_cascades, const ocean_ray* rays_dev, int n, const float4* scales_dev, float step,
                            int max_samples, float tolerance, int max_iterations, unsigned* bounds_dev, ocean_ray_hit* out_dev,
-                           cudaStream_t stream);
+                           const WakeRead* wake, cudaStream_t stream);
 
 // ocean_buoyancy.cu: buoyancy (oracle/buoyancy.py).  bodies_dev = [num_bodies], offsets_dev = the exclusive prefix of their
 // num_points (body-major world points), q_dev / samples_dev = [n] world points' (x, z) / surface records, results_dev = [num_bodies]
@@ -184,14 +194,16 @@ cudaError_t launch_sample_velocity(const uint2* velocity_dev, int map_size, int 
 // ocean_spray.cu: spray candidates (sea_spray_particle.gdshader:80-94) as a stable stream compaction; counts_dev is
 // [spray_blocks(n) + 1] ints of scratch whose last element receives the number of active candidates
 int spray_blocks(int n);
+// wake (may be null): the wake forms of the kernels, which add the layer's h and F to the spawn test (and h to the particle height)
 cudaError_t launch_extract_spray(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
-                                 float3 particle_scale, int* counts_dev, ocean_spray_record* records_dev, int max_records, cudaStream_t stream);
+                                 float3 particle_scale, int* counts_dev, ocean_spray_record* records_dev, int max_records,
+                                 const WakeRead* wake, cudaStream_t stream);
 // ocean_spray.cu: one particle-process frame [t0, t1) of a spray emitter (oracle/spray_particles.py), three launches when
 // amount > 0.  states_dev = [amount] (updated in place), counts_dev = [spray_blocks(amount) + 1] ints of scratch whose last
 // element receives the number of live particles, instances_dev = [max_instances][16] floats
 cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const ocean_spray_emitter& emitter,
                                    double t0, double t1, ocean_spray_particle* states_dev, int* counts_dev, float* instances_dev,
-                                   int max_instances, cudaStream_t stream);
+                                   int max_instances, const WakeRead* wake, cudaStream_t stream);
 
 // ocean_wake.cu: the wake layer (oracle/wake.py).  One sub-step of the layer: h / h_prev ([n][n], read at (i + di, j + dj),
 // 0 outside: the scroll folded into the reads) to out_h, and, when out_h_prev is not null, the scrolled h to out_h_prev.

@@ -17,10 +17,13 @@
 // first: for a world position Q it solves P + D_xz(P) = Q by damped Newton steps (four displacement texels per cascade and
 // trial give D and its exact bilinear Jacobian), then samples the maps at P with the same per-point body as k_sample_maps.
 // The ray cast (ocean_raycast; oracle/raycast.py is the specification) marches each ray through the height slab of the maps
-// with the same inversion, warm-started from sample to sample, and refines the first crossing.
+// with the same inversion, warm-started from sample to sample, and refines the first crossing.  Its wake form
+// (ocean_wake_set_readers; oracle/wake_readers.py) adds the wake free surface e to the height of every evaluation, widens
+// the slab by e's bounds (k_raycast_wake_bound) and adds e's sample and slopes to the record.
 #include "../../include/ocean.h"
 #include "ocean_kernels.cuh"
 #include "ocean_texture.cuh"
+#include "wake_sample.cuh"
 
 namespace ocean {
 
@@ -290,16 +293,39 @@ __global__ void __launch_bounds__(256) k_raycast_bound(const uint2* __restrict__
     }
 }
 
+// The NaN-dropping extrema of the wake free surface e ([n][n]) as k_raycast_bound's: bounds[0] = max e, bounds[1] = max -e
+// (as order_key).  bounds must be zero on entry.
+__global__ void __launch_bounds__(256) k_raycast_wake_bound(const float* __restrict__ e, int n, unsigned* __restrict__ bounds) {
+    const size_t cells = (size_t)n * n;
+    float hi = -INFINITY, nlo = -INFINITY;
+    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < cells; t += (size_t)gridDim.x * blockDim.x) {
+        const float v = e[t];
+        hi = fmaxf(hi, v);
+        nlo = fmaxf(nlo, -v);
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+        nlo = fmaxf(nlo, __shfl_xor_sync(0xffffffffu, nlo, o));
+    }
+    if ((threadIdx.x & 31) == 0) {
+        atomicMax(&bounds[0], order_key(hi));
+        atomicMax(&bounds[1], order_key(nlo));
+    }
+}
+
 // An evaluated point of a ray: parameter, position, source point P, inversion residual, gap.
 struct RayPoint {
     float t, x, y, z, px, pz, r, g;
 };
 
 // One gap evaluation at parameter t, started at Q or (warm) from the evaluated point `base` shifted by the ray's horizontal
-// advance since it, with the surface query's restarts when that start does not converge.
+// advance since it, with the surface query's restarts when that start does not converge.  With Wake the gap is taken to
+// eta + we, we = the sample of the wake free surface w.field at (x, z).
+template <bool Wake>
 __device__ __forceinline__ RayPoint ray_gap(const uint2* __restrict__ displacement, int N, int C, const float4* __restrict__ scales,
                                             const ocean_ray& ray, float t, bool warm, float base_x, float base_z, float base_px, float base_pz,
-                                            float tol, int max_iterations, float rho, uint32_t& iterations, uint32_t& unconverged) {
+                                            float tol, int max_iterations, float rho, uint32_t& iterations, uint32_t& unconverged,
+                                            const WakeRead& w) {
     RayPoint e;
     e.t = t;
     e.x = ray.origin[0] + t * ray.direction[0];
@@ -349,18 +375,27 @@ __device__ __forceinline__ RayPoint ray_gap(const uint2* __restrict__ displaceme
     e.px = px;
     e.pz = pz;
     e.r = r;
-    e.g = e.y - eta;
+    if constexpr (Wake) {
+        float we = 0.0f;
+        sample_field<false>(w.field, w.n, w.cell, w.x0, w.z0, q, &we);
+        e.g = e.y - (eta + we);
+    } else {
+        e.g = e.y - eta;
+    }
     iterations += (uint32_t)total;
     unconverged += (r <= tol) ? 0u : 1u;
     return e;
 }
 
 // One thread per ray: slab clip, march, Illinois refinement, and the map sample at the reported point.  bounds = the
-// per-layer maxima of k_raycast_bound.  (128, 4) lets ptxas keep the ray's state in registers (no spill).
+// per-layer maxima of k_raycast_bound.  (128, 4) lets ptxas keep the ray's state in registers (no spill).  With Wake (the
+// coupled surface) bounds[3C], bounds[3C + 1] are k_raycast_wake_bound's extrema of w.field = e, and the reported point's
+// record carries e's sample and slopes as ocean_query_surface's coupled record.
+template <bool Wake>
 __global__ void __launch_bounds__(128, 4) k_raycast(const uint2* __restrict__ displacement, const uint2* __restrict__ normal, int N, int C,
                                                  const ocean_ray* __restrict__ rays, int n, const float4* __restrict__ scales, float step,
                                                  int max_samples, float tol, int max_iterations, const unsigned* __restrict__ bounds,
-                                                 ocean_ray_hit* __restrict__ out) {
+                                                 ocean_ray_hit* __restrict__ out, const WakeRead w) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const ocean_ray ray = rays[i];
@@ -382,6 +417,13 @@ __global__ void __launch_bounds__(128, 4) k_raycast(const uint2* __restrict__ di
         y_hi = y_hi + fmaxf(a, b);
         acc = acc + fabsf(s) * fmaxf(fabsf(ymin), fabsf(ymax));
         rho = rho + fabsf(s) * __uint_as_float(bounds[3 * c + 2]);
+    }
+    if constexpr (Wake) {
+        // the sample of e is 0 outside its window, and its bilinear interpolant lies between its extrema
+        const float emax = order_value(bounds[3 * C + 0]), emin = -order_value(bounds[3 * C + 1]);
+        y_lo = y_lo + fminf(emin, 0.0f);
+        y_hi = y_hi + fmaxf(emax, 0.0f);
+        acc = acc + fmaxf(fabsf(emin), fabsf(emax));
     }
     rho = rho * 0.5f;
     const float pad = tol + acc * 0x1p-13f;
@@ -414,8 +456,8 @@ __global__ void __launch_bounds__(128, 4) k_raycast(const uint2* __restrict__ di
     float t = t_in, base_x = 0.0f, base_z = 0.0f, base_px = 0.0f, base_pz = 0.0f, wa = 0.0f, wb = 0.0f;
     int k = 0, steps = 0, last = 0;
     for (;;) {
-        const RayPoint e = ray_gap(displacement, N, C, scales, ray, t, evaluations > 0, base_x, base_z, base_px, base_pz, tol, max_iterations,
-                                   rho, iterations, unconverged);
+        const RayPoint e = ray_gap<Wake>(displacement, N, C, scales, ray, t, evaluations > 0, base_x, base_z, base_px, base_pz, tol,
+                                         max_iterations, rho, iterations, unconverged, w);
         ++evaluations;
         if (isnan(e.g)) { status = OCEAN_RAY_INVALID; rep = e; break; }
         if (!refining) {
@@ -460,6 +502,13 @@ __global__ void __launch_bounds__(128, 4) k_raycast(const uint2* __restrict__ di
     }
     float3 d, g;
     sample_point(displacement, normal, N, C, make_float2(rep.px, rep.pz), scales, d, g);
+    if constexpr (Wake) {
+        float r[3] = {0.0f, 0.0f, 0.0f};
+        sample_field<true>(w.field, w.n, w.cell, w.x0, w.z0, make_float2(rep.x, rep.z), r);
+        d.y = __fadd_rn(d.y, r[0]);
+        g.x = __fadd_rn(g.x, r[1]);
+        g.y = __fadd_rn(g.y, r[2]);
+    }
     hit.t = rep.t;
     hit.position[0] = rep.x; hit.position[1] = rep.y; hit.position[2] = rep.z;
     hit.source_x = rep.px;
@@ -518,19 +567,29 @@ cudaError_t launch_query_surface(const DeviceBuffers& b, int num_cascades, const
     return cudaGetLastError();
 }
 
-// bounds_dev: [3 * num_cascades] unsigned, cleared here, then filled by k_raycast_bound; k_raycast reads them.
+// bounds_dev: [3 * num_cascades] unsigned (+ 2 with a wake), cleared here, then filled by k_raycast_bound (and
+// k_raycast_wake_bound, e is taken per call: it changes with every step call); k_raycast reads them.
 cudaError_t launch_raycast(const DeviceBuffers& b, int num_cascades, const ocean_ray* rays_dev, int n, const float4* scales_dev, float step,
                            int max_samples, float tolerance, int max_iterations, unsigned* bounds_dev, ocean_ray_hit* out_dev,
-                           cudaStream_t stream) {
+                           const WakeRead* wake, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     const int N = b.map_size;
-    cudaError_t e = cudaMemsetAsync(bounds_dev, 0, sizeof(unsigned) * 3 * (size_t)num_cascades, stream);
+    cudaError_t e = cudaMemsetAsync(bounds_dev, 0, sizeof(unsigned) * (3 * (size_t)num_cascades + (wake ? 2 : 0)), stream);
     if (e != cudaSuccess) return e;
     const unsigned bound_blocks = (unsigned)(((size_t)N * N + 4095) / 4096);     // 16 texels per thread
     k_raycast_bound<<<dim3(bound_blocks, (unsigned)num_cascades), 256, 0, stream>>>(b.displacement, N, bounds_dev);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    k_raycast<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(b.displacement, b.normal, N, num_cascades, rays_dev, n, scales_dev, step,
-                                                              max_samples, tolerance, max_iterations, bounds_dev, out_dev);
+    const unsigned ray_blocks = (unsigned)((n + 127) / 128);
+    if (!wake) {
+        k_raycast<false><<<ray_blocks, 128, 0, stream>>>(b.displacement, b.normal, N, num_cascades, rays_dev, n, scales_dev, step, max_samples,
+                                                         tolerance, max_iterations, bounds_dev, out_dev, WakeRead{});
+        return cudaGetLastError();
+    }
+    const unsigned wake_blocks = (unsigned)(((size_t)wake->n * wake->n + 4095) / 4096);    // 16 cells per thread
+    k_raycast_wake_bound<<<wake_blocks, 256, 0, stream>>>(wake->field, wake->n, bounds_dev + 3 * num_cascades);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    k_raycast<true><<<ray_blocks, 128, 0, stream>>>(b.displacement, b.normal, N, num_cascades, rays_dev, n, scales_dev, step, max_samples,
+                                                    tolerance, max_iterations, bounds_dev, out_dev, *wake);
     return cudaGetLastError();
 }
 

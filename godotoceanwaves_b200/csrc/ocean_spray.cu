@@ -19,10 +19,15 @@
 //           particles are counted per block of 256
 //   scan    k_spray_scan on the block counts
 //   write   the instances of the live particles at block offset + rank (warp ballots): a stable compaction in INDEX order
+//
+// The wake forms of k_spray_count, k_spray_write and k_spray_particles_update (ocean_wake_set_readers; oracle/wake_readers.py)
+// add the wake layer's slopes and foam F at START_POS.xz to the spawn test's gradient and foam, and its height h to the
+// particle's height: spray from the white water the render map shows on the wake.  Same launches.
 #include "../../include/ocean.h"
 #include "ocean_kernels.cuh"
 #include "ocean_texture.cuh"
 #include "detmath.cuh"
+#include "wake_sample.cuh"
 
 namespace ocean {
 
@@ -37,9 +42,10 @@ struct SprayFactors {
     float normal_factor, foam_factor, foam;
 };
 
-// :80-87: the gradient and foam at START_POS.xz, and the two factors
+// :80-87: the gradient and foam at START_POS.xz, and the two factors; with Wake plus the wake's (dh/dx, dh/dz) and F there
+template <bool Wake>
 __device__ __forceinline__ SprayFactors spray_factors(const uint2* __restrict__ normal, int N, int C, float2 p,
-                                                      const float4* __restrict__ scales) {
+                                                      const float4* __restrict__ scales, const WakeRead& w) {
     float gx = 0.0f, gy = 0.0f, gf = 0.0f;
     for (int c = 0; c < C; ++c) {
         const float4 s = __ldg(&scales[c]);
@@ -47,6 +53,14 @@ __device__ __forceinline__ SprayFactors spray_factors(const uint2* __restrict__ 
         gx = gx + t.x;
         gy = gy + t.y;
         gf = gf + t.w;
+    }
+    if constexpr (Wake) {
+        float r[3] = {0.0f, 0.0f, 0.0f}, fw = 0.0f;
+        sample_field<true>(w.field, w.n, w.cell, w.x0, w.z0, p, r);
+        if (w.foam) sample_field<false>(w.foam, w.n, w.cell, w.x0, w.z0, p, &fw);
+        gx = gx + r[1];
+        gy = gy + r[2];
+        gf = gf + fw;
     }
     const float nx = -gx, nz = -gy;
     const float ny = __fdiv_rn(1.0f, __fsqrt_rn((nx * nx + 1.0f * 1.0f) + nz * nz));               // normalize(...).y  :84
@@ -57,9 +71,10 @@ __device__ __forceinline__ SprayFactors spray_factors(const uint2* __restrict__ 
     return f;
 }
 
+template <bool Wake>
 __device__ __forceinline__ SprayEval spray_eval(const uint2* __restrict__ normal, int N, int C, float2 p, const float4* __restrict__ scales,
-                                                float3 particle_scale) {
-    const SprayFactors f = spray_factors(normal, N, C, p, scales);
+                                                float3 particle_scale, const WakeRead& w) {
+    const SprayFactors f = spray_factors<Wake>(normal, N, C, p, scales, w);
     const float nf = f.normal_factor, ff = f.foam_factor, gf = f.foam;
     SprayEval e;
     e.active = nf >= 0.0f && nf <= 1.0f && gf > 0.9f;                                               // :89
@@ -74,11 +89,13 @@ __device__ __forceinline__ SprayEval spray_eval(const uint2* __restrict__ normal
 
 constexpr int kSprayBlock = 256;
 
+template <bool Wake>
 __global__ void __launch_bounds__(kSprayBlock) k_spray_count(const uint2* __restrict__ normal, int N, int C, const float2* __restrict__ points, int n,
-                                                             const float4* __restrict__ scales, float3 particle_scale, int* __restrict__ block_counts) {
+                                                             const float4* __restrict__ scales, float3 particle_scale, int* __restrict__ block_counts,
+                                                             const WakeRead w) {
     const int i = blockIdx.x * kSprayBlock + threadIdx.x;
     bool active = false;
-    if (i < n) active = spray_eval(normal, N, C, points[i], scales, particle_scale).active;
+    if (i < n) active = spray_eval<Wake>(normal, N, C, points[i], scales, particle_scale, w).active;
     const int total = __syncthreads_count(active);
     if (threadIdx.x == 0) block_counts[blockIdx.x] = total;
 }
@@ -120,10 +137,11 @@ __global__ void __launch_bounds__(1024) k_spray_scan(int* __restrict__ counts, i
     if (threadIdx.x == 0) counts[blocks] = s_carry;
 }
 
+template <bool Wake>
 __global__ void __launch_bounds__(kSprayBlock) k_spray_write(const uint2* __restrict__ normal, int N, int C, const float2* __restrict__ points, int n,
                                                              const float4* __restrict__ scales, float3 particle_scale,
                                                              const int* __restrict__ block_offsets, ocean_spray_record* __restrict__ out,
-                                                             int max_records) {
+                                                             int max_records, const WakeRead w) {
     __shared__ int s_warp[kSprayBlock / 32];
     const int i = blockIdx.x * kSprayBlock + threadIdx.x;
     SprayEval e;
@@ -131,7 +149,7 @@ __global__ void __launch_bounds__(kSprayBlock) k_spray_write(const uint2* __rest
     float2 p = make_float2(0.f, 0.f);
     if (i < n) {
         p = points[i];
-        e = spray_eval(normal, N, C, p, scales, particle_scale);
+        e = spray_eval<Wake>(normal, N, C, p, scales, particle_scale, w);
     }
     const unsigned ballot = __ballot_sync(0xffffffffu, e.active);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -230,10 +248,11 @@ __device__ __forceinline__ void spray_start(ocean_spray_particle& p, const ocean
     spray_set_scale(p.transform, 1e-3f, 1e-3f, 1e-3f);
 }
 
-// process() :74-126 of an ACTIVE particle
+// process() :74-126 of an ACTIVE particle; with Wake the spawn test reads the wake and the height adds its h at START_POS.xz
+template <bool Wake>
 __device__ __forceinline__ void spray_process(ocean_spray_particle& p, const ocean_spray_emitter& e, float time,
                                               const uint2* __restrict__ disp, const uint2* __restrict__ normal, int N, int C,
-                                              const float4* __restrict__ scales) {
+                                              const float4* __restrict__ scales, const WakeRead& w) {
     const float st = p.userdata1[3], pl = p.userdata2[3];
     if (time > st + pl) {
         p.flags &= ~OCEAN_SPRAY_ACTIVE;
@@ -242,7 +261,7 @@ __device__ __forceinline__ void spray_process(ocean_spray_particle& p, const oce
     if (!(time >= st)) return;
     const float2 sp = make_float2(p.userdata1[0], p.userdata1[2]);
     if (p.userdata3[3] == 0.0f) {                                                                  // :78-96
-        const SprayFactors f = spray_factors(normal, N, C, sp, scales);
+        const SprayFactors f = spray_factors<Wake>(normal, N, C, sp, scales, w);
         const float nf = f.normal_factor, ff = f.foam_factor;
         const bool active = nf >= 0.0f && nf <= 1.0f && f.foam > 0.9f;
         p.flags = active ? (p.flags | OCEAN_SPRAY_ACTIVE) : (p.flags & ~OCEAN_SPRAY_ACTIVE);
@@ -260,6 +279,11 @@ __device__ __forceinline__ void spray_process(ocean_spray_particle& p, const oce
     for (int c = 0; c < C; ++c) {                                                                  // :105-108
         const float4 s = __ldg(&scales[c]);
         add_displacement(disp + (size_t)c * N * N, N, sp.x * s.x, sp.y * s.y, s.z, dx, dy, dz);
+    }
+    if constexpr (Wake) {
+        float hw = 0.0f;
+        sample_field<false>(w.field, w.n, w.cell, w.x0, w.z0, sp, &hw);
+        dy = dy + hw;
     }
     dx = dx * 0.75f;                                                                               // :111
     dy = dy * 1.0f;
@@ -283,11 +307,12 @@ __device__ __forceinline__ bool spray_live(const ocean_spray_particle& p) {
     return (p.flags & OCEAN_SPRAY_ACTIVE) && p.userdata3[3] != 0.0f;
 }
 
+template <bool Wake>
 __global__ void __launch_bounds__(kSprayBlock) k_spray_particles_update(const ocean_spray_emitter e, double t0, double t1, float time,
                                                                         const uint2* __restrict__ disp, const uint2* __restrict__ normal,
                                                                         int N, int C, const float4* __restrict__ scales,
                                                                         ocean_spray_particle* __restrict__ states,
-                                                                        int* __restrict__ block_counts) {
+                                                                        int* __restrict__ block_counts, const WakeRead w) {
     const int i = blockIdx.x * kSprayBlock + threadIdx.x;
     bool live = false;
     if (i < e.amount) {
@@ -303,7 +328,7 @@ __global__ void __launch_bounds__(kSprayBlock) k_spray_particles_update(const oc
             p.flags |= OCEAN_SPRAY_ACTIVE | OCEAN_SPRAY_EMITTED;
             spray_start(p, e, (uint32_t)i, time);
         }
-        if (p.flags & OCEAN_SPRAY_ACTIVE) spray_process(p, e, time, disp, normal, N, C, scales);
+        if (p.flags & OCEAN_SPRAY_ACTIVE) spray_process<Wake>(p, e, time, disp, normal, N, C, scales, w);
         states[i] = p;
         live = spray_live(p);
     }
@@ -341,17 +366,28 @@ int spray_blocks(int n) { return (n + kSprayBlock - 1) / kSprayBlock; }
 // counts_dev: [spray_blocks(n) + 1] ints of scratch; on completion counts_dev[spray_blocks(n)] = number of active
 // candidates (which may exceed max_records: the records beyond it are dropped, the count is not clamped).
 cudaError_t launch_extract_spray(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
-                                 float3 particle_scale, int* counts_dev, ocean_spray_record* records_dev, int max_records, cudaStream_t stream) {
+                                 float3 particle_scale, int* counts_dev, ocean_spray_record* records_dev, int max_records,
+                                 const WakeRead* wake, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     const int blocks = spray_blocks(n);
-    k_spray_count<<<blocks, kSprayBlock, 0, stream>>>(b.normal, b.map_size, num_cascades, points_dev, n, scales_dev, particle_scale, counts_dev);
+    const WakeRead w = wake ? *wake : WakeRead{};
+    if (wake)
+        k_spray_count<true><<<blocks, kSprayBlock, 0, stream>>>(b.normal, b.map_size, num_cascades, points_dev, n, scales_dev, particle_scale,
+                                                                counts_dev, w);
+    else
+        k_spray_count<false><<<blocks, kSprayBlock, 0, stream>>>(b.normal, b.map_size, num_cascades, points_dev, n, scales_dev, particle_scale,
+                                                                 counts_dev, w);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     k_spray_scan<<<1, 1024, 0, stream>>>(counts_dev, blocks);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    k_spray_write<<<blocks, kSprayBlock, 0, stream>>>(b.normal, b.map_size, num_cascades, points_dev, n, scales_dev, particle_scale, counts_dev,
-                                                      records_dev, max_records);
+    if (wake)
+        k_spray_write<true><<<blocks, kSprayBlock, 0, stream>>>(b.normal, b.map_size, num_cascades, points_dev, n, scales_dev, particle_scale,
+                                                                counts_dev, records_dev, max_records, w);
+    else
+        k_spray_write<false><<<blocks, kSprayBlock, 0, stream>>>(b.normal, b.map_size, num_cascades, points_dev, n, scales_dev, particle_scale,
+                                                                 counts_dev, records_dev, max_records, w);
     return cudaGetLastError();
 }
 
@@ -359,11 +395,16 @@ cudaError_t launch_extract_spray(const DeviceBuffers& b, int num_cascades, const
 // particles (which may exceed max_instances: the instances beyond it are dropped, the count is not clamped).
 cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const ocean_spray_emitter& emitter,
                                    double t0, double t1, ocean_spray_particle* states_dev, int* counts_dev, float* instances_dev,
-                                   int max_instances, cudaStream_t stream) {
+                                   int max_instances, const WakeRead* wake, cudaStream_t stream) {
     if (emitter.amount <= 0) return cudaSuccess;
     const int blocks = spray_blocks(emitter.amount);
-    k_spray_particles_update<<<blocks, kSprayBlock, 0, stream>>>(emitter, t0, t1, (float)t1, b.displacement, b.normal, b.map_size, num_cascades,
-                                                                 scales_dev, states_dev, counts_dev);
+    const WakeRead w = wake ? *wake : WakeRead{};
+    if (wake)
+        k_spray_particles_update<true><<<blocks, kSprayBlock, 0, stream>>>(emitter, t0, t1, (float)t1, b.displacement, b.normal, b.map_size,
+                                                                           num_cascades, scales_dev, states_dev, counts_dev, w);
+    else
+        k_spray_particles_update<false><<<blocks, kSprayBlock, 0, stream>>>(emitter, t0, t1, (float)t1, b.displacement, b.normal, b.map_size,
+                                                                            num_cascades, scales_dev, states_dev, counts_dev, w);
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) return err;
     k_spray_scan<<<1, 1024, 0, stream>>>(counts_dev, blocks);

@@ -582,6 +582,14 @@ class WaveGenerator:
         check(load_library().ocean_wake_set_obstacles(self.context, m.ctypes.data, m.shape[1], m.shape[0], int(origin[0]),
                                                       int(origin[1])))
 
+    def wake_set_readers(self, raycast: bool = False, spray: bool = False) -> None:
+        """Let the ray cast and spray read the wake layer (include/ocean.h, ocean_wake_set_readers): raycast=True makes the
+        ray cast hit the coupled surface while the coupling is live; spray=True adds the layer's slopes and foam to the spawn
+        test and its height to the spray particles.  Both False (the default) reads nothing."""
+        self._require()
+        readers = (1 if raycast else 0) | (2 if spray else 0)
+        check(load_library().ocean_wake_set_readers(self.context, readers))
+
     def twiddles_to_host(self) -> np.ndarray:
         self._require()
         out = np.empty((self.map_size - 1, 2), np.float32)

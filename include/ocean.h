@@ -251,7 +251,10 @@ int ocean_query_surface_device(ocean_generator* gen, int num_points, const float
  * other field.  step must be finite and > 0, max_samples in [2, 2^20]; tolerance, max_iterations, num_cascades and
  * map_scales as for ocean_query_surface; an invalid call launches nothing.  map_scales is a host array in both entry points;
  * ocean_raycast takes host rays and records and is synchronous; ocean_raycast_device takes device pointers for them and is
- * asynchronous on the generator's stream.  A call with rays launches 2 kernels. */
+ * asynchronous on the generator's stream.  A call with rays launches 2 kernels, 3 while it reads the wake layer.
+ * With OCEAN_WAKE_READ_RAYCAST set (ocean_wake_set_readers) and the wake coupling live, the surface is the coupled one that
+ * ocean_query_surface describes: the wake free surface e is added to the height, the slab and the record ("Wake layer",
+ * Readers). */
 #define OCEAN_RAY_MISS 0
 #define OCEAN_RAY_HIT_FROM_ABOVE 1
 #define OCEAN_RAY_HIT_FROM_BELOW 2
@@ -484,7 +487,9 @@ int ocean_copy_f32_velocity_to_host(ocean_generator* gen, int cascade, float* ho
  * Only the ACTIVE candidates are returned, in candidate order (stable compaction, deterministic).  *num_active receives their
  * number even when it exceeds max_records (records beyond max_records are dropped).  oracle/spray.py is the specification.
  * ocean_spray_grid fills the start positions of the emitter's particle grid (sea_spray_particle.gdshader:47,52-54):
- * emission_transform = 3 x 4 row-major (basis columns, origin), NULL = identity; points_xz_host: [num_particles][2]. */
+ * emission_transform = 3 x 4 row-major (basis columns, origin), NULL = identity; points_xz_host: [num_particles][2].
+ * With OCEAN_WAKE_READ_SPRAY set (ocean_wake_set_readers) the gradient and foam also read the wake layer's slopes and foam
+ * ("Wake layer", Readers); the launches are the same. */
 typedef struct ocean_spray_record {
     uint32_t index;            /* candidate (particle INDEX) */
     float start_x, start_z;    /* START_POS.xz */
@@ -532,6 +537,8 @@ int ocean_extract_spray_device(ocean_generator* gen, int num_candidates, const f
  * t1 / emitter_lifetime < 2^32, num_cascades in [1, num_cascades of the generator], max_instances >= 0, and no NULL except
  * states when amount = 0 and instances when max_instances = 0.  An invalid call returns OCEAN_ERR_INVALID_ARGUMENT, launches
  * nothing and leaves the states untouched.  A valid call with amount > 0 launches three kernels (update, scan, write).
+ * With OCEAN_WAKE_READ_SPRAY set (ocean_wake_set_readers) the spawn test reads the wake layer as ocean_extract_spray's does,
+ * and the height adds the layer's h at START_POS.xz every frame ("Wake layer", Readers).
  * ocean_spray_particles takes host states (updated in place), instances and count and is synchronous;
  * ocean_spray_particles_device takes device pointers for them and is asynchronous on the generator's stream.  A zero-filled
  * state is a particle that was never emitted. */
@@ -649,8 +656,8 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *   launches  none extra: while foam is on each sub-step runs the foam form of the same kernel, and the render map the
  *             foam form of its kernel.
  *   limits    foam is not advected (the wake has no horizontal velocity; it stays where it forms, as the cascades' foam
- *             does); wake foam emits no spray; the ray cast and the sampling ops do not read it; there is no per-source
- *             foam rate; the cascades' foam is unchanged.
+ *             does); ocean_sample_maps and ocean_sample_velocity do not read it (spray does, under
+ *             OCEAN_WAKE_READ_SPRAY); there is no per-source foam rate; the cascades' foam is unchanged.
  * Obstacles (ocean_wake_set_obstacles, opt-in per generator; without a mask every kernel and record is as above): a
  * world-fixed binary mask of blocked cells (quays, breakwaters, islands, the shore) that wake waves reflect from and cannot
  * cross.  oracle/wake_obstacles.py is the specification, bit for bit.
@@ -684,8 +691,34 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *             removes the mask, since the cell size may change; ocean_wake_set_state, ocean_wake_set_foam and
  *             ocean_wake_set_coupling leave it as it is.
  *   launches  none extra: while a mask is set each sub-step and the free surface run the obstacle forms of their kernels.
- * Limits: the ray cast, spray, ocean_sample_maps and ocean_sample_velocity read the FFT maps only (the ray cast's slab
- * would also need a bound on e); the wake has no horizontal water velocity (iWave is vertical only); static obstacles block
+ * Readers (ocean_wake_set_readers, opt-in per generator; with readers 0 every op is byte-identical to a generator without a
+ * layer, whatever the coupling, foam and mask): the ray cast and spray read the layer too, so every op that answers "where is
+ * the water" or "where is the white water" reads the same layers.  oracle/wake_readers.py is the specification, bit for bit.
+ *   raycast   OCEAN_WAKE_READ_RAYCAST takes effect while the coupling is live (on and primed): ocean_raycast[_device] then
+ *             reads what the surface query reads, the free surface e in its own window.  Each evaluation's gap is
+ *             g = y - (eta + we), eta the cascades' height at the inverted source point as before and we the sample of e at
+ *             the evaluated point's (x, z) (one binary32 add; the wake has no horizontal displacement, so the inversion, warm
+ *             starts, restarts, march and refinement are unchanged).  The slab is widened by e's NaN-dropping extrema, taken
+ *             per call by one more kernel: y_lo += fminf(e_min, 0), y_hi += fmaxf(e_max, 0) (the sample is 0 outside the
+ *             window) and the padding's magnitude sum acc += fmaxf(|e_min|, |e_max|).  The record at the reported point gets
+ *             the coupled record's additions at Q = (position.x, position.z): displacement[1] += we, gradient_foam[0] += gx,
+ *             gradient_foam[1] += gz, so gap == position.y - displacement[1] holds as without the wake.  While the coupling
+ *             is off or unprimed the bit does nothing and launches nothing.
+ *   spray     OCEAN_WAKE_READ_SPRAY takes effect whenever a layer exists (no coupling needed: spray follows what the render
+ *             map draws).  With (hw, hgx, hgz) = ocean_sample_wake's sample of h and Fw that of F (+0 while foam is off) at
+ *             the candidate's START_POS.xz in the current window: the spawn test of ocean_extract_spray[_device] and
+ *             ocean_spray_particles[_device] adds, right after the cascade sum and before the normalize, gradient.x += hgx,
+ *             gradient.y += hgz, foam += Fw (so ocean_spray_record.foam is the sum); ocean_spray_particles adds hw to the
+ *             particle's displacement y right after the cascade sum, every frame, so the spray rises from the wake surface.
+ *   order     the ops read the layer as the last step call left it: a ray cast or spray call enqueued after
+ *             ocean_wake_step[_device] on the generator's stream sees that tick's wake.
+ *   limits    the coupled surface has a step at the edge of e's window (the sample drops to 0 there), as the surface query
+ *             and the physics see it: a crossing bracketed across the step ends the refinement without |gap| <= tolerance.
+ *             There is no cap on spray candidates per wake, and hull contact makes spray only where it makes wake foam.
+ *   launches  one more kernel per ray cast with rays while the ray cast reader is in effect; none extra for spray (its
+ *             kernels run their wake forms).
+ * Limits: ocean_sample_maps and ocean_sample_velocity read the FFT maps only; the wake has no horizontal water velocity
+ * (iWave is vertical only); static obstacles block
  * waves (ocean_wake_set_obstacles) but hulls do not (they are pressure sources); linear deep water only (no breaking,
  * shallow water or nonlinearity); the layer and the cascades interact by superposition only.  Far from the world origin
  * positions are binary32: phi, the cull and the samples use the cell centres x0 + (float)(i + 1/2) * dx, which lie within
@@ -726,7 +759,11 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
  *   ocean_wake_set_obstacles mask_host = NULL with width = depth = 0 removes the mask and releases it; otherwise width and
  *                            depth >= 1, width * depth <= 2^28 (a 16384^2 mask: 8 km on a side at dx = 0.5 m), and
  *                            origin + width and origin + depth representable in int64.  An invalid call keeps the previous
- *                            mask.  Synchronous: returns once the mask is on the device. */
+ *                            mask.  Synchronous: returns once the mask is on the device.
+ *   ocean_wake_set_readers   readers = a combination of OCEAN_WAKE_READ_RAYCAST and OCEAN_WAKE_READ_SPRAY (any other bit:
+ *                            OCEAN_ERR_INVALID_ARGUMENT, nothing changes); 0 (the default) reads nothing.  Host only, launches
+ *                            nothing.  ocean_wake_init (re-create or release) clears the readers; ocean_wake_set_state,
+ *                            ocean_wake_set_foam, ocean_wake_set_coupling and ocean_wake_set_obstacles leave them as they are. */
 typedef struct ocean_wake_params {
     int32_t size;               /* N: 0 (release) or a power of two in [128, 2048] */
     int32_t sponge_cells;       /* width of the absorbing ring, [0, 64] and <= size / 2 */
@@ -765,6 +802,9 @@ int ocean_wake_get_foam_state(ocean_generator* gen, float* foam_host);
 int ocean_wake_set_foam_state(ocean_generator* gen, const float* foam_host);
 int ocean_wake_set_obstacles(ocean_generator* gen, const uint8_t* mask_host, int32_t width, int32_t depth, int64_t origin_x,
                              int64_t origin_z);
+#define OCEAN_WAKE_READ_RAYCAST 1u      /* ocean_raycast[_device] reads the wake free surface e */
+#define OCEAN_WAKE_READ_SPRAY 2u        /* ocean_extract_spray[_device], ocean_spray_particles[_device] read h and F */
+int ocean_wake_set_readers(ocean_generator* gen, uint32_t readers);
 
 /* Parity/debug taps (not timed): binary32 maps before the half conversion, the row-pass output
  * ([4][N][N][2] float, == fft_buffer half 1 after the first fft_compute, wave_generator.gd:79) and

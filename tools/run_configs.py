@@ -3,6 +3,7 @@ config.
 
     python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast] [--spray-particles]
                                 [--wake] [--wake-coupling] [--wake-foam] [--wake-obstacles]
+                                [--wake-readers]
 
 Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
 --query.  An unknown argument exits before anything touches the GPU."""
@@ -550,6 +551,70 @@ def run_wake_step_coupling(N, sources, reps, label, substeps=8, dx=0.5):
     print(json.dumps(out), flush=True)
 
 
+def run_wake_readers(reps, label, N=256, C=4, wake=512, dx=0.5):
+    """Wake readers' cost (ocean_wake_set_readers): readers off against on, alternating windows on one generator, over C
+    cascades of N x N and a coupled, foamed wake x wake layer stirred by 64 moving sources:
+      the ray cast, 2^20 picking rays (run_raycast's scene a): one more kernel (the bounds of e) and one bilinear sample of e
+      per evaluation;
+      ocean_extract_spray_device on 2^20 candidates over the wake's window;
+      ocean_spray_particles_device with 32768 and 2^20 particles, one 30 Hz frame per call after 6 s of emitter time."""
+    g, _, scales = warmed_generator(N, C, 2)
+    g.wake_init(wake, dx, 0.05, 32, 3.0)
+    g.wake_set_coupling(True)
+    g.wake_set_foam(0.05, 1.0, 0.2, 0.3)
+    ext = wake * dx
+    rng = np.random.default_rng(wake)
+    s = np.zeros(64, gow.WaveGenerator.WAKE_SOURCE)
+    s["x"], s["z"] = rng.uniform(-0.4 * ext, 0.4 * ext, 64), rng.uniform(-0.4 * ext, 0.4 * ext, 64)
+    s["vx"], s["vz"] = rng.uniform(-6, 6, 64), rng.uniform(-6, 6, 64)
+    s["radius"], s["head"], s["body"] = 2.0, 0.2, -1
+    for _ in range(20):
+        g.wake_step(0.1, 4, (-wake // 2, -wake // 2), s)
+    lib = load_library()
+    gpu = card()
+    readers = lambda on: (lambda: g.wake_set_readers(raycast=on, spray=on))
+    out = {"config": label, **gpu, "map_size": N, "cascades": C, "wake_size": wake, "cell_size": dx}
+    rays = _picking_rays(1024)
+    n = len(rays)
+    rays_d = upload(rays)
+    hits = records(n, rc.HIT)
+    cast = lambda: check(lib.ocean_raycast_device(g.context, n, rays_d.data_ptr(), C, scales.ctypes.data, 0.5, 1024, 1e-3, 8,
+                                                  hits.data_ptr()))
+    t_off, t_on = alternate(lambda: timed(g, cast, reps, 2, readers(False)), lambda: timed(g, cast, reps, 2, readers(True)))
+    out["raycast_2^20_ms"] = {"off": t_off, "on": t_on, "on_over_off": min(t_on) / min(t_off) - 1.0}
+    m = 1 << 20
+    E = np.array([[ext / 20, 0, 0, 0], [0, 1, 0, 0], [0, 0, ext / 20, 0]], np.float32)
+    pts = torch.from_numpy(gow.WaveGenerator.spray_grid(m, E)).to(DEV)
+    recs = records(m, gow.WaveGenerator.SPRAY_RECORD)
+    count = torch.zeros(1, dtype=torch.int32, device=DEV)
+    ps = np.array([1, 1, 1], np.float32)
+    extract = lambda: check(lib.ocean_extract_spray_device(g.context, m, pts.data_ptr(), C, scales.ctypes.data, ps.ctypes.data, m,
+                                                           recs.data_ptr(), count.data_ptr()))
+    t_off, t_on = alternate(lambda: timed(g, extract, reps, 2, readers(False)), lambda: timed(g, extract, reps, 2, readers(True)))
+    out["extract_spray_2^20_ms"] = {"off": t_off, "on": t_on, "on_over_off": min(t_on) / min(t_off) - 1.0, "active_on": int(count.item())}
+    for amount in (32768, 1 << 20):
+        e = gow.WaveGenerator.default_spray_emitter()
+        e["amount"] = e["num_particles"] = amount
+        e["emission_transform"] = E.reshape(12) if amount > 32768 else (15 * np.eye(3, 4)).reshape(12)
+        states = torch.zeros(amount * gow.WaveGenerator.SPRAY_PARTICLE.itemsize, dtype=torch.uint8, device=DEV)
+        inst = torch.empty(amount * 16, dtype=torch.float32, device=DEV)
+        live = torch.zeros(1, dtype=torch.int32, device=DEV)
+        clock = [0.0]
+
+        def frame():
+            t0 = clock[0]
+            clock[0] = t0 + 1.0 / 30.0
+            check(lib.ocean_spray_particles_device(g.context, e.ctypes.data, t0, clock[0], C, scales.ctypes.data, states.data_ptr(), amount,
+                                                   inst.data_ptr(), live.data_ptr()))
+
+        for _ in range(180):                           # 6 s of emitter time: every particle emitted
+            frame()
+        t_off, t_on = alternate(lambda: timed(g, frame, reps, 2, readers(False)), lambda: timed(g, frame, reps, 2, readers(True)))
+        out[f"spray_particles_{amount}_ms"] = {"off": t_off, "on": t_on, "on_over_off": min(t_on) / min(t_off) - 1.0}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
 def run_wake_step_foam(N, sources, reps, label, substeps=8, dx=0.5):
     """Wake foam's cost in the step call: run_wake's ocean_wake_step_device with foam off and on (the foam form of the
     sub-step kernel: |v|^2 carried by the cull, w^2 |v|^2 summed beside phi, one more 4 B read and write per cell);
@@ -725,6 +790,10 @@ GROUPS = {          # flag: its configs, in the order they run
     "--wake-foam": [
         partial(run_wake_step_foam, N, k, 200 if N < 1024 else 50, f"wake foam, step: {N}x{N} cells, {k} source(s), 8 sub-steps")
         for N in (256, 512, 1024) for k in (1, 64, 1024)
+    ],
+    "--wake-readers": [
+        partial(run_wake_readers, 20, "wake readers: ray cast, spray and spray particles, readers off vs on, 4 cascades of 256x256, "
+                                      "coupled 512x512 wake with foam"),
     ],
     "--wake-obstacles": [
         partial(run_wake_step_obstacles, N, k, 200 if N < 1024 else 50, f"wake obstacles, step: {N}x{N} cells, {k} source(s), 8 sub-steps")
