@@ -144,6 +144,11 @@ struct ocean_generator {
     int pass_num_cascades_remaining = 0;                // wave_generator.gd:15
     uint64_t kernel_launches = 0;
     uint64_t cascade_updates = 0;
+    // Entry points entered so far, and the value it had when the stream's last operation was a persistent single-update
+    // launch (0: it is not).  The next update's launch is queued as that launch's programmatic dependent only if no entry
+    // point ran in between (any of them may have put work on the stream), see run_cascades.
+    uint64_t entries = 0;
+    uint64_t update_tail = 0;
     DeviceArray<unsigned> ray_bounds;                   // ray cast scratch: [3 * num_cascades] per-layer bounds (first use)
     // wake layer (ocean_wake_init): four [size][size] fields -- h, h_prev and the two a sub-step writes
     DeviceArray<float> wake_fields;
@@ -193,6 +198,7 @@ int enter_gen(ocean_generator* g, DeviceScope& scope) {
     if (!g) return fail(OCEAN_ERR_INVALID_ARGUMENT, "generator handle is NULL");
     cudaError_t e = scope.enter(g->device);
     if (e != cudaSuccess) return fail(OCEAN_ERR_CUDA, "cudaSetDevice(%d) failed: %s", g->device, cudaGetErrorString(e));
+    g->entries += 1;
     return OCEAN_OK;
 }
 #define OCEAN_ENTER(gen)                 \
@@ -473,7 +479,16 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
     const bool two_kernel = g->profiling;              // profiled updates time the row and the column pass apart
     if (two_kernel)   // the persistent launch takes its dispatch records by value
         RUN_CUDA(cudaMemcpyAsync(g->d_cascade.ptr, hc, sizeof(ocean::CascadeDispatch) * n, cudaMemcpyHostToDevice, g->stream));
-    RUN_CUDA(cudaEventRecord(g->ring_done[slot], g->stream));
+    // The staging slot is free again once the copies above have read it.  Without them (the persistent path with no spectrum
+    // or table to rebuild: every step of a steady simulation) nothing on the device reads the slot, no event is recorded, and
+    // the last record of ring_done[slot] -- older work -- is what the next use of the slot waits for.
+    const bool staged = n_dirty || n_tables || two_kernel;
+    if (staged) RUN_CUDA(cudaEventRecord(g->ring_done[slot], g->stream));
+    // The first persistent launch follows the previous update's persistent launch directly when no entry point ran in between
+    // and nothing was enqueued above: it is then queued as that launch's programmatic dependent.  Later launches of this call
+    // follow one of its own.
+    bool chained = !staged && g->update_tail != 0 && g->entries - g->update_tail <= 1;
+    g->update_tail = 0;
     int launched = 0;
     if (g->profiling) RUN_CUDA(cudaEventRecord(g->prof[1], g->stream));
     if (!two_kernel) {
@@ -484,10 +499,12 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
                 return ocean::build_item_table(g->map_size, m, ocean::persistent_group(g->map_size), ocean::persistent_lag(g->map_size), out);
             };
             const DeviceArray<int>* table = nullptr;
+            const bool cached = g->item_tables.count(m) != 0;        // a first use uploads the table: a copy on the stream
             RUN_CUDA(item_table(g, g->item_tables, m, build, &table));
             counters_touched = true;
             RUN_CUDA(ocean::launch_cascade_update_persistent(g->buf, hc + first, m, g->stream, g->d_queue.ptr, table->ptr,
-                                                             (int)table->capacity, g->resident_ctas));
+                                                             (int)table->capacity, g->resident_ctas, false, chained && cached));
+            chained = true;
             launched += 1;
         }
     } else {
@@ -511,6 +528,7 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
     if (two_kernel)
         RUN_CUDA(cudaMemcpyAsync(g->d_queue.ptr + 1, g->done_count.data(), sizeof(uint32_t) * g->done_count.size(), cudaMemcpyHostToDevice, g->stream));
 #undef RUN_CUDA
+    if (!two_kernel) g->update_tail = g->entries;
     g->ring_next = (g->ring_next + 1) % kRing;
     g->kernel_launches += (uint64_t)launched + (n_dirty ? 1 : 0) + (n_tables ? 1 : 0);
     g->cascade_updates += (uint64_t)n;
@@ -788,6 +806,7 @@ int ocean_update_frames(ocean_generator* gen, double delta, ocean_cascade_params
     }
     // frame 0 exactly as ocean_update_all: flush of a pending pass, time/rate advance, spectra and tables where needed
     if ((rc = ocean_update_all(gen, delta, parameters, count))) return rc;
+    gen->update_tail = 0;                                              // the fused launches below are not single updates
     const uint32_t a_per = (uint32_t)ocean::a_items_per_cascade(gen->map_size), b_per = (uint32_t)ocean::b_items_per_cascade(gen->map_size);
     const int C = gen->num_cascades;
     std::vector<ocean::CascadeDispatch> rec;

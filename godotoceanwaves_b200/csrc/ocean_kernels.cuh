@@ -98,9 +98,12 @@ int chunk_cascades(int map_size);
 constexpr int kMaxPersistentCascades = 256;
 // multi_frame: the records describe several consecutive updates of the same cascades (build_item_table_frames): B items then
 // publish their completion in queue_dev[1 + num_cascades + c] and A items wait for wait_target there.
+// The work counter queue_dev[0] must be 0 at the launch and is 0 again once the launch is complete (no host reset).
+// chained: the stream's previous operation is a persistent launch; this one is queued as its programmatic dependent, so its teams
+// start their prologue while that launch drains (the kernel waits for the previous grid's completion before its first item).
 cudaError_t launch_cascade_update_persistent(const DeviceBuffers& b, const CascadeDispatch* dispatch_host, int count,
                                              cudaStream_t stream, int* queue_dev, const int* item_table_dev, int total_items,
-                                             int resident_ctas, bool multi_frame = false);
+                                             int resident_ctas, bool multi_frame = false, bool chained = false);
 int build_item_table(int map_size, int count, int group, int lag, int* out);
 // Queue order of `frames` consecutive updates of the same `count` cascades in one launch: A(f0) A(f1) B(f0) A(f2) B(f1) ... with
 // A(f) = the row-pass items of every cascade; slot of (frame f, cascade position c) = f * count + c.  Frames alternate between the
