@@ -68,6 +68,77 @@ enum StagedOp {
     kStageSampleVelocity, kStageBodyForces, kStageSimulateBodies, kStageDeviceMath, kStageWakeStep, kStageSampleWake,
     kNumStagedOps
 };
+
+// The parts of the wake layer WakeLayer::off turns off; kWakeLayer is the whole layer.
+enum : unsigned { kWakeCoupling = 1, kWakeFoam = 2, kWakeMask = 4, kWakeFields = 8, kWakeLayer = 15 };
+
+// The wake layer (ocean_wake_init) and its parts.  The coupling, foam and mask are on exactly while their buffers are
+// allocated: the calls that turn a part on leave it allocated (and cleared where the kernels read it) or off.
+struct WakeLayer {
+    ocean_wake_params params{};                         // size 0: no layer
+    // four [size][size] fields -- h, h_prev and the two a sub-step writes -- and the window's origin in whole cells
+    DeviceArray<float> fields;
+    int h = 0, hp = 1;                                  // which fields hold h and h_prev
+    int64_t origin[2] = {0, 0};
+    // coupling (ocean_wake_set_coupling): two [size][size] snapshots of the free surface e = h + phi, each with its window
+    // origin, the interval between them, and the drag pass's per-world-point vertical velocity
+    DeviceArray<float> snapshots;
+    DeviceArray<float> wv;
+    bool primed = false;                                // the snapshots describe the layer
+    int e = 0;                                          // which snapshot holds e (the other holds e_old)
+    int64_t snapshot_origin[2][2] = {};                 // [snapshot][x, z]
+    float interval = 0.0f;                              // T
+    // foam (ocean_wake_set_foam): two [size][size] foam fields, F and the one a sub-step writes, and the parameters
+    DeviceArray<float> foam;
+    ocean_wake_foam_params foam_params{};
+    int f = 0;                                          // which foam field holds F
+    // obstacles (ocean_wake_set_obstacles): the mask's bytes ([depth][width], nonzero = blocked) and its world cell origin
+    DeviceArray<uint8_t> mask;
+    int32_t mask_size[2] = {0, 0};                      // width, depth
+    int64_t mask_origin[2] = {0, 0};
+    // readers (ocean_wake_set_readers): OCEAN_WAKE_READ_* bits of the ops that read the layer besides the coupling's
+    uint32_t readers = 0;
+
+    bool on() const { return params.size > 0; }
+    bool coupled() const { return snapshots.ptr != nullptr; }
+    bool foamed() const { return foam.ptr != nullptr; }
+    bool masked() const { return mask.ptr != nullptr; }
+    // the surface query reads the layer while the coupling is on and primed
+    bool coupling_live() const { return on() && coupled() && primed; }
+    bool reads(uint32_t reader) const { return on() && (readers & reader); }
+    size_t cells() const { return (size_t)params.size * params.size; }
+    float* field(int k) const { return fields.ptr + k * cells(); }
+    float* foam_field(int k) const { return foam.ptr + k * cells(); }
+    float* snapshot(int k) const { return snapshots.ptr + k * cells(); }
+    // (float)((double)origin * dx), the world corner of a window at `origin`
+    float corner(int64_t o) const { return (float)((double)o * (double)params.cell_size); }
+
+    // h in the current window, with F while foam is on
+    ocean::WakeRead read_h() const {
+        return {field(h), foamed() ? foam_field(f) : nullptr, params.size, params.cell_size, corner(origin[0]), corner(origin[1])};
+    }
+    // e in its own window
+    ocean::WakeRead read_e() const {
+        return {snapshot(e), nullptr, params.size, params.cell_size, corner(snapshot_origin[e][0]), corner(snapshot_origin[e][1])};
+    }
+    ocean::WakeCoupleArgs couple_args() const {
+        const int o = e ^ 1;
+        return {snapshot(e), snapshot(o), params.size, params.cell_size, corner(snapshot_origin[e][0]), corner(snapshot_origin[e][1]),
+                corner(snapshot_origin[o][0]), corner(snapshot_origin[o][1]), interval};
+    }
+    // The mask in the window at (origin_x, origin_z): the mask cell of window cell (0, 0), exact in __int128 and clamped to
+    // [-2^30, 2^30] per axis.  The halo spans window cells [-6, size + 6) and the mask at most 2^28 cells, so a clamped offset
+    // leaves the whole halo outside the mask exactly when the exact one does.
+    ocean::WakeObstacles obstacles(int64_t origin_x, int64_t origin_z) const {
+        auto offset = [](int64_t window, int64_t m) -> int {
+            constexpr __int128 kClamp = (__int128)1 << 30;
+            const __int128 d = (__int128)window - (__int128)m;
+            return (int)(d > kClamp ? kClamp : d < -kClamp ? -kClamp : d);
+        };
+        return {mask.ptr, mask_size[0], mask_size[1], offset(origin_x, mask_origin[0]), offset(origin_z, mask_origin[1])};
+    }
+    int off(ocean_generator* g, unsigned parts);
+};
 }  // namespace
 
 struct ocean_generator {
@@ -150,30 +221,7 @@ struct ocean_generator {
     uint64_t entries = 0;
     uint64_t update_tail = 0;
     DeviceArray<unsigned> ray_bounds;                   // ray cast scratch: [3 * num_cascades] per-layer bounds (first use)
-    // wake layer (ocean_wake_init): four [size][size] fields -- h, h_prev and the two a sub-step writes
-    DeviceArray<float> wake_fields;
-    ocean_wake_params wake{};                           // size 0: no layer
-    int wake_h = 0, wake_hp = 1;                        // which fields hold h and h_prev
-    int64_t wake_origin[2] = {0, 0};
-    // wake coupling (ocean_wake_set_coupling): two [size][size] snapshots of the free surface e = h + phi, each with its window
-    // origin, the interval between them, and the drag pass's per-world-point vertical velocity
-    DeviceArray<float> wake_snapshots;
-    DeviceArray<float> wake_wv;
-    bool wake_coupled = false, wake_primed = false;
-    int wake_e = 0;                                     // which snapshot holds e (the other holds e_old)
-    int64_t wake_snapshot_origin[2][2] = {};            // [snapshot][x, z]
-    float wake_interval = 0.0f;                         // T
-    // wake foam (ocean_wake_set_foam): two [size][size] foam fields, F and the one a sub-step writes, and the parameters
-    DeviceArray<float> wake_foam;
-    ocean_wake_foam_params wake_foam_params{};
-    bool wake_foam_on = false;
-    int wake_f = 0;                                     // which foam field holds F
-    // wake obstacles (ocean_wake_set_obstacles): the mask's bytes ([depth][width], nonzero = blocked) and its world cell origin
-    DeviceArray<uint8_t> wake_mask;
-    int32_t wake_mask_size[2] = {0, 0};                 // width, depth; 0: no mask
-    int64_t wake_mask_origin[2] = {0, 0};
-    // wake readers (ocean_wake_set_readers): OCEAN_WAKE_READ_* bits of the ops that read the layer besides the coupling's
-    uint32_t wake_readers = 0;
+    WakeLayer wake;
 };
 
 namespace {
@@ -1167,11 +1215,6 @@ int ocean_spray_grid(int num_particles, const float* emission_transform, float* 
     return OCEAN_OK;
 }
 
-namespace {
-// The layer's h and F in its current window, when the spray reader is set (ocean_wake_set_readers); false otherwise.
-bool wake_spray_read(ocean_generator* g, ocean::WakeRead* out);
-}  // namespace
-
 int ocean_extract_spray_device(ocean_generator* gen, int num_candidates, const float* points_xz_dev, int num_cascades,
                                const float* map_scales_host, const float* particle_scale, int max_records,
                                ocean_spray_record* records_dev, int* num_active_dev) {
@@ -1187,8 +1230,8 @@ int ocean_extract_spray_device(ocean_generator* gen, int num_candidates, const f
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
     const int blocks = ocean::spray_blocks(num_candidates);
     OCEAN_CUDA(gen->spray_counts.grow(gen, (size_t)blocks + 1));
-    ocean::WakeRead wake;
-    const bool wk = wake_spray_read(gen, &wake);
+    const bool wk = gen->wake.reads(OCEAN_WAKE_READ_SPRAY);
+    const ocean::WakeRead wake = wk ? gen->wake.read_h() : ocean::WakeRead{};
     OCEAN_CUDA(ocean::launch_extract_spray(gen->buf, num_cascades, reinterpret_cast<const float2*>(points_xz_dev), num_candidates,
                                            gen->q_scales.ptr, make_float3(particle_scale[0], particle_scale[1], particle_scale[2]),
                                            gen->spray_counts.ptr, records_dev, max_records, wk ? &wake : nullptr, gen->stream));
@@ -1284,8 +1327,8 @@ int ocean_spray_particles_device(ocean_generator* gen, const ocean_spray_emitter
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
     const int blocks = ocean::spray_blocks(emitter->amount);
     OCEAN_CUDA(gen->spray_counts.grow(gen, (size_t)blocks + 1));
-    ocean::WakeRead wake;
-    const bool wk = wake_spray_read(gen, &wake);
+    const bool wk = gen->wake.reads(OCEAN_WAKE_READ_SPRAY);
+    const ocean::WakeRead wake = wk ? gen->wake.read_h() : ocean::WakeRead{};
     OCEAN_CUDA(ocean::launch_spray_particles(gen->buf, num_cascades, gen->q_scales.ptr, *emitter, t0, t1, states_dev, gen->spray_counts.ptr,
                                              instances_dev, max_instances, wk ? &wake : nullptr, gen->stream));
     gen->kernel_launches += 3;
@@ -1329,11 +1372,6 @@ int check_surface_args(int num_points, float tolerance, int max_iterations) {
     return OCEAN_OK;
 }
 
-float wake_corner(int64_t origin, float cell);
-
-// The surface query reads the wake layer while its coupling is on and primed (ocean_wake_set_coupling).
-bool wake_coupling_live(const ocean_generator* g) { return g->wake.size > 0 && g->wake_coupled && g->wake_primed; }
-
 // The surface query on validated arguments, with the map scales already in gen->q_scales (ocean_query_surface_device and
 // ocean_buoyancy_device).  With the wake coupling live, one more kernel adds the wake free surface to the records and, when
 // wv_dev is not null (a drag pass follows), writes the wake's vertical velocity of each point there.
@@ -1343,21 +1381,8 @@ int run_query_surface(ocean_generator* gen, int num_points, const float2* points
     OCEAN_CUDA(ocean::launch_query_surface(gen->buf, num_cascades, points_xz_dev, num_points, gen->q_scales.ptr, tolerance, max_iterations,
                                            out_dev, gen->surf_scratch.ptr, gen->stream));
     gen->kernel_launches += max_iterations > 0 ? 3 : 1;
-    if (wake_coupling_live(gen)) {
-        const size_t cells = (size_t)gen->wake.size * gen->wake.size;
-        const int e = gen->wake_e, o = e ^ 1;
-        const float dx = gen->wake.cell_size;
-        ocean::WakeCoupleArgs a{};
-        a.e = gen->wake_snapshots.ptr + e * cells;
-        a.e_old = gen->wake_snapshots.ptr + o * cells;
-        a.n = gen->wake.size;
-        a.cell = dx;
-        a.x0 = wake_corner(gen->wake_snapshot_origin[e][0], dx);
-        a.z0 = wake_corner(gen->wake_snapshot_origin[e][1], dx);
-        a.x0_old = wake_corner(gen->wake_snapshot_origin[o][0], dx);
-        a.z0_old = wake_corner(gen->wake_snapshot_origin[o][1], dx);
-        a.interval = gen->wake_interval;
-        OCEAN_CUDA(ocean::launch_wake_couple(a, points_xz_dev, num_points, out_dev, wv_dev, gen->stream));
+    if (gen->wake.coupling_live()) {
+        OCEAN_CUDA(ocean::launch_wake_couple(gen->wake.couple_args(), points_xz_dev, num_points, out_dev, wv_dev, gen->stream));
         gen->kernel_launches += 1;
     }
     return OCEAN_OK;
@@ -1413,16 +1438,8 @@ int ocean_raycast_device(ocean_generator* gen, int num_rays, const ocean_ray* ra
     if (!rays_dev || !out_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
     // with the ray cast reader set and the coupling live, the coupled surface: e in its own window, and one more kernel (its bounds)
-    const bool wk = (gen->wake_readers & OCEAN_WAKE_READ_RAYCAST) && wake_coupling_live(gen);
-    ocean::WakeRead wake{};
-    if (wk) {
-        const int e = gen->wake_e;
-        wake.field = gen->wake_snapshots.ptr + e * (size_t)gen->wake.size * gen->wake.size;
-        wake.n = gen->wake.size;
-        wake.cell = gen->wake.cell_size;
-        wake.x0 = wake_corner(gen->wake_snapshot_origin[e][0], wake.cell);
-        wake.z0 = wake_corner(gen->wake_snapshot_origin[e][1], wake.cell);
-    }
+    const bool wk = gen->wake.reads(OCEAN_WAKE_READ_RAYCAST) && gen->wake.coupling_live();
+    const ocean::WakeRead wake = wk ? gen->wake.read_e() : ocean::WakeRead{};
     OCEAN_CUDA(gen->ray_bounds.grow(gen, 3 * (size_t)gen->num_cascades + (wk ? 2 : 0)));
     OCEAN_CUDA(ocean::launch_raycast(gen->buf, num_cascades, rays_dev, num_rays, gen->q_scales.ptr, step, max_samples, tolerance, max_iterations,
                                      gen->ray_bounds.ptr, out_dev, wk ? &wake : nullptr, gen->stream));
@@ -1707,9 +1724,9 @@ int ocean_body_forces_device(ocean_generator* gen, int num_bodies, const ocean_b
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
     OCEAN_CUDA(gen->drag_velocities.upload(gen, velocities_host, (size_t)num_bodies));
     float* wv = nullptr;
-    if (world > 0 && wake_coupling_live(gen)) {
-        OCEAN_CUDA(gen->wake_wv.grow(gen, (size_t)world));
-        wv = gen->wake_wv.ptr;
+    if (world > 0 && gen->wake.coupling_live()) {
+        OCEAN_CUDA(gen->wake.wv.grow(gen, (size_t)world));
+        wv = gen->wake.wv.ptr;
     }
     ocean_surface_sample* samples = nullptr;
     if ((rc = run_buoyancy(gen, num_bodies, bodies_host, world, points_dev, num_cascades, density, tolerance, max_iterations, hydrostatic_dev,
@@ -1801,9 +1818,9 @@ int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const oce
     OCEAN_CUDA(gen->buoy_q.grow(gen, (size_t)world));
     OCEAN_CUDA(gen->buoy_samples.grow(gen, (size_t)world));
     float* wv = nullptr;                                // every sub-step reads the same snapshots
-    if (world > 0 && wake_coupling_live(gen)) {
-        OCEAN_CUDA(gen->wake_wv.grow(gen, (size_t)world));
-        wv = gen->wake_wv.ptr;
+    if (world > 0 && gen->wake.coupling_live()) {
+        OCEAN_CUDA(gen->wake.wv.grow(gen, (size_t)world));
+        wv = gen->wake.wv.ptr;
     }
     if (!hydrostatic_dev) {
         OCEAN_CUDA(gen->buoy_results.grow(gen, B));
@@ -1981,10 +1998,8 @@ int ocean_wake_kernel_taps(float* taps_host) {
 namespace {
 constexpr double kWakeCap = 4.0;                        // max Ghat of the stencil (tools/fit_wake_kernel.py)
 
-float* wake_field(ocean_generator* g, int k) { return g->wake_fields.ptr + (size_t)k * g->wake.size * g->wake.size; }
-
 int check_wake_layer(ocean_generator* g) {
-    if (g->wake.size == 0) return fail(OCEAN_ERR_STATE, "the generator has no wake layer (ocean_wake_init)");
+    if (!g->wake.on()) return fail(OCEAN_ERR_STATE, "the generator has no wake layer (ocean_wake_init)");
     return OCEAN_OK;
 }
 
@@ -1995,7 +2010,7 @@ int wake_step_args(ocean_generator* g, double dt, int substeps, int num_sources,
     if (substeps < 1 || substeps > 256) return fail(OCEAN_ERR_INVALID_ARGUMENT, "substeps %d outside [1, 256]", substeps);
     if (num_sources < 0 || num_states < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "negative source or state count");
     if ((num_sources > 0 && !sources) || (num_states > 0 && !states)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "sources or states is NULL");
-    const ocean_wake_params& p = g->wake;
+    const ocean_wake_params& p = g->wake.params;
     const float hf = (float)(dt / substeps);
     const double h = hf, dx = p.cell_size;
     if (kG * h * h / dx * kWakeCap > 4.0)
@@ -2023,69 +2038,47 @@ int wake_step_args(ocean_generator* g, double dt, int substeps, int num_sources,
     return OCEAN_OK;
 }
 
-// (float)((double)origin * dx), the window's world corner
-float wake_corner(int64_t origin, float cell) { return (float)((double)origin * (double)cell); }
-
-// Turns the coupling off and releases its buffers (the caller has entered the generator).
-int wake_uncouple(ocean_generator* g) {
-    if (g->wake_snapshots.ptr || g->wake_wv.ptr) OCEAN_CUDA(cudaStreamSynchronize(g->stream));    // kernels may still read them
-    g->wake_snapshots.release();
-    g->wake_wv.release();
-    g->wake_coupled = g->wake_primed = false;
-    g->wake_e = 0;
-    g->wake_interval = 0.0f;
-    for (auto& o : g->wake_snapshot_origin) o[0] = o[1] = 0;
+// Turns off the chosen parts of the layer (kWake*; kWakeFields removes the layer itself): one synchronise when a buffer of
+// theirs is live, since kernels may still read it, then their buffers are released and their state reset.  The caller has
+// entered the generator.
+int WakeLayer::off(ocean_generator* g, unsigned parts) {
+    const bool live = ((parts & kWakeCoupling) && (snapshots.ptr || wv.ptr)) || ((parts & kWakeFoam) && foam.ptr) ||
+                      ((parts & kWakeMask) && mask.ptr) || ((parts & kWakeFields) && fields.ptr);
+    if (live) OCEAN_CUDA(cudaStreamSynchronize(g->stream));
+    if (parts & kWakeCoupling) {
+        snapshots.release();
+        wv.release();
+        primed = false;
+        e = 0;
+        interval = 0.0f;
+        for (auto& o : snapshot_origin) o[0] = o[1] = 0;
+    }
+    if (parts & kWakeFoam) {
+        foam.release();
+        foam_params = ocean_wake_foam_params{};
+        f = 0;
+    }
+    if (parts & kWakeMask) {
+        mask.release();
+        mask_size[0] = mask_size[1] = 0;
+        mask_origin[0] = mask_origin[1] = 0;
+    }
+    if (parts & kWakeFields) {
+        fields.release();
+        params = ocean_wake_params{};
+        h = 0;
+        hp = 1;
+        origin[0] = origin[1] = 0;
+        readers = 0;
+    }
     return OCEAN_OK;
 }
 
-// Turns foam off and releases its fields (the caller has entered the generator).
-int wake_foam_off(ocean_generator* g) {
-    if (g->wake_foam.ptr) OCEAN_CUDA(cudaStreamSynchronize(g->stream));     // kernels may still read them
-    g->wake_foam.release();
-    g->wake_foam_on = false;
-    g->wake_foam_params = ocean_wake_foam_params{};
-    g->wake_f = 0;
-    return OCEAN_OK;
-}
-
-float* wake_foam_field(ocean_generator* g, int k) { return g->wake_foam.ptr + (size_t)k * g->wake.size * g->wake.size; }
-
-bool wake_spray_read(ocean_generator* g, ocean::WakeRead* out) {
-    if (!(g->wake_readers & OCEAN_WAKE_READ_SPRAY) || g->wake.size == 0) return false;
-    out->field = wake_field(g, g->wake_h);
-    out->foam = g->wake_foam_on ? wake_foam_field(g, g->wake_f) : nullptr;
-    out->n = g->wake.size;
-    out->cell = g->wake.cell_size;
-    out->x0 = wake_corner(g->wake_origin[0], out->cell);
-    out->z0 = wake_corner(g->wake_origin[1], out->cell);
-    return true;
-}
-
-// Removes the obstacle mask and releases it (the caller has entered the generator).
-int wake_obstacles_off(ocean_generator* g) {
-    if (g->wake_mask.ptr) OCEAN_CUDA(cudaStreamSynchronize(g->stream));     // kernels may still read it
-    g->wake_mask.release();
-    g->wake_mask_size[0] = g->wake_mask_size[1] = 0;
-    g->wake_mask_origin[0] = g->wake_mask_origin[1] = 0;
-    return OCEAN_OK;
-}
-
-// The mask in the window at (origin_x, origin_z): the mask cell of window cell (0, 0), exact in __int128 and clamped to
-// [-2^30, 2^30] per axis.  The halo spans window cells [-6, size + 6) and the mask at most 2^28 cells, so a clamped offset
-// leaves the whole halo outside the mask exactly when the exact one does.
-ocean::WakeObstacles wake_obstacles(const ocean_generator* g, int64_t origin_x, int64_t origin_z) {
-    auto offset = [](int64_t window, int64_t mask) -> int {
-        constexpr __int128 kClamp = (__int128)1 << 30;
-        const __int128 d = (__int128)window - (__int128)mask;
-        return (int)(d > kClamp ? kClamp : d < -kClamp ? -kClamp : d);
-    };
-    ocean::WakeObstacles o{};
-    o.mask = g->wake_mask.ptr;
-    o.width = g->wake_mask_size[0];
-    o.depth = g->wake_mask_size[1];
-    o.qx = offset(origin_x, g->wake_mask_origin[0]);
-    o.qz = offset(origin_z, g->wake_mask_origin[1]);
-    return o;
+// The status of the set-up step `what` of a part that has just been allocated; a failed set-up turns the part off.
+int wake_part_setup(ocean_generator* g, unsigned part, cudaError_t e, const char* what) {
+    if (e == cudaSuccess) return OCEAN_OK;
+    g->wake.off(g, part);
+    return fail(OCEAN_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(e));
 }
 
 int check_wake_points(int num_points, const void* points, const void* out) {
@@ -2100,16 +2093,12 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
     if (rc) return rc;
     if (!params) return fail(OCEAN_ERR_INVALID_ARGUMENT, "params is NULL");
     const ocean_wake_params p = *params;
+    WakeLayer& w = gen->wake;
     if (p.size == 0) {
-        if ((rc = wake_uncouple(gen))) return rc;
-        if ((rc = wake_foam_off(gen))) return rc;
-        if ((rc = wake_obstacles_off(gen))) return rc;
-        gen->wake_readers = 0;
-        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-        gen->wake_fields.release();
+        if ((rc = w.off(gen, kWakeLayer))) return rc;
+        // only wake kernels read these, and none is queued once the layer's buffers are released
         gen->staging[kStageWakeStep].release();
         gen->staging[kStageSampleWake].release();
-        gen->wake = ocean_wake_params{};
         return OCEAN_OK;
     }
     if (p.size < 128 || p.size > 2048 || (p.size & (p.size - 1)))
@@ -2120,21 +2109,16 @@ int ocean_wake_init(ocean_generator* gen, const ocean_wake_params* params) {
     if (p.sponge_cells < 0 || p.sponge_cells > ocean::kWakeMaxSponge || 2 * p.sponge_cells > p.size)
         return fail(OCEAN_ERR_INVALID_ARGUMENT, "sponge_cells %d outside [0, min(64, size / 2)]", p.sponge_cells);
     const size_t cells = 4 * (size_t)p.size * p.size;  // h, h_prev and two fields a scrolled sub-step writes
-    if ((rc = wake_uncouple(gen))) return rc;
-    if ((rc = wake_foam_off(gen))) return rc;
-    if ((rc = wake_obstacles_off(gen))) return rc;      // the mask's cells are cells of the old cell size
-    gen->wake_readers = 0;
-    gen->wake = ocean_wake_params{};                    // no layer until the fields below are allocated and cleared
-    if (gen->wake_fields.capacity != cells) {
-        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-        gen->wake_fields.release();
-    }
-    OCEAN_CUDA(gen->wake_fields.grow(gen, cells));
-    OCEAN_CUDA(cudaMemsetAsync(gen->wake_fields.ptr, 0, cells * sizeof(float), gen->stream));
-    gen->wake = p;
-    gen->wake_h = 0;
-    gen->wake_hp = 1;
-    gen->wake_origin[0] = gen->wake_origin[1] = 0;
+    // every part goes (the mask's cells are cells of the old cell size); the fields' block stays when its size does
+    if ((rc = w.off(gen, w.fields.capacity == cells ? kWakeLayer & ~kWakeFields : kWakeLayer))) return rc;
+    w.params = ocean_wake_params{};                     // no layer until the fields below are allocated and cleared
+    w.readers = 0;
+    OCEAN_CUDA(w.fields.grow(gen, cells));
+    OCEAN_CUDA(cudaMemsetAsync(w.fields.ptr, 0, cells * sizeof(float), gen->stream));
+    w.params = p;
+    w.h = 0;
+    w.hp = 1;
+    w.origin[0] = w.origin[1] = 0;
     return OCEAN_OK;
 }
 
@@ -2146,89 +2130,79 @@ int ocean_wake_step_device(ocean_generator* gen, double dt, int substeps, int64_
     ocean::WakeStepArgs a;
     float h = 0.0f;
     if ((rc = wake_step_args(gen, dt, substeps, num_sources, sources_dev, num_states, states_dev, &a, &h))) return rc;
-    const int n = gen->wake.size;
+    WakeLayer& w = gen->wake;
+    const int n = w.params.size;
     // the scroll, clamped to [-n, n] per axis (a move of n cells or more reads nothing but zeros)
     auto shift = [n](int64_t to, int64_t from) -> int {
         const __int128 d = (__int128)to - (__int128)from;
         return d > n ? n : d < -n ? -n : (int)d;
     };
-    a.di = shift(origin_x, gen->wake_origin[0]);
-    a.dj = shift(origin_z, gen->wake_origin[1]);
-    a.x0 = wake_corner(origin_x, gen->wake.cell_size);
-    a.z0 = wake_corner(origin_z, gen->wake.cell_size);
+    a.di = shift(origin_x, w.origin[0]);
+    a.dj = shift(origin_z, w.origin[1]);
+    a.x0 = w.corner(origin_x);
+    a.z0 = w.corner(origin_z);
     ocean::WakeFoamStepArgs f{};
-    if (gen->wake_foam_on) {
-        const ocean_wake_foam_params& fp = gen->wake_foam_params;
+    const ocean::WakeFoamStepArgs* foam = w.foamed() ? &f : nullptr;
+    if (foam) {
+        const ocean_wake_foam_params& fp = w.foam_params;
         f.whitecap = fp.whitecap;
         f.decay = exp_det_host(-(fp.decay_rate * h));  // binary32 products, the cascades' DETMATH exp
         f.grow = fp.grow_rate * h;
         f.stir = fp.stir_rate * h;
     }
     // while a mask is set every kernel of the call runs its obstacle form, the mask read in the call's window
-    const bool masked = gen->wake_mask.ptr != nullptr;
-    const ocean::WakeObstacles ob = wake_obstacles(gen, origin_x, origin_z);
+    const ocean::WakeObstacles ob = w.obstacles(origin_x, origin_z);
+    const ocean::WakeObstacles* obstacles = w.masked() ? &ob : nullptr;
     for (int k = 0; k < substeps; ++k) {
         int spare[2], m = 0;
         for (int b = 0; b < 4 && m < 2; ++b)
-            if (b != gen->wake_h && b != gen->wake_hp) spare[m++] = b;
+            if (b != w.h && b != w.hp) spare[m++] = b;
         const bool scrolled = a.di != 0 || a.dj != 0;
-        a.h = wake_field(gen, gen->wake_h);
-        a.h_prev = wake_field(gen, gen->wake_hp);
-        a.out_h = wake_field(gen, spare[0]);
-        a.out_h_prev = scrolled ? wake_field(gen, spare[1]) : nullptr;
+        a.h = w.field(w.h);
+        a.h_prev = w.field(w.hp);
+        a.out_h = w.field(spare[0]);
+        a.out_h_prev = scrolled ? w.field(spare[1]) : nullptr;
         a.tau = (float)k * h;
-        if (gen->wake_foam_on) {
-            f.step = a;
-            f.foam = wake_foam_field(gen, gen->wake_f);
-            f.out_foam = wake_foam_field(gen, gen->wake_f ^ 1);
-            if (masked)
-                OCEAN_CUDA(ocean::launch_wake_step_foam_obstacles(f, ob, gen->stream));
-            else
-                OCEAN_CUDA(ocean::launch_wake_step_foam(f, gen->stream));
-            gen->wake_f ^= 1;
-        } else if (masked) {
-            OCEAN_CUDA(ocean::launch_wake_step_obstacles(a, ob, gen->stream));
-        } else {
-            OCEAN_CUDA(ocean::launch_wake_step(a, gen->stream));
+        if (foam) {
+            f.foam = w.foam_field(w.f);
+            f.out_foam = w.foam_field(w.f ^ 1);
         }
+        OCEAN_CUDA(ocean::launch_wake_step(a, foam, obstacles, gen->stream));
         gen->kernel_launches += 1;
-        gen->wake_hp = scrolled ? spare[1] : gen->wake_h;
-        gen->wake_h = spare[0];
+        if (foam) w.f ^= 1;
+        w.hp = scrolled ? spare[1] : w.h;
+        w.h = spare[0];
         // the fields are now those of the new origin: record it at once, so a later failed launch leaves them consistent
-        gen->wake_origin[0] = origin_x;
-        gen->wake_origin[1] = origin_z;
+        w.origin[0] = origin_x;
+        w.origin[1] = origin_z;
         a.di = a.dj = 0;
     }
-    if (gen->wake_coupled) {
+    if (w.coupled()) {
         // e = h + phi at the end of the call into the snapshot that held e_old (on a priming call into both)
-        const size_t cells = (size_t)n * n;
-        const int e = gen->wake_primed ? gen->wake_e ^ 1 : gen->wake_e;
-        ocean::WakeFreeSurfaceArgs f{};
-        f.h = wake_field(gen, gen->wake_h);
-        f.e = gen->wake_snapshots.ptr + e * cells;
-        f.e_old = gen->wake_primed ? nullptr : gen->wake_snapshots.ptr + (e ^ 1) * cells;
-        f.sources = a.sources;
-        f.states = a.states;
-        f.num_sources = a.num_sources;
-        f.num_states = a.num_states;
-        f.n = n;
-        f.cell = a.cell;
-        f.x0 = a.x0;
-        f.z0 = a.z0;
-        f.tau = (float)substeps * h;
-        if (masked)
-            OCEAN_CUDA(ocean::launch_wake_free_surface_obstacles(f, ob, gen->stream));
-        else
-            OCEAN_CUDA(ocean::launch_wake_free_surface(f, gen->stream));
+        const int e = w.primed ? w.e ^ 1 : w.e;
+        ocean::WakeFreeSurfaceArgs fs{};
+        fs.h = w.field(w.h);
+        fs.e = w.snapshot(e);
+        fs.e_old = w.primed ? nullptr : w.snapshot(e ^ 1);
+        fs.sources = a.sources;
+        fs.states = a.states;
+        fs.num_sources = a.num_sources;
+        fs.num_states = a.num_states;
+        fs.n = n;
+        fs.cell = a.cell;
+        fs.x0 = a.x0;
+        fs.z0 = a.z0;
+        fs.tau = (float)substeps * h;
+        OCEAN_CUDA(ocean::launch_wake_free_surface(fs, obstacles, gen->stream));
         gen->kernel_launches += 1;
         for (int k = 0; k < 2; ++k) {
-            if (k != e && gen->wake_primed) continue;
-            gen->wake_snapshot_origin[k][0] = origin_x;
-            gen->wake_snapshot_origin[k][1] = origin_z;
+            if (k != e && w.primed) continue;
+            w.snapshot_origin[k][0] = origin_x;
+            w.snapshot_origin[k][1] = origin_z;
         }
-        gen->wake_e = e;
-        gen->wake_interval = f.tau;
-        gen->wake_primed = true;
+        w.e = e;
+        w.interval = fs.tau;
+        w.primed = true;
     }
     return OCEAN_OK;
 }
@@ -2256,14 +2230,13 @@ int ocean_wake_render_map(ocean_generator* gen, void* map_dev, float* world_rect
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
     if (!map_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "map_dev is NULL");
-    const ocean_wake_params& p = gen->wake;
-    const float* foam = gen->wake_foam_on ? wake_foam_field(gen, gen->wake_f) : nullptr;
-    OCEAN_CUDA(ocean::launch_wake_map(wake_field(gen, gen->wake_h), foam, p.size, p.cell_size, map_dev, gen->stream));
+    const ocean::WakeRead r = gen->wake.read_h();
+    OCEAN_CUDA(ocean::launch_wake_map(r, map_dev, gen->stream));
     gen->kernel_launches += 1;
     if (world_rect) {
-        world_rect[0] = wake_corner(gen->wake_origin[0], p.cell_size);
-        world_rect[1] = wake_corner(gen->wake_origin[1], p.cell_size);
-        world_rect[2] = world_rect[3] = (float)p.size * p.cell_size;
+        world_rect[0] = r.x0;
+        world_rect[1] = r.z0;
+        world_rect[2] = world_rect[3] = (float)r.n * r.cell;
     }
     return OCEAN_OK;
 }
@@ -2274,10 +2247,7 @@ int ocean_sample_wake_device(ocean_generator* gen, int num_points, const float* 
     if ((rc = check_wake_layer(gen))) return rc;
     if ((rc = check_wake_points(num_points, points_xz_dev, out_dev))) return rc;
     if (num_points == 0) return OCEAN_OK;
-    const ocean_wake_params& p = gen->wake;
-    OCEAN_CUDA(ocean::launch_wake_sample(wake_field(gen, gen->wake_h), p.size, p.cell_size, wake_corner(gen->wake_origin[0], p.cell_size),
-                                         wake_corner(gen->wake_origin[1], p.cell_size), reinterpret_cast<const float2*>(points_xz_dev),
-                                         num_points, out_dev, gen->stream));
+    OCEAN_CUDA(ocean::launch_wake_sample(gen->wake.read_h(), reinterpret_cast<const float2*>(points_xz_dev), num_points, out_dev, gen->stream));
     gen->kernel_launches += 1;
     return OCEAN_OK;
 }
@@ -2300,12 +2270,12 @@ int ocean_wake_get_state(ocean_generator* gen, float* h_host, float* h_prev_host
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
     if (!h_host || !h_prev_host || !origin_xz) return fail(OCEAN_ERR_INVALID_ARGUMENT, "NULL argument");
-    const size_t bytes = sizeof(float) * gen->wake.size * gen->wake.size;
-    OCEAN_CUDA(cudaMemcpyAsync(h_host, wake_field(gen, gen->wake_h), bytes, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(h_prev_host, wake_field(gen, gen->wake_hp), bytes, cudaMemcpyDeviceToHost, gen->stream));
+    const WakeLayer& w = gen->wake;
+    OCEAN_CUDA(cudaMemcpyAsync(h_host, w.field(w.h), sizeof(float) * w.cells(), cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(h_prev_host, w.field(w.hp), sizeof(float) * w.cells(), cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    origin_xz[0] = gen->wake_origin[0];
-    origin_xz[1] = gen->wake_origin[1];
+    origin_xz[0] = w.origin[0];
+    origin_xz[1] = w.origin[1];
     return OCEAN_OK;
 }
 
@@ -2314,13 +2284,13 @@ int ocean_wake_set_state(ocean_generator* gen, const float* h_host, const float*
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
     if (!h_host || !h_prev_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "NULL argument");
-    const size_t bytes = sizeof(float) * gen->wake.size * gen->wake.size;
-    OCEAN_CUDA(cudaMemcpyAsync(wake_field(gen, gen->wake_h), h_host, bytes, cudaMemcpyHostToDevice, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(wake_field(gen, gen->wake_hp), h_prev_host, bytes, cudaMemcpyHostToDevice, gen->stream));
+    WakeLayer& w = gen->wake;
+    OCEAN_CUDA(cudaMemcpyAsync(w.field(w.h), h_host, sizeof(float) * w.cells(), cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(w.field(w.hp), h_prev_host, sizeof(float) * w.cells(), cudaMemcpyHostToDevice, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    gen->wake_origin[0] = origin_x;
-    gen->wake_origin[1] = origin_z;
-    gen->wake_primed = false;                           // the snapshots no longer describe the layer
+    w.origin[0] = origin_x;
+    w.origin[1] = origin_z;
+    w.primed = false;                                   // the snapshots no longer describe the layer
     return OCEAN_OK;
 }
 
@@ -2329,11 +2299,9 @@ int ocean_wake_set_coupling(ocean_generator* gen, int enable) {
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
     if (enable != 0 && enable != 1) return fail(OCEAN_ERR_INVALID_ARGUMENT, "enable %d is not 0 or 1", enable);
-    if (!enable) return wake_uncouple(gen);
-    if (gen->wake_coupled) return OCEAN_OK;
-    OCEAN_CUDA(gen->wake_snapshots.grow(gen, 2 * (size_t)gen->wake.size * gen->wake.size));
-    gen->wake_coupled = true;
-    gen->wake_primed = false;
+    if (!enable) return gen->wake.off(gen, kWakeCoupling);
+    if (gen->wake.coupled()) return OCEAN_OK;
+    OCEAN_CUDA(gen->wake.snapshots.grow(gen, 2 * gen->wake.cells()));   // unprimed: nothing reads them before a step
     return OCEAN_OK;
 }
 
@@ -2341,25 +2309,26 @@ int ocean_wake_get_coupling(ocean_generator* gen, float* e_host, float* e_old_ho
     OCEAN_ENTER(gen);
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
-    if (!gen->wake_coupled) return fail(OCEAN_ERR_STATE, "the wake layer's coupling is off (ocean_wake_set_coupling)");
+    const WakeLayer& w = gen->wake;
+    if (!w.coupled()) return fail(OCEAN_ERR_STATE, "the wake layer's coupling is off (ocean_wake_set_coupling)");
     if (!e_host || !e_old_host || !origins || !interval) return fail(OCEAN_ERR_INVALID_ARGUMENT, "NULL argument");
-    const size_t cells = (size_t)gen->wake.size * gen->wake.size;
-    if (!gen->wake_primed) {
+    const size_t cells = w.cells();
+    if (!w.primed) {
         std::fill(e_host, e_host + cells, 0.0f);
         std::fill(e_old_host, e_old_host + cells, 0.0f);
         std::fill(origins, origins + 4, (int64_t)0);
         *interval = 0.0f;
         return OCEAN_OK;
     }
-    const int e = gen->wake_e, o = e ^ 1;
-    OCEAN_CUDA(cudaMemcpyAsync(e_host, gen->wake_snapshots.ptr + e * cells, sizeof(float) * cells, cudaMemcpyDeviceToHost, gen->stream));
-    OCEAN_CUDA(cudaMemcpyAsync(e_old_host, gen->wake_snapshots.ptr + o * cells, sizeof(float) * cells, cudaMemcpyDeviceToHost, gen->stream));
+    const int e = w.e, o = e ^ 1;
+    OCEAN_CUDA(cudaMemcpyAsync(e_host, w.snapshot(e), sizeof(float) * cells, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(e_old_host, w.snapshot(o), sizeof(float) * cells, cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    origins[0] = gen->wake_snapshot_origin[e][0];
-    origins[1] = gen->wake_snapshot_origin[e][1];
-    origins[2] = gen->wake_snapshot_origin[o][0];
-    origins[3] = gen->wake_snapshot_origin[o][1];
-    *interval = gen->wake_interval;
+    origins[0] = w.snapshot_origin[e][0];
+    origins[1] = w.snapshot_origin[e][1];
+    origins[2] = w.snapshot_origin[o][0];
+    origins[3] = w.snapshot_origin[o][1];
+    *interval = w.interval;
     return OCEAN_OK;
 }
 
@@ -2367,21 +2336,21 @@ int ocean_wake_set_foam(ocean_generator* gen, const ocean_wake_foam_params* para
     OCEAN_ENTER(gen);
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
-    if (!params) return wake_foam_off(gen);
+    WakeLayer& w = gen->wake;
+    if (!params) return w.off(gen, kWakeFoam);
     const ocean_wake_foam_params p = *params;
     if (!std::isfinite(p.whitecap) || !std::isfinite(p.grow_rate) || !std::isfinite(p.stir_rate) || !std::isfinite(p.decay_rate))
         return fail(OCEAN_ERR_INVALID_ARGUMENT, "foam parameters not finite");
     if (!(p.grow_rate >= 0.0f) || !(p.stir_rate >= 0.0f) || !(p.decay_rate >= 0.0f))
         return fail(OCEAN_ERR_INVALID_ARGUMENT, "grow_rate %g, stir_rate %g or decay_rate %g is negative", p.grow_rate, p.stir_rate,
                     p.decay_rate);
-    if (!gen->wake_foam_on) {
-        const size_t cells = (size_t)gen->wake.size * gen->wake.size;
-        OCEAN_CUDA(gen->wake_foam.grow(gen, 2 * cells));
-        OCEAN_CUDA(cudaMemsetAsync(gen->wake_foam.ptr, 0, 2 * cells * sizeof(float), gen->stream));
-        gen->wake_f = 0;
-        gen->wake_foam_on = true;
+    if (!w.foamed()) {
+        OCEAN_CUDA(w.foam.grow(gen, 2 * w.cells()));
+        const cudaError_t e = cudaMemsetAsync(w.foam.ptr, 0, 2 * w.cells() * sizeof(float), gen->stream);
+        if ((rc = wake_part_setup(gen, kWakeFoam, e, "clearing the foam"))) return rc;
+        w.f = 0;
     }
-    gen->wake_foam_params = p;
+    w.foam_params = p;
     return OCEAN_OK;
 }
 
@@ -2390,7 +2359,8 @@ int ocean_wake_set_obstacles(ocean_generator* gen, const uint8_t* mask_host, int
     OCEAN_ENTER(gen);
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
-    if (!mask_host && width == 0 && depth == 0) return wake_obstacles_off(gen);
+    WakeLayer& w = gen->wake;
+    if (!mask_host && width == 0 && depth == 0) return w.off(gen, kWakeMask);
     if (!mask_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "mask_host is NULL with width %d, depth %d", width, depth);
     if (width < 1 || depth < 1) return fail(OCEAN_ERR_INVALID_ARGUMENT, "mask size %d x %d is not at least 1 x 1", width, depth);
     if ((int64_t)width * depth > ((int64_t)1 << 28))
@@ -2398,17 +2368,18 @@ int ocean_wake_set_obstacles(ocean_generator* gen, const uint8_t* mask_host, int
     if (origin_x > INT64_MAX - width || origin_z > INT64_MAX - depth)
         return fail(OCEAN_ERR_INVALID_ARGUMENT, "mask origin + size not representable in int64");
     const size_t cells = (size_t)width * depth;
-    if (gen->wake_mask.capacity != cells) {
-        if ((rc = wake_obstacles_off(gen))) return rc;
-        OCEAN_CUDA(gen->wake_mask.grow(gen, cells));
+    if (w.mask.capacity != cells) {
+        if ((rc = w.off(gen, kWakeMask))) return rc;
+        OCEAN_CUDA(w.mask.grow(gen, cells));
     }
     // stream order puts the copy after the steps that read the old mask; the call returns once the copy is done
-    OCEAN_CUDA(cudaMemcpyAsync(gen->wake_mask.ptr, mask_host, cells, cudaMemcpyHostToDevice, gen->stream));
-    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    gen->wake_mask_size[0] = width;
-    gen->wake_mask_size[1] = depth;
-    gen->wake_mask_origin[0] = origin_x;
-    gen->wake_mask_origin[1] = origin_z;
+    cudaError_t e = cudaMemcpyAsync(w.mask.ptr, mask_host, cells, cudaMemcpyHostToDevice, gen->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(gen->stream);
+    if ((rc = wake_part_setup(gen, kWakeMask, e, "copying the mask"))) return rc;
+    w.mask_size[0] = width;
+    w.mask_size[1] = depth;
+    w.mask_origin[0] = origin_x;
+    w.mask_origin[1] = origin_z;
     return OCEAN_OK;
 }
 
@@ -2417,7 +2388,7 @@ int ocean_wake_set_readers(ocean_generator* gen, uint32_t readers) {
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
     if (readers & ~(OCEAN_WAKE_READ_RAYCAST | OCEAN_WAKE_READ_SPRAY)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "readers 0x%x: unknown bits", readers);
-    gen->wake_readers = readers;
+    gen->wake.readers = readers;
     return OCEAN_OK;
 }
 
@@ -2425,10 +2396,10 @@ int ocean_wake_get_foam_state(ocean_generator* gen, float* foam_host) {
     OCEAN_ENTER(gen);
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
-    if (!gen->wake_foam_on) return fail(OCEAN_ERR_STATE, "the wake layer's foam is off (ocean_wake_set_foam)");
+    const WakeLayer& w = gen->wake;
+    if (!w.foamed()) return fail(OCEAN_ERR_STATE, "the wake layer's foam is off (ocean_wake_set_foam)");
     if (!foam_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "foam_host is NULL");
-    const size_t bytes = sizeof(float) * gen->wake.size * gen->wake.size;
-    OCEAN_CUDA(cudaMemcpyAsync(foam_host, wake_foam_field(gen, gen->wake_f), bytes, cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(foam_host, w.foam_field(w.f), sizeof(float) * w.cells(), cudaMemcpyDeviceToHost, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }
@@ -2437,10 +2408,10 @@ int ocean_wake_set_foam_state(ocean_generator* gen, const float* foam_host) {
     OCEAN_ENTER(gen);
     if (rc) return rc;
     if ((rc = check_wake_layer(gen))) return rc;
-    if (!gen->wake_foam_on) return fail(OCEAN_ERR_STATE, "the wake layer's foam is off (ocean_wake_set_foam)");
+    const WakeLayer& w = gen->wake;
+    if (!w.foamed()) return fail(OCEAN_ERR_STATE, "the wake layer's foam is off (ocean_wake_set_foam)");
     if (!foam_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "foam_host is NULL");
-    const size_t bytes = sizeof(float) * gen->wake.size * gen->wake.size;
-    OCEAN_CUDA(cudaMemcpyAsync(wake_foam_field(gen, gen->wake_f), foam_host, bytes, cudaMemcpyHostToDevice, gen->stream));
+    OCEAN_CUDA(cudaMemcpyAsync(w.foam_field(w.f), foam_host, sizeof(float) * w.cells(), cudaMemcpyHostToDevice, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
 }

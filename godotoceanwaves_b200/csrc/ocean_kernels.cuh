@@ -131,9 +131,10 @@ cudaError_t launch_sample_maps(const DeviceBuffers& b, int num_cascades, const f
 size_t surface_scratch_ints(int num_cascades, int n);
 cudaError_t launch_query_surface(const DeviceBuffers& b, int num_cascades, const float2* points_dev, int n, const float4* scales_dev,
                                  float tolerance, int max_iterations, ocean_surface_sample* out_dev, int* scratch_dev, cudaStream_t stream);
-// A wake field the ray cast or spray reads (ocean_wake_set_readers; oracle/wake_readers.py): field and foam are [n][n]
-// binary32 in the window at world corner (x0, z0), sampled as ocean_sample_wake (0 outside).  The ray cast reads the
-// coupling's free surface e in `field`; spray reads h in `field` and F in `foam` (null while wake foam is off: F reads +0).
+// A wake field the ray cast, spray, render map or sample reads (ocean_wake_set_readers; oracle/wake_readers.py): field and
+// foam are [n][n] binary32 in the window at world corner (x0, z0), sampled as ocean_sample_wake (0 outside).  The ray cast
+// reads the coupling's free surface e in `field`; the others read h in `field` and F in `foam` (null while wake foam is off:
+// F reads +0).
 struct WakeRead {
     const float* field;
     const float* foam;
@@ -234,10 +235,6 @@ struct WakeObstacles {
     int width, depth;
     int qx, qz;
 };
-cudaError_t launch_wake_step(const WakeStepArgs& args, cudaStream_t stream);
-// The obstacle forms of the sub-step, the foam sub-step and the free surface: blocked cells read s = 0 and are written 0
-// (h, F and e); h_prev is written unmasked.
-cudaError_t launch_wake_step_obstacles(const WakeStepArgs& args, const WakeObstacles& obstacles, cudaStream_t stream);
 // The foam sub-step (ocean_wake_set_foam; oracle/wake_foam.py): the sub-step of `step`, and F ([n][n], read at (i + di, j + dj),
 // 0 outside) advanced to out_foam (another [n][n] field) with the call's constants.
 struct WakeFoamStepArgs {
@@ -248,12 +245,12 @@ struct WakeFoamStepArgs {
     float decay;                                    // d = exp(-decay_rate h)
     float grow, stir;                               // grow_rate h, stir_rate h
 };
-cudaError_t launch_wake_step_foam(const WakeFoamStepArgs& args, cudaStream_t stream);
-cudaError_t launch_wake_step_foam_obstacles(const WakeFoamStepArgs& args, const WakeObstacles& obstacles, cudaStream_t stream);
-// map_dev = [n][n][4] half (h, dh/dx, dh/dz, F), F = foam_dev or 0 when foam_dev is null; out_dev = [count][3] floats
-cudaError_t launch_wake_map(const float* h_dev, const float* foam_dev, int n, float cell, void* map_dev, cudaStream_t stream);
-cudaError_t launch_wake_sample(const float* h_dev, int n, float cell, float x0, float z0, const float2* xz_dev, int count, float* out_dev,
-                               cudaStream_t stream);
+// One sub-step of args; with foam not null the foam sub-step (foam->step is replaced by args), with obstacles not null the
+// obstacle form: blocked cells read s = 0 and are written 0 (h and F; h_prev is written unmasked).
+cudaError_t launch_wake_step(const WakeStepArgs& args, const WakeFoamStepArgs* foam, const WakeObstacles* obstacles, cudaStream_t stream);
+// map_dev = [n][n][4] half (h, dh/dx, dh/dz, F) of wake.field and wake.foam (F = 0 when it is null); out_dev = [count][3] floats
+cudaError_t launch_wake_map(const WakeRead& wake, void* map_dev, cudaStream_t stream);
+cudaError_t launch_wake_sample(const WakeRead& wake, const float2* xz_dev, int count, float* out_dev, cudaStream_t stream);
 // The coupling (ocean_wake_set_coupling; oracle/wake_coupling.py).  free_surface: e = h + phi of the sources at tau (the end
 // of the step call) in the window at corner (x0, z0), into e, and into e_old when it is not null (a priming call).
 struct WakeFreeSurfaceArgs {
@@ -266,8 +263,8 @@ struct WakeFreeSurfaceArgs {
     int n;
     float cell, x0, z0, tau;
 };
-cudaError_t launch_wake_free_surface(const WakeFreeSurfaceArgs& args, cudaStream_t stream);
-cudaError_t launch_wake_free_surface_obstacles(const WakeFreeSurfaceArgs& args, const WakeObstacles& obstacles, cudaStream_t stream);
+// With obstacles not null, e = 0 on blocked cells.
+cudaError_t launch_wake_free_surface(const WakeFreeSurfaceArgs& args, const WakeObstacles* obstacles, cudaStream_t stream);
 // The snapshots e and e_old ([n][n]) with their window corners, and the interval T between them.
 struct WakeCoupleArgs {
     const float* e;

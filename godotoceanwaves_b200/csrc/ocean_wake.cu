@@ -417,55 +417,46 @@ void wake_kernel_taps(float* out) {
     for (int t = 0; t < 28; ++t) out[t] = wake_tap(t);
 }
 
-cudaError_t launch_wake_step(const WakeStepArgs& args, cudaStream_t stream) {
+cudaError_t launch_wake_step(const WakeStepArgs& args, const WakeFoamStepArgs* foam, const WakeObstacles* obstacles, cudaStream_t stream) {
     const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
-    k_wake_step<<<grid, kThreads, 0, stream>>>(args);
+    if (foam) {
+        WakeFoamStepArgs f = *foam;
+        f.step = args;
+        if (obstacles)
+            k_wake_step_foam_obstacles<<<grid, kThreads, 0, stream>>>(f, *obstacles);
+        else
+            k_wake_step_foam<<<grid, kThreads, 0, stream>>>(f);
+    } else if (obstacles) {
+        k_wake_step_obstacles<<<grid, kThreads, 0, stream>>>(args, *obstacles);
+    } else {
+        k_wake_step<<<grid, kThreads, 0, stream>>>(args);
+    }
     return cudaGetLastError();
 }
 
-cudaError_t launch_wake_step_foam(const WakeFoamStepArgs& args, cudaStream_t stream) {
-    const dim3 grid((unsigned)(args.step.n / kTile), (unsigned)(args.step.n / kTile));
-    k_wake_step_foam<<<grid, kThreads, 0, stream>>>(args);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_wake_free_surface(const WakeFreeSurfaceArgs& args, cudaStream_t stream) {
+cudaError_t launch_wake_free_surface(const WakeFreeSurfaceArgs& args, const WakeObstacles* obstacles, cudaStream_t stream) {
     const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
-    k_wake_free_surface<<<grid, kThreads, 0, stream>>>(args);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_wake_step_obstacles(const WakeStepArgs& args, const WakeObstacles& obstacles, cudaStream_t stream) {
-    const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
-    k_wake_step_obstacles<<<grid, kThreads, 0, stream>>>(args, obstacles);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_wake_step_foam_obstacles(const WakeFoamStepArgs& args, const WakeObstacles& obstacles, cudaStream_t stream) {
-    const dim3 grid((unsigned)(args.step.n / kTile), (unsigned)(args.step.n / kTile));
-    k_wake_step_foam_obstacles<<<grid, kThreads, 0, stream>>>(args, obstacles);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_wake_free_surface_obstacles(const WakeFreeSurfaceArgs& args, const WakeObstacles& obstacles, cudaStream_t stream) {
-    const dim3 grid((unsigned)(args.n / kTile), (unsigned)(args.n / kTile));
-    k_wake_free_surface_obstacles<<<grid, kThreads, 0, stream>>>(args, obstacles);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_wake_map(const float* h_dev, const float* foam_dev, int n, float cell, void* map_dev, cudaStream_t stream) {
-    const unsigned blocks = (unsigned)(((size_t)n * n + 255) / 256);
-    if (foam_dev)
-        k_wake_map_foam<<<blocks, 256, 0, stream>>>(h_dev, foam_dev, n, 2.0f * cell, static_cast<__half2*>(map_dev));
+    if (obstacles)
+        k_wake_free_surface_obstacles<<<grid, kThreads, 0, stream>>>(args, *obstacles);
     else
-        k_wake_map<<<blocks, 256, 0, stream>>>(h_dev, n, 2.0f * cell, static_cast<__half2*>(map_dev));    // exact
+        k_wake_free_surface<<<grid, kThreads, 0, stream>>>(args);
     return cudaGetLastError();
 }
 
-cudaError_t launch_wake_sample(const float* h_dev, int n, float cell, float x0, float z0, const float2* xz_dev, int count, float* out_dev,
-                               cudaStream_t stream) {
+cudaError_t launch_wake_map(const WakeRead& wake, void* map_dev, cudaStream_t stream) {
+    const int n = wake.n;
+    const unsigned blocks = (unsigned)(((size_t)n * n + 255) / 256);
+    if (wake.foam)
+        k_wake_map_foam<<<blocks, 256, 0, stream>>>(wake.field, wake.foam, n, 2.0f * wake.cell, static_cast<__half2*>(map_dev));
+    else
+        k_wake_map<<<blocks, 256, 0, stream>>>(wake.field, n, 2.0f * wake.cell, static_cast<__half2*>(map_dev));    // exact
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wake_sample(const WakeRead& wake, const float2* xz_dev, int count, float* out_dev, cudaStream_t stream) {
     if (count <= 0) return cudaSuccess;
-    k_wake_sample<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(h_dev, n, cell, x0, z0, xz_dev, count, out_dev);
+    k_wake_sample<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(wake.field, wake.n, wake.cell, wake.x0, wake.z0, xz_dev, count,
+                                                                         out_dev);
     return cudaGetLastError();
 }
 
