@@ -89,6 +89,37 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanSeaState                              // struct ocean_sea_state (144 B)
+    {
+        public double m_minus1, m0, m1, m2;                         // spectral moments
+        public fixed double direction[2];                           // sum E d, world (x, z)
+        public fixed double slope[2];                               // sum E kx^2, sum E kz^2
+        public fixed double stokes[2];                              // surface Stokes drift, m/s
+        public double significant_wave_height, mean_period, zero_crossing_period, energy_period;
+        public double mean_direction;                               // degrees, wind_direction's convention
+        public double directional_spread;                           // radians
+        public double mean_square_slope, stokes_speed;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public struct OceanDrifter                                      // struct ocean_drifter (40 B)
+    {
+        public double x, z;                                         // the label: undisplaced point P
+        public float yaw, yaw_rate;                                 // radians, rad/s
+        public float windage, tilt, offset, scale;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanDriftParams                           // struct ocean_drift_params (56 B)
+    {
+        public fixed float current[2];                              // m/s, world x and z
+        public fixed float wind[2];                                 // m/s, world x and z
+        public float stokes_scale;                                  // 1 physical, 0 off
+        public uint flags;                                          // OCEAN_DRIFT_WRAP (1) | OCEAN_DRIFT_READ_WAKE (2)
+        public fixed double box[4];                                 // wrap box (x0, z0, width, depth)
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public unsafe struct OceanSurfaceSample                         // struct ocean_surface_sample (40 B) <- water.gdshader:28,37 inverted
     {
         public float source_x, source_z;
@@ -300,6 +331,17 @@ namespace OceanB200
         // wake readers: OCEAN_WAKE_READ_RAYCAST (1) makes the ray cast hit the coupled surface, OCEAN_WAKE_READ_SPRAY (2) lets spray read h and F
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_wake_set_readers(IntPtr handle, uint readers);
+        // sea state: per-cascade moments (may be null) and the total under map_scales[num_cascades][4] (synchronous)
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_get_sea_state(IntPtr handle, int num_cascades, float* map_scales, OceanSeaState* per_cascade,
+                                                        OceanSeaState* total);
+        // drifters: advance by dt (0 only renders) and write 12-float MultiMesh instances (may be null)
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_drift(IntPtr handle, double dt, OceanDriftParams* parameters, int num_drifters, OceanDrifter* drifters,
+                                                int num_cascades, float* map_scales, float* instances);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_drift_device(IntPtr handle, double dt, OceanDriftParams* parameters, int num_drifters, IntPtr drifters_dev,
+                                                       int num_cascades, float* map_scales, IntPtr instances_dev);
         // surface query: the surface at world positions points [n][2] (P + D_xz(P) = Q solved for P, then the map query at P)
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_query_surface(IntPtr handle, int num_points, float* points_xz, int num_cascades, float* map_scales,

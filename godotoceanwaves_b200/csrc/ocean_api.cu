@@ -65,7 +65,7 @@ struct DeviceArray {
 // The host entry points that stage the caller's arrays, one staging block each (ocean_generator::staging, see Staging).
 enum StagedOp {
     kStageSampleMaps, kStageExtractSpray, kStageSprayParticles, kStageQuerySurface, kStageRaycast, kStageBuoyancy,
-    kStageSampleVelocity, kStageBodyForces, kStageSimulateBodies, kStageDeviceMath, kStageWakeStep, kStageSampleWake,
+    kStageSampleVelocity, kStageBodyForces, kStageSimulateBodies, kStageDeviceMath, kStageWakeStep, kStageSampleWake, kStageDrift,
     kNumStagedOps
 };
 
@@ -186,6 +186,11 @@ struct ocean_generator {
     std::vector<ocean::VelocityDispatch> vel_source;    // [num_cascades] table slot and time of the update that built the current maps
     std::vector<char> vel_has_source;                   // the cascade's maps were written at least once
     std::vector<char> vel_stale;                        // its velocity layer does not describe its current maps yet
+    // the sea-state cache, allocated by the first sea-state or drift call: per cascade the moments (zero until computed) and
+    // whether they describe its current spectrum and dispersion table; partial = the reduction's block sums
+    DeviceArray<double> sea_moments;                    // [num_cascades][kSeaStateMoments]
+    DeviceArray<double> sea_partial;
+    std::vector<char> sea_stale;
     DeviceArray<ocean::CascadeDispatch> d_cascade;      // [num_cascades] (two-kernel path only)
     DeviceArray<ocean::SpectrumDispatch> d_spectrum;    // [num_cascades]
     DeviceArray<ocean::TableDispatch> d_tables;         // [num_cascades]
@@ -444,6 +449,7 @@ int assign_table_slot(ocean_generator* g, int i, const ocean_cascade_params& p, 
     };
     int cur = g->cascade_slot[i];
     if (cur >= 0 && g->slot_valid[cur] && same(g->slot_key[cur])) return cur;
+    g->sea_stale[i] = 1;                                                    // the sea state reads the cascade's table
     if (cur >= 0) {
         g->slot_refs[cur] -= 1;
         g->cascade_slot[i] = -1;
@@ -491,7 +497,10 @@ int run_cascades(ocean_generator* g, const int* indices, int n) {
     for (int k = 0; k < n; ++k) {
         const int i = indices[k];
         const ocean_cascade_params& p = g->pass_parameters[i];
-        if (p.should_generate_spectrum) hs[n_dirty++] = make_spectrum_dispatch(p, i);   // :68-72
+        if (p.should_generate_spectrum) {
+            hs[n_dirty++] = make_spectrum_dispatch(p, i);   // :68-72
+            g->sea_stale[i] = 1;
+        }
         const int ts = assign_table_slot(g, i, p, ht, &n_tables);
         if (ts < 0) return fail(OCEAN_ERR_STATE, "no free dispersion-table slot (internal error)");
         hc[k] = make_cascade_dispatch(p, i, ts);                     // :73,85
@@ -707,6 +716,7 @@ int ocean_create(int device, int map_size, int num_cascades, ocean_generator** o
     g->vel_source.assign(C, ocean::VelocityDispatch{0, 0, 0.0f});
     g->vel_has_source.assign(C, 0);
     g->vel_stale.assign(C, 0);
+    g->sea_stale.assign(C, 0);
     for (int i = 0; i < C; ++i) g->scratch_layer_of[i] = 2 * i;
     CREATE_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&g->h_cascade), sizeof(ocean::CascadeDispatch) * kRing * C, cudaHostAllocDefault));
     CREATE_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&g->h_spectrum), sizeof(ocean::SpectrumDispatch) * kRing * C, cudaHostAllocDefault));
@@ -1071,6 +1081,7 @@ int ocean_set_spectrum_amplitudes(ocean_generator* gen, int cascade, const float
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     OCEAN_CUDA(cudaMemcpy(gen->buf.spectrum + (size_t)cascade * N * N, tex.data(), sizeof(float) * tex.size(), cudaMemcpyHostToDevice));
     if (gen->vel_has_source[cascade]) gen->vel_stale[cascade] = 1;       // the velocity layer reads the spectrum as stored
+    gen->sea_stale[cascade] = 1;                                         // and so does the sea state
     return OCEAN_OK;
 }
 
@@ -2414,6 +2425,130 @@ int ocean_wake_set_foam_state(ocean_generator* gen, const float* foam_host) {
     OCEAN_CUDA(cudaMemcpyAsync(w.foam_field(w.f), foam_host, sizeof(float) * w.cells(), cudaMemcpyHostToDevice, gen->stream));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
     return OCEAN_OK;
+}
+
+// ---- sea state and drifters (ocean_drift.cu; oracle/sea_state.py, oracle/drifters.py) ----
+namespace {
+// Allocates the cache on first use, zeroed, then recomputes every stale cascade that has a dispersion table in one launch
+// sequence.  A cascade without a table has never been updated: it keeps zero moments and stays stale until it gets one.
+// The cache is allocated whole or not at all: a failure releases both buffers, so the next call starts over.
+int refresh_sea_state(ocean_generator* gen) {
+    if (!gen->sea_moments.ptr || !gen->sea_partial.ptr) {
+        const size_t n = (size_t)gen->num_cascades * ocean::kSeaStateMoments;
+        const int per_launch = std::min(gen->num_cascades, ocean::kMaxSeaStateLaunch);
+        cudaError_t e = gen->sea_moments.grow(gen, n);
+        if (e == cudaSuccess) e = cudaMemsetAsync(gen->sea_moments.ptr, 0, sizeof(double) * n, gen->stream);
+        if (e == cudaSuccess) e = gen->sea_partial.grow(gen, (size_t)per_launch * ocean::sea_state_blocks(gen->map_size) * ocean::kSeaStateMoments);
+        if (e != cudaSuccess) {
+            gen->sea_moments.release();
+            gen->sea_partial.release();
+            return fail(OCEAN_ERR_CUDA, "sea-state cache allocation failed: %s", cudaGetErrorString(e));
+        }
+    }
+    std::vector<ocean::SeaStateJob> jobs;
+    for (int i = 0; i < gen->num_cascades; ++i)
+        if (gen->sea_stale[i] && gen->cascade_slot[i] >= 0) jobs.push_back(ocean::SeaStateJob{i, gen->cascade_slot[i]});
+    if (jobs.empty()) return OCEAN_OK;
+    int launched = 0;
+    OCEAN_CUDA(ocean::launch_sea_state(gen->buf, jobs.data(), (int)jobs.size(), gen->sea_partial.ptr, gen->sea_moments.ptr, gen->stream,
+                                       &launched));
+    gen->kernel_launches += (uint64_t)launched;
+    for (const auto& j : jobs) gen->sea_stale[j.cascade] = 0;
+    return OCEAN_OK;
+}
+
+// The record of moments m (ocean::kSeaStateMoments, the device order) with its derived fields (include/ocean.h).
+ocean_sea_state sea_state_record(const double* m) {
+    ocean_sea_state s;
+    std::memset(&s, 0, sizeof s);
+    s.m_minus1 = m[0]; s.m0 = m[1]; s.m1 = m[2]; s.m2 = m[3];
+    s.direction[0] = m[4]; s.direction[1] = m[5];
+    s.slope[0] = m[6]; s.slope[1] = m[7];
+    s.stokes[0] = m[8]; s.stokes[1] = m[9];
+    if (s.m0 == 0.0) return s;
+    const double two_pi = 2.0 * M_PI;
+    s.significant_wave_height = 4.0 * std::sqrt(s.m0);
+    s.mean_period = two_pi * s.m0 / s.m1;
+    s.zero_crossing_period = two_pi * std::sqrt(s.m0 / s.m2);
+    s.energy_period = two_pi * s.m_minus1 / s.m0;
+    s.mean_direction = std::atan2(-s.direction[1], -s.direction[0]) * (180.0 / M_PI);
+    const double R = std::hypot(s.direction[0], s.direction[1]) / s.m0;
+    s.directional_spread = std::sqrt(2.0 * std::fmax(0.0, 1.0 - R));
+    s.mean_square_slope = s.slope[0] + s.slope[1];
+    s.stokes_speed = std::hypot(s.stokes[0], s.stokes[1]);
+    return s;
+}
+
+int check_drift_args(ocean_generator* gen, double dt, const ocean_drift_params* p, int num_drifters, const void* drifters, int num_cascades,
+                     const float* map_scales) {
+    if (!std::isfinite(dt) || !(dt >= 0.0)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "dt %g is not finite and >= 0", dt);
+    if (!p) return fail(OCEAN_ERR_INVALID_ARGUMENT, "params is NULL");
+    const float fs[5] = {p->current[0], p->current[1], p->wind[0], p->wind[1], p->stokes_scale};
+    for (float f : fs)
+        if (!std::isfinite(f)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a drift parameter (%g) is not finite", f);
+    for (double b : p->box)
+        if (!std::isfinite(b)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a box coordinate (%g) is not finite", b);
+    if (p->flags & ~(OCEAN_DRIFT_WRAP | OCEAN_DRIFT_READ_WAKE)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "flags 0x%x: unknown bits", p->flags);
+    if ((p->flags & OCEAN_DRIFT_WRAP) && !(p->box[2] > 0.0 && p->box[3] > 0.0))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "wrap box %g x %g: width and depth must be > 0", p->box[2], p->box[3]);
+    if (num_cascades < 1 || num_cascades > gen->num_cascades)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_cascades %d outside [1, %d]", num_cascades, gen->num_cascades);
+    if (!map_scales) return fail(OCEAN_ERR_INVALID_ARGUMENT, "map_scales is NULL");
+    if (num_drifters < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_drifters %d is negative", num_drifters);
+    if (num_drifters > 0 && !drifters) return fail(OCEAN_ERR_INVALID_ARGUMENT, "drifters is NULL");
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_get_sea_state(ocean_generator* gen, int num_cascades, const float* map_scales_host, ocean_sea_state* per_cascade_host,
+                    ocean_sea_state* total_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if (num_cascades < 1 || num_cascades > gen->num_cascades)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_cascades %d outside [1, %d]", num_cascades, gen->num_cascades);
+    if (!map_scales_host || !total_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "map_scales or total is NULL");
+    if ((rc = refresh_sea_state(gen))) return rc;
+    std::vector<double> m((size_t)num_cascades * ocean::kSeaStateMoments);
+    OCEAN_CUDA(cudaMemcpyAsync(m.data(), gen->sea_moments.ptr, sizeof(double) * m.size(), cudaMemcpyDeviceToHost, gen->stream));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    double total[ocean::kSeaStateMoments] = {};
+    for (int i = 0; i < num_cascades; ++i) {
+        const double* mi = m.data() + (size_t)i * ocean::kSeaStateMoments;
+        if (per_cascade_host) per_cascade_host[i] = sea_state_record(mi);
+        const double s = (double)map_scales_host[4 * (size_t)i + 2], s2 = s * s;
+        for (int k = 0; k < ocean::kSeaStateMoments; ++k) total[k] = total[k] + s2 * mi[k];
+    }
+    *total_host = sea_state_record(total);
+    return OCEAN_OK;
+}
+
+int ocean_drift_device(ocean_generator* gen, double dt, const ocean_drift_params* params, int num_drifters, ocean_drifter* drifters_dev,
+                       int num_cascades, const float* map_scales_host, float* instances_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_drift_args(gen, dt, params, num_drifters, drifters_dev, num_cascades, map_scales_host))) return rc;
+    if (num_drifters == 0) return OCEAN_OK;
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;
+    if (dt > 0.0 && (rc = refresh_sea_state(gen))) return rc;
+    const bool wk = instances_dev && (params->flags & OCEAN_DRIFT_READ_WAKE) && gen->wake.on();
+    const ocean::WakeRead wake = wk ? gen->wake.read_h() : ocean::WakeRead{};
+    OCEAN_CUDA(ocean::launch_drift(gen->buf, num_cascades, gen->q_scales.ptr, gen->sea_moments.ptr, *params, dt, drifters_dev, num_drifters,
+                                   instances_dev, wk ? &wake : nullptr, gen->stream));
+    gen->kernel_launches += 1;
+    return OCEAN_OK;
+}
+
+int ocean_drift(ocean_generator* gen, double dt, const ocean_drift_params* params, int num_drifters, ocean_drifter* drifters_host,
+                int num_cascades, const float* map_scales_host, float* instances_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    if ((rc = check_drift_args(gen, dt, params, num_drifters, drifters_host, num_cascades, map_scales_host))) return rc;
+    if (num_drifters == 0) return OCEAN_OK;
+    Staging st;
+    const auto drifters = st.inout(drifters_host, (size_t)num_drifters);
+    const auto instances = st.out(instances_host, 12 * (size_t)num_drifters);
+    if ((rc = st.upload(gen, kStageDrift))) return rc;
+    return st.finish(gen, ocean_drift_device(gen, dt, params, num_drifters, st[drifters], num_cascades, map_scales_host, st[instances]));
 }
 
 int ocean_get_info(ocean_generator* gen, ocean_info* out) {

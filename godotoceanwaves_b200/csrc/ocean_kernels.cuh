@@ -209,6 +209,25 @@ cudaError_t launch_spray_particles(const DeviceBuffers& b, int num_cascades, con
                                    double t0, double t1, ocean_spray_particle* states_dev, int* counts_dev, float* instances_dev,
                                    int max_instances, const WakeRead* wake, cudaStream_t stream);
 
+// ocean_drift.cu: the sea state (oracle/sea_state.py).  One job per cascade to recompute: its spectrum layer and the dispersion
+// table its updates use.  moments_dev = [num_cascades][kSeaStateMoments] binary64 (m-1, m0, m1, m2, sum E d.x, sum E d.z,
+// sum E kx^2, sum E kz^2, u_s.x, u_s.z); partial_dev = [min(count, kMaxSeaStateLaunch)][sea_state_blocks(N)][kSeaStateMoments]
+// of scratch.  Two launches per kMaxSeaStateLaunch jobs; *launched receives the number of kernels launched.
+struct SeaStateJob {
+    int32_t cascade;
+    int32_t table_slot;
+};
+constexpr int kSeaStateMoments = 10;
+constexpr int kMaxSeaStateLaunch = 256;
+int sea_state_blocks(int map_size);
+cudaError_t launch_sea_state(const DeviceBuffers& b, const SeaStateJob* jobs_host, int count, double* partial_dev, double* moments_dev,
+                             cudaStream_t stream, int* launched);
+// ocean_drift.cu: the drifters (oracle/drifters.py), one launch.  drifters_dev = [n] (advanced in place when dt > 0),
+// instances_dev = [n][12] floats or null (no render); wake (may be null) = the layer's h the render reads.
+cudaError_t launch_drift(const DeviceBuffers& b, int num_cascades, const float4* scales_dev, const double* moments_dev,
+                         const ocean_drift_params& params, double dt, ocean_drifter* drifters_dev, int n, float* instances_dev,
+                         const WakeRead* wake, cudaStream_t stream);
+
 // ocean_wake.cu: the wake layer (oracle/wake.py).  One sub-step of the layer: h / h_prev ([n][n], read at (i + di, j + dj),
 // 0 outside: the scroll folded into the reads) to out_h, and, when out_h_prev is not null, the scrolled h to out_h_prev.
 // a1..a3 are the per-ring coefficients, index min(cells to the window edge, sponge_cells).

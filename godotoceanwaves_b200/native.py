@@ -117,6 +117,9 @@ SIGNATURES = {
     "ocean_wake_set_foam_state": (C.c_int, [_H, C.c_void_p]),
     "ocean_wake_set_obstacles": (C.c_int, [_H, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int64]),
     "ocean_wake_set_readers": (C.c_int, [_H, C.c_uint32]),
+    "ocean_get_sea_state": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ocean_drift": (C.c_int, [_H, C.c_double, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ocean_drift_device": (C.c_int, [_H, C.c_double, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "ocean_get_foam_state": (C.c_int, [_H, C.c_int, C.c_void_p]),
     "ocean_set_foam_state": (C.c_int, [_H, C.c_int, C.c_void_p]),
     "ocean_jonswap_alpha": (C.c_double, [C.c_double, C.c_double]),

@@ -590,6 +590,53 @@ class WaveGenerator:
         readers = (1 if raycast else 0) | (2 if spray else 0)
         check(load_library().ocean_wake_set_readers(self.context, readers))
 
+    # -- sea state and drifters: the spectra's moments, and debris that rides the waves and drifts with the Stokes drift --
+    SEA_STATE = np.dtype([("m_minus1", np.float64), ("m0", np.float64), ("m1", np.float64), ("m2", np.float64),
+                          ("direction", np.float64, 2), ("slope", np.float64, 2), ("stokes", np.float64, 2),
+                          ("significant_wave_height", np.float64), ("mean_period", np.float64), ("zero_crossing_period", np.float64),
+                          ("energy_period", np.float64), ("mean_direction", np.float64), ("directional_spread", np.float64),
+                          ("mean_square_slope", np.float64), ("stokes_speed", np.float64)])      # struct ocean_sea_state
+    DRIFTER = np.dtype([("x", np.float64), ("z", np.float64), ("yaw", np.float32), ("yaw_rate", np.float32), ("windage", np.float32),
+                        ("tilt", np.float32), ("offset", np.float32), ("scale", np.float32)])   # struct ocean_drifter
+    DRIFT_PARAMS = np.dtype([("current", np.float32, 2), ("wind", np.float32, 2), ("stokes_scale", np.float32), ("flags", np.uint32),
+                             ("box", np.float64, 4)])                                            # struct ocean_drift_params
+    DRIFT_WRAP, DRIFT_READ_WAKE = 1, 2                                                           # OCEAN_DRIFT_*
+
+    def sea_state(self, map_scales):
+        """The sea state of the len(map_scales) first cascades (include/ocean.h, ocean_get_sea_state): (total, per_cascade),
+        a 0-d SEA_STATE of the surface as rendered (moments scaled by displacement_scale^2 and summed) and the unscaled
+        SEA_STATE of each cascade."""
+        self._require()
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        per = np.zeros(sc.shape[0], self.SEA_STATE)
+        total = np.zeros((), self.SEA_STATE)
+        check(load_library().ocean_get_sea_state(self.context, sc.shape[0], sc.ctypes.data, per.ctypes.data, total.ctypes.data))
+        return total, per
+
+    @staticmethod
+    def drift_params(current=(0.0, 0.0), wind=(0.0, 0.0), stokes_scale: float = 1.0, box=None, read_wake: bool = False) -> np.ndarray:
+        """A 0-d DRIFT_PARAMS: box = (x0, z0, width, depth) turns the wrap on; read_wake makes the render read the wake layer."""
+        p = np.zeros((), WaveGenerator.DRIFT_PARAMS)
+        p["current"] = current
+        p["wind"] = wind
+        p["stokes_scale"] = stokes_scale
+        p["flags"] = (WaveGenerator.DRIFT_WRAP if box is not None else 0) | (WaveGenerator.DRIFT_READ_WAKE if read_wake else 0)
+        if box is not None:
+            p["box"] = box
+        return p
+
+    def drift(self, drifters, dt: float, map_scales, params=None, render: bool = True):
+        """Advance the DRIFTER rows of `drifters` by dt (include/ocean.h, ocean_drift; dt = 0 only renders) under params
+        (a DRIFT_PARAMS, default drift_params()).  Returns (new drifters, instances [n][12] float32 or None without render)."""
+        self._require()
+        d = np.array(drifters, self.DRIFTER, copy=True).reshape(-1)
+        p = self.drift_params() if params is None else np.array(params, self.DRIFT_PARAMS).reshape(())
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        inst = np.zeros((len(d), 12), np.float32) if render else None
+        check(load_library().ocean_drift(self.context, float(dt), p.ctypes.data, len(d), d.ctypes.data, sc.shape[0], sc.ctypes.data,
+                                         None if inst is None else inst.ctypes.data))
+        return d, inst
+
     def twiddles_to_host(self) -> np.ndarray:
         self._require()
         out = np.empty((self.map_size - 1, 2), np.float32)

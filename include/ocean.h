@@ -806,6 +806,122 @@ int ocean_wake_set_obstacles(ocean_generator* gen, const uint8_t* mask_host, int
 #define OCEAN_WAKE_READ_SPRAY 2u        /* ocean_extract_spray[_device], ocean_spray_particles[_device] read h and F */
 int ocean_wake_set_readers(ocean_generator* gen, uint32_t readers);
 
+/* Sea state -- the statistics of the sea the cascades' spectra describe: wave height, periods, direction, slope and Stokes
+ * drift, for authoring parameters, driving audio and choosing the knobs other ops take (a ray cast's step against crest
+ * thickness, the wake layer's cell_size, query tolerances).  oracle/sea_state.py is the specification, bit for bit.
+ *   terms     per texel id of a cascade's spectrum texture as stored, A(id) = its .xy (each wave once), with the binary32
+ *             k_vec, k_unit and omega of the dispersion table its updates use (rows y > N/2 are the mirror of row N - y:
+ *             omega the same, k_vec and k_unit negated except k_vec.x and k_unit.x in column 0) and
+ *             k = sqrt(k_vec.x k_vec.x + k_vec.y k_vec.y) + 1e-6 (spectrum_modulate.glsl:60), in binary64:
+ *               E = 2 |A|^2 = 2 (A.x A.x + A.y A.y)   the texel's share of the height variance (the transform is
+ *                                                      unnormalised: one A of modulus a is a height cosine of amplitude 2a)
+ *               d = -(k_unit.y, k_unit.x)            world direction of travel (the maps are the transpose of the
+ *                                                      spectrum's field, and h0 e^{+i w t} under e^{+i k.x} travels along -k)
+ *               kw = (k_vec.y, k_vec.x)              world wave vector
+ *               q = ocean_detmath_expf(-((2 k) * 20)), F = (1 + q q) / ((1 - q)(1 - q)) = cosh 2kD / (2 sinh^2 kD) at the
+ *                                                      library's depth D = 20 m
+ *             moments (sums over the texels): m_minus1 = E / w, m0 = E, m1 = w E, m2 = (w w) E, direction = E d,
+ *             slope = (E kw.x^2, E kw.z^2), stokes = (((2 w) k) E) F d.  The DC texel (N/2, N/2) and texels with E = 0 or
+ *             1 - q = 0 contribute nothing.
+ *   order     binary64, fixed: thread t of T = N^2 / 16 sums texels t, t + T, ... from +0; a warp shuffle tree (lane l adds
+ *             lane l + 16, then + 8, + 4, + 2, + 1); the 8 warps of a 256-thread block in warp order from +0; the N^2 / 4096
+ *             blocks in block order from +0.  No floating-point atomics: the moments are a function of the spectrum.
+ *   cache     the moments of each cascade are cached on the device (allocated by the first sea-state or drift call, counted
+ *             in device_bytes).  A cascade becomes stale when its spectrum is written (regeneration on
+ *             should_generate_spectrum, ocean_set_spectrum_amplitudes) or its dispersion table changes (a new tile_length);
+ *             a call recomputes the stale cascades in one launch sequence of 2 kernels (none when nothing is stale).  A
+ *             cascade that has not been updated yet has zero moments.
+ *   total     sum over i in [0, num_cascades) in cascade order of (s_i s_i) moments_i, s_i = (double)map_scales[i].z (the
+ *             displacement scale): the statistics of the surface as rendered, the cascades being independent fields whose
+ *             variances add.  per_cascade[i] (may be NULL) holds the unscaled moments.
+ *   derived   on the host, binary64, every one 0 when m0 = 0:
+ *               significant_wave_height  Hs = 4 sqrt(m0)
+ *               mean_period              Tm01 = 2 pi m0 / m1
+ *               zero_crossing_period     Tm02 = 2 pi sqrt(m0 / m2)
+ *               energy_period            Te = 2 pi m_minus1 / m0
+ *               mean_direction           degrees(atan2(-direction[1], -direction[0])): the wind_direction whose spectrum
+ *                                        peaks there (spectrum_compute.glsl's theta); the waves travel towards it + 180
+ *               directional_spread       sqrt(2 max(0, 1 - R)) radians, R = |direction| / m0 (circular spread)
+ *               mean_square_slope        slope[0] + slope[1]
+ *               stokes_speed             |stokes| (m/s); stokes itself is the surface Stokes drift vector
+ *             The peak period is not a moment: 2 pi / ocean_jonswap_peak_angular_frequency is the model's.
+ * ocean_get_sea_state is host-only and synchronous (the sea state changes only when a spectrum does); the drifters read the
+ * cache on the device.  num_cascades in [1, num_cascades of the generator], map_scales and total non-NULL.  The entry point
+ * is ocean_get_sea_state rather than ocean_sea_state because C gives a function and a typedef one namespace, and the record
+ * below holds that name. */
+typedef struct ocean_sea_state {
+    double m_minus1, m0, m1, m2;        /* spectral moments: sum E / w, E, w E, w^2 E (m^2 s, m^2, m^2 / s, m^2 / s^2) */
+    double direction[2];                /* sum E d, world (x, z) */
+    double slope[2];                    /* sum E kw.x^2, sum E kw.z^2 */
+    double stokes[2];                   /* surface Stokes drift, m/s, world (x, z) */
+    double significant_wave_height;     /* derived fields (above) */
+    double mean_period;
+    double zero_crossing_period;
+    double energy_period;
+    double mean_direction;              /* degrees */
+    double directional_spread;          /* radians */
+    double mean_square_slope;
+    double stokes_speed;                /* m/s */
+} ocean_sea_state;                      /* 144 B */
+int ocean_get_sea_state(ocean_generator* gen, int num_cascades, const float* map_scales_host, ocean_sea_state* per_cascade_host,
+                    ocean_sea_state* total_host);
+
+/* Drifters -- the bulk of what floats in a scene (debris, crates, seaweed, foam patches, buoys used as props): thousands of
+ * objects that ride the waves and drift with the sea, one thread each, with render-ready MultiMesh instances.  A drifter is
+ * a Lagrangian label: the undisplaced point P whose surface point P + D(P, t) it sits at.  Tessendorf's choppy displacement
+ * is the first-order Lagrangian displacement of the surface, so a fixed label moves on a closed orbit (the bodies of
+ * ocean_simulate_bodies bob in place); real floating matter drifts with the Stokes drift, the second-order mean of those
+ * orbits, which is a label velocity.  oracle/drifters.py is the specification, bit for bit.  One call, per drifter:
+ *   drift   (dt > 0 only) u = stokes_scale * us + current + windage * wind, with us = sum over i in cascade order of
+ *           (s_i s_i) stokes_i (the sea-state cache under the call's map_scales, s_i = map_scales[i].z), binary64:
+ *           u = ((stokes_scale us) + current) + (windage wind);  x += dt u.x, z += dt u.z;
+ *           yaw = (float)((double)yaw + dt yaw_rate)
+ *   wrap    (dt > 0, OCEAN_DRIFT_WRAP) r = x - x0, x = x0 + (r - W floor(r / W)), z likewise with (z0, D): labels stay in
+ *           [x0, x0 + W] x [z0, z0 + D] (the closed box: the last rounding may land on the far edge), the ambient debris
+ *           field around a moving camera
+ *   render  (instances not NULL) the maps at (float)P with ocean_sample_maps' filter (displacement D, gradient g), then
+ *           X = ((float)(x + D.x), (float)((D.y [+ hw]) + offset), (float)(z + D.z)), each sum binary64 and rounded once;
+ *           n = normalize(-g.x, 1, -g.y), n_t = normalize(up + tilt (n - up)) (every operation binary32, as written);
+ *           basis y = n_t, z = normalize(f - (f . n_t) n_t) with f = (sin yaw, 0, cos yaw) (DETMATH sincos), x = y cross z,
+ *           each column times scale -- with tilt = 0 it is Godot's Basis(Vector3.UP, yaw) * scale up to rounding.  12 floats
+ *           per drifter in drifter order, the 3 x 4 row-major layout of ocean_simulate_bodies' transforms (a MultiMesh
+ *           TRANSFORM_3D buffer).
+ *   wake    with OCEAN_DRIFT_READ_WAKE and a wake layer present, ocean_sample_wake's (hw, hgx, hgz) at (X.x, X.z) is added
+ *           to the height (in binary64, above) and to g (g.x += hgx, g.y += hgz) before the normal, so drifters sit on the
+ *           surface the render maps draw.  The wake has no horizontal velocity: drifters bob on wakes but are not pushed.
+ * dt = 0 only renders (the labels are not written).  A drifter is not validated: a NaN or infinite one affects only itself.
+ * Limits: the Stokes drift is the surface value of linear theory (no vertical profile, no wave-current interaction); it is
+ * uniform in space (the mean of the whole spectrum, not the local wave group's); drifters do not collide with each other or
+ * with bodies; the render is the surface within 150 m of the camera (ocean_query_surface's limit).
+ * Validation: dt finite and >= 0, params non-NULL with every field finite, box width and depth > 0 with OCEAN_DRIFT_WRAP,
+ * no unknown flag, num_cascades in [1, num_cascades of the generator], map_scales non-NULL, num_drifters >= 0 and drifters
+ * non-NULL when num_drifters > 0.  An invalid call returns OCEAN_ERR_INVALID_ARGUMENT, launches nothing and leaves the
+ * drifters untouched.  A call with drifters and dt > 0 first brings stale sea-state cascades up to date (2 kernels when any
+ * is stale), then launches 1 kernel; with dt = 0 only the 1.  ocean_drift takes host drifters (updated in place) and
+ * instances and is synchronous; ocean_drift_device takes device pointers for them and is asynchronous on the generator's
+ * stream. */
+#define OCEAN_DRIFT_WRAP 1u             /* wrap the labels into params.box */
+#define OCEAN_DRIFT_READ_WAKE 2u        /* the render reads the wake layer's h and slopes */
+typedef struct ocean_drifter {
+    double x, z;                /* the label: undisplaced point P, world metres (binary64: mm per frame kilometres out) */
+    float yaw, yaw_rate;        /* radians and rad/s, about the surface normal */
+    float windage;              /* fraction of the wind vector added to the drift */
+    float tilt;                 /* 0 stays upright, 1 follows the surface normal */
+    float offset;               /* metres added to the height */
+    float scale;                /* uniform instance scale */
+} ocean_drifter;                /* 40 B */
+typedef struct ocean_drift_params {
+    float current[2];           /* m/s, world x and z */
+    float wind[2];              /* m/s, world x and z */
+    float stokes_scale;         /* 1 is physical, 0 turns the Stokes drift off */
+    uint32_t flags;             /* OCEAN_DRIFT_* */
+    double box[4];              /* wrap box (x0, z0, width, depth), metres */
+} ocean_drift_params;           /* 56 B */
+int ocean_drift(ocean_generator* gen, double dt, const ocean_drift_params* params, int num_drifters, ocean_drifter* drifters_host,
+                int num_cascades, const float* map_scales_host, float* instances_host);
+int ocean_drift_device(ocean_generator* gen, double dt, const ocean_drift_params* params, int num_drifters, ocean_drifter* drifters_dev,
+                       int num_cascades, const float* map_scales_host, float* instances_dev);
+
 /* Parity/debug taps (not timed): binary32 maps before the half conversion, the row-pass output
  * ([4][N][N][2] float, == fft_buffer half 1 after the first fft_compute, wave_generator.gd:79) and
  * the twiddle table ([N-1][2] float: stage s, index j at (1<<s)-1+j; fft_butterfly.glsl:27).

@@ -3,7 +3,7 @@ config.
 
     python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast] [--spray-particles]
                                 [--wake] [--wake-coupling] [--wake-foam] [--wake-obstacles]
-                                [--wake-readers]
+                                [--wake-readers] [--sea-state] [--drifters]
 
 Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
 --query.  An unknown argument exits before anything touches the GPU."""
@@ -615,6 +615,66 @@ def run_wake_readers(reps, label, N=256, C=4, wake=512, dx=0.5):
     print(json.dumps(out), flush=True)
 
 
+def run_sea_state(N, C, reps, label):
+    """The sea-state reduction (ocean_get_sea_state) with every cascade stale: each of `reps` rounds injects the spectra again
+    (ocean_set_spectrum_amplitudes, outside the window), then the generator's CUDA events bracket one call -- its two kernels
+    and the 10 C binary64 moments' copy to the host; the host wall time of the call, synchronise included, beside them."""
+    g, p, scales = warmed_generator(N, C, 1)
+    g.sea_state(scales)
+    amps = [g.spectrum_to_host(c)[..., :2].copy().view(np.complex64)[..., 0] for c in range(C)]
+    dev_ms, wall_us = [], []
+    for _ in range(reps):
+        for c in range(C):
+            g.set_spectrum_amplitudes(c, amps[c])
+        g.synchronize()
+        t0 = time.perf_counter()
+        g.timer_start()
+        g.sea_state(scales)
+        dev_ms.append(g.timer_stop())
+        wall_us.append((time.perf_counter() - t0) * 1e6)
+    spectrum_bytes = C * N * N * 16
+    best = min(dev_ms)
+    print(json.dumps({"config": label, **card(), "map_size": N, "cascades": C, "device_ms": sorted(dev_ms), "host_wall_us": sorted(wall_us),
+                      "spectrum_MiB": spectrum_bytes / 2**20, "spectrum_GBps_at_best": spectrum_bytes / (best * 1e-3) / 1e9}), flush=True)
+    g.free()
+
+
+def run_drift(N, C, n, reps, label, wake=512, dx=0.5):
+    """ocean_drift_device on n drifters with dt = 1/60 s, a current, wind and the wrap, wake read off against on (alternating
+    windows on one generator; the sea state is fresh, so each call is the drift kernel alone).  The drifters lie in a 400 m box
+    around the 512 x 512 wake window (16 moving sources), so the wake form samples the layer for part of them.  Per drifter the
+    kernel reads and writes its 40 B record and writes a 48 B instance: 128 B of state traffic, beside the map gathers."""
+    g, _, scales = warmed_generator(N, C, 2)
+    g.wake_init(wake, dx, 0.05, 32, 3.0)
+    ext = wake * dx
+    rng = np.random.default_rng(n)
+    s = np.zeros(16, gow.WaveGenerator.WAKE_SOURCE)
+    s["x"], s["z"] = rng.uniform(-0.4 * ext, 0.4 * ext, 16), rng.uniform(-0.4 * ext, 0.4 * ext, 16)
+    s["vx"], s["vz"] = rng.uniform(-6, 6, 16), rng.uniform(-6, 6, 16)
+    s["radius"], s["head"], s["body"] = 2.0, 0.2, -1
+    for _ in range(10):
+        g.wake_step(0.1, 4, (-wake // 2, -wake // 2), s)
+    d = np.zeros(n, gow.WaveGenerator.DRIFTER)
+    d["x"], d["z"] = rng.uniform(-200, 200, n), rng.uniform(-200, 200, n)
+    d["yaw"], d["yaw_rate"] = rng.uniform(-3, 3, n), rng.uniform(-1, 1, n)
+    d["windage"], d["tilt"], d["scale"] = 0.02, 0.5, 1.0
+    drifters = upload(d)
+    inst = torch.empty(n * 12, dtype=torch.float32, device=DEV)
+    lib = load_library()
+    params = {on: gow.WaveGenerator.drift_params(current=(0.2, 0.1), wind=(6.0, 2.0), box=(-200.0, -200.0, 400.0, 400.0), read_wake=on)
+              for on in (False, True)}
+    call = lambda on: (lambda: check(lib.ocean_drift_device(g.context, 1.0 / 60.0, params[on].ctypes.data, n, drifters.data_ptr(), C,
+                                                             scales.ctypes.data, inst.data_ptr())))
+    call(False)()
+    t_off, t_on = alternate(lambda: timed(g, call(False), reps, 3), lambda: timed(g, call(True), reps, 3))
+    state_bytes = n * (2 * gow.WaveGenerator.DRIFTER.itemsize + 48)
+    print(json.dumps({"config": label, **card(), "map_size": N, "cascades": C, "drifters": n, "wake_size": wake,
+                      "ms_per_call": {"wake_off": t_off, "wake_on": t_on}, "us_per_call_best": {"wake_off": 1e3 * min(t_off), "wake_on": 1e3 * min(t_on)},
+                      "state_GBps_at_best": {"wake_off": state_bytes / (min(t_off) * 1e-3) / 1e9, "wake_on": state_bytes / (min(t_on) * 1e-3) / 1e9}}),
+          flush=True)
+    g.free()
+
+
 def run_wake_step_foam(N, sources, reps, label, substeps=8, dx=0.5):
     """Wake foam's cost in the step call: run_wake's ocean_wake_step_device with foam off and on (the foam form of the
     sub-step kernel: |v|^2 carried by the cull, w^2 |v|^2 summed beside phi, one more 4 B read and write per cell);
@@ -794,6 +854,14 @@ GROUPS = {          # flag: its configs, in the order they run
     "--wake-readers": [
         partial(run_wake_readers, 20, "wake readers: ray cast, spray and spray particles, readers off vs on, 4 cascades of 256x256, "
                                       "coupled 512x512 wake with foam"),
+    ],
+    "--sea-state": [
+        partial(run_sea_state, 1024, 8, 10, "sea state: the reduction over 8 cascades of 1024x1024, every cascade stale"),
+    ],
+    "--drifters": [
+        partial(run_drift, N, 4, n, 200 if n < (1 << 20) else 50, f"drifters: {'2^16' if n < (1 << 20) else '2^20'} over 4 cascades of {N}x{N}, "
+                "wake read off vs on")
+        for N in (256, 1024) for n in (1 << 16, 1 << 20)
     ],
     "--wake-obstacles": [
         partial(run_wake_step_obstacles, N, k, 200 if N < 1024 else 50, f"wake obstacles, step: {N}x{N} cells, {k} source(s), 8 sub-steps")

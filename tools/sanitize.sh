@@ -1,5 +1,6 @@
 #!/bin/bash
-# compute-sanitizer passes over a small but queue-exercising workload (run under gpurun): 256x256 x 12 cascades, 3 updates + 5 fused frames.
+# compute-sanitizer passes over a small but queue-exercising workload: 256x256 x 12 cascades, 3 updates + 5 fused frames, then
+# the map query, the sea-state reduction and 4096 drifters reading a 256x256 wake layer.
 cat > /tmp/san.py <<'PY'
 import sys, numpy as np
 sys.path.insert(0, ".")
@@ -12,10 +13,21 @@ for _ in range(3):
 g.update_frames(0.02, p, 5)        # fused frames: alternating scratch halves, column pass waiting for the previous frame's
 d, n = g.maps_to_host()
 pts = np.random.default_rng(0).uniform(-100, 100, (4096, 2)).astype(np.float32)
-g.sample(pts, gow.WaveGenerator.map_scales(p))
+sc = gow.WaveGenerator.map_scales(p)
+g.sample(pts, sc)
+total, _ = g.sea_state(sc)                        # the sea-state reduction over every cascade
+g.wake_init(256, 0.5)                             # drifters on the wake: the drift kernel's wake form
+src = np.zeros(4, gow.WaveGenerator.WAKE_SOURCE)
+src["x"], src["z"], src["vx"], src["radius"], src["head"], src["body"] = 20.0, 30.0, 3.0, 2.0, 0.2, -1
+g.wake_step(0.05, 4, (0, 0), src)
+dr = np.zeros(len(pts), gow.WaveGenerator.DRIFTER)
+dr["x"], dr["z"], dr["scale"], dr["tilt"] = pts[:, 0], pts[:, 1], 1.0, 0.5
+dp = gow.WaveGenerator.drift_params(current=(0.1, 0.0), box=(-100.0, -100.0, 200.0, 200.0), read_wake=True)
+dr, inst = g.drift(dr, 1.0 / 60.0, sc, dp)
+print("sea state", float(total["significant_wave_height"]), "drift", float(np.nansum(inst)))
 print("checksum", int(d.view(np.uint16).astype(np.uint64).sum()), int(n.view(np.uint16).astype(np.uint64).sum()))
 g.free()
 PY
 for tool in memcheck racecheck synccheck; do
-  echo "== $tool"; timeout 600 compute-sanitizer --tool $tool python /tmp/san.py 2>&1 | grep -i "checksum\|ERROR SUMMARY\|hazard\|error" | head -8
+  echo "== $tool"; timeout 600 compute-sanitizer --tool $tool python /tmp/san.py 2>&1 | grep -i "checksum\|sea state\|ERROR SUMMARY\|hazard\|error" | head -8
 done
