@@ -189,6 +189,52 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanThruster                              // struct ocean_thruster (36 B): an engine or jet
+    {
+        public int body;
+        public fixed float position[3];                             // hull-local
+        public fixed float direction[3];                            // hull-local; rotate it to steer an outboard
+        public float thrust;                                        // N, scaled by the point's immersion
+        public float half_height;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanFoil                                  // struct ocean_foil (36 B): a keel, rudder or fin
+    {
+        public int body;
+        public fixed float position[3];                             // hull-local centre of pressure
+        public fixed float normal[3];                               // hull-local plate normal; rotate it to turn a rudder
+        public float area;                                          // C_n A, m^2, finite and >= 0
+        public float half_height;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanBodyLoad                              // struct ocean_body_load (24 B): sails, gusts, impulses
+    {
+        public fixed float force[3];                                // world frame
+        public fixed float torque[3];                               // world frame, about the centre of mass
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanTether                                // struct ocean_tether (44 B): a mooring or tow line
+    {
+        public int body_a;
+        public int body_b;                                          // -1: point_b is a world anchor
+        public fixed float point_a[3];
+        public fixed float point_b[3];
+        public float rest_length, stiffness, damping;               // finite and >= 0
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanDriveResult                           // struct ocean_drive_result (32 B)
+    {
+        public fixed float force[3];                                // what the thrusters, foils, tethers and load added
+        public fixed float torque[3];
+        public float wetted_foil_area;
+        public float max_normal_speed;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public unsafe struct OceanRay                                   // struct ocean_ray (28 B)
     {
         public fixed float origin[3];
@@ -387,6 +433,24 @@ namespace OceanB200
                                                                  int num_points, void* points_dev, void* drag_areas_dev, int num_cascades,
                                                                  float* map_scales, float density, float dt, int substeps, float tolerance,
                                                                  int max_iterations, void* hydrostatic_dev, void* drag_dev, void* transforms_dev);
+        // driven and moored bodies: ocean_simulate_bodies with thrusters, foils, loads (may be null) and tethers, host arrays in
+        // both forms; drive and tensions ([num_tethers], for drawing or snapping ropes) are the last sub-step's and may be null
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_simulate_driven_bodies(IntPtr handle, int num_bodies, OceanFloatingBody* bodies, OceanBodyState* states,
+                                                                 int num_points, OceanBuoyancyPoint* points, float* drag_areas, int num_cascades,
+                                                                 float* map_scales, float density, float dt, int substeps, float tolerance,
+                                                                 int max_iterations, int num_thrusters, OceanThruster* thrusters, int num_foils,
+                                                                 OceanFoil* foils, OceanBodyLoad* loads, int num_tethers, OceanTether* tethers,
+                                                                 OceanBuoyancyResult* hydrostatic, OceanDragResult* drag, OceanDriveResult* drive,
+                                                                 float* tensions, float* transforms);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_simulate_driven_bodies_device(IntPtr handle, int num_bodies, OceanFloatingBody* bodies, void* states_dev,
+                                                                        int num_points, void* points_dev, void* drag_areas_dev, int num_cascades,
+                                                                        float* map_scales, float density, float dt, int substeps, float tolerance,
+                                                                        int max_iterations, int num_thrusters, OceanThruster* thrusters,
+                                                                        int num_foils, OceanFoil* foils, OceanBodyLoad* loads, int num_tethers,
+                                                                        OceanTether* tethers, void* hydrostatic_dev, void* drag_dev, void* drive_dev,
+                                                                        void* tensions_dev, void* transforms_dev);
         // velocity maps: d/dt of the displacement map, recomputed for the cascades whose maps changed; recomputed may be null
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_update_velocity(IntPtr handle, int* recomputed);

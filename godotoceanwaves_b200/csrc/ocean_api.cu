@@ -66,7 +66,7 @@ struct DeviceArray {
 enum StagedOp {
     kStageSampleMaps, kStageExtractSpray, kStageSprayParticles, kStageQuerySurface, kStageRaycast, kStageBuoyancy,
     kStageSampleVelocity, kStageBodyForces, kStageSimulateBodies, kStageDeviceMath, kStageWakeStep, kStageSampleWake, kStageDrift,
-    kNumStagedOps
+    kStageDrivenBodies, kNumStagedOps
 };
 
 // The parts of the wake layer WakeLayer::off turns off; kWakeLayer is the whole layer.
@@ -179,6 +179,19 @@ struct ocean_generator {
     // drag_velocities)
     DeviceArray<ocean_floating_body> sim_bodies;
     DeviceArray<float> sim_r2;
+    // driven-body scratch (ocean_simulate_driven_bodies): the actuator, load and tether arrays, the by-body incidence list
+    // (offsets, then entries, in one block; its host copy is kept because the upload is asynchronous), the tether records,
+    // the integrator's sums, and the drive and tension outputs when the caller passes NULL for them
+    DeviceArray<ocean_thruster> drive_thrusters;
+    DeviceArray<ocean_foil> drive_foils;
+    DeviceArray<ocean_body_load> drive_loads;
+    DeviceArray<ocean_tether> drive_tethers;
+    DeviceArray<int> drive_incidence;
+    std::vector<int> drive_incidence_host;
+    DeviceArray<ocean::TetherForce> drive_tether_forces;
+    DeviceArray<ocean::DriveSum> drive_sums;
+    DeviceArray<ocean_drive_result> drive_results;
+    DeviceArray<float> drive_tensions;
     // velocity maps, allocated by the first velocity call: row-pass scratch, the map, its binary32 tap while the taps are on
     DeviceArray<float4> vel_scratch;                    // [num_cascades][N][N]
     DeviceArray<uint2> velocity;                        // [num_cascades][N][N] 4 x half
@@ -1521,16 +1534,19 @@ int upload_offsets(ocean_generator* gen, int num_bodies, const Body* bodies_host
 
 // The buoyancy launches on a body table and offsets already in device memory (bodies_dev may be written by earlier kernels on
 // the stream), with the map scales in gen->q_scales and gen->buoy_q grown to `world`: samples receives the surface records, and
-// wv_dev (may be null) the wake's vertical velocity of each world point while the wake coupling is live.
+// wv_dev (may be null) the wake's vertical velocity of each world point while the wake coupling is live.  With queried > world
+// the query also takes the points gen->buoy_q holds after the world points (written earlier on the stream).
 int launch_buoyancy_sequence(ocean_generator* gen, const ocean_buoyancy_body* bodies_dev, const int* offsets_dev, int num_bodies, int world,
                              const ocean_buoyancy_point* points_dev, int num_cascades, float density, float tolerance, int max_iterations,
-                             ocean_buoyancy_result* results_dev, ocean_surface_sample* samples, float* wv_dev = nullptr) {
+                             ocean_buoyancy_result* results_dev, ocean_surface_sample* samples, float* wv_dev = nullptr, int queried = -1) {
     int rc;
+    if (queried < 0) queried = world;                   // more query points than world ones: the driven bodies' actuators
     if (world > 0) {
         OCEAN_CUDA(ocean::launch_buoyancy_transform(bodies_dev, offsets_dev, num_bodies, points_dev, world, gen->buoy_q.ptr, gen->stream));
         gen->kernel_launches += 1;
-        if ((rc = run_query_surface(gen, world, gen->buoy_q.ptr, num_cascades, tolerance, max_iterations, samples, wv_dev))) return rc;
     }
+    if (queried > 0)
+        if ((rc = run_query_surface(gen, queried, gen->buoy_q.ptr, num_cascades, tolerance, max_iterations, samples, wv_dev))) return rc;
     const float rho_g = density * 9.81f;                                 // G, wave_generator.gd:5, in binary32
     OCEAN_CUDA(ocean::launch_buoyancy_reduce(bodies_dev, offsets_dev, num_bodies, points_dev, samples, rho_g, tolerance, results_dev,
                                              gen->stream));
@@ -1808,30 +1824,135 @@ int check_simulate_args(int num_bodies, const ocean_floating_body* bodies, const
 }
 }  // namespace
 
-int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_dev,
-                                 int num_points, const ocean_buoyancy_point* points_dev, const float* drag_areas_dev, int num_cascades,
-                                 const float* map_scales_host, float density, float dt, int substeps, float tolerance, int max_iterations,
-                                 ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev, float* transforms_dev) {
-    OCEAN_ENTER(gen);
-    if (rc) return rc;
-    int world = 0;
-    if ((rc = check_simulate_args(num_bodies, bodies_host, states_dev, num_points, drag_areas_dev, density, dt, substeps, tolerance,
-                                  max_iterations, &world)))
-        return rc;
-    if (num_bodies == 0) return OCEAN_OK;
-    if (world > 0 && !points_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
-    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
+namespace {
+// The drive arguments of ocean_simulate_driven_bodies[_device] (host arrays), as validated by check_drive_args.
+struct DriveHost {
+    int num_thrusters = 0;
+    const ocean_thruster* thrusters = nullptr;
+    int num_foils = 0;
+    const ocean_foil* foils = nullptr;
+    const ocean_body_load* loads = nullptr;
+    int num_tethers = 0;
+    const ocean_tether* tethers = nullptr;
+    int actuators() const { return num_thrusters + num_foils; }
+    bool any() const { return num_thrusters > 0 || num_foils > 0 || num_tethers > 0 || loads; }
+};
+
+bool finite_nonnegative(float x) { return x >= 0.0f && std::isfinite(x); }
+
+// The counts and arrays, the body indices, and the foil areas and tether constants that enter the stability bound; the world
+// points plus the actuators must stay below 2^31 (one surface query takes them all).
+int check_drive_args(int num_bodies, int world, const DriveHost& d) {
+    if (d.num_thrusters < 0 || d.num_foils < 0 || d.num_tethers < 0)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "a count is negative (thrusters %d, foils %d, tethers %d)", d.num_thrusters, d.num_foils,
+                    d.num_tethers);
+    if ((d.num_thrusters > 0 && !d.thrusters) || (d.num_foils > 0 && !d.foils) || (d.num_tethers > 0 && !d.tethers))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "an actuator or tether array is NULL");
+    if ((long long)world + d.num_thrusters + d.num_foils > 2147483647LL)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "world points plus actuators exceed 2^31 - 1");
+    for (int k = 0; k < d.num_thrusters; ++k)
+        if (d.thrusters[k].body < 0 || d.thrusters[k].body >= num_bodies)
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "thruster %d: body %d outside [0, %d)", k, d.thrusters[k].body, num_bodies);
+    for (int k = 0; k < d.num_foils; ++k) {
+        const ocean_foil& f = d.foils[k];
+        if (f.body < 0 || f.body >= num_bodies) return fail(OCEAN_ERR_INVALID_ARGUMENT, "foil %d: body %d outside [0, %d)", k, f.body, num_bodies);
+        if (!finite_nonnegative(f.area)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "foil %d: area %g is not finite and >= 0", k, f.area);
+    }
+    for (int k = 0; k < d.num_tethers; ++k) {
+        const ocean_tether& t = d.tethers[k];
+        if (t.body_a < 0 || t.body_a >= num_bodies)
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "tether %d: body_a %d outside [0, %d)", k, t.body_a, num_bodies);
+        if (t.body_b != -1 && (t.body_b < 0 || t.body_b >= num_bodies || t.body_b == t.body_a))
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "tether %d: body_b %d is not -1 or another body", k, t.body_b);
+        if (!finite_nonnegative(t.rest_length) || !finite_nonnegative(t.stiffness) || !finite_nonnegative(t.damping))
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "tether %d: rest_length, stiffness and damping must be finite and >= 0", k);
+    }
+    return OCEAN_OK;
+}
+
+// The by-body incidence list into gen->drive_incidence_host: [num_bodies + 1] offsets, then per body its thrusters, foils
+// and tether ends in array order (thruster k -> k, foil k -> T + k, end e of tether k -> T + F + 2 k + e).
+void build_incidence(ocean_generator* gen, int num_bodies, const DriveHost& d) {
+    const size_t B = (size_t)num_bodies;
+    std::vector<int>& v = gen->drive_incidence_host;
+    const size_t entries = (size_t)d.actuators() + 2 * (size_t)d.num_tethers;
+    v.assign(B + 1 + entries, 0);
+    int* off = v.data();
+    int* list = off + B + 1;
+    for (int k = 0; k < d.num_thrusters; ++k) off[d.thrusters[k].body + 1] += 1;
+    for (int k = 0; k < d.num_foils; ++k) off[d.foils[k].body + 1] += 1;
+    for (int k = 0; k < d.num_tethers; ++k) {
+        off[d.tethers[k].body_a + 1] += 1;
+        if (d.tethers[k].body_b >= 0) off[d.tethers[k].body_b + 1] += 1;
+    }
+    for (size_t b = 0; b < B; ++b) off[b + 1] += off[b];
+    std::vector<int> next(off, off + B);
+    const int T = d.num_thrusters, F = d.num_foils;
+    for (int k = 0; k < T; ++k) list[next[d.thrusters[k].body]++] = k;
+    for (int k = 0; k < F; ++k) list[next[d.foils[k].body]++] = T + k;
+    for (int k = 0; k < d.num_tethers; ++k) {
+        list[next[d.tethers[k].body_a]++] = T + F + 2 * k;
+        if (d.tethers[k].body_b >= 0) list[next[d.tethers[k].body_b]++] = T + F + 2 * k + 1;
+    }
+    v.resize(B + 1 + (size_t)off[B]);                   // anchored tethers have one end
+}
+
+// ocean_simulate_bodies_device after its checks (num_bodies > 0, scales uploaded), with drive null: the plain integrator;
+// with drive: the driven one (drive->any()), its arrays validated, and drive_dev / tensions_dev the outputs or null.
+int run_simulate(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_dev, int world,
+                 const ocean_buoyancy_point* points_dev, const float* drag_areas_dev, int num_cascades, float density, float dt, int substeps,
+                 float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
+                 float* transforms_dev, const DriveHost* drive = nullptr, ocean_drive_result* drive_dev = nullptr, float* tensions_dev = nullptr) {
+    int rc;
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
     const size_t B = (size_t)num_bodies;
+    const int actuators = drive ? drive->actuators() : 0;
+    const int queried = world + actuators;              // the hull's world points, then the actuators'
     OCEAN_CUDA(gen->sim_r2.grow(gen, B));
     OCEAN_CUDA(gen->buoy_bodies.grow(gen, B));
     OCEAN_CUDA(gen->drag_velocities.grow(gen, B));
-    OCEAN_CUDA(gen->buoy_q.grow(gen, (size_t)world));
-    OCEAN_CUDA(gen->buoy_samples.grow(gen, (size_t)world));
+    OCEAN_CUDA(gen->buoy_q.grow(gen, (size_t)queried));
+    OCEAN_CUDA(gen->buoy_samples.grow(gen, (size_t)queried));
     float* wv = nullptr;                                // every sub-step reads the same snapshots
-    if (world > 0 && gen->wake.coupling_live()) {
-        OCEAN_CUDA(gen->wake.wv.grow(gen, (size_t)world));
+    if (queried > 0 && gen->wake.coupling_live()) {
+        OCEAN_CUDA(gen->wake.wv.grow(gen, (size_t)queried));
         wv = gen->wake.wv.ptr;
+    }
+    ocean::DriveArgs da{};
+    if (drive) {
+        da.num_thrusters = drive->num_thrusters;
+        da.num_foils = drive->num_foils;
+        da.num_tethers = drive->num_tethers;
+        if (drive->num_thrusters > 0) {
+            OCEAN_CUDA(gen->drive_thrusters.upload(gen, drive->thrusters, (size_t)drive->num_thrusters));
+            da.thrusters = gen->drive_thrusters.ptr;
+        }
+        if (drive->num_foils > 0) {
+            OCEAN_CUDA(gen->drive_foils.upload(gen, drive->foils, (size_t)drive->num_foils));
+            da.foils = gen->drive_foils.ptr;
+        }
+        if (drive->num_tethers > 0) {
+            OCEAN_CUDA(gen->drive_tethers.upload(gen, drive->tethers, (size_t)drive->num_tethers));
+            OCEAN_CUDA(gen->drive_tether_forces.grow(gen, (size_t)drive->num_tethers));
+            da.tethers = gen->drive_tethers.ptr;
+            if (!tensions_dev) {
+                OCEAN_CUDA(gen->drive_tensions.grow(gen, (size_t)drive->num_tethers));
+                tensions_dev = gen->drive_tensions.ptr;
+            }
+        }
+        if (drive->loads) {
+            OCEAN_CUDA(gen->drive_loads.upload(gen, drive->loads, B));
+            da.loads = gen->drive_loads.ptr;
+        }
+        build_incidence(gen, num_bodies, *drive);
+        OCEAN_CUDA(gen->drive_incidence.upload(gen, gen->drive_incidence_host.data(), gen->drive_incidence_host.size()));
+        da.incidence_offsets = gen->drive_incidence.ptr;
+        da.incidence = gen->drive_incidence.ptr + B + 1;
+        OCEAN_CUDA(gen->drive_sums.grow(gen, B));
+        if (!drive_dev) {
+            OCEAN_CUDA(gen->drive_results.grow(gen, B));
+            drive_dev = gen->drive_results.ptr;
+        }
     }
     if (!hydrostatic_dev) {
         OCEAN_CUDA(gen->buoy_results.grow(gen, B));
@@ -1851,17 +1972,54 @@ int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const oce
     const float h = dt / (float)substeps;
     const float half_rho = 0.5f * density;
     for (int s = 0; s < substeps; ++s) {
+        float* transforms = s == substeps - 1 ? transforms_dev : nullptr;
+        if (actuators > 0) {
+            OCEAN_CUDA(ocean::launch_actuator_transform(da, poses, gen->buoy_q.ptr + world, gen->stream));
+            gen->kernel_launches += 1;
+        }
         if ((rc = launch_buoyancy_sequence(gen, poses, gen->buoy_offsets.ptr, num_bodies, world, points_dev, num_cascades, density, tolerance,
-                                           max_iterations, hydrostatic_dev, gen->buoy_samples.ptr, wv)))
+                                           max_iterations, hydrostatic_dev, gen->buoy_samples.ptr, wv, queried)))
             return rc;
         OCEAN_CUDA(ocean::launch_drag_reduce(poses, velocities, gen->buoy_offsets.ptr, num_bodies, points_dev, drag_areas_dev,
                                              gen->buoy_samples.ptr, gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, half_rho,
                                              drag_dev, wv, gen->stream));
-        OCEAN_CUDA(ocean::launch_bodies_integrate(bodies, gen->sim_r2.ptr, num_bodies, hydrostatic_dev, drag_dev, density, h, states_dev, poses,
-                                                  velocities, s == substeps - 1 ? transforms_dev : nullptr, gen->stream));
-        gen->kernel_launches += 2;
+        if (!drive) {
+            OCEAN_CUDA(ocean::launch_bodies_integrate(bodies, gen->sim_r2.ptr, num_bodies, hydrostatic_dev, drag_dev, density, h, states_dev,
+                                                      poses, velocities, transforms, gen->stream));
+            gen->kernel_launches += 2;
+            continue;
+        }
+        if (da.num_tethers > 0) {
+            OCEAN_CUDA(ocean::launch_tethers(da, poses, velocities, gen->drive_tether_forces.ptr, tensions_dev, gen->stream));
+            gen->kernel_launches += 1;
+        }
+        OCEAN_CUDA(ocean::launch_drive_reduce(da, num_bodies, bodies, gen->sim_r2.ptr, poses, velocities, hydrostatic_dev, drag_dev,
+                                              gen->buoy_samples.ptr + world, wv ? wv + world : nullptr, gen->drive_tether_forces.ptr,
+                                              gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, density, h, gen->drive_sums.ptr,
+                                              drive_dev, gen->stream));
+        OCEAN_CUDA(ocean::launch_bodies_integrate_driven(bodies, num_bodies, gen->drive_sums.ptr, h, states_dev, poses, velocities, transforms,
+                                                         gen->stream));
+        gen->kernel_launches += 3;
     }
     return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_dev,
+                                 int num_points, const ocean_buoyancy_point* points_dev, const float* drag_areas_dev, int num_cascades,
+                                 const float* map_scales_host, float density, float dt, int substeps, float tolerance, int max_iterations,
+                                 ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev, float* transforms_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_simulate_args(num_bodies, bodies_host, states_dev, num_points, drag_areas_dev, density, dt, substeps, tolerance,
+                                  max_iterations, &world)))
+        return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (world > 0 && !points_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
+    return run_simulate(gen, num_bodies, bodies_host, states_dev, world, points_dev, drag_areas_dev, num_cascades, density, dt, substeps,
+                        tolerance, max_iterations, hydrostatic_dev, drag_dev, transforms_dev);
 }
 
 int ocean_simulate_bodies(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_host,
@@ -1888,6 +2046,72 @@ int ocean_simulate_bodies(ocean_generator* gen, int num_bodies, const ocean_floa
     return st.finish(gen, ocean_simulate_bodies_device(gen, num_bodies, bodies_host, st[states], num_points, st[points], st[areas],
                                                        num_cascades, map_scales_host, density, dt, substeps, tolerance, max_iterations,
                                                        st[hydrostatic], st[drag], st[transforms]));
+}
+
+// ---- driven and moored bodies: thrusters, foils, loads and tethers in the integrator (ocean_drive.cu; oracle/drive.py) ----
+static_assert(sizeof(ocean_thruster) == 36 && sizeof(ocean_foil) == 36, "actuator layouts");
+static_assert(sizeof(ocean_body_load) == 24 && sizeof(ocean_tether) == 44 && sizeof(ocean_drive_result) == 32, "drive record layouts");
+
+int ocean_simulate_driven_bodies_device(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host,
+                                        ocean_body_state* states_dev, int num_points, const ocean_buoyancy_point* points_dev,
+                                        const float* drag_areas_dev, int num_cascades, const float* map_scales_host, float density, float dt,
+                                        int substeps, float tolerance, int max_iterations, int num_thrusters, const ocean_thruster* thrusters_host,
+                                        int num_foils, const ocean_foil* foils_host, const ocean_body_load* loads_host, int num_tethers,
+                                        const ocean_tether* tethers_host, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
+                                        ocean_drive_result* drive_dev, float* tensions_dev, float* transforms_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_simulate_args(num_bodies, bodies_host, states_dev, num_points, drag_areas_dev, density, dt, substeps, tolerance,
+                                  max_iterations, &world)))
+        return rc;
+    const DriveHost drive{num_thrusters, thrusters_host, num_foils, foils_host, num_bodies > 0 ? loads_host : nullptr, num_tethers, tethers_host};
+    if ((rc = check_drive_args(num_bodies, world, drive))) return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (world > 0 && !points_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
+    if (!drive.any()) {                                 // ocean_simulate_bodies, with a zero drive record
+        if (drive_dev) OCEAN_CUDA(cudaMemsetAsync(drive_dev, 0, sizeof(ocean_drive_result) * (size_t)num_bodies, gen->stream));
+        return run_simulate(gen, num_bodies, bodies_host, states_dev, world, points_dev, drag_areas_dev, num_cascades, density, dt, substeps,
+                            tolerance, max_iterations, hydrostatic_dev, drag_dev, transforms_dev);
+    }
+    return run_simulate(gen, num_bodies, bodies_host, states_dev, world, points_dev, drag_areas_dev, num_cascades, density, dt, substeps,
+                        tolerance, max_iterations, hydrostatic_dev, drag_dev, transforms_dev, &drive, drive_dev, tensions_dev);
+}
+
+int ocean_simulate_driven_bodies(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_host,
+                                 int num_points, const ocean_buoyancy_point* points_host, const float* drag_areas_host, int num_cascades,
+                                 const float* map_scales_host, float density, float dt, int substeps, float tolerance, int max_iterations,
+                                 int num_thrusters, const ocean_thruster* thrusters_host, int num_foils, const ocean_foil* foils_host,
+                                 const ocean_body_load* loads_host, int num_tethers, const ocean_tether* tethers_host,
+                                 ocean_buoyancy_result* hydrostatic_host, ocean_drag_result* drag_host, ocean_drive_result* drive_host,
+                                 float* tensions_host, float* transforms_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_simulate_args(num_bodies, bodies_host, states_host, num_points, drag_areas_host, density, dt, substeps, tolerance,
+                                  max_iterations, &world)))
+        return rc;
+    const DriveHost drive{num_thrusters, thrusters_host, num_foils, foils_host, num_bodies > 0 ? loads_host : nullptr, num_tethers, tethers_host};
+    if ((rc = check_drive_args(num_bodies, world, drive))) return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (world > 0 && !points_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
+    const size_t P = world > 0 ? (size_t)num_points : 0, B = (size_t)num_bodies;
+    Staging st;                                         // an output not asked for stays NULL: the twin uses its own
+    const auto points = st.in(points_host, P);
+    const auto areas = st.in(drag_areas_host, P);
+    const auto states = st.inout(states_host, B);
+    const auto hydrostatic = st.out(hydrostatic_host, B);
+    const auto drag = st.out(drag_host, B);
+    const auto drive_out = st.out(drive_host, B);
+    const auto tensions = st.out(tensions_host, (size_t)num_tethers);
+    const auto transforms = st.out(transforms_host, 12 * B);
+    if ((rc = st.upload(gen, kStageDrivenBodies))) return rc;
+    return st.finish(gen, ocean_simulate_driven_bodies_device(gen, num_bodies, bodies_host, st[states], num_points, st[points], st[areas],
+                                                              num_cascades, map_scales_host, density, dt, substeps, tolerance, max_iterations,
+                                                              num_thrusters, thrusters_host, num_foils, foils_host, loads_host, num_tethers,
+                                                              tethers_host, st[hydrostatic], st[drag], st[drive_out], st[tensions],
+                                                              st[transforms]));
 }
 
 int ocean_copy_twiddles_to_host(ocean_generator* gen, float* host) {

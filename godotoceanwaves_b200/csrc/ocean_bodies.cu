@@ -10,6 +10,8 @@
 //   k_bodies_integrate   one thread per body: the semi-implicit step of the specification from the state, the pose the
 //                        sub-step started from and its two records; writes the new state, the next sub-step's pose and
 //                        velocity rows, and on the last sub-step the 3 x 4 transform of the final state when asked to.
+// ocean_simulate_driven_bodies runs k_bodies_integrate_driven instead, the same step on the forces and denominators of
+// ocean_drive.cu's reduce (both are forms of one inlined template).
 // Nothing crosses PCIe between sub-steps.  Numeric policy: binary32, the specification's operation order, no contraction
 // (-fmad=false), IEEE division and square root.
 #include "../../include/ocean.h"
@@ -73,35 +75,41 @@ __global__ void __launch_bounds__(256) k_bodies_prepare(const ocean_floating_bod
     vel[body] = v;
 }
 
-__global__ void __launch_bounds__(256) k_bodies_integrate(const ocean_floating_body* __restrict__ bodies, const float* __restrict__ r2,
-                                                          int num_bodies, const ocean_buoyancy_result* __restrict__ hyd,
-                                                          const ocean_drag_result* __restrict__ drg, float density, float h,
-                                                          ocean_body_state* __restrict__ states, ocean_buoyancy_body* __restrict__ pose,
-                                                          ocean_body_velocity* __restrict__ vel, float* __restrict__ transforms) {
+// One sub-step of the specification's step per body.  The plain form (k_bodies_integrate) forms F, tau and the denominators
+// m + h c_v, I + h c_w from the two records; the driven form (k_bodies_integrate_driven, ocean_drive.cu's reduce) reads them
+// from the body's DriveSum, where the drive contributions are already added.
+template <bool kDriven>
+__device__ __forceinline__ void bodies_integrate(const ocean_floating_body* __restrict__ bodies, const float* __restrict__ r2, int num_bodies,
+                                                 const ocean_buoyancy_result* __restrict__ hyd, const ocean_drag_result* __restrict__ drg,
+                                                 float density, float h, ocean_body_state* __restrict__ states, ocean_buoyancy_body* __restrict__ pose,
+                                                 ocean_body_velocity* __restrict__ vel, float* __restrict__ transforms,
+                                                 const DriveSum* __restrict__ sums) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= num_bodies) return;
     const ocean_floating_body b = bodies[i];
     ocean_body_state s = states[i];
     float R[12];                                    // the pose this sub-step started from: [R(q) | position]
     for (int k = 0; k < 12; ++k) R[k] = pose[i].transform[k];
-    const ocean_buoyancy_result fh = hyd[i];
-    const ocean_drag_result fd = drg[i];
+    ocean_buoyancy_result fh{};
+    ocean_drag_result fd{};
+    DriveSum ds{};
+    if constexpr (kDriven) ds = sums[i]; else { fh = hyd[i]; fd = drg[i]; }
     const float cv = (density * fd.wetted_drag_area) * fd.max_relative_speed;
-    const float cw = cv * __ldg(&r2[i]);
+    const float cw = kDriven ? 0.0f : cv * __ldg(&r2[i]);
     // linear: v' = v + (h / (m + h c_v)) F
     float F[3];
-    for (int k = 0; k < 3; ++k) F[k] = fh.force[k] + fd.force[k];
+    for (int k = 0; k < 3; ++k) F[k] = kDriven ? ds.force[k] : fh.force[k] + fd.force[k];
     F[1] = F[1] - b.mass * kG;
-    const float kv = __fdiv_rn(h, b.mass + h * cv);
+    const float kv = __fdiv_rn(h, kDriven ? ds.den_v : b.mass + h * cv);
     for (int k = 0; k < 3; ++k) s.linear_velocity[k] = s.linear_velocity[k] + kv * F[k];
     // angular, in body axes: w_b' = w_b + h tau_b / (I + h c_w), then w' = R w_b'
     float tau[3], tb[3], wb[3];
-    for (int k = 0; k < 3; ++k) tau[k] = fh.torque[k] + fd.torque[k];
+    for (int k = 0; k < 3; ++k) tau[k] = kDriven ? ds.torque[k] : fh.torque[k] + fd.torque[k];
     for (int k = 0; k < 3; ++k) {
         tb[k] = (R[k] * tau[0] + R[4 + k] * tau[1]) + R[8 + k] * tau[2];
         wb[k] = (R[k] * s.angular_velocity[0] + R[4 + k] * s.angular_velocity[1]) + R[8 + k] * s.angular_velocity[2];
     }
-    for (int k = 0; k < 3; ++k) wb[k] = wb[k] + __fdiv_rn(h * tb[k], b.inertia[k] + h * cw);
+    for (int k = 0; k < 3; ++k) wb[k] = wb[k] + __fdiv_rn(h * tb[k], kDriven ? ds.den_w[k] : b.inertia[k] + h * cw);
     for (int k = 0; k < 3; ++k) s.angular_velocity[k] = (R[4 * k] * wb[0] + R[4 * k + 1] * wb[1]) + R[4 * k + 2] * wb[2];
     // position and orientation: p' = p + h v',  q' = normalize(q + (h/2) (w' (x) q))
     for (int k = 0; k < 3; ++k) s.position[k] = s.position[k] + h * s.linear_velocity[k];
@@ -129,6 +137,21 @@ __global__ void __launch_bounds__(256) k_bodies_integrate(const ocean_floating_b
         for (int k = 0; k < 12; ++k) transforms[(size_t)i * 12 + k] = R[k];
 }
 
+__global__ void __launch_bounds__(256) k_bodies_integrate(const ocean_floating_body* __restrict__ bodies, const float* __restrict__ r2,
+                                                          int num_bodies, const ocean_buoyancy_result* __restrict__ hyd,
+                                                          const ocean_drag_result* __restrict__ drg, float density, float h,
+                                                          ocean_body_state* __restrict__ states, ocean_buoyancy_body* __restrict__ pose,
+                                                          ocean_body_velocity* __restrict__ vel, float* __restrict__ transforms) {
+    bodies_integrate<false>(bodies, r2, num_bodies, hyd, drg, density, h, states, pose, vel, transforms, nullptr);
+}
+
+__global__ void __launch_bounds__(256) k_bodies_integrate_driven(const ocean_floating_body* __restrict__ bodies, int num_bodies,
+                                                                 const DriveSum* __restrict__ sums, float h, ocean_body_state* __restrict__ states,
+                                                                 ocean_buoyancy_body* __restrict__ pose, ocean_body_velocity* __restrict__ vel,
+                                                                 float* __restrict__ transforms) {
+    bodies_integrate<true>(bodies, nullptr, num_bodies, nullptr, nullptr, 0.0f, h, states, pose, vel, transforms, sums);
+}
+
 }  // namespace
 
 cudaError_t launch_bodies_prepare(const ocean_floating_body* bodies_dev, const ocean_body_state* states_dev, int num_bodies,
@@ -148,6 +171,15 @@ cudaError_t launch_bodies_integrate(const ocean_floating_body* bodies_dev, const
     k_bodies_integrate<<<(unsigned)((num_bodies + 255) / 256), 256, 0, stream>>>(bodies_dev, r2_dev, num_bodies, hydrostatic_dev, drag_dev,
                                                                                  density, h, states_dev, pose_dev, velocities_dev,
                                                                                  transforms_dev);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_bodies_integrate_driven(const ocean_floating_body* bodies_dev, int num_bodies, const DriveSum* sums_dev, float h,
+                                           ocean_body_state* states_dev, ocean_buoyancy_body* pose_dev, ocean_body_velocity* velocities_dev,
+                                           float* transforms_dev, cudaStream_t stream) {
+    if (num_bodies <= 0) return cudaSuccess;
+    k_bodies_integrate_driven<<<(unsigned)((num_bodies + 255) / 256), 256, 0, stream>>>(bodies_dev, num_bodies, sums_dev, h, states_dev, pose_dev,
+                                                                                        velocities_dev, transforms_dev);
     return cudaGetLastError();
 }
 

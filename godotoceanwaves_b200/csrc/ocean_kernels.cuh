@@ -176,6 +176,42 @@ cudaError_t launch_bodies_integrate(const ocean_floating_body* bodies_dev, const
                                     const ocean_buoyancy_result* hydrostatic_dev, const ocean_drag_result* drag_dev, float density, float h,
                                     ocean_body_state* states_dev, ocean_buoyancy_body* pose_dev, ocean_body_velocity* velocities_dev,
                                     float* transforms_dev, cudaStream_t stream);
+// The driven form of integrate: the forces, torques and step denominators of each body from launch_drive_reduce's sums_dev.
+struct DriveSum {
+    float force[3], torque[3];      // hyd + drg, then the drive contributions in incidence order
+    float den_v, den_w[3];          // mass + h c_v (+ tethers), inertia + h c_w (+ tethers)
+};
+cudaError_t launch_bodies_integrate_driven(const ocean_floating_body* bodies_dev, int num_bodies, const DriveSum* sums_dev, float h,
+                                           ocean_body_state* states_dev, ocean_buoyancy_body* pose_dev, ocean_body_velocity* velocities_dev,
+                                           float* transforms_dev, cudaStream_t stream);
+
+// ocean_drive.cu: thrusters, foils, loads and tethers of the driven integrator (oracle/drive.py).  Actuator k (the thrusters,
+// then the foils) has world point world + k of the surface query.  One tether record per tether from the sub-step's tables:
+struct TetherForce {
+    float force[3];                 // T u, on body_a; body_b gets -T u
+    float torque_a[3], torque_b[3]; // r_a x (T u), r_b x (-T u)
+    float tension;                  // 0: slack, the tether adds nothing
+};
+struct DriveArgs {
+    const ocean_thruster* thrusters;    // [num_thrusters] device
+    int num_thrusters;
+    const ocean_foil* foils;            // [num_foils] device
+    int num_foils;
+    const ocean_tether* tethers;        // [num_tethers] device
+    int num_tethers;
+    const ocean_body_load* loads;       // [num_bodies] device, or null
+    const int* incidence_offsets;       // [num_bodies + 1] device: each body's range of incidence
+    const int* incidence;               // thruster k -> k, foil k -> T + k, tether k end e -> T + F + 2 k + e
+};
+cudaError_t launch_actuator_transform(const DriveArgs& d, const ocean_buoyancy_body* pose_dev, float2* q_dev, cudaStream_t stream);
+cudaError_t launch_tethers(const DriveArgs& d, const ocean_buoyancy_body* pose_dev, const ocean_body_velocity* velocities_dev,
+                           TetherForce* forces_dev, float* tensions_dev, cudaStream_t stream);
+cudaError_t launch_drive_reduce(const DriveArgs& d, int num_bodies, const ocean_floating_body* bodies_dev, const float* r2_dev,
+                                const ocean_buoyancy_body* pose_dev, const ocean_body_velocity* velocities_dev,
+                                const ocean_buoyancy_result* hydrostatic_dev, const ocean_drag_result* drag_dev,
+                                const ocean_surface_sample* actuator_samples_dev, const float* actuator_wv_dev, const TetherForce* tether_forces_dev,
+                                const uint2* velocity_dev, int map_size, int num_cascades, const float4* scales_dev, float density, float h,
+                                DriveSum* sums_dev, ocean_drive_result* drive_dev, cudaStream_t stream);
 
 // ocean_velocity.cu: velocity maps (oracle_velocity_update).  One record per cascade to recompute: the table slot and time of
 // the update that built the cascade's current maps.

@@ -393,6 +393,55 @@ class WaveGenerator:
             out += (transforms,)
         return out if len(out) > 1 else s
 
+    # -- driven and moored bodies: thrusters, hull foils, applied loads and tethers in the integrator ------------------
+    THRUSTER = np.dtype([("body", np.int32), ("position", np.float32, 3), ("direction", np.float32, 3), ("thrust", np.float32),
+                         ("half_height", np.float32)])                                    # struct ocean_thruster
+    FOIL = np.dtype([("body", np.int32), ("position", np.float32, 3), ("normal", np.float32, 3), ("area", np.float32),
+                     ("half_height", np.float32)])                                        # struct ocean_foil
+    BODY_LOAD = np.dtype([("force", np.float32, 3), ("torque", np.float32, 3)])           # struct ocean_body_load
+    TETHER = np.dtype([("body_a", np.int32), ("body_b", np.int32), ("point_a", np.float32, 3), ("point_b", np.float32, 3),
+                       ("rest_length", np.float32), ("stiffness", np.float32), ("damping", np.float32)])      # struct ocean_tether
+    DRIVE_RESULT = np.dtype([("force", np.float32, 3), ("torque", np.float32, 3), ("wetted_foil_area", np.float32),
+                             ("max_normal_speed", np.float32)])                           # struct ocean_drive_result
+
+    def drive_bodies(self, bodies, states, points, drag_areas, map_scales, dt: float, substeps: int = 1, density: float = 1025.0,
+                     tolerance: float = 1e-3, max_iterations: int = 8, thrusters=None, foils=None, loads=None, tethers=None,
+                     return_records: bool = False, return_tensions: bool = False, return_transforms: bool = False):
+        """simulate_bodies with the THRUSTER, FOIL and TETHER rows and one BODY_LOAD row per body (loads may be None) acting on
+        the bodies (include/ocean.h, ocean_simulate_driven_bodies).  Returns the new states; with return_records also the
+        (BUOYANCY_RESULT, DRAG_RESULT, DRIVE_RESULT) rows of the last sub-step, with return_tensions the last sub-step's tension
+        of each tether (float32), with return_transforms the [n][12] float32 transforms of the new states."""
+        self._require()
+        b = np.ascontiguousarray(bodies, self.FLOATING_BODY).reshape(-1)
+        s = np.array(states, self.BODY_STATE, copy=True).reshape(-1)
+        p = np.ascontiguousarray(points, self.BUOYANCY_POINT).reshape(-1)
+        a = np.ascontiguousarray(drag_areas, np.float32).reshape(-1)
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        th = np.ascontiguousarray(np.zeros(0, self.THRUSTER) if thrusters is None else thrusters, self.THRUSTER).reshape(-1)
+        fo = np.ascontiguousarray(np.zeros(0, self.FOIL) if foils is None else foils, self.FOIL).reshape(-1)
+        te = np.ascontiguousarray(np.zeros(0, self.TETHER) if tethers is None else tethers, self.TETHER).reshape(-1)
+        ld = None if loads is None else np.ascontiguousarray(loads, self.BODY_LOAD).reshape(-1)
+        if len(s) != len(b) or len(a) != len(p) or (ld is not None and len(ld) != len(b)):
+            raise ValueError(f"{len(s)} states for {len(b)} bodies, {len(a)} drag areas for {len(p)} points, or loads of another length")
+        hydro = np.zeros(len(b), self.BUOYANCY_RESULT) if return_records else None
+        drag = np.zeros(len(b), self.DRAG_RESULT) if return_records else None
+        drive = np.zeros(len(b), self.DRIVE_RESULT) if return_records else None
+        tensions = np.zeros(len(te), np.float32) if return_tensions else None
+        transforms = np.zeros((len(b), 12), np.float32) if return_transforms else None
+        ptr = lambda x: None if x is None or x.size == 0 else x.ctypes.data  # noqa: E731
+        check(load_library().ocean_simulate_driven_bodies(
+            self.context, len(b), ptr(b), ptr(s), len(p), ptr(p), ptr(a), sc.shape[0], sc.ctypes.data, float(density), float(dt),
+            int(substeps), float(tolerance), int(max_iterations), len(th), ptr(th), len(fo), ptr(fo), ptr(ld), len(te), ptr(te),
+            ptr(hydro), ptr(drag), ptr(drive), ptr(tensions), ptr(transforms)))
+        out = (s,)
+        if return_records:
+            out += (hydro, drag, drive)
+        if return_tensions:
+            out += (tensions,)
+        if return_transforms:
+            out += (transforms,)
+        return out if len(out) > 1 else s
+
     # -- spray candidates: the spawn test of sea_spray_particle.gdshader:80-94 as a stream compaction --------------
     SPRAY_RECORD = np.dtype([("index", np.uint32), ("start_x", np.float32), ("start_z", np.float32), ("scale_factor", np.float32),
                              ("particle_scale", np.float32, 3), ("foam", np.float32)])     # struct ocean_spray_record

@@ -443,6 +443,87 @@ int ocean_simulate_bodies_device(ocean_generator* gen, int num_bodies, const oce
                                  const float* map_scales_host, float density, float dt, int substeps, float tolerance, int max_iterations,
                                  ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev, float* transforms_dev);
 
+/* Driven and moored bodies -- ocean_simulate_bodies with thrusters, hull foils, applied loads and tethers (oracle/drive.py is
+ * the specification, bit for bit).  A boat is driven by a thruster, steered by a rudder foil, kept on course by a keel foil
+ * and moored or towed by a tether; the body state stays on the device as in ocean_simulate_bodies.  Per sub-step, with R, t,
+ * v and w the pose and velocity the sub-step starts from, r = R p for a hull-local point p, and f the submerged fraction of
+ * ocean_buoyancy at r + t with the actuator's half_height (its world point is queried with the hull's):
+ *   thruster  F = (f * thrust) * (R direction), T = r x F; a dry thruster (f = 0) adds nothing, so a propeller that leaves
+ *             the water on a crest pushes nothing
+ *   foil      d = u - (v + w x r), u the water velocity at the point as ocean_body_forces computes it (plus the wake's
+ *             vertical velocity while the coupling is live); n = R normal, dn = (d.x n.x + d.y n.y) + d.z n.z,
+ *             F = (((rho/2 * (f * area)) * dn) * |dn|) * n, T = r x F: normal-only drag of a flat plate, area = C_n A; dry adds
+ *             nothing
+ *   tether    x_a, x_b the end points (x_b = point_b, a world anchor, when body_b = -1), L = |x_b - x_a|, u = (x_b - x_a) / L,
+ *             s = k (L - L0) + c ((v_b - v_a) . u) with v_a, v_b the end points' velocities (0 at an anchor); the tension is
+ *             s when L > 0 and s > 0, else 0 (slack: the tether adds nothing); +T u acts at x_a and -T u at x_b
+ *   load      force and torque added as given (world frame, about the centre of mass)
+ *   step      ocean_simulate_bodies' step with the forces added onto F and tau in a fixed order (each body's thrusters,
+ *             foils and tether ends in array order, then its load), and the denominators widened by the new Jacobian
+ *             bounds: c_v += (density * sum f area) * max |dn| and c_w += that * max |p|^2 over the body's foil points; each
+ *             taut tether end adds h c + h^2 k to mass + h c_v and (h c) |p|^2 + (h^2 k) |p|^2 to every inertia + h c_w.
+ * For a linear spring this step has determinant 1 and trace in (-2, 2] at any h, for one body on an anchor and for bodies
+ * joined by lines: stiff mooring and tow lines do not blow up at 60 Hz.  No floating-point atomics: the result does not
+ * depend on the schedule.  A NaN or infinite actuator or load affects only its body, and a tether only the two bodies it
+ * joins.  A body with nothing attached and no load row takes ocean_simulate_bodies' step bit for bit, and a call with no
+ * thrusters, foils or tethers and loads = NULL is ocean_simulate_bodies (drive, when given, is zeroed).
+ * The actuator arrays and loads are host arrays in both entry points (a game changes them every tick).  Validation is
+ * ocean_simulate_bodies', plus: counts >= 0 and their arrays non-NULL when positive; every actuator's body and a tether's
+ * body_a in [0, num_bodies), body_b -1 or a body other than body_a; foil areas, rest lengths, stiffnesses and dampings finite
+ * and >= 0 (they enter the stability bound); world points plus actuators below 2^31.  Positions, directions, thrust and loads
+ * are not validated.  An invalid call launches nothing.  drive (may be NULL) receives per body the last sub-step's sum of the
+ * forces and torques the drive arguments added, the wetted foil area sum f area and max |dn|; tensions (may be NULL) the last
+ * sub-step's tension per tether.  With A = num_thrusters + num_foils, S sub-steps and anything attached, the call launches
+ * 1 + S (7 + a + t + 1) kernels, a = 1 when A > 0, t = 1 when num_tethers > 0 (1 + S (5 + a + t + 1) with max_iterations = 0,
+ * 1 + S (3 + t + 1) when there are no world points at all), and S more while the wake coupling is live. */
+typedef struct ocean_thruster {
+    int32_t body;
+    float position[3];          /* hull-local point of the propeller */
+    float direction[3];         /* hull-local direction of the push (not normalised: thrust scales it) */
+    float thrust;               /* N */
+    float half_height;          /* of the immersion column, as ocean_buoyancy_point's */
+} ocean_thruster;               /* 36 B */
+typedef struct ocean_foil {
+    int32_t body;
+    float position[3];          /* hull-local centre of pressure */
+    float normal[3];            /* hull-local unit normal of the plate */
+    float area;                 /* C_n A, m^2, finite and >= 0 */
+    float half_height;
+} ocean_foil;                   /* 36 B */
+typedef struct ocean_body_load {
+    float force[3];             /* world frame, N */
+    float torque[3];            /* world frame, about the centre of mass, N m */
+} ocean_body_load;              /* 24 B */
+typedef struct ocean_tether {
+    int32_t body_a;
+    int32_t body_b;             /* -1: point_b is a world anchor */
+    float point_a[3];           /* hull-local point of body_a */
+    float point_b[3];           /* hull-local point of body_b, or the world anchor */
+    float rest_length;          /* m, finite and >= 0 */
+    float stiffness;            /* N/m, finite and >= 0 */
+    float damping;              /* N s/m, finite and >= 0 */
+} ocean_tether;                 /* 44 B */
+typedef struct ocean_drive_result {
+    float force[3];             /* sum of the forces the thrusters, foils, tethers and load added */
+    float torque[3];            /* and of their torques about the centre of mass */
+    float wetted_foil_area;     /* sum f * area over the body's foils, m^2 */
+    float max_normal_speed;     /* max |dn| over the body's wet foils, m/s */
+} ocean_drive_result;           /* 32 B */
+int ocean_simulate_driven_bodies(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_host,
+                                 int num_points, const ocean_buoyancy_point* points_host, const float* drag_areas_host, int num_cascades,
+                                 const float* map_scales_host, float density, float dt, int substeps, float tolerance, int max_iterations,
+                                 int num_thrusters, const ocean_thruster* thrusters_host, int num_foils, const ocean_foil* foils_host,
+                                 const ocean_body_load* loads_host, int num_tethers, const ocean_tether* tethers_host,
+                                 ocean_buoyancy_result* hydrostatic_host, ocean_drag_result* drag_host, ocean_drive_result* drive_host,
+                                 float* tensions_host, float* transforms_host);
+int ocean_simulate_driven_bodies_device(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host,
+                                        ocean_body_state* states_dev, int num_points, const ocean_buoyancy_point* points_dev,
+                                        const float* drag_areas_dev, int num_cascades, const float* map_scales_host, float density, float dt,
+                                        int substeps, float tolerance, int max_iterations, int num_thrusters, const ocean_thruster* thrusters_host,
+                                        int num_foils, const ocean_foil* foils_host, const ocean_body_load* loads_host, int num_tethers,
+                                        const ocean_tether* tethers_host, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
+                                        ocean_drive_result* drive_dev, float* tensions_dev, float* transforms_dev);
+
 /* Velocity maps -- the water velocity: the time derivative of the displacement map, what drag, damping and floating debris
  * need.  A cascade's velocity layer is (vx, vy, vz, 0) = d/dt of its displacement texel (hx, hy, hz, 0): same layout, same
  * orientation (ocean_get_maps), RGBA16F, in m/s before the displacement scale.  It is computed exactly, as one more inverse

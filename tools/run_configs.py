@@ -3,7 +3,7 @@ config.
 
     python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast] [--spray-particles]
                                 [--wake] [--wake-coupling] [--wake-foam] [--wake-obstacles]
-                                [--wake-readers] [--sea-state] [--drifters]
+                                [--wake-readers] [--sea-state] [--drifters] [--drive]
 
 Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
 --query.  An unknown argument exits before anything touches the GPU."""
@@ -25,6 +25,7 @@ from godotoceanwaves_b200.native import check, load_library
 from oracle import bodies as ob
 from oracle import buoyancy as bu
 from oracle import drag as dr
+from oracle import drive as od
 from oracle import raycast as rc
 
 DEV = torch.device("cuda", 0)
@@ -493,6 +494,56 @@ def run_bodies(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, t
     print(json.dumps(out), flush=True)
 
 
+def run_drive(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, tolerance=1e-3, max_iterations=8):
+    """Driven bodies (ocean_simulate_driven_bodies_device) against ocean_simulate_bodies_device on the same fleet: every body
+    with 2 thrusters, 2 foils and a tether to its neighbour (the last one anchored), loads on every body.  Device times from
+    CUDA events, states restored before each window, alternating windows; the card's name, power limit and max SM clock are
+    read in the same run."""
+    g, _, scales = warmed_generator(N, C, 2)
+    bodies, states, hull, cda = _floating_scene(n_bodies, per_body)
+    rng = np.random.default_rng(5)
+    B = n_bodies
+    th = np.zeros(2 * B, od.THRUSTER)
+    th["body"] = np.repeat(np.arange(B), 2)
+    th["position"] = rng.uniform(-1.0, 1.0, (2 * B, 3))
+    th["direction"] = (1.0, 0.0, 0.0)
+    th["thrust"], th["half_height"] = 200.0, 0.3
+    fo = np.zeros(2 * B, od.FOIL)
+    fo["body"] = np.repeat(np.arange(B), 2)
+    fo["position"] = rng.uniform(-1.0, 1.0, (2 * B, 3))
+    fo["normal"] = (0.0, 0.0, 1.0)
+    fo["area"], fo["half_height"] = 0.5, 0.3
+    te = np.zeros(B, od.TETHER)
+    te["body_a"] = np.arange(B)
+    te["body_b"] = np.append(np.arange(1, B), -1)
+    te["point_b"][-1] = states["position"][-1]
+    ends = np.append(states["position"][1:], states["position"][-1:], 0)
+    te["rest_length"] = np.linalg.norm(ends - states["position"], axis=1) * 0.99       # just taut at the start
+    te["stiffness"], te["damping"] = 1e3, 50.0
+    loads = np.zeros(B, od.LOAD)
+    loads["force"] = (10.0, 0.0, 0.0)
+    hull_d = upload(hull)
+    cda_d = torch.from_numpy(cda).to(DEV)
+    st0_d = upload(states)
+    st_d = st0_d.clone()
+    torch.cuda.synchronize()
+    lib = load_library()
+    plain = lambda: check(lib.ocean_simulate_bodies_device(g.context, B, bodies.ctypes.data, st_d.data_ptr(), len(hull), hull_d.data_ptr(),  # noqa: E731
+                                                           cda_d.data_ptr(), C, scales.ctypes.data, 1025.0, dt, substeps, tolerance,
+                                                           max_iterations, None, None, None))
+    driven = lambda: check(lib.ocean_simulate_driven_bodies_device(  # noqa: E731
+        g.context, B, bodies.ctypes.data, st_d.data_ptr(), len(hull), hull_d.data_ptr(), cda_d.data_ptr(), C, scales.ctypes.data, 1025.0, dt,
+        substeps, tolerance, max_iterations, len(th), th.ctypes.data, len(fo), fo.ctypes.data, loads.ctypes.data, len(te), te.ctypes.data,
+        None, None, None, None, None))
+    restore = lambda: st_d.copy_(st0_d)  # noqa: E731
+    t_p, t_d = alternate(lambda: timed(g, plain, reps, 3, restore), lambda: timed(g, driven, reps, 3, restore), rounds=5)
+    out = {"config": label, **card(), "map_size": N, "cascades": C, "bodies": B, "points_per_body": per_body, "substeps": substeps,
+           "thrusters": len(th), "foils": len(fo), "tethers": len(te), "simulate_us_per_call": [1e3 * v for v in t_p],
+           "driven_us_per_call": [1e3 * v for v in t_d], "driven_over_simulate": min(t_d) / min(t_p) - 1.0}
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
 def run_simulate_coupling(N, C, n_bodies, per_body, substeps, reps, label, wake=512, dx=1.0, dt=1.0 / 60.0):
     """Wake coupling's cost in the body integrator: ocean_simulate_bodies_device on two generators with the same maps and a
     wake layer of wake x wake cells of dx centred on the world origin (it covers [-256, 256]^2 m of the scene's
@@ -862,6 +913,12 @@ GROUPS = {          # flag: its configs, in the order they run
         partial(run_drift, N, 4, n, 200 if n < (1 << 20) else 50, f"drifters: {'2^16' if n < (1 << 20) else '2^20'} over 4 cascades of {N}x{N}, "
                 "wake read off vs on")
         for N in (256, 1024) for n in (1 << 16, 1 << 20)
+    ],
+    "--drive": [
+        partial(run_drive, N, C, 1 << 14, 64, S, reps,
+                f"driven bodies: 2^14 bodies x 64 points, 2 thrusters, 2 foils and a tether each, {S} sub-step(s), {C} cascades of {N}x{N}, "
+                "vs simulate_bodies")
+        for S in (1, 4) for N, C, reps in ((256, 4, 50), (1024, 8, 20))
     ],
     "--wake-obstacles": [
         partial(run_wake_step_obstacles, N, k, 200 if N < 1024 else 50, f"wake obstacles, step: {N}x{N} cells, {k} source(s), 8 sub-steps")
