@@ -235,6 +235,30 @@ namespace OceanB200
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    public struct OceanHullMesh                                     // struct ocean_hull_mesh (24 B): a triangle-mesh hull
+    {
+        public int first_vertex, num_vertices;                      // range of the vertices ([3] float each, hull-local)
+        public int first_triangle, num_triangles;                   // range of the triangles ([3] int each, Godot's clockwise winding)
+        public float normal_drag, tangential_drag;                  // C_n, C_t, finite and >= 0
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanHullBody                              // struct ocean_hull_body (56 B)
+    {
+        public fixed float transform[12];                           // 3 x 4 row-major [R | t]
+        public int mesh;
+        public int reserved;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    public unsafe struct OceanFloatingHull                          // struct ocean_floating_hull (20 B)
+    {
+        public float mass;
+        public fixed float inertia[3];
+        public int mesh;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     public unsafe struct OceanRay                                   // struct ocean_ray (28 B)
     {
         public fixed float origin[3];
@@ -451,6 +475,28 @@ namespace OceanB200
                                                                         int num_foils, OceanFoil* foils, OceanBodyLoad* loads, int num_tethers,
                                                                         OceanTether* tethers, void* hydrostatic_dev, void* drag_dev, void* drive_dev,
                                                                         void* tensions_dev, void* transforms_dev);
+        // hull meshes: register triangle-mesh hulls once (volumes may be null), then pressure and drag over their wetted triangles
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_hull_set_meshes(IntPtr handle, int num_meshes, OceanHullMesh* meshes, int num_vertices, float* vertices,
+                                                          int num_triangles, int* triangles, float* volumes);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_hull_forces(IntPtr handle, int num_bodies, OceanHullBody* bodies, OceanBodyVelocity* velocities,
+                                                      int num_cascades, float* map_scales, float density, float tolerance, int max_iterations,
+                                                      OceanBuoyancyResult* hydrostatic, OceanDragResult* drag, OceanSurfaceSample* samples);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_hull_forces_device(IntPtr handle, int num_bodies, OceanHullBody* bodies, OceanBodyVelocity* velocities,
+                                                             int num_cascades, float* map_scales, float density, float tolerance, int max_iterations,
+                                                             void* hydrostatic_dev, void* drag_dev, void* samples_dev);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_simulate_hull_bodies(IntPtr handle, int num_bodies, OceanFloatingHull* bodies, OceanBodyState* states,
+                                                               int num_cascades, float* map_scales, float density, float dt, int substeps,
+                                                               float tolerance, int max_iterations, OceanBuoyancyResult* hydrostatic,
+                                                               OceanDragResult* drag, float* transforms);
+        [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
+        internal static partial int ocean_simulate_hull_bodies_device(IntPtr handle, int num_bodies, OceanFloatingHull* bodies, void* states_dev,
+                                                                      int num_cascades, float* map_scales, float density, float dt, int substeps,
+                                                                      float tolerance, int max_iterations, void* hydrostatic_dev, void* drag_dev,
+                                                                      void* transforms_dev);
         // velocity maps: d/dt of the displacement map, recomputed for the cascades whose maps changed; recomputed may be null
         [LibraryImport(Lib)] [UnmanagedCallConv(CallConvs = new[] { typeof(System.Runtime.CompilerServices.CallConvCdecl) })]
         internal static partial int ocean_update_velocity(IntPtr handle, int* recomputed);

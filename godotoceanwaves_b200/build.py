@@ -9,7 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libocean.so")
 SOURCES = ["ocean_kernels.cu", "ocean_sample.cu", "ocean_spray.cu", "ocean_buoyancy.cu", "ocean_bodies.cu", "ocean_velocity.cu",
-           "ocean_wake.cu", "ocean_drift.cu", "ocean_drive.cu", "ocean_api.cu"]
+           "ocean_wake.cu", "ocean_drift.cu", "ocean_drive.cu", "ocean_hull.cu", "ocean_api.cu"]
 HEADERS = ["ocean_kernels.cuh", "ocean_texture.cuh", "detmath.cuh", "fft_core.cuh", "wake_sample.cuh", os.path.join("..", "..", "include", "ocean.h")]
 
 NVCC_FLAGS = [

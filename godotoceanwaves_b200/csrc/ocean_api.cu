@@ -66,7 +66,7 @@ struct DeviceArray {
 enum StagedOp {
     kStageSampleMaps, kStageExtractSpray, kStageSprayParticles, kStageQuerySurface, kStageRaycast, kStageBuoyancy,
     kStageSampleVelocity, kStageBodyForces, kStageSimulateBodies, kStageDeviceMath, kStageWakeStep, kStageSampleWake, kStageDrift,
-    kStageDrivenBodies, kNumStagedOps
+    kStageDrivenBodies, kStageHullForces, kStageSimulateHulls, kNumStagedOps
 };
 
 // The parts of the wake layer WakeLayer::off turns off; kWakeLayer is the whole layer.
@@ -192,6 +192,16 @@ struct ocean_generator {
     DeviceArray<ocean::DriveSum> drive_sums;
     DeviceArray<ocean_drive_result> drive_results;
     DeviceArray<float> drive_tensions;
+    // hull meshes (ocean_hull_set_meshes): the registered set, and a host copy of its mesh records (the calls validate the
+    // bodies' mesh indices and count their world vertices from it); the calls' scratch: the pose table, the per-world-vertex
+    // (r, d) and (u, 0) of k_hull_vertex, and the integrator's hull rows
+    DeviceArray<ocean_hull_mesh> hull_meshes;
+    DeviceArray<float> hull_vertices;
+    DeviceArray<int32_t> hull_triangles;
+    std::vector<ocean_hull_mesh> hull_meshes_host;
+    DeviceArray<ocean_hull_body> hull_poses;
+    DeviceArray<float4> hull_corners;
+    DeviceArray<ocean_floating_hull> hull_bodies;
     // velocity maps, allocated by the first velocity call: row-pass scratch, the map, its binary32 tap while the taps are on
     DeviceArray<float4> vel_scratch;                    // [num_cascades][N][N]
     DeviceArray<uint2> velocity;                        // [num_cascades][N][N] 4 x half
@@ -2112,6 +2122,300 @@ int ocean_simulate_driven_bodies(ocean_generator* gen, int num_bodies, const oce
                                                               num_thrusters, thrusters_host, num_foils, foils_host, loads_host, num_tethers,
                                                               tethers_host, st[hydrostatic], st[drag], st[drive_out], st[tensions],
                                                               st[transforms]));
+}
+
+// ---- hull meshes: pressure and drag integrated over the wetted triangles (ocean_hull.cu; oracle/hull.py) ----
+static_assert(sizeof(ocean_hull_mesh) == 24 && sizeof(ocean_hull_body) == 56 && sizeof(ocean_floating_hull) == 20, "hull record layouts");
+static_assert(offsetof(ocean_hull_body, transform) == offsetof(ocean_buoyancy_body, transform) && sizeof(ocean_hull_body) == sizeof(ocean_buoyancy_body),
+              "k_bodies_integrate writes hull pose rows as ocean_buoyancy_body rows");
+
+namespace {
+bool finite_nonnegative_coefficient(float x) { return x >= 0.0f && std::isfinite(x); }
+
+// Every check of ocean_hull_set_meshes, on the host, before anything is uploaded; volumes (may be null) receives each mesh's
+// signed volume, sum over its triangles of p0 . (p2 x p1) / 6 in binary64 (Godot's clockwise winding: positive when closed
+// and wound outward).
+int check_hull_meshes(int num_meshes, const ocean_hull_mesh* meshes, int num_vertices, const float* vertices, int num_triangles,
+                      const int32_t* triangles, float* volumes) {
+    constexpr int kMaxElements = INT32_MAX / 3;         // 3 * index stays an int32
+    if (num_meshes < 0 || num_vertices < 0 || num_triangles < 0)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "a count is negative (meshes %d, vertices %d, triangles %d)", num_meshes, num_vertices,
+                    num_triangles);
+    if (num_vertices > kMaxElements || num_triangles > kMaxElements)
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "%d vertices or %d triangles above (2^31 - 1) / 3", num_vertices, num_triangles);
+    if ((num_meshes > 0 && !meshes) || (num_vertices > 0 && !vertices) || (num_triangles > 0 && !triangles))
+        return fail(OCEAN_ERR_INVALID_ARGUMENT, "an array is NULL where its count is positive");
+    for (size_t k = 0; k < 3 * (size_t)num_vertices; ++k)
+        if (!std::isfinite(vertices[k])) return fail(OCEAN_ERR_INVALID_ARGUMENT, "vertex %zu is not finite", k / 3);
+    for (int m = 0; m < num_meshes; ++m) {
+        const ocean_hull_mesh& h = meshes[m];
+        const long long fv = h.first_vertex, nv = h.num_vertices, ft = h.first_triangle, nt = h.num_triangles;
+        if (nv < 0 || fv < 0 || fv + nv > num_vertices)
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "mesh %d: vertices [%lld, %lld) outside [0, %d)", m, fv, fv + nv, num_vertices);
+        if (nt < 0 || ft < 0 || ft + nt > num_triangles)
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "mesh %d: triangles [%lld, %lld) outside [0, %d)", m, ft, ft + nt, num_triangles);
+        if (!finite_nonnegative_coefficient(h.normal_drag) || !finite_nonnegative_coefficient(h.tangential_drag))
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "mesh %d: drag coefficients %g, %g are not finite and >= 0", m, h.normal_drag,
+                        h.tangential_drag);
+        const int32_t* tri = triangles + 3 * ft;
+        for (long long k = 0; k < 3 * nt; ++k)
+            if (tri[k] < 0 || tri[k] >= nv)
+                return fail(OCEAN_ERR_INVALID_ARGUMENT, "mesh %d: triangle %lld index %d outside [0, %lld)", m, k / 3, tri[k], nv);
+    }
+    if (!volumes) return OCEAN_OK;
+    for (int m = 0; m < num_meshes; ++m) {
+        const ocean_hull_mesh& h = meshes[m];
+        const float* p = vertices + 3 * (size_t)h.first_vertex;
+        const int32_t* tri = triangles + 3 * (size_t)h.first_triangle;
+        double v = 0.0;
+        for (int j = 0; j < h.num_triangles; ++j) {
+            const float* a = p + 3 * (size_t)tri[3 * j];
+            const float* b = p + 3 * (size_t)tri[3 * j + 1];
+            const float* c = p + 3 * (size_t)tri[3 * j + 2];
+            const double cx = (double)c[1] * b[2] - (double)c[2] * b[1];
+            const double cy = (double)c[2] * b[0] - (double)c[0] * b[2];
+            const double cz = (double)c[0] * b[1] - (double)c[1] * b[0];
+            v += (double)a[0] * cx + (double)a[1] * cy + (double)a[2] * cz;
+        }
+        volumes[m] = (float)(v / 6.0);
+    }
+    return OCEAN_OK;
+}
+
+// The bodies' mesh indices against the registered set; *world receives the number of world vertices.
+extern "C++" template <typename Row>
+int check_hull_bodies(const ocean_generator* gen, int num_bodies, const Row* bodies, int* world) {
+    if (num_bodies < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_bodies %d is negative", num_bodies);
+    if (num_bodies > 0 && !bodies) return fail(OCEAN_ERR_INVALID_ARGUMENT, "bodies is NULL");
+    const int meshes = (int)gen->hull_meshes_host.size();
+    if (num_bodies > 0 && meshes == 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "no hull meshes are registered (ocean_hull_set_meshes)");
+    long long total = 0;
+    for (int b = 0; b < num_bodies; ++b) {
+        if (bodies[b].mesh < 0 || bodies[b].mesh >= meshes)
+            return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: mesh %d outside [0, %d)", b, bodies[b].mesh, meshes);
+        total += gen->hull_meshes_host[bodies[b].mesh].num_vertices;
+    }
+    if (total > INT32_MAX) return fail(OCEAN_ERR_INVALID_ARGUMENT, "%lld world vertices exceed INT32_MAX", total);
+    *world = (int)total;
+    return OCEAN_OK;
+}
+
+// The exclusive prefix of the bodies' meshes' num_vertices into gen->buoy_offsets_host, uploaded to gen->buoy_offsets.
+extern "C++" template <typename Row>
+int upload_hull_offsets(ocean_generator* gen, int num_bodies, const Row* bodies_host) {
+    std::vector<int>& offsets = gen->buoy_offsets_host;
+    offsets.resize((size_t)num_bodies);
+    for (int b = 0, start = 0; b < num_bodies; start += gen->hull_meshes_host[bodies_host[b].mesh].num_vertices, ++b) offsets[b] = start;
+    OCEAN_CUDA(gen->buoy_offsets.upload(gen, offsets.data(), (size_t)num_bodies));
+    return OCEAN_OK;
+}
+
+int check_hull_forces_args(const ocean_generator* gen, int num_bodies, const ocean_hull_body* bodies, const ocean_body_velocity* velocities,
+                           float density, float tolerance, int max_iterations, int* world) {
+    int rc = check_surface_args(0, tolerance, max_iterations);
+    if (rc) return rc;
+    if (!(density > 0.0f) || !std::isfinite(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
+    if ((rc = check_hull_bodies(gen, num_bodies, bodies, world))) return rc;
+    if (num_bodies > 0 && !velocities) return fail(OCEAN_ERR_INVALID_ARGUMENT, "velocities is NULL");
+    return OCEAN_OK;
+}
+
+// Grows the per-world-vertex scratch of a hull call: query points, corners, the surface records when the caller wants none
+// (returned in *samples) and the wake's vertical velocities while the coupling is live (*wv, else null).
+int grow_hull_scratch(ocean_generator* gen, int world, ocean_surface_sample** samples, float** wv) {
+    const size_t n = (size_t)world;
+    OCEAN_CUDA(gen->buoy_q.grow(gen, n));
+    OCEAN_CUDA(gen->hull_corners.grow(gen, 2 * n));
+    if (!*samples) {
+        OCEAN_CUDA(gen->buoy_samples.grow(gen, n));
+        *samples = gen->buoy_samples.ptr;
+    }
+    *wv = nullptr;
+    if (world > 0 && gen->wake.coupling_live()) {
+        OCEAN_CUDA(gen->wake.wv.grow(gen, n));
+        *wv = gen->wake.wv.ptr;
+    }
+    return OCEAN_OK;
+}
+
+// The hull-forces launches on a pose table, velocities and offsets already in device memory (the poses may be written by
+// earlier kernels on the stream), with the map scales in gen->q_scales and the scratch grown to `world`.
+int launch_hull_sequence(ocean_generator* gen, const ocean_hull_body* poses_dev, const ocean_body_velocity* velocities_dev, int num_bodies,
+                         int world, int num_cascades, float density, float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_dev,
+                         ocean_drag_result* drag_dev, ocean_surface_sample* samples, float* wv) {
+    int rc;
+    float4* corner_r = gen->hull_corners.ptr;
+    float4* corner_u = corner_r + world;
+    if (world > 0) {
+        OCEAN_CUDA(ocean::launch_hull_transform(poses_dev, gen->buoy_offsets.ptr, num_bodies, gen->hull_meshes.ptr, gen->hull_vertices.ptr, world,
+                                                gen->buoy_q.ptr, corner_r, gen->stream));
+        gen->kernel_launches += 1;
+        if ((rc = run_query_surface(gen, world, gen->buoy_q.ptr, num_cascades, tolerance, max_iterations, samples, wv))) return rc;
+        OCEAN_CUDA(ocean::launch_hull_vertex(samples, world, gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, wv, corner_r,
+                                             corner_u, gen->stream));
+        gen->kernel_launches += 1;
+    }
+    const float rho_g = density * 9.81f;                                 // G, wave_generator.gd:5, in binary32
+    const float half_rho = 0.5f * density;
+    OCEAN_CUDA(ocean::launch_hull_reduce(poses_dev, velocities_dev, gen->buoy_offsets.ptr, num_bodies, gen->hull_meshes.ptr, gen->hull_triangles.ptr,
+                                         corner_r, corner_u, samples, rho_g, half_rho, tolerance, hydrostatic_dev, drag_dev, gen->stream));
+    gen->kernel_launches += 1;
+    return OCEAN_OK;
+}
+
+// ocean_simulate_bodies' checks on hull bodies; *world as for check_hull_bodies.
+int check_simulate_hull_args(const ocean_generator* gen, int num_bodies, const ocean_floating_hull* bodies, const ocean_body_state* states,
+                             float density, float dt, int substeps, float tolerance, int max_iterations, int* world) {
+    int rc = check_surface_args(0, tolerance, max_iterations);
+    if (rc) return rc;
+    if (!finite_positive(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
+    if (!finite_positive(dt)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "dt %g is not finite and > 0", dt);
+    if (substeps < 1 || substeps > 64) return fail(OCEAN_ERR_INVALID_ARGUMENT, "substeps %d outside [1, 64]", substeps);
+    if ((rc = check_hull_bodies(gen, num_bodies, bodies, world))) return rc;
+    if (num_bodies > 0 && !states) return fail(OCEAN_ERR_INVALID_ARGUMENT, "states is NULL");
+    for (int b = 0; b < num_bodies; ++b) {
+        const ocean_floating_hull& fb = bodies[b];
+        if (!finite_positive(fb.mass)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: mass %g is not finite and > 0", b, fb.mass);
+        for (int k = 0; k < 3; ++k)
+            if (!finite_positive(fb.inertia[k]))
+                return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: inertia[%d] %g is not finite and > 0", b, k, fb.inertia[k]);
+    }
+    return OCEAN_OK;
+}
+}  // namespace
+
+int ocean_hull_set_meshes(ocean_generator* gen, int num_meshes, const ocean_hull_mesh* meshes_host, int num_vertices,
+                          const float* vertices_host, int num_triangles, const int32_t* triangles_host, float* volumes_host) {
+    int rc = check_hull_meshes(num_meshes, meshes_host, num_vertices, vertices_host, num_triangles, triangles_host, volumes_host);
+    if (rc) return rc;
+    DeviceScope device_scope__;
+    if ((rc = enter_gen(gen, device_scope__))) return rc;
+    gen->hull_meshes_host.clear();                      // off until the new set is in place
+    if (num_meshes == 0) {
+        OCEAN_CUDA(cudaStreamSynchronize(gen->stream));  // an earlier call may still read the set
+        gen->hull_meshes.release();
+        gen->hull_vertices.release();
+        gen->hull_triangles.release();
+        return OCEAN_OK;
+    }
+    // stream order puts the copies after the calls that read the old set; the call returns once they are done
+    OCEAN_CUDA(gen->hull_meshes.upload(gen, meshes_host, (size_t)num_meshes));
+    if (num_vertices > 0) OCEAN_CUDA(gen->hull_vertices.upload(gen, vertices_host, 3 * (size_t)num_vertices));
+    if (num_triangles > 0) OCEAN_CUDA(gen->hull_triangles.upload(gen, triangles_host, 3 * (size_t)num_triangles));
+    OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
+    gen->hull_meshes_host.assign(meshes_host, meshes_host + num_meshes);
+    return OCEAN_OK;
+}
+
+int ocean_hull_forces_device(ocean_generator* gen, int num_bodies, const ocean_hull_body* bodies_host,
+                             const ocean_body_velocity* velocities_host, int num_cascades, const float* map_scales_host, float density,
+                             float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
+                             ocean_surface_sample* samples_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_hull_forces_args(gen, num_bodies, bodies_host, velocities_host, density, tolerance, max_iterations, &world))) return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (!hydrostatic_dev || !drag_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
+    if ((rc = refresh_velocity(gen, nullptr))) return rc;
+    ocean_surface_sample* samples = samples_dev;
+    float* wv = nullptr;
+    if ((rc = grow_hull_scratch(gen, world, &samples, &wv))) return rc;
+    OCEAN_CUDA(gen->hull_poses.upload(gen, bodies_host, (size_t)num_bodies));
+    OCEAN_CUDA(gen->drag_velocities.upload(gen, velocities_host, (size_t)num_bodies));
+    if ((rc = upload_hull_offsets(gen, num_bodies, bodies_host))) return rc;
+    return launch_hull_sequence(gen, gen->hull_poses.ptr, gen->drag_velocities.ptr, num_bodies, world, num_cascades, density, tolerance,
+                                max_iterations, hydrostatic_dev, drag_dev, samples, wv);
+}
+
+int ocean_hull_forces(ocean_generator* gen, int num_bodies, const ocean_hull_body* bodies_host, const ocean_body_velocity* velocities_host,
+                      int num_cascades, const float* map_scales_host, float density, float tolerance, int max_iterations,
+                      ocean_buoyancy_result* hydrostatic_host, ocean_drag_result* drag_host, ocean_surface_sample* samples_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_hull_forces_args(gen, num_bodies, bodies_host, velocities_host, density, tolerance, max_iterations, &world))) return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if (!hydrostatic_host || !drag_host) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a host buffer is NULL");
+    const size_t B = (size_t)num_bodies;
+    Staging st;
+    const auto hydrostatic = st.out(hydrostatic_host, B);
+    const auto drag = st.out(drag_host, B);
+    const auto samples = st.out(samples_host, (size_t)world);
+    if ((rc = st.upload(gen, kStageHullForces))) return rc;
+    return st.finish(gen, ocean_hull_forces_device(gen, num_bodies, bodies_host, velocities_host, num_cascades, map_scales_host, density,
+                                                   tolerance, max_iterations, st[hydrostatic], st[drag], st[samples]));
+}
+
+int ocean_simulate_hull_bodies_device(ocean_generator* gen, int num_bodies, const ocean_floating_hull* bodies_host,
+                                      ocean_body_state* states_dev, int num_cascades, const float* map_scales_host, float density, float dt,
+                                      int substeps, float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_dev,
+                                      ocean_drag_result* drag_dev, float* transforms_dev) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_simulate_hull_args(gen, num_bodies, bodies_host, states_dev, density, dt, substeps, tolerance, max_iterations, &world)))
+        return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
+    if ((rc = refresh_velocity(gen, nullptr))) return rc;
+    const size_t B = (size_t)num_bodies;
+    ocean_surface_sample* samples = nullptr;
+    float* wv = nullptr;                                // every sub-step reads the same snapshots
+    if ((rc = grow_hull_scratch(gen, world, &samples, &wv))) return rc;
+    OCEAN_CUDA(gen->sim_r2.grow(gen, B));
+    OCEAN_CUDA(gen->sim_bodies.grow(gen, B));
+    OCEAN_CUDA(gen->hull_poses.grow(gen, B));
+    OCEAN_CUDA(gen->drag_velocities.grow(gen, B));
+    if (!hydrostatic_dev) {
+        OCEAN_CUDA(gen->buoy_results.grow(gen, B));
+        hydrostatic_dev = gen->buoy_results.ptr;
+    }
+    if (!drag_dev) {
+        OCEAN_CUDA(gen->drag_results.grow(gen, B));
+        drag_dev = gen->drag_results.ptr;
+    }
+    OCEAN_CUDA(gen->hull_bodies.upload(gen, bodies_host, B));
+    if ((rc = upload_hull_offsets(gen, num_bodies, bodies_host))) return rc;
+    ocean_hull_body* poses = gen->hull_poses.ptr;
+    ocean_body_velocity* velocities = gen->drag_velocities.ptr;
+    OCEAN_CUDA(ocean::launch_hull_prepare(gen->hull_bodies.ptr, states_dev, num_bodies, gen->hull_meshes.ptr, gen->hull_vertices.ptr,
+                                          gen->sim_r2.ptr, poses, velocities, gen->sim_bodies.ptr, gen->stream));
+    gen->kernel_launches += 1;
+    const float h = dt / (float)substeps;
+    for (int s = 0; s < substeps; ++s) {
+        if ((rc = launch_hull_sequence(gen, poses, velocities, num_bodies, world, num_cascades, density, tolerance, max_iterations,
+                                       hydrostatic_dev, drag_dev, samples, wv)))
+            return rc;
+        OCEAN_CUDA(ocean::launch_bodies_integrate(gen->sim_bodies.ptr, gen->sim_r2.ptr, num_bodies, hydrostatic_dev, drag_dev, density, h,
+                                                  states_dev, reinterpret_cast<ocean_buoyancy_body*>(poses), velocities,
+                                                  s == substeps - 1 ? transforms_dev : nullptr, gen->stream));
+        gen->kernel_launches += 1;
+    }
+    return OCEAN_OK;
+}
+
+int ocean_simulate_hull_bodies(ocean_generator* gen, int num_bodies, const ocean_floating_hull* bodies_host, ocean_body_state* states_host,
+                               int num_cascades, const float* map_scales_host, float density, float dt, int substeps, float tolerance,
+                               int max_iterations, ocean_buoyancy_result* hydrostatic_host, ocean_drag_result* drag_host,
+                               float* transforms_host) {
+    OCEAN_ENTER(gen);
+    if (rc) return rc;
+    int world = 0;
+    if ((rc = check_simulate_hull_args(gen, num_bodies, bodies_host, states_host, density, dt, substeps, tolerance, max_iterations, &world)))
+        return rc;
+    if (num_bodies == 0) return OCEAN_OK;
+    const size_t B = (size_t)num_bodies;
+    Staging st;                                         // an output not asked for stays NULL: the twin uses its own
+    const auto states = st.inout(states_host, B);
+    const auto hydrostatic = st.out(hydrostatic_host, B);
+    const auto drag = st.out(drag_host, B);
+    const auto transforms = st.out(transforms_host, 12 * B);
+    if ((rc = st.upload(gen, kStageSimulateHulls))) return rc;
+    return st.finish(gen, ocean_simulate_hull_bodies_device(gen, num_bodies, bodies_host, st[states], num_cascades, map_scales_host, density,
+                                                            dt, substeps, tolerance, max_iterations, st[hydrostatic], st[drag],
+                                                            st[transforms]));
 }
 
 int ocean_copy_twiddles_to_host(ocean_generator* gen, float* host) {

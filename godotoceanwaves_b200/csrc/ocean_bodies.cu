@@ -10,6 +10,8 @@
 //   k_bodies_integrate   one thread per body: the semi-implicit step of the specification from the state, the pose the
 //                        sub-step started from and its two records; writes the new state, the next sub-step's pose and
 //                        velocity rows, and on the last sub-step the 3 x 4 transform of the final state when asked to.
+// ocean_simulate_hull_bodies (ocean_hull.cu) runs k_hull_prepare, the same prepare over a hull mesh's vertices, in place of
+// k_bodies_prepare, and k_bodies_integrate on pose rows of ocean_hull_body (ocean_buoyancy_body's layout).
 // ocean_simulate_driven_bodies runs k_bodies_integrate_driven instead, the same step on the forces and denominators of
 // ocean_drive.cu's reduce (both are forms of one inlined template).
 // Nothing crosses PCIe between sub-steps.  Numeric policy: binary32, the specification's operation order, no contraction
@@ -152,6 +154,44 @@ __global__ void __launch_bounds__(256) k_bodies_integrate_driven(const ocean_flo
     bodies_integrate<true>(bodies, nullptr, num_bodies, nullptr, nullptr, 0.0f, h, states, pose, vel, transforms, sums);
 }
 
+// r2 = the NaN-dropping max of |p|^2 over the mesh's vertices, the first sub-step's pose row ([R(q) | position], the mesh) and
+// velocity row: k_bodies_prepare on a hull mesh; and the body's ocean_floating_body row (its mass and inertia, the mesh's
+// vertex range), the table k_bodies_integrate reads.
+__global__ void __launch_bounds__(256) k_hull_prepare(const ocean_floating_hull* __restrict__ bodies, const ocean_body_state* __restrict__ states,
+                                                      int num_bodies, const ocean_hull_mesh* __restrict__ meshes,
+                                                      const float* __restrict__ vertices, float* __restrict__ r2, ocean_hull_body* __restrict__ pose,
+                                                      ocean_body_velocity* __restrict__ vel, ocean_floating_body* __restrict__ rows) {
+    const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (warp >= (size_t)num_bodies) return;        // whole warps: the shuffles below see all 32 lanes
+    const int body = (int)warp;
+    const int lane = threadIdx.x & 31;
+    const ocean_floating_hull b = bodies[body];
+    const ocean_hull_mesh mesh = meshes[b.mesh];
+    const float* p0 = vertices + 3 * (size_t)mesh.first_vertex;
+    float m = 0.0f;
+    for (int j = lane; j < mesh.num_vertices; j += 32) {
+        const float* p = p0 + 3 * (size_t)j;
+        m = fmaxf(m, (p[0] * p[0] + p[1] * p[1]) + p[2] * p[2]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_down_sync(0xffffffffu, m, o));
+    if (lane != 0) return;
+    r2[body] = m;
+    rows[body] = ocean_floating_body{b.mass, {b.inertia[0], b.inertia[1], b.inertia[2]}, mesh.first_vertex, mesh.num_vertices};
+    const ocean_body_state& s = states[body];
+    ocean_hull_body pb;
+    pose_transform(s.orientation, s.position, pb.transform);
+    pb.mesh = b.mesh;
+    pb.reserved = 0;
+    pose[body] = pb;
+    ocean_body_velocity v;
+    for (int k = 0; k < 3; ++k) {
+        v.linear[k] = s.linear_velocity[k];
+        v.angular[k] = s.angular_velocity[k];
+    }
+    vel[body] = v;
+}
+
 }  // namespace
 
 cudaError_t launch_bodies_prepare(const ocean_floating_body* bodies_dev, const ocean_body_state* states_dev, int num_bodies,
@@ -180,6 +220,16 @@ cudaError_t launch_bodies_integrate_driven(const ocean_floating_body* bodies_dev
     if (num_bodies <= 0) return cudaSuccess;
     k_bodies_integrate_driven<<<(unsigned)((num_bodies + 255) / 256), 256, 0, stream>>>(bodies_dev, num_bodies, sums_dev, h, states_dev, pose_dev,
                                                                                         velocities_dev, transforms_dev);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_hull_prepare(const ocean_floating_hull* bodies_dev, const ocean_body_state* states_dev, int num_bodies,
+                                const ocean_hull_mesh* meshes_dev, const float* vertices_dev, float* r2_dev, ocean_hull_body* pose_dev,
+                                ocean_body_velocity* velocities_dev, ocean_floating_body* rows_dev, cudaStream_t stream) {
+    if (num_bodies <= 0) return cudaSuccess;
+    const unsigned blocks = (unsigned)(((size_t)num_bodies * 32 + 255) / 256);      // 8 bodies per block
+    k_hull_prepare<<<blocks, 256, 0, stream>>>(bodies_dev, states_dev, num_bodies, meshes_dev, vertices_dev, r2_dev, pose_dev, velocities_dev,
+                                               rows_dev);
     return cudaGetLastError();
 }
 

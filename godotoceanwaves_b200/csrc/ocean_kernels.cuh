@@ -165,6 +165,20 @@ cudaError_t launch_drag_reduce(const ocean_buoyancy_body* bodies_dev, const ocea
                                const float4* scales_dev, float half_rho, ocean_drag_result* results_dev, const float* wake_wv_dev,
                                cudaStream_t stream);
 
+// ocean_hull.cu: hull-mesh forces (oracle/hull.py).  bodies_dev / velocities_dev = [num_bodies], offsets_dev = the exclusive
+// prefix of their meshes' num_vertices (body-major world vertices), meshes / vertices / triangles = the registered set;
+// q_dev = [n] query points, corner_r_dev / corner_u_dev = [n] (r, w.y then d) and (u, 0) per world vertex, samples_dev = [n]
+// surface records, wake_wv_dev (may be null) = [n] the wake's vertical velocities
+cudaError_t launch_hull_transform(const ocean_hull_body* bodies_dev, const int* offsets_dev, int num_bodies, const ocean_hull_mesh* meshes_dev,
+                                  const float* vertices_dev, int n, float2* q_dev, float4* corner_r_dev, cudaStream_t stream);
+cudaError_t launch_hull_vertex(const ocean_surface_sample* samples_dev, int n, const uint2* velocity_dev, int map_size, int num_cascades,
+                               const float4* scales_dev, const float* wake_wv_dev, float4* corner_r_dev, float4* corner_u_dev,
+                               cudaStream_t stream);
+cudaError_t launch_hull_reduce(const ocean_hull_body* bodies_dev, const ocean_body_velocity* velocities_dev, const int* offsets_dev,
+                               int num_bodies, const ocean_hull_mesh* meshes_dev, const int* triangles_dev, const float4* corner_r_dev,
+                               const float4* corner_u_dev, const ocean_surface_sample* samples_dev, float rho_g, float half_rho,
+                               float tolerance, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev, cudaStream_t stream);
+
 // ocean_bodies.cu: the floating-body integrator (oracle/bodies.py).  bodies_dev / states_dev = [num_bodies], r2_dev =
 // [num_bodies] max |p|^2 over each hull, pose_dev / velocities_dev = the tables the body-forces kernels read.  prepare fills r2
 // and the first sub-step's tables; integrate takes one sub-step of h from the records of the tables' pose and writes the next
@@ -176,6 +190,12 @@ cudaError_t launch_bodies_integrate(const ocean_floating_body* bodies_dev, const
                                     const ocean_buoyancy_result* hydrostatic_dev, const ocean_drag_result* drag_dev, float density, float h,
                                     ocean_body_state* states_dev, ocean_buoyancy_body* pose_dev, ocean_body_velocity* velocities_dev,
                                     float* transforms_dev, cudaStream_t stream);
+// prepare for hull meshes (ocean_simulate_hull_bodies): r2 over the mesh's vertices, pose rows of ocean_hull_body, which
+// launch_bodies_integrate takes as ocean_buoyancy_body rows (same layout; it writes only the transform), and rows_dev =
+// [num_bodies] the ocean_floating_body rows (mass, inertia) launch_bodies_integrate reads
+cudaError_t launch_hull_prepare(const ocean_floating_hull* bodies_dev, const ocean_body_state* states_dev, int num_bodies,
+                                const ocean_hull_mesh* meshes_dev, const float* vertices_dev, float* r2_dev, ocean_hull_body* pose_dev,
+                                ocean_body_velocity* velocities_dev, ocean_floating_body* rows_dev, cudaStream_t stream);
 // The driven form of integrate: the forces, torques and step denominators of each body from launch_drive_reduce's sums_dev.
 struct DriveSum {
     float force[3], torque[3];      // hyd + drg, then the drive contributions in incidence order

@@ -94,6 +94,15 @@ SIGNATURES = {
                                                       C.c_void_p, C.c_float, C.c_float, C.c_int, C.c_float, C.c_int, C.c_int, C.c_void_p,
                                                       C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                                       C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ocean_hull_set_meshes": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ocean_hull_forces": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int, C.c_void_p,
+                                    C.c_void_p, C.c_void_p]),
+    "ocean_hull_forces_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ocean_simulate_hull_bodies": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int,
+                                             C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ocean_simulate_hull_bodies_device": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_int,
+                                                    C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ocean_update_velocity": (C.c_int, [_H, _P(C.c_int)]),
     "ocean_get_velocity_map": (C.c_int, [_H, _P(C.c_void_p), _P(C.c_size_t)]),
     "ocean_copy_velocity_to_host": (C.c_int, [_H, C.c_int, C.c_int, C.c_void_p]),

@@ -41,6 +41,7 @@ class WaveGenerator:
         self._carr = None
         self._seen = None
         self._wake_size = 0
+        self._hull_vertex_counts = np.zeros(0, np.int64)      # num_vertices of each registered hull mesh
 
     # ---- wave_generator.gd:17-54
     def init_gpu(self, num_cascades: int) -> None:
@@ -51,6 +52,7 @@ class WaveGenerator:
         check(lib.ocean_create(int(self.device), int(self.map_size), int(num_cascades), C.byref(h)))
         self.context = h
         self._num_cascades = int(num_cascades)
+        self._hull_vertex_counts = np.zeros(0, np.int64)
         disp, norm, layer = C.c_void_p(), C.c_void_p(), C.c_size_t()
         check(lib.ocean_get_maps(h, C.byref(disp), C.byref(norm), C.byref(layer)))
         self.descriptors = {"displacement_map": _Descriptor(disp.value, layer.value),
@@ -438,6 +440,89 @@ class WaveGenerator:
             out += (hydro, drag, drive)
         if return_tensions:
             out += (tensions,)
+        if return_transforms:
+            out += (transforms,)
+        return out if len(out) > 1 else s
+
+    # -- hull meshes: pressure and drag integrated over the wetted triangles of a triangle-mesh hull -------------------
+    HULL_MESH = np.dtype([("first_vertex", np.int32), ("num_vertices", np.int32), ("first_triangle", np.int32), ("num_triangles", np.int32),
+                          ("normal_drag", np.float32), ("tangential_drag", np.float32)])     # struct ocean_hull_mesh
+    HULL_BODY = np.dtype([("transform", np.float32, 12), ("mesh", np.int32), ("reserved", np.int32)])      # struct ocean_hull_body
+    FLOATING_HULL = np.dtype([("mass", np.float32), ("inertia", np.float32, 3), ("mesh", np.int32)])      # struct ocean_floating_hull
+
+    @staticmethod
+    def weld_faces(faces):
+        """(vertices [V][3] float32, triangles [T][3] int32) from triangle soup [T * 3][3] (Godot's Mesh.get_faces()): corners with
+        identical coordinates become one vertex, numbered in order of first appearance, and each triangle keeps its winding.
+        A welded hull queries each vertex once where the soup queries it once per triangle that touches it."""
+        f = np.ascontiguousarray(faces, np.float32).reshape(-1, 3)
+        if len(f) % 3:
+            raise ValueError(f"{len(f)} corners are not whole triangles")
+        _, first, inverse = np.unique(f.view(np.dtype((np.void, 12))).reshape(-1), return_index=True, return_inverse=True)
+        order = np.argsort(first, kind="stable")           # unique rows in order of first appearance
+        rank = np.empty_like(order)
+        rank[order] = np.arange(len(order))
+        return f[first[order]].copy(), rank[inverse.reshape(-1)].astype(np.int32).reshape(-1, 3)
+
+    def set_hull_meshes(self, meshes, vertices, triangles) -> np.ndarray:
+        """Registers the HULL_MESH rows of `meshes` (ranges of `vertices` [V][3] float32 and of `triangles` [T][3] int32, indices
+        local to each mesh's vertex range, Godot's clockwise winding) on the device (include/ocean.h, ocean_hull_set_meshes);
+        an empty `meshes` releases the set.  Returns each mesh's enclosed signed volume (float32, negative when wound inward)."""
+        self._require()
+        m = np.ascontiguousarray(meshes, self.HULL_MESH).reshape(-1)
+        v = np.ascontiguousarray(vertices, np.float32).reshape(-1, 3)
+        t = np.ascontiguousarray(triangles, np.int32).reshape(-1, 3)
+        volumes = np.zeros(len(m), np.float32)
+        ptr = lambda x: None if x.size == 0 else x.ctypes.data  # noqa: E731
+        check(load_library().ocean_hull_set_meshes(self.context, len(m), ptr(m), len(v), ptr(v), len(t), ptr(t), ptr(volumes)))
+        self._hull_vertex_counts = m["num_vertices"].astype(np.int64)
+        return volumes
+
+    def hull_forces(self, bodies, velocities, map_scales, density: float = 1025.0, tolerance: float = 1e-3, max_iterations: int = 8,
+                    return_samples: bool = False):
+        """(BUOYANCY_RESULT rows, DRAG_RESULT rows), one each per HULL_BODY row of `bodies` (a 3 x 4 row-major transform and the
+        index of a registered mesh) with its BODY_VELOCITY row: hydrostatic pressure and drag integrated over the mesh's wetted
+        triangles (include/ocean.h, ocean_hull_forces).  With return_samples, also the SURFACE_SAMPLE of every world vertex."""
+        self._require()
+        b = np.ascontiguousarray(bodies, self.HULL_BODY).reshape(-1)
+        v = np.ascontiguousarray(velocities, self.BODY_VELOCITY).reshape(-1)
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        if len(v) != len(b):
+            raise ValueError(f"{len(v)} velocities for {len(b)} bodies")
+        hydro = np.zeros(len(b), self.BUOYANCY_RESULT)
+        drag = np.zeros(len(b), self.DRAG_RESULT)
+        samples = None
+        if return_samples:                                      # an unknown mesh index is rejected by the call itself
+            counts = self._hull_vertex_counts
+            known = b["mesh"][(b["mesh"] >= 0) & (b["mesh"] < len(counts))]
+            samples = np.zeros(int(counts[known].sum()), self.SURFACE_SAMPLE)
+        ptr = lambda x: None if x is None or x.size == 0 else x.ctypes.data  # noqa: E731
+        check(load_library().ocean_hull_forces(self.context, len(b), ptr(b), ptr(v), sc.shape[0], sc.ctypes.data, float(density),
+                                               float(tolerance), int(max_iterations), ptr(hydro), ptr(drag), ptr(samples)))
+        return (hydro, drag, samples) if return_samples else (hydro, drag)
+
+    def simulate_hull_bodies(self, bodies, states, map_scales, dt: float, substeps: int = 1, density: float = 1025.0,
+                             tolerance: float = 1e-3, max_iterations: int = 8, return_records: bool = False,
+                             return_transforms: bool = False):
+        """simulate_bodies on hull meshes (include/ocean.h, ocean_simulate_hull_bodies): each FLOATING_HULL row of `bodies` (mass,
+        principal inertia, a registered mesh) advanced from its BODY_STATE row.  Returns the new states; with return_records also
+        the (BUOYANCY_RESULT, DRAG_RESULT) rows of the last sub-step, with return_transforms the [n][12] float32 transforms."""
+        self._require()
+        b = np.ascontiguousarray(bodies, self.FLOATING_HULL).reshape(-1)
+        s = np.array(states, self.BODY_STATE, copy=True).reshape(-1)
+        sc = np.ascontiguousarray(map_scales, np.float32).reshape(-1, 4)
+        if len(s) != len(b):
+            raise ValueError(f"{len(s)} states for {len(b)} bodies")
+        hydro = np.zeros(len(b), self.BUOYANCY_RESULT) if return_records else None
+        drag = np.zeros(len(b), self.DRAG_RESULT) if return_records else None
+        transforms = np.zeros((len(b), 12), np.float32) if return_transforms else None
+        ptr = lambda x: None if x is None or x.size == 0 else x.ctypes.data  # noqa: E731
+        check(load_library().ocean_simulate_hull_bodies(self.context, len(b), ptr(b), ptr(s), sc.shape[0], sc.ctypes.data, float(density),
+                                                        float(dt), int(substeps), float(tolerance), int(max_iterations), ptr(hydro),
+                                                        ptr(drag), ptr(transforms)))
+        out = (s,)
+        if return_records:
+            out += (hydro, drag)
         if return_transforms:
             out += (transforms,)
         return out if len(out) > 1 else s

@@ -524,6 +524,98 @@ int ocean_simulate_driven_bodies_device(ocean_generator* gen, int num_bodies, co
                                         const ocean_tether* tethers_host, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
                                         ocean_drive_result* drive_dev, float* tensions_dev, float* transforms_dev);
 
+/* Hull meshes -- floating bodies whose hull is a closed triangle mesh: hydrostatic pressure and drag integrated over the
+ * wetted triangles (oracle/hull.py is the specification, bit for bit).  This is the per-triangle pressure model of game boat
+ * physics (Kerner, "Water interaction model for boats in video games"): unlike the point hulls above, the pressure force is
+ * normal to the hull, so a hull on a wave slope feels a horizontal force, and on flat water the displaced volume and the
+ * centre of buoyancy are exact at any heel.
+ * ocean_hull_set_meshes registers the meshes once; the generator keeps them in device memory until the next set, a call with
+ * num_meshes = 0 (which releases them) or ocean_destroy.  A mesh is a range of the vertices ([3] float each, hull-local, m) and
+ * a range of the triangles ([3] int32 each, indices into the mesh's own vertex range), with its drag coefficients.  Winding is
+ * Godot's: front faces are CLOCKWISE seen from outside (Mesh.get_faces(), ArrayMesh triangles), so the outward area vector of
+ * triangle (a, b, c) is a = 0.5 (c - a) x (b - a).  Meshes are shared: a thousand crates name one mesh.  The call rejects,
+ * with nothing uploaded and the previous set kept: negative counts, NULL arrays where a count needs them, ranges outside the
+ * arrays, triangle indices outside their mesh's vertex range, non-finite vertices, negative or non-finite coefficients and
+ * more than (2^31 - 1) / 3 vertices or triangles.  The arguments are checked before the generator handle, so they can be
+ * validated without a device.  volumes (may be NULL) receives each mesh's enclosed signed volume by the divergence theorem
+ * (binary64 on the host, stored as float): negative for a mesh wound the other way, which lets a host catch a wrong winding
+ * and derive a mass.
+ * ocean_hull_forces: per body (ocean_hull_body: the transform of ocean_buoyancy_body and a mesh index) and its velocity
+ * (ocean_body_velocity, as for ocean_body_forces), with rho_g = density * 9.81f and half_rho = 0.5f * density:
+ *   vertex    r = R p, w = r + t (k_buoyancy_transform's operations); one surface query at (w.x, w.z) (with the wake coupling
+ *             while it is live); depth d = eta - w.y; water velocity u at the record's source point (ocean_body_forces' u,
+ *             plus the wake's vertical velocity while the coupling is live)
+ *   clip      per triangle, dropped if any corner's d is NaN: corners with d > 0 are wet; 3 wet: the triangle; 1 wet (i, then
+ *             j, k in winding order): (P_i, X_ij, X_ik); 2 wet (k dry, i, j after it in winding order): (P_i, P_j, X_jk) and
+ *             (P_i, X_jk, X_ki); X_ab = P_a + t (P_b - P_a), t = d_a / (d_a - d_b) from the wet corner a, with d = 0 and
+ *             u = u_a + t (u_b - u_a) there
+ *   pressure  per wet sub-triangle with area vector a, for data linear over it: force -rho g integral(d n dA) = -rho g a sum(d) / 3,
+ *             torque -rho g integral(d r x n dA), V = -integral(d n_y dA), S1 = -integral((d r + y d^2 / 2) n_y dA), from
+ *             integral(f n dA) = a sum(f) / 3 and integral(f g n dA) = a (sum(f_i g_i) + sum(f) sum(g)) / 12; no square root
+ *   drag      per wet sub-triangle: d_c = the mean of its corners' u - (v + w x r), A = |a|, n = a / A, dn = d_c . n; normal drag
+ *             -(rho/2) C_n A dn^2 n on impinging faces (dn < 0) only, tangential (rho/2) C_t A |d_t| d_t, d_t = d_c - dn n,
+ *             torque r_c x F about the origin (r_c the sub-triangle's centroid); a zero-area sub-triangle adds nothing
+ * The records are ocean_body_forces': hydrostatic.force, torque (about the body origin), submerged_volume = V, center_offset =
+ * S1 / V (0 unless V > 0), max_residual and unconverged over the body's world vertices; drag.force and torque, wetted_drag_area
+ * = sum (C_n + C_t) A and max_relative_speed = max |d_c| from 0, so c_v = density * wetted_drag_area * max_relative_speed
+ * bounds the drag's Jacobian as ocean_simulate_bodies' step assumes.  On flat water, for a closed hull, V and t + S1 / V are
+ * exactly the displaced volume and the centre of buoyancy (the waterplane cap has d = 0 and adds nothing), and force =
+ * (0, rho g V, 0).  A body whose mesh has no vertices gets all-zero records.  Sums are in the fixed order of ocean_buoyancy
+ * (triangle j in lane j mod 32, each triangle's pieces added together first, then the shuffle tree): no atomics, and the result
+ * does not depend on the schedule.  A NaN pose affects only its body.  The limits: one warp per body (a 2^16-triangle hull is
+ * one warp's loop), the SURFACE water velocity at every depth, no added mass, slamming or wave-making terms, nothing written
+ * back into the maps.
+ * The bodies, velocities and map_scales are host arrays in both entry points; num_cascades, map_scales, tolerance and
+ * max_iterations are ocean_query_surface's.  The call validates every body's mesh index (a call with no meshes registered and
+ * bodies is invalid), density, and world vertices (the sum of the bodies' meshes' num_vertices) at most INT32_MAX; an invalid
+ * call launches nothing.  It brings stale velocity layers up to date (as ocean_body_forces), then with world vertices launches
+ * 6 kernels (4 with max_iterations = 0): the vertex transform, the surface query, a per-vertex pass that writes the depth and
+ * the water velocity once per vertex, and one reduce per body that clips and integrates; one more while the wake coupling is
+ * live.  With no world vertices only the reduce runs.  samples (may be NULL) receives the surface record of every world
+ * vertex, body-major.  ocean_hull_forces takes host outputs and is synchronous; ocean_hull_forces_device takes device outputs
+ * and is asynchronous on the generator's stream.
+ * ocean_simulate_hull_bodies is ocean_simulate_bodies on hull meshes: per sub-step these kernels on the pose and velocity
+ * tables, then the integrator's k_bodies_integrate unchanged, with r2 = max |p|^2 over the mesh's vertices (clip points lie
+ * on triangle edges, so c_w = c_v r2 stays a bound).  Its states, dt, substeps and outputs, and its validation beyond the
+ * meshes, are ocean_simulate_bodies'.  It launches 1 + 7 S kernels (1 + 5 S with max_iterations = 0, 1 + 2 S with no world
+ * vertices) and S more while the wake coupling is live.  Hull bodies keep ocean_body_state, so ocean_wake_step drives wakes
+ * from them unchanged. */
+typedef struct ocean_hull_mesh {
+    int32_t first_vertex;       /* range into the hull vertices ([3] float each, hull-local, m) */
+    int32_t num_vertices;
+    int32_t first_triangle;     /* range into the triangles ([3] int32 each, indices local to this mesh's vertex range) */
+    int32_t num_triangles;
+    float normal_drag;          /* C_n, finite and >= 0 */
+    float tangential_drag;      /* C_t, finite and >= 0 */
+} ocean_hull_mesh;              /* 24 B */
+typedef struct ocean_hull_body {
+    float transform[12];        /* 3 x 4 row-major [R | t], as ocean_buoyancy_body's */
+    int32_t mesh;
+    int32_t reserved;
+} ocean_hull_body;              /* 56 B, the layout of ocean_buoyancy_body */
+typedef struct ocean_floating_hull {
+    float mass;                 /* kg, finite and > 0 */
+    float inertia[3];           /* principal moments about the centre of mass (the hull origin), kg m^2, finite and > 0 */
+    int32_t mesh;
+} ocean_floating_hull;          /* 20 B */
+int ocean_hull_set_meshes(ocean_generator* gen, int num_meshes, const ocean_hull_mesh* meshes_host, int num_vertices,
+                          const float* vertices_host, int num_triangles, const int32_t* triangles_host, float* volumes_host);
+int ocean_hull_forces(ocean_generator* gen, int num_bodies, const ocean_hull_body* bodies_host, const ocean_body_velocity* velocities_host,
+                      int num_cascades, const float* map_scales_host, float density, float tolerance, int max_iterations,
+                      ocean_buoyancy_result* hydrostatic_host, ocean_drag_result* drag_host, ocean_surface_sample* samples_host);
+int ocean_hull_forces_device(ocean_generator* gen, int num_bodies, const ocean_hull_body* bodies_host,
+                             const ocean_body_velocity* velocities_host, int num_cascades, const float* map_scales_host, float density,
+                             float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
+                             ocean_surface_sample* samples_dev);
+int ocean_simulate_hull_bodies(ocean_generator* gen, int num_bodies, const ocean_floating_hull* bodies_host, ocean_body_state* states_host,
+                               int num_cascades, const float* map_scales_host, float density, float dt, int substeps, float tolerance,
+                               int max_iterations, ocean_buoyancy_result* hydrostatic_host, ocean_drag_result* drag_host,
+                               float* transforms_host);
+int ocean_simulate_hull_bodies_device(ocean_generator* gen, int num_bodies, const ocean_floating_hull* bodies_host,
+                                      ocean_body_state* states_dev, int num_cascades, const float* map_scales_host, float density, float dt,
+                                      int substeps, float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_dev,
+                                      ocean_drag_result* drag_dev, float* transforms_dev);
+
 /* Velocity maps -- the water velocity: the time derivative of the displacement map, what drag, damping and floating debris
  * need.  A cascade's velocity layer is (vx, vy, vz, 0) = d/dt of its displacement texel (hx, hy, hz, 0): same layout, same
  * orientation (ocean_get_maps), RGBA16F, in m/s before the displacement scale.  It is computed exactly, as one more inverse

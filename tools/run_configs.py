@@ -3,7 +3,7 @@ config.
 
     python tools/run_configs.py [--updates] [--query] [--velocity] [--buoyancy] [--drag] [--bodies] [--raycast] [--spray-particles]
                                 [--wake] [--wake-coupling] [--wake-foam] [--wake-obstacles]
-                                [--wake-readers] [--sea-state] [--drifters] [--drive]
+                                [--wake-readers] [--sea-state] [--drifters] [--drive] [--hull]
 
 Each flag runs its group of GROUPS; several flags run their groups in the table's order.  No flag runs --updates and then
 --query.  An unknown argument exits before anything touches the GPU."""
@@ -26,6 +26,7 @@ from oracle import bodies as ob
 from oracle import buoyancy as bu
 from oracle import drag as dr
 from oracle import drive as od
+from oracle import hull as oh
 from oracle import raycast as rc
 
 DEV = torch.device("cuda", 0)
@@ -544,6 +545,73 @@ def run_drive(N, C, n_bodies, per_body, substeps, reps, label, dt=1.0 / 60.0, to
     print(json.dumps(out), flush=True)
 
 
+def _ellipsoid(nu, nv, radii):
+    """A closed ellipsoid on a (u, v) grid with pinched poles, in Godot's winding: (vertices [(nv + 1) nu][3], triangles
+    [2 nu nv][3])."""
+    th = np.linspace(0, np.pi, nv + 1)
+    ph = np.linspace(0, 2 * np.pi, nu, endpoint=False)
+    grid = np.stack([np.outer(np.sin(th), np.cos(ph)), np.outer(np.cos(th), np.ones(nu)), np.outer(np.sin(th), np.sin(ph))], 2)
+    idx = np.arange((nv + 1) * nu).reshape(nv + 1, nu)
+    a, b, c, d = idx[:-1], np.roll(idx[:-1], -1, 1), idx[1:], np.roll(idx[1:], -1, 1)
+    tris = np.concatenate([np.stack([a, c, b], -1).reshape(-1, 3), np.stack([b, c, d], -1).reshape(-1, 3)]).astype(np.int32)
+    return (grid.reshape(-1, 3) * radii).astype(np.float32), tris
+
+
+def run_hull(N, C, n_bodies, nu, nv, substeps, reps, label, dt=1.0 / 60.0):
+    """Hull meshes (ocean_hull_forces_device, ocean_simulate_hull_bodies_device) on n_bodies sharing one ellipsoid of 2 nu nv
+    triangles, against ocean_body_forces_device and ocean_simulate_bodies_device with hull points at the same vertices (the
+    same surface queries): what the clip-and-reduce costs.  Device times from CUDA events, states restored before each window,
+    alternating windows; the card's name, power limit and max SM clock are read in the same run."""
+    g, _, scales = warmed_generator(N, C, 2)
+    v, t = _ellipsoid(nu, nv, (3.0, 1.0, 1.5))
+    meshes = np.zeros(1, oh.MESH)
+    meshes[0] = (0, len(v), 0, len(t), 1.0, 0.05)
+    vol = float(g.set_hull_meshes(meshes, v, t)[0])
+    B = n_bodies
+    rng = np.random.default_rng(9)
+    states = np.zeros(B, ob.STATE)
+    states["position"] = np.stack([rng.uniform(-300, 300, B), rng.uniform(-1, 1, B), rng.uniform(-300, 300, B)], 1)
+    q = rng.standard_normal((B, 4))
+    states["orientation"] = q / np.linalg.norm(q, axis=1, keepdims=True)
+    states["linear_velocity"] = rng.uniform(-2.0, 2.0, (B, 3))
+    hulls = np.zeros(B, oh.FLOATING)
+    hulls["mass"], hulls["inertia"] = 0.5 * 1025.0 * vol, 0.5 * 1025.0 * vol
+    table, vel = oh.pose(hulls, states)
+    points = np.zeros(len(v), bu.POINT)
+    points["position"], points["volume"], points["half_height"] = v, vol / len(v), 0.3
+    bodies = np.zeros(B, ob.BODY)
+    bodies["mass"], bodies["inertia"], bodies["num_points"] = hulls["mass"], hulls["inertia"], len(v)
+    ptable, _ = ob.pose(bodies, states)
+    hull_d = upload(points)
+    cda_d = torch.from_numpy(np.full(len(v), 0.05, np.float32)).to(DEV)
+    hyd_d, drag_d = records(B, bu.RESULT), records(B, dr.RESULT)
+    st0_d = upload(states)
+    st_d = st0_d.clone()
+    torch.cuda.synchronize()
+    lib = load_library()
+    hull_forces = lambda: check(lib.ocean_hull_forces_device(g.context, B, table.ctypes.data, vel.ctypes.data, C, scales.ctypes.data,  # noqa: E731
+                                                             1025.0, 1e-3, 8, hyd_d.data_ptr(), drag_d.data_ptr(), None))
+    point_forces = lambda: check(lib.ocean_body_forces_device(g.context, B, ptable.ctypes.data, vel.ctypes.data, len(points),  # noqa: E731
+                                                              hull_d.data_ptr(), cda_d.data_ptr(), C, scales.ctypes.data, 1025.0, 1e-3, 8,
+                                                              hyd_d.data_ptr(), drag_d.data_ptr(), None))
+    t_h, t_p = alternate(lambda: timed(g, hull_forces, reps, 3), lambda: timed(g, point_forces, reps, 3), rounds=5)
+    out = {"config": label, **card(), "map_size": N, "cascades": C, "bodies": B, "triangles": len(t), "vertices": len(v),
+           "hull_forces_us": [1e3 * x for x in t_h], "point_forces_us": [1e3 * x for x in t_p],
+           "hull_over_points": min(t_h) / min(t_p) - 1.0}
+    if substeps:
+        restore = lambda: st_d.copy_(st0_d)  # noqa: E731
+        hull_sim = lambda: check(lib.ocean_simulate_hull_bodies_device(g.context, B, hulls.ctypes.data, st_d.data_ptr(), C,  # noqa: E731
+                                                                       scales.ctypes.data, 1025.0, dt, substeps, 1e-3, 8, None, None, None))
+        point_sim = lambda: check(lib.ocean_simulate_bodies_device(g.context, B, bodies.ctypes.data, st_d.data_ptr(), len(points),  # noqa: E731
+                                                                   hull_d.data_ptr(), cda_d.data_ptr(), C, scales.ctypes.data, 1025.0, dt,
+                                                                   substeps, 1e-3, 8, None, None, None))
+        s_h, s_p = alternate(lambda: timed(g, hull_sim, reps, 3, restore), lambda: timed(g, point_sim, reps, 3, restore), rounds=5)
+        out.update(substeps=substeps, simulate_hull_us=[1e3 * x for x in s_h], simulate_points_us=[1e3 * x for x in s_p],
+                   simulate_hull_over_points=min(s_h) / min(s_p) - 1.0)
+    g.free()
+    print(json.dumps(out), flush=True)
+
+
 def run_simulate_coupling(N, C, n_bodies, per_body, substeps, reps, label, wake=512, dx=1.0, dt=1.0 / 60.0):
     """Wake coupling's cost in the body integrator: ocean_simulate_bodies_device on two generators with the same maps and a
     wake layer of wake x wake cells of dx centred on the world origin (it covers [-256, 256]^2 m of the scene's
@@ -919,6 +987,14 @@ GROUPS = {          # flag: its configs, in the order they run
                 f"driven bodies: 2^14 bodies x 64 points, 2 thrusters, 2 foils and a tether each, {S} sub-step(s), {C} cascades of {N}x{N}, "
                 "vs simulate_bodies")
         for S in (1, 4) for N, C, reps in ((256, 4, 50), (1024, 8, 20))
+    ],
+    "--hull": [
+        partial(run_hull, 256, 4, 1 << 14, 16, 16, 4, 50, "hull meshes: 2^14 bodies sharing a 512-triangle ellipsoid (272 vertices), "
+                "4 cascades of 256x256, vs points at the vertices; simulate at 4 sub-steps"),
+        partial(run_hull, 1024, 8, 1 << 14, 16, 16, 4, 20, "hull meshes: 2^14 bodies sharing a 512-triangle ellipsoid (272 vertices), "
+                "8 cascades of 1024x1024, vs points at the vertices; simulate at 4 sub-steps"),
+        partial(run_hull, 256, 4, 1, 256, 128, 0, 50, "hull meshes: one body of 2^16 triangles (one warp), 4 cascades of 256x256, "
+                "vs points at its vertices"),
     ],
     "--wake-obstacles": [
         partial(run_wake_step_obstacles, N, k, 200 if N < 1024 else 50, f"wake obstacles, step: {N}x{N} cells, {k} source(s), 8 sub-steps")

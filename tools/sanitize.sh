@@ -24,7 +24,16 @@ dr = np.zeros(len(pts), gow.WaveGenerator.DRIFTER)
 dr["x"], dr["z"], dr["scale"], dr["tilt"] = pts[:, 0], pts[:, 1], 1.0, 0.5
 dp = gow.WaveGenerator.drift_params(current=(0.1, 0.0), box=(-100.0, -100.0, 200.0, 200.0), read_wake=True)
 dr, inst = g.drift(dr, 1.0 / 60.0, sc, dp)
-print("sea state", float(total["significant_wave_height"]), "drift", float(np.nansum(inst)))
+hv = np.array([[0, 0, 0], [2, 0, 0], [0, 1, 0], [0, 0, 1.5]], np.float32) - 0.4      # hull meshes: a shared tetrahedron
+ht = np.array([[0, 1, 2], [0, 3, 1], [0, 2, 3], [1, 3, 2]], np.int32)
+hm = np.array([(0, 4, 0, 4, 1.0, 0.05)], gow.WaveGenerator.HULL_MESH)
+g.set_hull_meshes(hm, hv, ht)
+hb = np.zeros(256, gow.WaveGenerator.FLOATING_HULL)
+hb["mass"], hb["inertia"] = 200.0, 50.0
+hs = np.zeros(256, gow.WaveGenerator.BODY_STATE)
+hs["position"][:, [0, 2]], hs["orientation"][:, 3] = pts[:256], 1.0
+hs = g.simulate_hull_bodies(hb, hs, sc, 1.0 / 60.0, 4)
+print("sea state", float(total["significant_wave_height"]), "drift", float(np.nansum(inst)), "hulls", float(np.nansum(hs["position"])))
 print("checksum", int(d.view(np.uint16).astype(np.uint64).sum()), int(n.view(np.uint16).astype(np.uint64).sum()))
 g.free()
 PY
