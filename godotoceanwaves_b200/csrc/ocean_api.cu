@@ -14,6 +14,7 @@
 #include <new>
 #include <string>
 #include <map>
+#include <type_traits>
 #include <vector>
 
 namespace {
@@ -138,6 +139,59 @@ struct WakeLayer {
         return {mask.ptr, mask_size[0], mask_size[1], offset(origin_x, mask_origin[0]), offset(origin_z, mask_origin[1])};
     }
     int off(ocean_generator* g, unsigned parts);
+    // the wake's vertical velocity of each of n query points for the drag passes, allocated while the coupling is live (else
+    // *out is null); every sub-step of a call reads the same snapshots
+    cudaError_t vertical_velocities(ocean_generator* g, size_t n, float** out) {
+        *out = nullptr;
+        if (n == 0 || !coupling_live()) return cudaSuccess;
+        cudaError_t e = wv.grow(g, n);
+        if (e == cudaSuccess) *out = wv.ptr;
+        return e;
+    }
+};
+
+// The scratch of the floating-body ops (buoyancy, body forces, hull forces and the three integrators), grown by the calls
+// that use it and kept for the next.  The point and mesh forms keep their own pose and row tables.
+struct BodyScratch {
+    // per body: the pose tables (ocean_buoyancy_body for point hulls, ocean_hull_body for meshes) and velocities the force
+    // passes read and the integrators rewrite each sub-step; the offsets of the bodies' first world points, with their host
+    // copy (kept here: the upload is asynchronous); max |p|^2 per hull; the integrators' rows (ocean_floating_body, written by
+    // k_hull_prepare for meshes, which are uploaded as ocean_floating_hull); the hydrostatic and drag results of an integrator
+    // whose caller passes NULL for them
+    DeviceArray<ocean_buoyancy_body> poses;
+    DeviceArray<ocean_hull_body> hull_poses;
+    DeviceArray<ocean_body_velocity> velocities;
+    DeviceArray<int> offsets;
+    std::vector<int> offsets_host;
+    DeviceArray<float> r2;
+    DeviceArray<ocean_floating_body> rows;
+    DeviceArray<ocean_floating_hull> hull_rows;
+    DeviceArray<ocean_buoyancy_result> hydrostatic;
+    DeviceArray<ocean_drag_result> drag;
+    // per queried point (the world points, then a driven call's actuators): the query positions, the surface records when
+    // the caller wants none, and for meshes the (r, d) and (u, 0) of k_hull_vertex per world vertex
+    DeviceArray<float2> q;
+    DeviceArray<ocean_surface_sample> samples;
+    DeviceArray<float4> corners;
+    // drive (ocean_simulate_driven_bodies): the actuator, load and tether arrays, the by-body incidence list (offsets, then
+    // entries, in one block) with its host copy, the tether records, the integrator's sums, and the drive and tension outputs
+    // when the caller passes NULL for them
+    DeviceArray<ocean_thruster> thrusters;
+    DeviceArray<ocean_foil> foils;
+    DeviceArray<ocean_body_load> loads;
+    DeviceArray<ocean_tether> tethers;
+    DeviceArray<int> incidence;
+    std::vector<int> incidence_host;
+    DeviceArray<ocean::TetherForce> tether_forces;
+    DeviceArray<ocean::DriveSum> sums;
+    DeviceArray<ocean_drive_result> drive;
+    DeviceArray<float> tensions;
+    // the registered mesh set (ocean_hull_set_meshes) and a host copy of its mesh records: the calls validate the bodies'
+    // mesh indices and count their world vertices from it
+    DeviceArray<ocean_hull_mesh> meshes;
+    DeviceArray<float> vertices;
+    DeviceArray<int32_t> triangles;
+    std::vector<ocean_hull_mesh> meshes_host;
 };
 }  // namespace
 
@@ -164,44 +218,7 @@ struct ocean_generator {
     DeviceArray<float4> q_scales;                       // map scales of the query ops
     DeviceArray<int> spray_counts;                      // spray op scratch: block counts / offsets (+ total)
     DeviceArray<int> surf_scratch;                      // surface query scratch: pending count, layer maxima, pending list
-    // buoyancy scratch: body table and world-point offsets, query positions, surface records (when the caller wants none)
-    DeviceArray<ocean_buoyancy_body> buoy_bodies;
-    DeviceArray<int> buoy_offsets;
-    std::vector<int> buoy_offsets_host;
-    DeviceArray<float2> buoy_q;
-    DeviceArray<ocean_surface_sample> buoy_samples;
-    // the body velocities of the drag pass
-    DeviceArray<ocean_body_velocity> drag_velocities;
-    // ocean_simulate_bodies_device's hydrostatic and drag results when its caller passes NULL for them
-    DeviceArray<ocean_buoyancy_result> buoy_results;
-    DeviceArray<ocean_drag_result> drag_results;
-    // floating-body scratch: the body table and max |p|^2 per hull (the pose and velocity tables are buoy_bodies and
-    // drag_velocities)
-    DeviceArray<ocean_floating_body> sim_bodies;
-    DeviceArray<float> sim_r2;
-    // driven-body scratch (ocean_simulate_driven_bodies): the actuator, load and tether arrays, the by-body incidence list
-    // (offsets, then entries, in one block; its host copy is kept because the upload is asynchronous), the tether records,
-    // the integrator's sums, and the drive and tension outputs when the caller passes NULL for them
-    DeviceArray<ocean_thruster> drive_thrusters;
-    DeviceArray<ocean_foil> drive_foils;
-    DeviceArray<ocean_body_load> drive_loads;
-    DeviceArray<ocean_tether> drive_tethers;
-    DeviceArray<int> drive_incidence;
-    std::vector<int> drive_incidence_host;
-    DeviceArray<ocean::TetherForce> drive_tether_forces;
-    DeviceArray<ocean::DriveSum> drive_sums;
-    DeviceArray<ocean_drive_result> drive_results;
-    DeviceArray<float> drive_tensions;
-    // hull meshes (ocean_hull_set_meshes): the registered set, and a host copy of its mesh records (the calls validate the
-    // bodies' mesh indices and count their world vertices from it); the calls' scratch: the pose table, the per-world-vertex
-    // (r, d) and (u, 0) of k_hull_vertex, and the integrator's hull rows
-    DeviceArray<ocean_hull_mesh> hull_meshes;
-    DeviceArray<float> hull_vertices;
-    DeviceArray<int32_t> hull_triangles;
-    std::vector<ocean_hull_mesh> hull_meshes_host;
-    DeviceArray<ocean_hull_body> hull_poses;
-    DeviceArray<float4> hull_corners;
-    DeviceArray<ocean_floating_hull> hull_bodies;
+    BodyScratch body;                                   // the floating-body ops (BodyScratch)
     // velocity maps, allocated by the first velocity call: row-pass scratch, the map, its binary32 tap while the taps are on
     DeviceArray<float4> vel_scratch;                    // [num_cascades][N][N]
     DeviceArray<uint2> velocity;                        // [num_cascades][N][N] 4 x half
@@ -1399,11 +1416,19 @@ int ocean_spray_particles(ocean_generator* gen, const ocean_spray_emitter* emitt
 static_assert(sizeof(ocean_surface_sample) == 40, "ocean_surface_sample layout");
 
 namespace {
-int check_surface_args(int num_points, float tolerance, int max_iterations) {
-    if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
-    if (!(tolerance > 0.0f) || !std::isfinite(tolerance)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "tolerance %g is not finite and > 0", tolerance);
+bool finite_positive(float x) { return x > 0.0f && std::isfinite(x); }
+bool finite_nonnegative(float x) { return x >= 0.0f && std::isfinite(x); }
+
+// The surface inversion's tolerance and iteration budget.
+int check_solver_args(float tolerance, int max_iterations) {
+    if (!finite_positive(tolerance)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "tolerance %g is not finite and > 0", tolerance);
     if (max_iterations < 0 || max_iterations > 64) return fail(OCEAN_ERR_INVALID_ARGUMENT, "max_iterations %d outside [0, 64]", max_iterations);
     return OCEAN_OK;
+}
+
+int check_surface_args(int num_points, float tolerance, int max_iterations) {
+    if (num_points < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_points %d is negative", num_points);
+    return check_solver_args(tolerance, max_iterations);
 }
 
 // The surface query on validated arguments, with the map scales already in gen->q_scales (ocean_query_surface_device and
@@ -1503,7 +1528,7 @@ static_assert(sizeof(ocean_buoyancy_result) == 48, "ocean_buoyancy_result layout
 
 namespace {
 // The bodies' ranges into the hull points, in 64-bit; *world receives the number of world points, the sum of their num_points.
-// (The templates here, over ocean_buoyancy_body and ocean_floating_body, need C++ linkage inside this extern "C" block.)
+// (The templates here, over the body row types, need C++ linkage inside this extern "C" block.)
 extern "C++" template <typename Body>
 int check_point_ranges(int num_bodies, const Body* bodies, int num_points, int* world) {
     long long total = 0;
@@ -1525,38 +1550,37 @@ int check_buoyancy_args(int num_bodies, const ocean_buoyancy_body* bodies, int n
     int rc = check_surface_args(num_points, tolerance, max_iterations);
     if (rc) return rc;
     if (num_bodies < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_bodies %d is negative", num_bodies);
-    if (!(density > 0.0f) || !std::isfinite(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
+    if (!finite_positive(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
     if (num_bodies > 0 && !bodies) return fail(OCEAN_ERR_INVALID_ARGUMENT, "bodies is NULL");
     return check_point_ranges(num_bodies, bodies, num_points, world);
 }
 
-// The exclusive prefix of the bodies' num_points into gen->buoy_offsets_host (kept in the generator: the upload of it is
-// asynchronous), uploaded to gen->buoy_offsets.
-extern "C++" template <typename Body>
-int upload_offsets(ocean_generator* gen, int num_bodies, const Body* bodies_host) {
-    const size_t B = (size_t)num_bodies;
-    std::vector<int>& offsets = gen->buoy_offsets_host;
-    offsets.resize(B);
-    for (size_t b = 0, start = 0; b < B; start += (size_t)bodies_host[b].num_points, ++b) offsets[b] = (int)start;
-    OCEAN_CUDA(gen->buoy_offsets.upload(gen, offsets.data(), B));
+// The exclusive prefix of count(b), body b's number of world points (hull points or mesh vertices), into
+// gen->body.offsets_host, uploaded to gen->body.offsets.  The counts were validated: their sum fits an int.
+extern "C++" template <typename Count>
+int upload_offsets(ocean_generator* gen, int num_bodies, Count count) {
+    std::vector<int>& offsets = gen->body.offsets_host;
+    offsets.resize((size_t)num_bodies);
+    for (int b = 0, start = 0; b < num_bodies; start += count(b), ++b) offsets[b] = start;
+    OCEAN_CUDA(gen->body.offsets.upload(gen, offsets.data(), (size_t)num_bodies));
     return OCEAN_OK;
 }
 
 // The buoyancy launches on a body table and offsets already in device memory (bodies_dev may be written by earlier kernels on
-// the stream), with the map scales in gen->q_scales and gen->buoy_q grown to `world`: samples receives the surface records, and
+// the stream), with the map scales in gen->q_scales and gen->body.q grown to `world`: samples receives the surface records, and
 // wv_dev (may be null) the wake's vertical velocity of each world point while the wake coupling is live.  With queried > world
-// the query also takes the points gen->buoy_q holds after the world points (written earlier on the stream).
+// the query also takes the points gen->body.q holds after the world points (written earlier on the stream).
 int launch_buoyancy_sequence(ocean_generator* gen, const ocean_buoyancy_body* bodies_dev, const int* offsets_dev, int num_bodies, int world,
                              const ocean_buoyancy_point* points_dev, int num_cascades, float density, float tolerance, int max_iterations,
                              ocean_buoyancy_result* results_dev, ocean_surface_sample* samples, float* wv_dev = nullptr, int queried = -1) {
     int rc;
     if (queried < 0) queried = world;                   // more query points than world ones: the driven bodies' actuators
     if (world > 0) {
-        OCEAN_CUDA(ocean::launch_buoyancy_transform(bodies_dev, offsets_dev, num_bodies, points_dev, world, gen->buoy_q.ptr, gen->stream));
+        OCEAN_CUDA(ocean::launch_buoyancy_transform(bodies_dev, offsets_dev, num_bodies, points_dev, world, gen->body.q.ptr, gen->stream));
         gen->kernel_launches += 1;
     }
     if (queried > 0)
-        if ((rc = run_query_surface(gen, queried, gen->buoy_q.ptr, num_cascades, tolerance, max_iterations, samples, wv_dev))) return rc;
+        if ((rc = run_query_surface(gen, queried, gen->body.q.ptr, num_cascades, tolerance, max_iterations, samples, wv_dev))) return rc;
     const float rho_g = density * 9.81f;                                 // G, wave_generator.gd:5, in binary32
     OCEAN_CUDA(ocean::launch_buoyancy_reduce(bodies_dev, offsets_dev, num_bodies, points_dev, samples, rho_g, tolerance, results_dev,
                                              gen->stream));
@@ -1565,19 +1589,20 @@ int launch_buoyancy_sequence(ocean_generator* gen, const ocean_buoyancy_body* bo
 }
 
 // The buoyancy launch sequence on validated arguments (num_bodies > 0), with the map scales already in gen->q_scales: the body
-// table and offsets are uploaded to gen->buoy_bodies / gen->buoy_offsets, and *samples_used receives the surface records
-// (samples_dev, or gen->buoy_samples when samples_dev is NULL) for a drag pass on the same points.
+// table and offsets are uploaded to gen->body.poses / gen->body.offsets, and *samples_used receives the surface records
+// (samples_dev, or gen->body.samples when samples_dev is NULL) for a drag pass on the same points.
 int run_buoyancy(ocean_generator* gen, int num_bodies, const ocean_buoyancy_body* bodies_host, int world, const ocean_buoyancy_point* points_dev,
                  int num_cascades, float density, float tolerance, int max_iterations, ocean_buoyancy_result* results_dev,
                  ocean_surface_sample* samples_dev, ocean_surface_sample** samples_used, float* wv_dev = nullptr) {
+    BodyScratch& sc = gen->body;
     int rc;
-    OCEAN_CUDA(gen->buoy_q.grow(gen, (size_t)world));
-    if (!samples_dev) OCEAN_CUDA(gen->buoy_samples.grow(gen, (size_t)world));
-    ocean_surface_sample* samples = samples_dev ? samples_dev : gen->buoy_samples.ptr;
-    OCEAN_CUDA(gen->buoy_bodies.upload(gen, bodies_host, (size_t)num_bodies));
-    if ((rc = upload_offsets(gen, num_bodies, bodies_host))) return rc;
-    if ((rc = launch_buoyancy_sequence(gen, gen->buoy_bodies.ptr, gen->buoy_offsets.ptr, num_bodies, world, points_dev, num_cascades, density,
-                                       tolerance, max_iterations, results_dev, samples, wv_dev)))
+    OCEAN_CUDA(sc.q.grow(gen, (size_t)world));
+    if (!samples_dev) OCEAN_CUDA(sc.samples.grow(gen, (size_t)world));
+    ocean_surface_sample* samples = samples_dev ? samples_dev : sc.samples.ptr;
+    OCEAN_CUDA(sc.poses.upload(gen, bodies_host, (size_t)num_bodies));
+    if ((rc = upload_offsets(gen, num_bodies, [&](int b) { return bodies_host[b].num_points; }))) return rc;
+    if ((rc = launch_buoyancy_sequence(gen, sc.poses.ptr, sc.offsets.ptr, num_bodies, world, points_dev, num_cascades, density, tolerance,
+                                       max_iterations, results_dev, samples, wv_dev)))
         return rc;
     if (samples_used) *samples_used = samples;
     return OCEAN_OK;
@@ -1759,20 +1784,17 @@ int ocean_body_forces_device(ocean_generator* gen, int num_bodies, const ocean_b
     if (!hydrostatic_dev || !drag_dev || (world > 0 && !points_dev)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
-    OCEAN_CUDA(gen->drag_velocities.upload(gen, velocities_host, (size_t)num_bodies));
+    BodyScratch& sc = gen->body;
+    OCEAN_CUDA(sc.velocities.upload(gen, velocities_host, (size_t)num_bodies));
     float* wv = nullptr;
-    if (world > 0 && gen->wake.coupling_live()) {
-        OCEAN_CUDA(gen->wake.wv.grow(gen, (size_t)world));
-        wv = gen->wake.wv.ptr;
-    }
+    OCEAN_CUDA(gen->wake.vertical_velocities(gen, (size_t)world, &wv));
     ocean_surface_sample* samples = nullptr;
     if ((rc = run_buoyancy(gen, num_bodies, bodies_host, world, points_dev, num_cascades, density, tolerance, max_iterations, hydrostatic_dev,
                            samples_dev, &samples, wv)))
         return rc;
     const float half_rho = 0.5f * density;
-    OCEAN_CUDA(ocean::launch_drag_reduce(gen->buoy_bodies.ptr, gen->drag_velocities.ptr, gen->buoy_offsets.ptr, num_bodies, points_dev,
-                                         drag_areas_dev, samples, gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, half_rho,
-                                         drag_dev, wv, gen->stream));
+    OCEAN_CUDA(ocean::launch_drag_reduce(sc.poses.ptr, sc.velocities.ptr, sc.offsets.ptr, num_bodies, points_dev, drag_areas_dev, samples,
+                                         gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, half_rho, drag_dev, wv, gen->stream));
     gen->kernel_launches += 1;
     return OCEAN_OK;
 }
@@ -1807,7 +1829,26 @@ static_assert(sizeof(ocean_floating_body) == 24, "ocean_floating_body layout");
 static_assert(sizeof(ocean_body_state) == 52, "ocean_body_state layout");
 
 namespace {
-bool finite_positive(float x) { return x > 0.0f && std::isfinite(x); }
+// The integrators' density, dt and substeps.
+int check_step_args(float density, float dt, int substeps) {
+    if (!finite_positive(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
+    if (!finite_positive(dt)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "dt %g is not finite and > 0", dt);
+    if (substeps < 1 || substeps > 64) return fail(OCEAN_ERR_INVALID_ARGUMENT, "substeps %d outside [1, 64]", substeps);
+    return OCEAN_OK;
+}
+
+// Each body's mass and principal inertia (ocean_floating_body or ocean_floating_hull rows).
+extern "C++" template <typename Row>
+int check_mass_inertia(int num_bodies, const Row* bodies) {
+    for (int b = 0; b < num_bodies; ++b) {
+        const Row& fb = bodies[b];
+        if (!finite_positive(fb.mass)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: mass %g is not finite and > 0", b, fb.mass);
+        for (int k = 0; k < 3; ++k)
+            if (!finite_positive(fb.inertia[k]))
+                return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: inertia[%d] %g is not finite and > 0", b, k, fb.inertia[k]);
+    }
+    return OCEAN_OK;
+}
 
 // ocean_body_forces' checks on the floating bodies, plus mass, inertia, dt, substeps and the states; *world as for
 // check_buoyancy_args.
@@ -1816,25 +1857,15 @@ int check_simulate_args(int num_bodies, const ocean_floating_body* bodies, const
     int rc = check_surface_args(num_points, tolerance, max_iterations);
     if (rc) return rc;
     if (num_bodies < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_bodies %d is negative", num_bodies);
-    if (!finite_positive(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
-    if (!finite_positive(dt)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "dt %g is not finite and > 0", dt);
-    if (substeps < 1 || substeps > 64) return fail(OCEAN_ERR_INVALID_ARGUMENT, "substeps %d outside [1, 64]", substeps);
+    if ((rc = check_step_args(density, dt, substeps))) return rc;
     if (num_bodies > 0 && !bodies) return fail(OCEAN_ERR_INVALID_ARGUMENT, "bodies is NULL");
     if (num_bodies > 0 && !states) return fail(OCEAN_ERR_INVALID_ARGUMENT, "states is NULL");
-    for (int b = 0; b < num_bodies; ++b) {
-        const ocean_floating_body& fb = bodies[b];
-        if (!finite_positive(fb.mass)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: mass %g is not finite and > 0", b, fb.mass);
-        for (int k = 0; k < 3; ++k)
-            if (!finite_positive(fb.inertia[k]))
-                return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: inertia[%d] %g is not finite and > 0", b, k, fb.inertia[k]);
-    }
+    if ((rc = check_mass_inertia(num_bodies, bodies))) return rc;
     if ((rc = check_point_ranges(num_bodies, bodies, num_points, world))) return rc;
     if (*world > 0 && !drag_areas) return fail(OCEAN_ERR_INVALID_ARGUMENT, "drag_areas is NULL");
     return OCEAN_OK;
 }
-}  // namespace
 
-namespace {
 // The drive arguments of ocean_simulate_driven_bodies[_device] (host arrays), as validated by check_drive_args.
 struct DriveHost {
     int num_thrusters = 0;
@@ -1847,8 +1878,6 @@ struct DriveHost {
     int actuators() const { return num_thrusters + num_foils; }
     bool any() const { return num_thrusters > 0 || num_foils > 0 || num_tethers > 0 || loads; }
 };
-
-bool finite_nonnegative(float x) { return x >= 0.0f && std::isfinite(x); }
 
 // The counts and arrays, the body indices, and the foil areas and tether constants that enter the stability bound; the world
 // points plus the actuators must stay below 2^31 (one surface query takes them all).
@@ -1880,11 +1909,11 @@ int check_drive_args(int num_bodies, int world, const DriveHost& d) {
     return OCEAN_OK;
 }
 
-// The by-body incidence list into gen->drive_incidence_host: [num_bodies + 1] offsets, then per body its thrusters, foils
+// The by-body incidence list into gen->body.incidence_host: [num_bodies + 1] offsets, then per body its thrusters, foils
 // and tether ends in array order (thruster k -> k, foil k -> T + k, end e of tether k -> T + F + 2 k + e).
 void build_incidence(ocean_generator* gen, int num_bodies, const DriveHost& d) {
     const size_t B = (size_t)num_bodies;
-    std::vector<int>& v = gen->drive_incidence_host;
+    std::vector<int>& v = gen->body.incidence_host;
     const size_t entries = (size_t)d.actuators() + 2 * (size_t)d.num_tethers;
     v.assign(B + 1 + entries, 0);
     int* off = v.data();
@@ -1907,109 +1936,137 @@ void build_incidence(ocean_generator* gen, int num_bodies, const DriveHost& d) {
     v.resize(B + 1 + (size_t)off[B]);                   // anchored tethers have one end
 }
 
-// ocean_simulate_bodies_device after its checks (num_bodies > 0, scales uploaded), with drive null: the plain integrator;
-// with drive: the driven one (drive->any()), its arrays validated, and drive_dev / tensions_dev the outputs or null.
-int run_simulate(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_dev, int world,
+int launch_hull_sequence(ocean_generator* gen, const ocean_hull_body* poses_dev, const ocean_body_velocity* velocities_dev, int num_bodies,
+                         int world, int num_cascades, float density, float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_dev,
+                         ocean_drag_result* drag_dev, ocean_surface_sample* samples, float* wv);      // with the hull meshes, below
+
+// The body integrator after an entry point's checks (num_bodies > 0, scales uploaded).  Row is the hull: ocean_floating_body
+// rows on the hull points points_dev with drag_areas_dev, or ocean_floating_hull rows on the registered meshes (points_dev and
+// drag_areas_dev unused).  With drive null the plain integrator runs; with drive (drive->any(), its arrays validated) the
+// driven one, drive_dev / tensions_dev the outputs or null.  Every sub-step runs the hull's force sequence on the current
+// poses, then the integrator, which writes transforms_dev on the last one.
+extern "C++" template <typename Row>
+int run_simulate(ocean_generator* gen, int num_bodies, const Row* bodies_host, ocean_body_state* states_dev, int world,
                  const ocean_buoyancy_point* points_dev, const float* drag_areas_dev, int num_cascades, float density, float dt, int substeps,
                  float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_dev, ocean_drag_result* drag_dev,
                  float* transforms_dev, const DriveHost* drive = nullptr, ocean_drive_result* drive_dev = nullptr, float* tensions_dev = nullptr) {
+    constexpr bool kMesh = std::is_same<Row, ocean_floating_hull>::value;
+    BodyScratch& sc = gen->body;
     int rc;
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
     const size_t B = (size_t)num_bodies;
     const int actuators = drive ? drive->actuators() : 0;
     const int queried = world + actuators;              // the hull's world points, then the actuators'
-    OCEAN_CUDA(gen->sim_r2.grow(gen, B));
-    OCEAN_CUDA(gen->buoy_bodies.grow(gen, B));
-    OCEAN_CUDA(gen->drag_velocities.grow(gen, B));
-    OCEAN_CUDA(gen->buoy_q.grow(gen, (size_t)queried));
-    OCEAN_CUDA(gen->buoy_samples.grow(gen, (size_t)queried));
-    float* wv = nullptr;                                // every sub-step reads the same snapshots
-    if (queried > 0 && gen->wake.coupling_live()) {
-        OCEAN_CUDA(gen->wake.wv.grow(gen, (size_t)queried));
-        wv = gen->wake.wv.ptr;
+    OCEAN_CUDA(sc.r2.grow(gen, B));
+    OCEAN_CUDA(sc.velocities.grow(gen, B));
+    OCEAN_CUDA(sc.q.grow(gen, (size_t)queried));
+    OCEAN_CUDA(sc.samples.grow(gen, (size_t)queried));
+    if constexpr (kMesh) {
+        OCEAN_CUDA(sc.hull_poses.grow(gen, B));
+        OCEAN_CUDA(sc.rows.grow(gen, B));
+        OCEAN_CUDA(sc.corners.grow(gen, 2 * (size_t)world));
+    } else {
+        OCEAN_CUDA(sc.poses.grow(gen, B));
     }
+    float* wv = nullptr;                                // every sub-step reads the same snapshots
+    OCEAN_CUDA(gen->wake.vertical_velocities(gen, (size_t)queried, &wv));
     ocean::DriveArgs da{};
     if (drive) {
         da.num_thrusters = drive->num_thrusters;
         da.num_foils = drive->num_foils;
         da.num_tethers = drive->num_tethers;
         if (drive->num_thrusters > 0) {
-            OCEAN_CUDA(gen->drive_thrusters.upload(gen, drive->thrusters, (size_t)drive->num_thrusters));
-            da.thrusters = gen->drive_thrusters.ptr;
+            OCEAN_CUDA(sc.thrusters.upload(gen, drive->thrusters, (size_t)drive->num_thrusters));
+            da.thrusters = sc.thrusters.ptr;
         }
         if (drive->num_foils > 0) {
-            OCEAN_CUDA(gen->drive_foils.upload(gen, drive->foils, (size_t)drive->num_foils));
-            da.foils = gen->drive_foils.ptr;
+            OCEAN_CUDA(sc.foils.upload(gen, drive->foils, (size_t)drive->num_foils));
+            da.foils = sc.foils.ptr;
         }
         if (drive->num_tethers > 0) {
-            OCEAN_CUDA(gen->drive_tethers.upload(gen, drive->tethers, (size_t)drive->num_tethers));
-            OCEAN_CUDA(gen->drive_tether_forces.grow(gen, (size_t)drive->num_tethers));
-            da.tethers = gen->drive_tethers.ptr;
+            OCEAN_CUDA(sc.tethers.upload(gen, drive->tethers, (size_t)drive->num_tethers));
+            OCEAN_CUDA(sc.tether_forces.grow(gen, (size_t)drive->num_tethers));
+            da.tethers = sc.tethers.ptr;
             if (!tensions_dev) {
-                OCEAN_CUDA(gen->drive_tensions.grow(gen, (size_t)drive->num_tethers));
-                tensions_dev = gen->drive_tensions.ptr;
+                OCEAN_CUDA(sc.tensions.grow(gen, (size_t)drive->num_tethers));
+                tensions_dev = sc.tensions.ptr;
             }
         }
         if (drive->loads) {
-            OCEAN_CUDA(gen->drive_loads.upload(gen, drive->loads, B));
-            da.loads = gen->drive_loads.ptr;
+            OCEAN_CUDA(sc.loads.upload(gen, drive->loads, B));
+            da.loads = sc.loads.ptr;
         }
         build_incidence(gen, num_bodies, *drive);
-        OCEAN_CUDA(gen->drive_incidence.upload(gen, gen->drive_incidence_host.data(), gen->drive_incidence_host.size()));
-        da.incidence_offsets = gen->drive_incidence.ptr;
-        da.incidence = gen->drive_incidence.ptr + B + 1;
-        OCEAN_CUDA(gen->drive_sums.grow(gen, B));
+        OCEAN_CUDA(sc.incidence.upload(gen, sc.incidence_host.data(), sc.incidence_host.size()));
+        da.incidence_offsets = sc.incidence.ptr;
+        da.incidence = sc.incidence.ptr + B + 1;
+        OCEAN_CUDA(sc.sums.grow(gen, B));
         if (!drive_dev) {
-            OCEAN_CUDA(gen->drive_results.grow(gen, B));
-            drive_dev = gen->drive_results.ptr;
+            OCEAN_CUDA(sc.drive.grow(gen, B));
+            drive_dev = sc.drive.ptr;
         }
     }
     if (!hydrostatic_dev) {
-        OCEAN_CUDA(gen->buoy_results.grow(gen, B));
-        hydrostatic_dev = gen->buoy_results.ptr;
+        OCEAN_CUDA(sc.hydrostatic.grow(gen, B));
+        hydrostatic_dev = sc.hydrostatic.ptr;
     }
     if (!drag_dev) {
-        OCEAN_CUDA(gen->drag_results.grow(gen, B));
-        drag_dev = gen->drag_results.ptr;
+        OCEAN_CUDA(sc.drag.grow(gen, B));
+        drag_dev = sc.drag.ptr;
     }
-    OCEAN_CUDA(gen->sim_bodies.upload(gen, bodies_host, B));
-    if ((rc = upload_offsets(gen, num_bodies, bodies_host))) return rc;
-    ocean_floating_body* bodies = gen->sim_bodies.ptr;
-    ocean_buoyancy_body* poses = gen->buoy_bodies.ptr;
-    ocean_body_velocity* velocities = gen->drag_velocities.ptr;
-    OCEAN_CUDA(ocean::launch_bodies_prepare(bodies, states_dev, num_bodies, points_dev, gen->sim_r2.ptr, poses, velocities, gen->stream));
+    if constexpr (kMesh) {
+        OCEAN_CUDA(sc.hull_rows.upload(gen, bodies_host, B));
+        if ((rc = upload_offsets(gen, num_bodies, [&](int b) { return sc.meshes_host[bodies_host[b].mesh].num_vertices; }))) return rc;
+        OCEAN_CUDA(ocean::launch_hull_prepare(sc.hull_rows.ptr, states_dev, num_bodies, sc.meshes.ptr, sc.vertices.ptr, sc.r2.ptr,
+                                              sc.hull_poses.ptr, sc.velocities.ptr, sc.rows.ptr, gen->stream));
+    } else {
+        OCEAN_CUDA(sc.rows.upload(gen, bodies_host, B));
+        if ((rc = upload_offsets(gen, num_bodies, [&](int b) { return bodies_host[b].num_points; }))) return rc;
+        OCEAN_CUDA(ocean::launch_bodies_prepare(sc.rows.ptr, states_dev, num_bodies, points_dev, sc.r2.ptr, sc.poses.ptr, sc.velocities.ptr,
+                                                gen->stream));
+    }
     gen->kernel_launches += 1;
+    const ocean_floating_body* bodies = sc.rows.ptr;
+    ocean_body_velocity* velocities = sc.velocities.ptr;
+    // the pose rows the integrators write: k_bodies_integrate writes a mesh hull's rows as ocean_buoyancy_body rows
+    ocean_buoyancy_body* poses = kMesh ? reinterpret_cast<ocean_buoyancy_body*>(sc.hull_poses.ptr) : sc.poses.ptr;
     const float h = dt / (float)substeps;
     const float half_rho = 0.5f * density;
     for (int s = 0; s < substeps; ++s) {
         float* transforms = s == substeps - 1 ? transforms_dev : nullptr;
-        if (actuators > 0) {
-            OCEAN_CUDA(ocean::launch_actuator_transform(da, poses, gen->buoy_q.ptr + world, gen->stream));
+        if constexpr (kMesh) {
+            if ((rc = launch_hull_sequence(gen, sc.hull_poses.ptr, velocities, num_bodies, world, num_cascades, density, tolerance,
+                                           max_iterations, hydrostatic_dev, drag_dev, sc.samples.ptr, wv)))
+                return rc;
+        } else {
+            if (actuators > 0) {
+                OCEAN_CUDA(ocean::launch_actuator_transform(da, poses, sc.q.ptr + world, gen->stream));
+                gen->kernel_launches += 1;
+            }
+            if ((rc = launch_buoyancy_sequence(gen, poses, sc.offsets.ptr, num_bodies, world, points_dev, num_cascades, density, tolerance,
+                                               max_iterations, hydrostatic_dev, sc.samples.ptr, wv, queried)))
+                return rc;
+            OCEAN_CUDA(ocean::launch_drag_reduce(poses, velocities, sc.offsets.ptr, num_bodies, points_dev, drag_areas_dev, sc.samples.ptr,
+                                                 gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, half_rho, drag_dev, wv,
+                                                 gen->stream));
             gen->kernel_launches += 1;
         }
-        if ((rc = launch_buoyancy_sequence(gen, poses, gen->buoy_offsets.ptr, num_bodies, world, points_dev, num_cascades, density, tolerance,
-                                           max_iterations, hydrostatic_dev, gen->buoy_samples.ptr, wv, queried)))
-            return rc;
-        OCEAN_CUDA(ocean::launch_drag_reduce(poses, velocities, gen->buoy_offsets.ptr, num_bodies, points_dev, drag_areas_dev,
-                                             gen->buoy_samples.ptr, gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, half_rho,
-                                             drag_dev, wv, gen->stream));
         if (!drive) {
-            OCEAN_CUDA(ocean::launch_bodies_integrate(bodies, gen->sim_r2.ptr, num_bodies, hydrostatic_dev, drag_dev, density, h, states_dev,
-                                                      poses, velocities, transforms, gen->stream));
-            gen->kernel_launches += 2;
+            OCEAN_CUDA(ocean::launch_bodies_integrate(bodies, sc.r2.ptr, num_bodies, hydrostatic_dev, drag_dev, density, h, states_dev, poses,
+                                                      velocities, transforms, gen->stream));
+            gen->kernel_launches += 1;
             continue;
         }
         if (da.num_tethers > 0) {
-            OCEAN_CUDA(ocean::launch_tethers(da, poses, velocities, gen->drive_tether_forces.ptr, tensions_dev, gen->stream));
+            OCEAN_CUDA(ocean::launch_tethers(da, poses, velocities, sc.tether_forces.ptr, tensions_dev, gen->stream));
             gen->kernel_launches += 1;
         }
-        OCEAN_CUDA(ocean::launch_drive_reduce(da, num_bodies, bodies, gen->sim_r2.ptr, poses, velocities, hydrostatic_dev, drag_dev,
-                                              gen->buoy_samples.ptr + world, wv ? wv + world : nullptr, gen->drive_tether_forces.ptr,
-                                              gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, density, h, gen->drive_sums.ptr,
-                                              drive_dev, gen->stream));
-        OCEAN_CUDA(ocean::launch_bodies_integrate_driven(bodies, num_bodies, gen->drive_sums.ptr, h, states_dev, poses, velocities, transforms,
+        OCEAN_CUDA(ocean::launch_drive_reduce(da, num_bodies, bodies, sc.r2.ptr, poses, velocities, hydrostatic_dev, drag_dev,
+                                              sc.samples.ptr + world, wv ? wv + world : nullptr, sc.tether_forces.ptr, gen->velocity.ptr,
+                                              gen->map_size, num_cascades, gen->q_scales.ptr, density, h, sc.sums.ptr, drive_dev, gen->stream));
+        OCEAN_CUDA(ocean::launch_bodies_integrate_driven(bodies, num_bodies, sc.sums.ptr, h, states_dev, poses, velocities, transforms,
                                                          gen->stream));
-        gen->kernel_launches += 3;
+        gen->kernel_launches += 2;
     }
     return OCEAN_OK;
 }
@@ -2080,13 +2137,11 @@ int ocean_simulate_driven_bodies_device(ocean_generator* gen, int num_bodies, co
     if (num_bodies == 0) return OCEAN_OK;
     if (world > 0 && !points_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
-    if (!drive.any()) {                                 // ocean_simulate_bodies, with a zero drive record
-        if (drive_dev) OCEAN_CUDA(cudaMemsetAsync(drive_dev, 0, sizeof(ocean_drive_result) * (size_t)num_bodies, gen->stream));
-        return run_simulate(gen, num_bodies, bodies_host, states_dev, world, points_dev, drag_areas_dev, num_cascades, density, dt, substeps,
-                            tolerance, max_iterations, hydrostatic_dev, drag_dev, transforms_dev);
-    }
+    if (!drive.any() && drive_dev)                      // ocean_simulate_bodies, with a zero drive record
+        OCEAN_CUDA(cudaMemsetAsync(drive_dev, 0, sizeof(ocean_drive_result) * (size_t)num_bodies, gen->stream));
     return run_simulate(gen, num_bodies, bodies_host, states_dev, world, points_dev, drag_areas_dev, num_cascades, density, dt, substeps,
-                        tolerance, max_iterations, hydrostatic_dev, drag_dev, transforms_dev, &drive, drive_dev, tensions_dev);
+                        tolerance, max_iterations, hydrostatic_dev, drag_dev, transforms_dev, drive.any() ? &drive : nullptr, drive_dev,
+                        tensions_dev);
 }
 
 int ocean_simulate_driven_bodies(ocean_generator* gen, int num_bodies, const ocean_floating_body* bodies_host, ocean_body_state* states_host,
@@ -2130,8 +2185,6 @@ static_assert(offsetof(ocean_hull_body, transform) == offsetof(ocean_buoyancy_bo
               "k_bodies_integrate writes hull pose rows as ocean_buoyancy_body rows");
 
 namespace {
-bool finite_nonnegative_coefficient(float x) { return x >= 0.0f && std::isfinite(x); }
-
 // Every check of ocean_hull_set_meshes, on the host, before anything is uploaded; volumes (may be null) receives each mesh's
 // signed volume, sum over its triangles of p0 . (p2 x p1) / 6 in binary64 (Godot's clockwise winding: positive when closed
 // and wound outward).
@@ -2154,7 +2207,7 @@ int check_hull_meshes(int num_meshes, const ocean_hull_mesh* meshes, int num_ver
             return fail(OCEAN_ERR_INVALID_ARGUMENT, "mesh %d: vertices [%lld, %lld) outside [0, %d)", m, fv, fv + nv, num_vertices);
         if (nt < 0 || ft < 0 || ft + nt > num_triangles)
             return fail(OCEAN_ERR_INVALID_ARGUMENT, "mesh %d: triangles [%lld, %lld) outside [0, %d)", m, ft, ft + nt, num_triangles);
-        if (!finite_nonnegative_coefficient(h.normal_drag) || !finite_nonnegative_coefficient(h.tangential_drag))
+        if (!finite_nonnegative(h.normal_drag) || !finite_nonnegative(h.tangential_drag))
             return fail(OCEAN_ERR_INVALID_ARGUMENT, "mesh %d: drag coefficients %g, %g are not finite and >= 0", m, h.normal_drag,
                         h.tangential_drag);
         const int32_t* tri = triangles + 3 * ft;
@@ -2187,78 +2240,53 @@ extern "C++" template <typename Row>
 int check_hull_bodies(const ocean_generator* gen, int num_bodies, const Row* bodies, int* world) {
     if (num_bodies < 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "num_bodies %d is negative", num_bodies);
     if (num_bodies > 0 && !bodies) return fail(OCEAN_ERR_INVALID_ARGUMENT, "bodies is NULL");
-    const int meshes = (int)gen->hull_meshes_host.size();
+    const std::vector<ocean_hull_mesh>& set = gen->body.meshes_host;
+    const int meshes = (int)set.size();
     if (num_bodies > 0 && meshes == 0) return fail(OCEAN_ERR_INVALID_ARGUMENT, "no hull meshes are registered (ocean_hull_set_meshes)");
     long long total = 0;
     for (int b = 0; b < num_bodies; ++b) {
         if (bodies[b].mesh < 0 || bodies[b].mesh >= meshes)
             return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: mesh %d outside [0, %d)", b, bodies[b].mesh, meshes);
-        total += gen->hull_meshes_host[bodies[b].mesh].num_vertices;
+        total += set[bodies[b].mesh].num_vertices;
     }
     if (total > INT32_MAX) return fail(OCEAN_ERR_INVALID_ARGUMENT, "%lld world vertices exceed INT32_MAX", total);
     *world = (int)total;
     return OCEAN_OK;
 }
 
-// The exclusive prefix of the bodies' meshes' num_vertices into gen->buoy_offsets_host, uploaded to gen->buoy_offsets.
-extern "C++" template <typename Row>
-int upload_hull_offsets(ocean_generator* gen, int num_bodies, const Row* bodies_host) {
-    std::vector<int>& offsets = gen->buoy_offsets_host;
-    offsets.resize((size_t)num_bodies);
-    for (int b = 0, start = 0; b < num_bodies; start += gen->hull_meshes_host[bodies_host[b].mesh].num_vertices, ++b) offsets[b] = start;
-    OCEAN_CUDA(gen->buoy_offsets.upload(gen, offsets.data(), (size_t)num_bodies));
-    return OCEAN_OK;
-}
-
 int check_hull_forces_args(const ocean_generator* gen, int num_bodies, const ocean_hull_body* bodies, const ocean_body_velocity* velocities,
                            float density, float tolerance, int max_iterations, int* world) {
-    int rc = check_surface_args(0, tolerance, max_iterations);
+    int rc = check_solver_args(tolerance, max_iterations);
     if (rc) return rc;
-    if (!(density > 0.0f) || !std::isfinite(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
+    if (!finite_positive(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
     if ((rc = check_hull_bodies(gen, num_bodies, bodies, world))) return rc;
     if (num_bodies > 0 && !velocities) return fail(OCEAN_ERR_INVALID_ARGUMENT, "velocities is NULL");
     return OCEAN_OK;
 }
 
-// Grows the per-world-vertex scratch of a hull call: query points, corners, the surface records when the caller wants none
-// (returned in *samples) and the wake's vertical velocities while the coupling is live (*wv, else null).
-int grow_hull_scratch(ocean_generator* gen, int world, ocean_surface_sample** samples, float** wv) {
-    const size_t n = (size_t)world;
-    OCEAN_CUDA(gen->buoy_q.grow(gen, n));
-    OCEAN_CUDA(gen->hull_corners.grow(gen, 2 * n));
-    if (!*samples) {
-        OCEAN_CUDA(gen->buoy_samples.grow(gen, n));
-        *samples = gen->buoy_samples.ptr;
-    }
-    *wv = nullptr;
-    if (world > 0 && gen->wake.coupling_live()) {
-        OCEAN_CUDA(gen->wake.wv.grow(gen, n));
-        *wv = gen->wake.wv.ptr;
-    }
-    return OCEAN_OK;
-}
-
 // The hull-forces launches on a pose table, velocities and offsets already in device memory (the poses may be written by
-// earlier kernels on the stream), with the map scales in gen->q_scales and the scratch grown to `world`.
+// earlier kernels on the stream), with the map scales in gen->q_scales, gen->body.q and gen->body.corners grown to `world`, and
+// wv the wake's vertical velocities (or null).
 int launch_hull_sequence(ocean_generator* gen, const ocean_hull_body* poses_dev, const ocean_body_velocity* velocities_dev, int num_bodies,
                          int world, int num_cascades, float density, float tolerance, int max_iterations, ocean_buoyancy_result* hydrostatic_dev,
                          ocean_drag_result* drag_dev, ocean_surface_sample* samples, float* wv) {
+    const BodyScratch& sc = gen->body;
     int rc;
-    float4* corner_r = gen->hull_corners.ptr;
+    float4* corner_r = sc.corners.ptr;
     float4* corner_u = corner_r + world;
     if (world > 0) {
-        OCEAN_CUDA(ocean::launch_hull_transform(poses_dev, gen->buoy_offsets.ptr, num_bodies, gen->hull_meshes.ptr, gen->hull_vertices.ptr, world,
-                                                gen->buoy_q.ptr, corner_r, gen->stream));
+        OCEAN_CUDA(ocean::launch_hull_transform(poses_dev, sc.offsets.ptr, num_bodies, sc.meshes.ptr, sc.vertices.ptr, world, sc.q.ptr, corner_r,
+                                                gen->stream));
         gen->kernel_launches += 1;
-        if ((rc = run_query_surface(gen, world, gen->buoy_q.ptr, num_cascades, tolerance, max_iterations, samples, wv))) return rc;
+        if ((rc = run_query_surface(gen, world, sc.q.ptr, num_cascades, tolerance, max_iterations, samples, wv))) return rc;
         OCEAN_CUDA(ocean::launch_hull_vertex(samples, world, gen->velocity.ptr, gen->map_size, num_cascades, gen->q_scales.ptr, wv, corner_r,
                                              corner_u, gen->stream));
         gen->kernel_launches += 1;
     }
     const float rho_g = density * 9.81f;                                 // G, wave_generator.gd:5, in binary32
     const float half_rho = 0.5f * density;
-    OCEAN_CUDA(ocean::launch_hull_reduce(poses_dev, velocities_dev, gen->buoy_offsets.ptr, num_bodies, gen->hull_meshes.ptr, gen->hull_triangles.ptr,
-                                         corner_r, corner_u, samples, rho_g, half_rho, tolerance, hydrostatic_dev, drag_dev, gen->stream));
+    OCEAN_CUDA(ocean::launch_hull_reduce(poses_dev, velocities_dev, sc.offsets.ptr, num_bodies, sc.meshes.ptr, sc.triangles.ptr, corner_r,
+                                         corner_u, samples, rho_g, half_rho, tolerance, hydrostatic_dev, drag_dev, gen->stream));
     gen->kernel_launches += 1;
     return OCEAN_OK;
 }
@@ -2266,21 +2294,12 @@ int launch_hull_sequence(ocean_generator* gen, const ocean_hull_body* poses_dev,
 // ocean_simulate_bodies' checks on hull bodies; *world as for check_hull_bodies.
 int check_simulate_hull_args(const ocean_generator* gen, int num_bodies, const ocean_floating_hull* bodies, const ocean_body_state* states,
                              float density, float dt, int substeps, float tolerance, int max_iterations, int* world) {
-    int rc = check_surface_args(0, tolerance, max_iterations);
+    int rc = check_solver_args(tolerance, max_iterations);
     if (rc) return rc;
-    if (!finite_positive(density)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "density %g is not finite and > 0", density);
-    if (!finite_positive(dt)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "dt %g is not finite and > 0", dt);
-    if (substeps < 1 || substeps > 64) return fail(OCEAN_ERR_INVALID_ARGUMENT, "substeps %d outside [1, 64]", substeps);
+    if ((rc = check_step_args(density, dt, substeps))) return rc;
     if ((rc = check_hull_bodies(gen, num_bodies, bodies, world))) return rc;
     if (num_bodies > 0 && !states) return fail(OCEAN_ERR_INVALID_ARGUMENT, "states is NULL");
-    for (int b = 0; b < num_bodies; ++b) {
-        const ocean_floating_hull& fb = bodies[b];
-        if (!finite_positive(fb.mass)) return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: mass %g is not finite and > 0", b, fb.mass);
-        for (int k = 0; k < 3; ++k)
-            if (!finite_positive(fb.inertia[k]))
-                return fail(OCEAN_ERR_INVALID_ARGUMENT, "body %d: inertia[%d] %g is not finite and > 0", b, k, fb.inertia[k]);
-    }
-    return OCEAN_OK;
+    return check_mass_inertia(num_bodies, bodies);
 }
 }  // namespace
 
@@ -2290,20 +2309,21 @@ int ocean_hull_set_meshes(ocean_generator* gen, int num_meshes, const ocean_hull
     if (rc) return rc;
     DeviceScope device_scope__;
     if ((rc = enter_gen(gen, device_scope__))) return rc;
-    gen->hull_meshes_host.clear();                      // off until the new set is in place
+    BodyScratch& sc = gen->body;
+    sc.meshes_host.clear();                             // off until the new set is in place
     if (num_meshes == 0) {
         OCEAN_CUDA(cudaStreamSynchronize(gen->stream));  // an earlier call may still read the set
-        gen->hull_meshes.release();
-        gen->hull_vertices.release();
-        gen->hull_triangles.release();
+        sc.meshes.release();
+        sc.vertices.release();
+        sc.triangles.release();
         return OCEAN_OK;
     }
     // stream order puts the copies after the calls that read the old set; the call returns once they are done
-    OCEAN_CUDA(gen->hull_meshes.upload(gen, meshes_host, (size_t)num_meshes));
-    if (num_vertices > 0) OCEAN_CUDA(gen->hull_vertices.upload(gen, vertices_host, 3 * (size_t)num_vertices));
-    if (num_triangles > 0) OCEAN_CUDA(gen->hull_triangles.upload(gen, triangles_host, 3 * (size_t)num_triangles));
+    OCEAN_CUDA(sc.meshes.upload(gen, meshes_host, (size_t)num_meshes));
+    if (num_vertices > 0) OCEAN_CUDA(sc.vertices.upload(gen, vertices_host, 3 * (size_t)num_vertices));
+    if (num_triangles > 0) OCEAN_CUDA(sc.triangles.upload(gen, triangles_host, 3 * (size_t)num_triangles));
     OCEAN_CUDA(cudaStreamSynchronize(gen->stream));
-    gen->hull_meshes_host.assign(meshes_host, meshes_host + num_meshes);
+    sc.meshes_host.assign(meshes_host, meshes_host + num_meshes);
     return OCEAN_OK;
 }
 
@@ -2319,14 +2339,19 @@ int ocean_hull_forces_device(ocean_generator* gen, int num_bodies, const ocean_h
     if (!hydrostatic_dev || !drag_dev) return fail(OCEAN_ERR_INVALID_ARGUMENT, "a device buffer is NULL");
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
     if ((rc = refresh_velocity(gen, nullptr))) return rc;
-    ocean_surface_sample* samples = samples_dev;
+    BodyScratch& sc = gen->body;
+    const size_t n = (size_t)world;
+    OCEAN_CUDA(sc.q.grow(gen, n));
+    OCEAN_CUDA(sc.corners.grow(gen, 2 * n));
+    if (!samples_dev) OCEAN_CUDA(sc.samples.grow(gen, n));
+    ocean_surface_sample* samples = samples_dev ? samples_dev : sc.samples.ptr;
     float* wv = nullptr;
-    if ((rc = grow_hull_scratch(gen, world, &samples, &wv))) return rc;
-    OCEAN_CUDA(gen->hull_poses.upload(gen, bodies_host, (size_t)num_bodies));
-    OCEAN_CUDA(gen->drag_velocities.upload(gen, velocities_host, (size_t)num_bodies));
-    if ((rc = upload_hull_offsets(gen, num_bodies, bodies_host))) return rc;
-    return launch_hull_sequence(gen, gen->hull_poses.ptr, gen->drag_velocities.ptr, num_bodies, world, num_cascades, density, tolerance,
-                                max_iterations, hydrostatic_dev, drag_dev, samples, wv);
+    OCEAN_CUDA(gen->wake.vertical_velocities(gen, n, &wv));
+    OCEAN_CUDA(sc.hull_poses.upload(gen, bodies_host, (size_t)num_bodies));
+    OCEAN_CUDA(sc.velocities.upload(gen, velocities_host, (size_t)num_bodies));
+    if ((rc = upload_offsets(gen, num_bodies, [&](int b) { return sc.meshes_host[bodies_host[b].mesh].num_vertices; }))) return rc;
+    return launch_hull_sequence(gen, sc.hull_poses.ptr, sc.velocities.ptr, num_bodies, world, num_cascades, density, tolerance, max_iterations,
+                                hydrostatic_dev, drag_dev, samples, wv);
 }
 
 int ocean_hull_forces(ocean_generator* gen, int num_bodies, const ocean_hull_body* bodies_host, const ocean_body_velocity* velocities_host,
@@ -2359,41 +2384,8 @@ int ocean_simulate_hull_bodies_device(ocean_generator* gen, int num_bodies, cons
         return rc;
     if (num_bodies == 0) return OCEAN_OK;
     if ((rc = upload_scales(gen, num_cascades, map_scales_host))) return rc;       // the last check: nothing is launched before it
-    if ((rc = refresh_velocity(gen, nullptr))) return rc;
-    const size_t B = (size_t)num_bodies;
-    ocean_surface_sample* samples = nullptr;
-    float* wv = nullptr;                                // every sub-step reads the same snapshots
-    if ((rc = grow_hull_scratch(gen, world, &samples, &wv))) return rc;
-    OCEAN_CUDA(gen->sim_r2.grow(gen, B));
-    OCEAN_CUDA(gen->sim_bodies.grow(gen, B));
-    OCEAN_CUDA(gen->hull_poses.grow(gen, B));
-    OCEAN_CUDA(gen->drag_velocities.grow(gen, B));
-    if (!hydrostatic_dev) {
-        OCEAN_CUDA(gen->buoy_results.grow(gen, B));
-        hydrostatic_dev = gen->buoy_results.ptr;
-    }
-    if (!drag_dev) {
-        OCEAN_CUDA(gen->drag_results.grow(gen, B));
-        drag_dev = gen->drag_results.ptr;
-    }
-    OCEAN_CUDA(gen->hull_bodies.upload(gen, bodies_host, B));
-    if ((rc = upload_hull_offsets(gen, num_bodies, bodies_host))) return rc;
-    ocean_hull_body* poses = gen->hull_poses.ptr;
-    ocean_body_velocity* velocities = gen->drag_velocities.ptr;
-    OCEAN_CUDA(ocean::launch_hull_prepare(gen->hull_bodies.ptr, states_dev, num_bodies, gen->hull_meshes.ptr, gen->hull_vertices.ptr,
-                                          gen->sim_r2.ptr, poses, velocities, gen->sim_bodies.ptr, gen->stream));
-    gen->kernel_launches += 1;
-    const float h = dt / (float)substeps;
-    for (int s = 0; s < substeps; ++s) {
-        if ((rc = launch_hull_sequence(gen, poses, velocities, num_bodies, world, num_cascades, density, tolerance, max_iterations,
-                                       hydrostatic_dev, drag_dev, samples, wv)))
-            return rc;
-        OCEAN_CUDA(ocean::launch_bodies_integrate(gen->sim_bodies.ptr, gen->sim_r2.ptr, num_bodies, hydrostatic_dev, drag_dev, density, h,
-                                                  states_dev, reinterpret_cast<ocean_buoyancy_body*>(poses), velocities,
-                                                  s == substeps - 1 ? transforms_dev : nullptr, gen->stream));
-        gen->kernel_launches += 1;
-    }
-    return OCEAN_OK;
+    return run_simulate(gen, num_bodies, bodies_host, states_dev, world, nullptr, nullptr, num_cascades, density, dt, substeps, tolerance,
+                        max_iterations, hydrostatic_dev, drag_dev, transforms_dev);
 }
 
 int ocean_simulate_hull_bodies(ocean_generator* gen, int num_bodies, const ocean_floating_hull* bodies_host, ocean_body_state* states_host,

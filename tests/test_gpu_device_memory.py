@@ -113,6 +113,61 @@ def _simulate_bodies(g, scales, n):
     g.simulate_bodies(b, s, pts, cda, scales, 1.0 / 60.0, 2, return_records=True, return_transforms=True)
 
 
+def _drive_bodies(g, scales, n):
+    """_simulate_bodies with one thruster, one foil and one load per body and a tether from each body to the next (the last one
+    anchored), so that every drive array is staged."""
+    pts, cda = _hull(g, n)
+    b, s = _floating(g, n)
+    k = np.arange(n)
+    th = np.zeros(n, g.THRUSTER)
+    th["body"], th["direction"], th["thrust"], th["half_height"] = k, (1.0, 0.0, 0.0), 50.0, 0.1
+    fo = np.zeros(n, g.FOIL)
+    fo["body"], fo["normal"], fo["area"], fo["half_height"] = k, (0.0, 0.0, 1.0), 0.5, 0.1
+    te = np.zeros(n, g.TETHER)
+    te["body_a"], te["body_b"] = k, np.where(k + 1 < n, k + 1, -1)
+    te["rest_length"], te["stiffness"], te["damping"] = 5.0, 100.0, 10.0
+    g.drive_bodies(b, s, pts, cda, scales, 1.0 / 60.0, 2, thrusters=th, foils=fo, loads=np.zeros(n, g.BODY_LOAD), tethers=te,
+                   return_records=True, return_tensions=True, return_transforms=True)
+
+
+def _hull_meshes(g):
+    """Registers one closed unit box (8 vertices, 12 triangles); the same set again keeps the count."""
+    v = np.array([[x, y, z] for x in (-0.5, 0.5) for y in (-0.5, 0.5) for z in (-0.5, 0.5)], np.float32)
+    t = np.array([[0, 1, 3], [0, 3, 2], [4, 6, 7], [4, 7, 5], [0, 4, 5], [0, 5, 1], [2, 3, 7], [2, 7, 6], [0, 2, 6], [0, 6, 4],
+                  [1, 5, 7], [1, 7, 3]], np.int32)
+    m = np.zeros(1, g.HULL_MESH)
+    m["num_vertices"], m["num_triangles"], m["normal_drag"], m["tangential_drag"] = len(v), len(t), 1.0, 0.1
+    g.set_hull_meshes(m, v, t)
+
+
+def _hull_poses(g, n):
+    b = np.zeros(n, g.HULL_BODY)
+    b["transform"][:, [0, 5, 10]] = 1.0
+    b["transform"][:, [3, 11]] = _points(n)
+    return b
+
+
+def _floating_hulls(g, n):
+    b = np.zeros(n, g.FLOATING_HULL)
+    b["mass"] = 200.0
+    b["inertia"] = 50.0
+    s = np.zeros(n, g.BODY_STATE)
+    s["position"][:, [0, 2]] = _points(n)
+    s["orientation"][:, 3] = 1.0
+    return b, s
+
+
+def _hull_forces(g, scales, n):
+    _hull_meshes(g)
+    g.hull_forces(_hull_poses(g, n), np.zeros(n, g.BODY_VELOCITY), scales, return_samples=True)
+
+
+def _simulate_hull_bodies(g, scales, n):
+    _hull_meshes(g)
+    b, s = _floating_hulls(g, n)
+    g.simulate_hull_bodies(b, s, scales, 1.0 / 60.0, 2, return_records=True, return_transforms=True)
+
+
 def _debug_device_math(g, scales, n):
     from godotoceanwaves_b200.native import check, load_library
     a = np.linspace(-10, 10, n, dtype=np.float32)
@@ -142,7 +197,7 @@ def _sample_wake(g, scales, n):
 
 
 OPS = [_sample_maps, _sample_velocity, _query_surface, _raycast, _extract_spray, _buoyancy, _body_forces, _simulate_bodies,
-       _debug_device_math, _wake_step, _sample_wake]
+       _drive_bodies, _hull_forces, _simulate_hull_bodies, _debug_device_math, _wake_step, _sample_wake]
 
 
 @pytest.mark.parametrize("op", OPS, ids=[op.__name__[1:] for op in OPS])
@@ -172,6 +227,9 @@ def _invalid_call(op, g, scales):
     rays, ps, emitter = _rays(g, n), np.ones(3, np.float32), g.default_spray_emitter()
     poses, velocities, (hull, cda) = _poses(g, 2), np.zeros(2, g.BODY_VELOCITY), _hull(g, 2)
     bodies, states = _floating(g, 2)
+    thrusters = np.zeros(2, g.THRUSTER)
+    thrusters["body"] = (0, 1)
+    hull_poses, (hulls, _) = _hull_poses(g, 2), _floating_hulls(g, 2)
     count = ctypes.c_int()
     calls = {
         "sample_maps": lambda: lib.ocean_sample_maps(h, n, P, C, S, None, O),
@@ -185,6 +243,13 @@ def _invalid_call(op, g, scales):
                                                      cda.ctypes.data, C, S, 1025.0, 1e-3, 8, None, O, None),
         "simulate_bodies": lambda: lib.ocean_simulate_bodies(h, 2, bodies.ctypes.data, states.ctypes.data, len(hull), None, cda.ctypes.data,
                                                              C, S, 1025.0, 1.0 / 60.0, 1, 1e-3, 8, None, None, None),
+        "drive_bodies": lambda: lib.ocean_simulate_driven_bodies(h, 2, bodies.ctypes.data, states.ctypes.data, len(hull), None,
+                                                                 cda.ctypes.data, C, S, 1025.0, 1.0 / 60.0, 1, 1e-3, 8, 2,
+                                                                 thrusters.ctypes.data, 0, None, None, 0, None, None, None, None, None, None),
+        "hull_forces": lambda: lib.ocean_hull_forces(h, 2, hull_poses.ctypes.data, velocities.ctypes.data, C, S, 1025.0, 1e-3, 8, None, O,
+                                                     None),
+        "simulate_hull_bodies": lambda: lib.ocean_simulate_hull_bodies(h, 2, hulls.ctypes.data, None, C, S, 1025.0, 1.0 / 60.0, 1, 1e-3, 8,
+                                                                       None, None, None),
         "debug_device_math": lambda: lib.ocean_debug_device_math(h, 0, n, P, P, None),
         "wake_step": lambda: lib.ocean_wake_step(h, 0.05, 1, 0, 0, n, None, 0, None),
         "sample_wake": lambda: lib.ocean_sample_wake(h, n, P, None),
@@ -193,7 +258,7 @@ def _invalid_call(op, g, scales):
 
 
 HOST_OPS = ["sample_maps", "sample_velocity", "query_surface", "raycast", "extract_spray", "spray_particles", "buoyancy", "body_forces",
-            "simulate_bodies", "debug_device_math", "wake_step", "sample_wake"]
+            "simulate_bodies", "drive_bodies", "hull_forces", "simulate_hull_bodies", "debug_device_math", "wake_step", "sample_wake"]
 
 
 @pytest.mark.parametrize("op", HOST_OPS)
@@ -203,6 +268,8 @@ def test_invalid_host_call_stages_nothing(op):
     g, _, scales = _gen()
     if op in ("wake_step", "sample_wake"):
         _wake_layer(g)
+    if op in ("hull_forces", "simulate_hull_bodies"):
+        _hull_meshes(g)                                         # so that the NULL buffer, not a missing mesh set, is rejected
     before = _bytes(g), g.info().kernel_launches
     assert _invalid_call(op, g, scales) == INVALID
     assert (_bytes(g), g.info().kernel_launches) == before
