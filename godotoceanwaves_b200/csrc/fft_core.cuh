@@ -147,15 +147,20 @@ constexpr int kE = 16;                                    // elements per thread
 __host__ __device__ constexpr int ilog2(int v) { return v <= 1 ? 0 : 1 + ilog2(v >> 1); }
 __device__ __forceinline__ int pad16(int idx) { return idx + (idx >> 4); }
 
+// pad16(x + c) == pad16(x) + pad16(c) whenever x or c is a multiple of 16.  The passes below split a padded index into the
+// thread's part, computed once, and a compile-time part, so that every element is an immediate offset from one address.
 // Loads the kE elements a thread owns in a pass of radix R from a (padded) shared buffer:
 // group g = t + TT*u, element a of the group sits at natural index a*(N/R) + g.
 template <int N, int R>
 __device__ __forceinline__ void pass_load(C2 (&v)[kE], const float4* __restrict__ buf, int t) {
     constexpr int TT = N / kE;
+    constexpr bool SPLIT = (N / R) % 16 == 0 && TT % 16 == 0;     // a*(N/R) + TT*u is a multiple of 16
+    const float4* base = SPLIT ? buf + pad16(t) : buf;
 #pragma unroll
     for (int u = 0; u < kE / R; ++u)
 #pragma unroll
-        for (int a = 0; a < R; ++a) v[u * R + a] = c2_from(buf[pad16(a * (N / R) + t + TT * u)]);
+        for (int a = 0; a < R; ++a)
+            v[u * R + a] = c2_from(SPLIT ? base[pad16(a * (N / R) + TT * u)] : buf[pad16(a * (N / R) + t + TT * u)]);
 }
 // Natural index of output b of group g after a pass of radix R that started at stride 2^LS0.
 template <int R, int LS0>
@@ -174,19 +179,40 @@ __device__ __forceinline__ void pass_compute(C2 (&v)[kE], int t, const float2* _
 template <int N, int R, int LS0>
 __device__ __forceinline__ void pass_store(const C2 (&v)[kE], float4* __restrict__ buf, int t) {
     constexpr int TT = N / kE;
+    // with TT a multiple of 2^LS0, out_index(t + TT*u, b) = out_index(t, 0) + TT*u*R + (b << LS0); the thread's part is a multiple
+    // of 16 when LS0 == 0 and R == 16, the element part when LS0 >= 4
+    constexpr bool SPLIT = TT % (1 << LS0) == 0 && ((LS0 == 0 && R % 16 == 0) || (LS0 >= 4 && (TT * R) % 16 == 0));
+    float4* base = SPLIT ? buf + pad16(out_index<R, LS0>(t, 0)) : buf;
 #pragma unroll
     for (int u = 0; u < kE / R; ++u)
 #pragma unroll
-        for (int b = 0; b < R; ++b) buf[pad16(out_index<R, LS0>(t + TT * u, b))] = c2_to(v[u * R + b]);
+        for (int b = 0; b < R; ++b) {
+            if (SPLIT) base[pad16(TT * u * R + (b << LS0))] = c2_to(v[u * R + b]);
+            else buf[pad16(out_index<R, LS0>(t + TT * u, b))] = c2_to(v[u * R + b]);
+        }
 }
-// Natural output index of register slot i (= u*RL + b) after the last pass.
+// Natural output index of register slot i (= u*RL + b) after the last pass, for 0 <= t < TT.  The group g = t + TT*u is below
+// TT * kE/RL = 2^LSL, so out_index<RL, LSL>(g, b) = g + (b << LSL): the thread's t plus a compile-time offset.
 template <int N>
 __device__ __forceinline__ int final_index(int t, int i) {
     using P = Plan<N>;
     constexpr int TT = N / kE;
     constexpr int RL = P::NP == 3 ? P::R2 : P::R1;
     constexpr int LSL = ilog2(N) - ilog2(RL);
+    static_assert(TT * (kE / RL) == (1 << LSL), "groups of the last pass");
     return out_index<RL, LSL>(t + TT * (i / RL), i % RL);
+}
+
+// For 0 <= t < TT the group g = t + TT*u of the last pass is below TT * kE/RL = 2^LSL, so final_index(t, i) = t + final_offset(i):
+// stores of the final outputs are compile-time offsets from the thread's first output.
+template <int N>
+__device__ __forceinline__ constexpr int final_offset(int i) {
+    using P = Plan<N>;
+    constexpr int TT = N / kE;
+    constexpr int RL = P::NP == 3 ? P::R2 : P::R1;
+    constexpr int LSL = ilog2(N) - ilog2(RL);
+    static_assert(TT * (kE / RL) == (1 << LSL), "groups of the last pass");
+    return TT * (i / RL) + ((i % RL) << LSL);
 }
 
 // Barrier among the N/16 threads that share one FFT's exchange buffer: they sit in one warp when
